@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py - headline benchmark of the Competitive-Collaboration training step on B200.
+"""bench.py - headline benchmark of the Competitive-Collaboration training step on H100.
 
   python bench.py --gpus N --steps K --warmup W          (N>1: launched under torch.distributed.run)
   python bench.py --impl reference ...                    (the reference algorithm's CPU path: oracle port)
+  python bench.py ... --dump-outputs DIR                  (also write what the last timed step computed, as .npy)
 
 One JSON line on rank 0.  metric = BASELINE.json's "train-step triplets/sec at 256x832x6lvl": frame
 snippets (target + 4 references) per second through forward + losses + backward + Adam.
@@ -10,7 +11,7 @@ snippets (target + 4 references) per second through forward + losses + backward 
   value     device-resident inputs, whole step replayed as one CUDA graph, CUDA-event timed, max over ranks
   e2e       same step through the public API with HOST (pinned) inputs: H2D of the 5 frames + intrinsics and
             a D2H read of the loss inside the timed region, every step
-  roofline  dominant kernel family (by measured share of the step) against the measured B200 peak;
+  roofline  dominant kernel family (by measured share of the step) against the H100 peak;
             roofline_warploss is the fused warp+loss kernel against the HBM peak (BASELINE metric, 2nd half)
   cpu_baseline  the oracle port of the reference step on this box's host cores (bounded sample)
 """
@@ -44,12 +45,13 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d['hbm_gbs'], tensor_burst=d['bf16_tflops'], tensor_sustained=d['bf16_tflops_sustained'],
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    # NVIDIA H100 SXM data sheet (700 W card, dense): 3.35 TB/s HBM3, 989 TFLOP/s BF16 - not measured here
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor_sustained=989.0, source='H100 SXM data sheet (not measured)')
 
 
 # ---------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -202,6 +204,8 @@ def measure_cfg(cfg, args, dev, rank, local, world, steps, full):
     ms_e2e = cdist.max_over_ranks(f0.elapsed_time(f1), dev)
     res = dict(ms_total=ms_total, ms_e2e=ms_e2e, steps=steps, warm=warm, launches_per_step=int(launches_per_step),
                in_bytes=in_bytes, loss=float(loss_host[0]), clocks=clocks, use_graph=use_graph, prof={})
+    if full and rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, loss, trainer)
     # the profile pass runs whole (eager) steps, all-reduce included: EVERY rank must take part
     if full and not args.no_profile:
         _say('%s: profile pass' % cfg)
@@ -232,7 +236,7 @@ def run_ours(args):
     if world == 1 and not args.no_side_configs:
         for c in ('cfg1', 'cfg2', 'cfg3'):
             if c != args.cfg:
-                side[c] = measure_cfg(c, args, dev, rank, local, world, max(5, min(args.steps, 10)), full=False)
+                side[c] = measure_cfg(c, args, dev, rank, local, world, args.steps, full=False)
     ref_gpu = None
     if world == 1 and not args.no_reference_gpu:
         _say('reference on the GPU')
@@ -251,9 +255,9 @@ def run_ours(args):
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': {'workload': CFG_WORKLOAD[args.cfg], 'global_batch': world * B, 'per_gpu_batch': B,
                        'frame': '%dx%d' % (H, W), 'levels': NLEVELS, 'parallelism': 'dp%d' % world,
-                       'conv_math': 'tcgen05 kind::tf32 x3 split precision (fp32-accurate, <=1e-4 parity)', 'cuda_graph': m['use_graph'],
+                       'conv_math': 'wgmma tf32 x3 split precision (fp32-accurate, <=1e-4 parity)', 'cuda_graph': m['use_graph'],
                        'numa_bound': numa_bound,
-                       'l2_policy': 'inputs and activations (>1 GB/step) exceed the 126 MB L2; no explicit flush',
+                       'l2_policy': 'inputs and activations (>1 GB/step) exceed the 50 MB L2; no explicit flush',
                        'e2e_input_path': ('pinned host batch -> H2D on a copy stream one step ahead (HostFeeder) -> D2D into the graph inputs; '
                                           'all steps+copies inside the timed region') if args.feed == 'prefetch' else
                                          'pinned host batch -> H2D into the graph inputs on the compute stream'},
@@ -274,6 +278,28 @@ def run_ours(args):
         if world == 1 and not args.no_cpu_baseline:
             out['cpu_baseline'] = cpu_baseline(args.cfg, budget_s=25.0)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 20          # elements per sampled array: 2 x 4 MB of float32
+
+
+def dump_outputs(out_dir, loss, trainer):
+    """What the last timed step handed its caller: the loss, and the parameters and gradients it produced (the flat
+    buffers of the optimiser, in its fixed parameter order).  Buffers longer than DUMP_SAMPLE are sampled at the same
+    seeded indices in every run, so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, 'loss.npy'), loss.detach().double().reshape(1).cpu().numpy())
+    opt = trainer.opt
+    for name, buf in (('params', opt.flat_p), ('grads', opt.flat_g)):
+        flat = buf.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(20240)
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, name + '.npy'), flat.float().cpu().numpy())
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -350,7 +376,7 @@ def profile_pass(trainer, tgt, refs, K, Kinv, steps=2):
                           'traffic': None, 'share_of_step': conv_ms / total, 'launches': sum(v['calls'] for v in conv.values()) // steps,
                           'executed_tensor_tflops': 3.0 * ach,
                           'peak_source': pk['source'] + ' bf16 sustained; achieved counts ALGORITHMIC flops - the fp32-accurate path '
-                                         'executes 3 tf32 MMAs per product (tf32 dense peak = bf16 / 2), see DESIGN.md'}
+                                         'executes 3 tf32 MMAs per product (tf32 dense peak = bf16 / 2)'}
     if photo_ms > 0:
         ach = photo_bytes / (photo_ms * 1e-3) / 1e9
         js['roofline_warploss'] = {'bound': 'hbm', 'kernel': 'photo_fwd+photo_bwd (fused warp+SSIM+loss)', 'achieved': ach,
@@ -365,10 +391,10 @@ def profile_pass(trainer, tgt, refs, K, Kinv, steps=2):
                                 for k, v in sorted(kern_ms.items(), key=lambda kv: -kv[1]['ms'])}
     try:
         single = single_kernel_roofline(pk)
-        nh = [v for k, v in kern_ms.items() if k.startswith('conv_nhwc')]
+        nh = [v for k, v in kern_ms.items() if k.startswith('conv_tc:')]
         if nh:
             single['share_of_step'] = sum(v['ms'] for v in nh) / total
-            single['share_source'] = 'live: CUDA events around every conv call of the profiled eager step that dispatched to conv_nhwc_kernel (fprop + dgrad)'
+            single['share_source'] = 'live: CUDA events around every conv call of the profiled eager step that dispatched to conv_tc_kernel (fprop + dgrad)'
 
         if 'roofline' in js:
             js['roofline_family'] = js['roofline']
@@ -383,10 +409,9 @@ def profile_pass(trainer, tgt, refs, K, Kinv, steps=2):
 
 def single_kernel_roofline(pk, iters=20):
     """The heaviest single convolution of the step, alone: DispResNet6's 7x7 32->32 layer (b4, 128x416, 21.4 GFLOP), which
-    the dispatcher gives to conv_nhwc_kernel (channels-last slab kernel).  Duration = CUDA events around `iters` calls on
-    the launching stream - a call = NCHW->NHWC copy + weight preparation + the kernel, as in the step (inputs 27 MB +
-    outputs 27 MB per launch).  DRAM traffic = the committed ncu --set full capture of the same launch
-    (profiles/r02_ncu_nhwc_7x7.txt), labelled as such; null if that file is absent."""
+    the dispatcher gives to conv_tc_kernel (wgmma implicit GEMM).  Duration = CUDA events around `iters` calls on the
+    launching stream - a call = weight preparation + the kernel, as in the step (inputs 27 MB + outputs 27 MB per
+    launch).  DRAM traffic is not measured (no hardware counters here): null."""
     from cc_b200 import nn as cnn, _lib
     dev = torch.device('cuda', torch.cuda.current_device())
     B, C, Hh, Ww, k = PER_GPU_BATCH, 32, H // 2, W // 2, 7
@@ -406,24 +431,11 @@ def single_kernel_roofline(pk, iters=20):
     us = e0.elapsed_time(e1) * 1e3 / iters
     flops = 2.0 * B * C * C * k * k * Hh * Ww
     ach = flops / (us * 1e-6) / 1e12
-    traffic, traffic_src = None, None
-    try:
-        unit = {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9}
-        vals = {}
-        for line in open(os.path.join(ROOT, 'profiles', 'r02_ncu_nhwc_7x7.txt')):
-            f = line.split()
-            if len(f) >= 3 and f[0] in ('dram__bytes_read.sum', 'dram__bytes_write.sum'):
-                vals[f[0]] = float(f[1]) * unit[f[2]]
-        if len(vals) == 2:
-            traffic = sum(vals.values())
-            traffic_src = 'committed capture profiles/r02_ncu_nhwc_7x7.txt (ncu --set full of this launch, kernel only), not re-measured in this run'
-    except Exception:
-        pass
-    return {'bound': 'tensor', 'kernel': '%s_kernel<3xTF32> + layout copy + weight prep (7x7 32->32 fprop, b%d %dx%d)' % (kern, B, Hh, Ww),
+    return {'bound': 'tensor', 'kernel': '%s_kernel<3xTF32> + weight prep (7x7 32->32 fprop, b%d %dx%d)' % (kern, B, Hh, Ww),
             'share_of_step': None, 'share_source': None,
             'achieved': ach, 'peak': pk['tensor_burst'], 'unit': 'TFLOP/s', 'frac': ach / pk['tensor_burst'],
             'us_per_launch': us, 'algorithmic_flops_per_launch': flops, 'algorithmic_bytes_per_launch': 2.0 * B * C * Hh * Ww * 4,
-            'traffic': traffic, 'traffic_source': traffic_src,
+            'traffic': None, 'traffic_source': None,
             'peak_source': pk['source'] + ' bf16 burst (kernel timed alone); 3 tf32 passes at half the bf16 rate: ceiling = peak / 6'}
 
 
@@ -456,17 +468,14 @@ def pick_cpu_threads():
 
 
 def _ref_module():
-    p = os.path.join(ROOT, 'baseline')
-    if p not in sys.path:
-        sys.path.insert(0, p)
-    import ref_step
+    from oracle import ref_step
     return ref_step
 
 
 def _cpu_step_timer(cfg, B, threads):
     """(run, kind, label): one reference train step on the host cores.  kind "reference" = the UNMODIFIED reference
-    modules under baseline/_ref driven by baseline/ref_step.py (stub correlation op); kind "port" = the oracle
-    restatement, only when baseline/_ref is absent."""
+    modules under oracle/_ref driven by oracle/ref_step.py (stub correlation op); kind "port" = the oracle
+    restatement, only when oracle/_ref is absent."""
     from cc_b200 import synth
     torch.set_num_threads(threads)
     tgt, refs = synth.frames(B, H, W, seed=7)
@@ -479,7 +488,7 @@ def _cpu_step_timer(cfg, B, threads):
             t0 = time.perf_counter()
             r.step(tgt, refs, K, Kinv)
             return time.perf_counter() - t0
-        return run, 'reference', 'unmodified reference modules (baseline/_ref), train.py:454-509,566-568 body, stub correlation op'
+        return run, 'reference', 'unmodified reference modules (oracle/_ref), train.py:454-509,566-568 body, stub correlation op'
     from oracle import step as OS
     P = OS.make_params(cfg)
     opt = OS.Adam(OS.all_params(P), OS.HP['lr'], OS.HP['beta1'], OS.HP['beta2'])
@@ -488,7 +497,7 @@ def _cpu_step_timer(cfg, B, threads):
         t0 = time.perf_counter()
         OS.train_step(cfg, P, opt, tgt, refs, K, Kinv)
         return time.perf_counter() - t0
-    return run, 'port', 'oracle port of the reference step (baseline/_ref absent)'
+    return run, 'port', 'oracle port of the reference step (oracle/_ref absent)'
 
 
 def cpu_baseline(cfg, budget_s=25.0):
@@ -508,20 +517,20 @@ def cpu_baseline(cfg, budget_s=25.0):
 
 
 def reference_gpu(cfg, dev, steps=5, warm=3):
-    """BASELINE.md section 4: the reference PyTorch path itself on this B200 (cudnn.benchmark=True as train.py:299; TF32
-    on = the reference's default on this hardware, TF32 off = the parity setting), same batch shape.  Context for
-    the north-star's ">= 10x reference PyTorch on 1xB200"; not the denominator of the driver's ratio."""
+    """BASELINE.md section 4: the reference PyTorch path itself on this GPU (cudnn.benchmark=True as train.py:299; TF32
+    on = the reference's default on this hardware, TF32 off = the parity setting), same batch shape.  Context only:
+    not the denominator of any ratio."""
     from cc_b200 import synth
     rs = _ref_module()
     if not rs.available():
-        return {'unavailable': 'baseline/_ref missing'}
+        return {'unavailable': 'oracle/_ref missing'}
     B = PER_GPU_BATCH
     tgt, refs = synth.frames(B, H, W, seed=7)
     K, Kinv = synth.intrinsics(B, H, W)
     tgt, refs, K, Kinv = tgt.to(dev), [r.to(dev) for r in refs], K.to(dev), Kinv.to(dev)
     saved = (torch.backends.cudnn.benchmark, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
     out = {'workload': CFG_WORKLOAD[cfg], 'per_gpu_batch': B, 'steps': steps, 'warmup': warm,
-           'note': 'unmodified reference modules (baseline/_ref) + pure-torch stub for the absent spatial_correlation_sampler; '
+           'note': 'unmodified reference modules (oracle/_ref) + pure-torch stub for the absent spatial_correlation_sampler; '
                    'loss.item() every step as train.py:563'}
     try:
         for tf32 in (True, False):
@@ -558,8 +567,8 @@ def reference_gpu(cfg, dev, steps=5, warm=3):
 
 
 def run_reference(args):
-    """--impl reference: the reference's own CPU implementation of the step (unmodified modules under baseline/_ref,
-    driven by baseline/ref_step.py; oracle port only if that copy is absent), all the host threads it can use, rank 0 only."""
+    """--impl reference: the reference's own CPU implementation of the step (unmodified modules under oracle/_ref,
+    driven by oracle/ref_step.py; oracle port only if that copy is absent), all the host threads it can use, rank 0 only."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
         return None
@@ -601,6 +610,8 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-side-configs', action='store_true', help='skip the cfg1/cfg2 side measurements (N=1)')
     ap.add_argument('--no-reference-gpu', action='store_true', help='skip the reference-PyTorch-on-this-GPU context run (N=1)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy')
     args = ap.parse_args()
     # Contract: rank 0 prints ONE JSON line on stdout.  Libraries chat on fd 1 (NCCL prints its version banner there):
     # park the real stdout, point fd 1 at stderr for the duration of the run, write the line to the real one at the end.
@@ -613,7 +624,7 @@ def main():
         os.write(real_stdout, (json.dumps(out) + '\n').encode())
     if args.impl == 'ours' and int(os.environ.get('WORLD_SIZE', '1')) > 1:
         # A captured CUDA graph that contains the NCCL all-reduce keeps the communicator busy: destroy_process_group()
-        # blocks forever on it (observed on 2xB200).  The result is printed; leave without the teardown.
+        # blocks forever on it.  The result is printed; leave without the teardown.
         torch.cuda.synchronize()
         torch.distributed.barrier()
         sys.stderr.flush()

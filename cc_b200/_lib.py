@@ -87,7 +87,7 @@ _SIGS = {
     'ccb_inverse_warp_bwd': (_I, [_P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     'ccb_warp_pose_partials_floats': (_LL, [_I, _I, _I]),
     'ccb_flow_warp_fwd': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),
-    'ccb_flow_warp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'ccb_flow_warp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     'ccb_pose2flow_fwd': (_I, [_P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
     'ccb_pose2flow_bwd': (_I, [_P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     'ccb_ssim_fwd': (_I, [_P, _P, _I, _I, _I, C.POINTER(_F), _P, _P]),
@@ -107,12 +107,8 @@ _SIGS = {
     'ccb_act_bwd_bias': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, _LL, _P]),
     'ccb_bias_grad_workspace_floats': (_LL, [_I, _I, _I]),
     'ccb_bias_grad': (_I, [_P, _P, _I, _I, _I, _P, _LL, _P]),
-    'ccb_debug_tc_swap_strides': (None, [_I]),
-    'ccb_debug_tma_status': (_I, [C.POINTER(C.c_uint)]),
     'ccb_debug_last_conv_kernel': (C.c_char_p, []),
-    'ccb_debug_nhwc': (None, [_I, _I, _I]),
-    'ccb_debug_nhwc_status': (_I, [C.POINTER(C.c_uint)]),
-    'ccb_debug_conv_plan': (_I, [C.POINTER(ConvDesc), _I, _I, _I, C.POINTER(_I)]),
+    'ccb_debug_tc_plan': (_I, [_I, C.POINTER(_I)]),
     'ccb_wcache_create': (C.c_void_p, []),
     'ccb_wcache_destroy': (None, [C.c_void_p]),
     'ccb_wcache_plan_floats': (_LL, [C.c_void_p]),
@@ -124,7 +120,7 @@ _SIGS = {
     'ccb_corr81_fwd': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _LL, _P]),
     'ccb_corr81_bwd': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
     'ccb_featwarp_fwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
-    'ccb_featwarp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'ccb_featwarp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     'ccb_bn_workspace_floats': (_LL, [_I, _I, _I]),
     'ccb_bn_fwd': (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _I, _P, _P]),
     'ccb_bn_bwd': (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
@@ -165,7 +161,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(DEFAULT_PATH):
             raise RuntimeError(
-                'cc_b200: %s is missing - build the sm_100a extension first '
+                'cc_b200: %s is missing - build the sm_90a extension first '
                 '(python -c "import __graft_entry__ as g; g.build()"); there is no CPU fallback.' % DEFAULT_PATH)
         use_library(DEFAULT_PATH)
     return _lib
@@ -191,9 +187,14 @@ def ptr(t, name='tensor', dtype=torch.float32):
     if not t.is_contiguous():
         raise ValueError('cc_b200: %s must be contiguous' % name)
     if not t.is_cuda and not is_simulator():
-        raise RuntimeError('cc_b200: %s is on %s - the sm_100a kernels need CUDA tensors (no CPU fallback)'
+        raise RuntimeError('cc_b200: %s is on %s - the sm_90a kernels need CUDA tensors (no CPU fallback)'
                            % (name, t.device))
     return t.data_ptr()
+
+
+def scatter_workspace(t):
+    """Fixed-point accumulators (+1 word) for the image gradient of a warp of `t` (ccb_flow_warp_bwd / ccb_featwarp_bwd)."""
+    return torch.empty(t.numel() + 1, dtype=torch.int64, device=t.device)
 
 
 def stream(t=None):

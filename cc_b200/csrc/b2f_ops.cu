@@ -28,7 +28,7 @@ constexpr int CG = 4;         // channels staged per barrier pair
 // per sample) but up to 192 channels, so the channel loop is what has to be spread over the SMs.
 __host__ __device__ __forceinline__ int corr_chunks(int B, int C, int h, int w) {
     const int tiles = cdiv(w, CT) * cdiv(h, CT) * B;
-    int chunks = cdiv(2 * 148, tiles);
+    int chunks = cdiv(2 * NUM_SMS, tiles);
     const int maxc = cdiv(C, CG);                  // at least one staged group per chunk
     if (chunks > maxc) chunks = maxc;
     if (chunks > 32) chunks = 32;
@@ -200,7 +200,7 @@ extern "C" int ccb_corr81_bwd(const float* f1, const float* f2, const float* gra
     if (d_f2) {
         const long long n = (long long)B * 81 * h * w;
         long long nb = (n + 255) / 256;
-        if (nb > 148 * 16) nb = 148 * 16;
+        if (nb > NUM_SMS * 16) nb = NUM_SMS * 16;
         CCB_LAUNCH(corr81_mirror_kernel, dim3((unsigned)nb), dim3(256), 0, stream, grad_out, work, B, h, w, reversed);
         CCB_LAUNCH(corr81_dgrad_kernel, grid, dim3(CT * CT), 0, stream, (const float*)work, f1, d_f2, B, C, h, w, reversed, 1, chunks);
     }

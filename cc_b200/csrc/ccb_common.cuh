@@ -1,4 +1,4 @@
-// ccb_common.cuh - shared host/device helpers for libccb200 (sm_100a).
+// ccb_common.cuh - shared host/device helpers for libccb200 (sm_90a).
 #pragma once
 #include "../../include/ccb200.h"
 #include "../../include/ccb200_debug.h"
@@ -33,7 +33,7 @@
 // CCB_PDL_TRIGGER: let the SUCCESSOR's blocks be scheduled as soon as every block of this grid has started (they park at their
 // own CCB_PDL_SYNC; no block of this grid is left unscheduled by then, so nothing can starve).  CCB_PDL_SYNC: wait for the
 // predecessor's completion + memory flush; must precede the first access to global data.  CCB_PDL_WAIT: both, at the top of
-// a kernel.  The tensor-core kernels trigger at the top and sync AFTER their prologue (barrier init, TMEM allocation), which
+// a kernel.  The tensor-core kernels trigger at the top and sync AFTER their prologue (barrier init), which
 // therefore overlaps the predecessor's tail.
 #define CCB_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 #define CCB_PDL_SYNC() asm volatile("griddepcontrol.wait;" ::: "memory")
@@ -65,12 +65,12 @@ int check_launch(const char* what);
     } while (0)
 
 // ---- weight preparation for the tensor-core conv kernels (wprep.cu) ----
-enum { WPREP_TC = 0, WPREP_TMA = 1, WPREP_SLAB = 2, WPREP_NHWC = 3 };
+enum { WPREP_TC = 0 };
 struct WPrepDesc {
     const float* w;
     float* wp;
     int N, Cc, KK, Ci, mode, Kp, ntaps;
-    int layout, p0, p1, p2;      // TC: p0 = cpad;  TMA: p0 = cb, p1 = cblocks, p2 = units;  SLAB: p0 = cs, p1 = cblocks, p2 = kt_full;  NHWC: p0 = 32, p1 = cblocks, p2 = ntaps
+    int layout, p0, p1, p2;      // TC: p0 = cpad
     signed char tap_index[64];
 };
 #ifndef CCB_CPU_SIM
@@ -110,5 +110,8 @@ __device__ __forceinline__ void block_sum(float (&v)[NV], float* scratch) {
 }
 
 __host__ __device__ __forceinline__ int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// streaming multiprocessors of the H100 SXM: grid and split-K plans aim at whole waves of this many CTAs
+constexpr int NUM_SMS = 132;
 
 }  // namespace ccb

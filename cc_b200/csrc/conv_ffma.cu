@@ -1,7 +1,7 @@
 // conv_ffma.cu - CUDA-core (FFMA) implicit-GEMM convolution: forward, data-gradient (also the
 // ConvTranspose2d forward) and weight-gradient, with fused bias / residual / activation epilogues.
 //
-// Role: (a) exact-fp32 baseline and fallback for shapes the tcgen05 path does not take (C_in = 3,
+// Role: (a) exact-fp32 baseline and fallback for shapes the wgmma tensor-core path does not take (C_in = 3,
 // C_out <= 4 heads, tiny deep levels), (b) numerical cross-check for the tensor-core kernels
 // (conv_tc.cu).  Replaces the cuDNN calls behind nn.Conv2d / nn.ConvTranspose2d in
 // models/{DispResNet6,PoseNetB6,MaskNet6,back2future}.py (SURVEY.md 2a K6/K7).
@@ -396,7 +396,7 @@ void launch_splitk_reduce(const float* work, float* out, const float* bias, cons
 
 // ------------------------------------------------------------------------------------------------
 static int pick_splits(int tiles, int ktiles, int max_splits) {
-    const int target = 148 * 4;
+    const int target = NUM_SMS * 4;
     if (tiles >= target || ktiles <= 2) return 1;
     int s = target / tiles;
     if (s > ktiles / 2) s = ktiles / 2;
@@ -460,36 +460,6 @@ int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const floa
 int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* work, long long work_floats,
              int three, cudaStream_t st);
 
-// TMA-fed tensor-core path (conv_tma.cu): stride-1 gathers (FPROP stride 1, every DGRAD parity class)
-bool tma_conv_supported(const ccb_conv_desc* d, int op);
-bool tma_direct_fprop(const ccb_conv_desc* d);
-bool tma_nhwc_takes(const ccb_conv_desc* d, int op);
-bool nhwc_wgrad_takes(const ccb_conv_desc* d);
-long long nhwc_wgrad_workspace_floats(const ccb_conv_desc* d);
-int nhwc_wgrad(const ccb_conv_desc* d, const float* x, const float* dz, float* dw, float* work, long long work_floats, int three,
-               cudaStream_t st);
-long long tma_workspace_floats(const ccb_conv_desc* d, int op);
-int tma_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias, const float* res, float* y,
-              float* work, long long work_floats, int three, cudaStream_t st);
-int tma_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const float* bias, const float* res, float* dx,
-              float* work, long long work_floats, int three, cudaStream_t st);
-bool tma_wgrad_supported(const ccb_conv_desc* d);
-long long tma_wgrad_workspace_floats(const ccb_conv_desc* d);
-int tma_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* work, long long work_floats, int three,
-              cudaStream_t st);
-static bool use_tma(const ccb_conv_desc* d, int op, const void* src) {
-    if ((((uintptr_t)src) & 15) != 0 || !tma_conv_supported(d, op) || tma_workspace_floats(d, op) < 0) return false;
-    // measured on B200 (tools/tma_probe.py): the slab kernel wins every DGRAD and the FPROPs with a long K loop or
-    // >= 64 output channels; short thin FPROPs (K <= 512, N <= 32) and stride-2 FPROPs stay on the register-gather kernel
-    if (op == CCB_CONV_FPROP && tma_direct_fprop(d)) return true;     // thin layers: CUDA-core direct kernel
-    if (op == CCB_CONV_FPROP && tma_nhwc_takes(d, op)) return true;   // channels-last slab kernel (measured: 32 -> 32 3x3 at 128x416 151 -> ~55 us)
-    if (op == CCB_CONV_FPROP && d->kh > 1) {
-        if (d->stride != 1) return false;
-        if (d->Co < 64 && (long long)d->Ci * d->kh * d->kw < 512) return false;
-    }
-    return true;
-}
-
 // the weight cache of the conv call in flight (wprep_get looks it up); sim builds have none
 struct WCacheScope {
 #ifndef CCB_CPU_SIM
@@ -500,7 +470,7 @@ struct WCacheScope {
 #endif
 };
 
-// 0: FFMA, 1: tcgen05 3xTF32, 2: tcgen05 single TF32
+// 0: FFMA, 1: wgmma 3xTF32, 2: wgmma single TF32
 static int pick_impl(const ccb_conv_desc* d, int op) {
     switch (d->impl) {
         case CCB_CONV_IMPL_FFMA: return 0;
@@ -547,26 +517,12 @@ extern "C" long long ccb_conv_workspace_floats(const ccb_conv_desc* d, int op) {
         ccb_conv_desc dp;
         long long xpf, dypf;
         if (wgrad_pad_desc(d, dp, xpf, dypf)) {
-            long long inner = tc_workspace_floats(&dp, op);
-            if (tma_wgrad_supported(&dp) && tma_wgrad_workspace_floats(&dp) > inner) inner = tma_wgrad_workspace_floats(&dp);
-            const long long t = xpf + dypf + inner;
+            const long long t = xpf + dypf + tc_workspace_floats(&dp, op);
             return t > bias_need ? t : bias_need;
         }
     }
     if (d->impl != CCB_CONV_IMPL_FFMA && tc_supported(d, op) && pick_impl(d, op) > 0) {
-        long long t = tc_workspace_floats(d, op);
-        if (op != CCB_CONV_WGRAD && tma_conv_supported(d, op)) {
-            long long t2 = tma_workspace_floats(d, op);
-            if (t2 > t) t = t2;
-        }
-        if (op == CCB_CONV_WGRAD && tma_wgrad_supported(d)) {
-            long long t2 = tma_wgrad_workspace_floats(d);
-            if (t2 > t) t = t2;
-        }
-        if (op == CCB_CONV_WGRAD && nhwc_wgrad_takes(d)) {
-            long long t2 = nhwc_wgrad_workspace_floats(d);
-            if (t2 > t) t = t2;
-        }
+        const long long t = tc_workspace_floats(d, op);
         return t > bias_need ? t : bias_need;
     }
     long long numel = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Co * d->Ho * d->Wo
@@ -590,8 +546,6 @@ extern "C" int ccb_conv2d_fprop(const ccb_conv_desc* d, const float* x, const fl
     {
         int impl = pick_impl(d, CCB_CONV_FPROP);
         CCB_REQUIRE(impl >= 0, CCB_ERR_UNSUPPORTED, "conv2d_fprop: shape not supported by the tensor-core path");
-        if (impl > 0 && use_tma(d, CCB_CONV_FPROP, x))
-            return tma_fprop(d, x, w, bias, res, y, work, work_floats, impl == 1, (cudaStream_t)stream);
         if (impl > 0) return tc_fprop(d, x, w, bias, res, y, work, work_floats, impl == 1, (cudaStream_t)stream);
     }
     a.x = x; a.w = w; a.bias = bias; a.res = res; a.out = y; a.work = work;
@@ -610,8 +564,6 @@ extern "C" int ccb_conv2d_dgrad(const ccb_conv_desc* d, const float* dy, const f
     {
         int impl = pick_impl(d, CCB_CONV_DGRAD);
         CCB_REQUIRE(impl >= 0, CCB_ERR_UNSUPPORTED, "conv2d_dgrad: shape not supported by the tensor-core path");
-        if (impl > 0 && use_tma(d, CCB_CONV_DGRAD, dy))
-            return tma_dgrad(d, dy, w, bias, res, dx, work, work_floats, impl == 1, (cudaStream_t)stream);
         if (impl > 0) return tc_dgrad(d, dy, w, bias, res, dx, work, work_floats, impl == 1, (cudaStream_t)stream);
     }
     a.dy = dy; a.w = w; a.bias = bias; a.res = res; a.out = dx; a.work = work;
@@ -646,12 +598,7 @@ extern "C" int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const fl
         int impl = pick_impl(d, CCB_CONV_WGRAD);
         CCB_REQUIRE(impl >= 0, CCB_ERR_UNSUPPORTED, "conv2d_wgrad: shape not supported by the tensor-core path");
         if (impl > 0) {
-            if (nhwc_wgrad_takes(d))
-                rc = nhwc_wgrad(d, x, dy, dw, work, work_floats, impl == 1, (cudaStream_t)stream);
-            else if (tma_wgrad_supported(d) && ((((uintptr_t)x) | ((uintptr_t)dy)) & 15) == 0)
-                rc = tma_wgrad(d, x, dy, dw, work, work_floats, impl == 1, (cudaStream_t)stream);
-            else
-                rc = tc_wgrad(d, x, dy, dw, work, work_floats, impl == 1, (cudaStream_t)stream);
+            rc = tc_wgrad(d, x, dy, dw, work, work_floats, impl == 1, (cudaStream_t)stream);
             if (rc) return rc;
             if (db) rc = launch_bias_grad(dy, db, d->B, d->Co, d->Ho * d->Wo, work, work_floats, (cudaStream_t)stream);
             return rc;
@@ -661,8 +608,7 @@ extern "C" int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const fl
         ccb_conv_desc dp;
         long long xpf, dypf;
         const bool padded = wgrad_pad_desc(d, dp, xpf, dypf);
-        const bool via_tma = padded && tma_wgrad_supported(&dp);
-        const long long inner = padded ? (via_tma ? tma_wgrad_workspace_floats(&dp) : tc_workspace_floats(&dp, CCB_CONV_WGRAD)) : 0;
+        const long long inner = padded ? tc_workspace_floats(&dp, CCB_CONV_WGRAD) : 0;
         if (padded && work && xpf + dypf + inner <= work_floats) {
             float* xp = work;
             float* dyp = work + xpf;
@@ -672,12 +618,8 @@ extern "C" int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const fl
                        d->Wo, dp.Wo);
             rc = check_launch("conv2d_wgrad pad");
             if (rc) return rc;
-            if (via_tma)
-                rc = tma_wgrad(&dp, xp, dyp, dw, work + xpf + dypf, work_floats - xpf - dypf, d->impl != CCB_CONV_IMPL_TC_TF32,
-                               (cudaStream_t)stream);
-            else
-                rc = tc_wgrad(&dp, xp, dyp, dw, work + xpf + dypf, work_floats - xpf - dypf, d->impl != CCB_CONV_IMPL_TC_TF32,
-                              (cudaStream_t)stream);
+            rc = tc_wgrad(&dp, xp, dyp, dw, work + xpf + dypf, work_floats - xpf - dypf, d->impl != CCB_CONV_IMPL_TC_TF32,
+                          (cudaStream_t)stream);
             if (rc) return rc;
             if (db) rc = launch_bias_grad(dy, db, d->B, d->Co, d->Ho * d->Wo, work, work_floats, (cudaStream_t)stream);
             return rc;

@@ -1,19 +1,22 @@
-// conv_tc.cu - implicit-GEMM convolution on the 5th-generation tensor cores (tcgen05 / TMEM), sm_100a.
+// conv_tc.cu - implicit-GEMM convolution on the Hopper tensor cores (wgmma), sm_90a.
 //
-//   D[128 pixels x N<=128 channels] (fp32, TMEM) += A[128 x 32] (im2col tile) * B[N x 32]^T (weights)
+//   D[128 pixels x N<=128 channels] (fp32, registers) += A[128 x 32] (im2col tile) * B[N x 32]^T (weights)
 //
-// * one CTA = one 128-pixel x N-channel output tile; 8 producer/epilogue warps + 1 MMA warp;
+// * one CTA = one 128-pixel x N-channel output tile; one producer warpgroup + two consumer warpgroups, each
+//   consumer owning 64 of the 128 rows (wgmma m64nNk8, N = the launch's channel tile rounded up to 16/32/64/128);
 // * A is gathered straight from the NCHW activations (no im2col buffer in HBM): a K-chunk is 4
 //   consecutive input channels of one filter tap, so the 4 loads of a chunk share the tap's bounds
 //   check and are coalesced across the 128 pixels of the tile;
-// * operands are staged in shared memory in the canonical K-major / no-swizzle UMMA layout
-//   [k-chunk][row][16 B] (8-row x 16 B core matrices contiguous, SBO = 128 B, LBO = rows*16 B);
+// * operands are staged in shared memory K-major with the 128-byte swizzle ([row][128 B], 16 B chunk ^= row & 7,
+//   8-row atoms 1 KB apart): the layout wgmma reads for tf32, which it accepts only K-major;
 // * fp32 parity: every fp32 operand is split hi = tf32(x), lo = x - hi and each k-step issues three
-//   kind::tf32 MMAs (hi*hi + lo*hi + hi*lo) into the same TMEM accumulator ("3xTF32", error ~2^-21);
+//   tf32 MMAs (hi*hi + lo*hi + hi*lo) ("3xTF32", error ~2^-21).  The tensor core only sums one 32-deep stage (small
+//   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
+//   fp32 adds, so no long accumulation chain runs through the tensor core's own rounding;
 //   CCB_CONV_IMPL_TC_TF32 issues hi*hi only (what cuDNN does by default for the reference on Ampere+);
-// * 3-stage mbarrier pipeline: producers -> full[s] -> MMA issuer -> tcgen05.commit -> empty[s];
-//   the epilogue reads the accumulator with tcgen05.ld (lane == pixel), adds bias / residual, applies
-//   the activation and stores NCHW (coalesced: consecutive lanes are consecutive pixels).
+// * mbarrier pipeline of up to 4 stages: producers -> full[s] -> consumers (wgmma, commit group, wait, fp32 add)
+//   -> empty[s];
+//   the epilogue adds bias / residual, applies the activation and stores NCHW straight from the accumulators.
 //
 // The same kernel serves FPROP, stride-1 DGRAD and the stride-parity classes of strided DGRAD /
 // ConvTranspose2d forward through a per-tap offset table ("generalised fprop").
@@ -23,12 +26,13 @@
 
 namespace ccb {
 
-constexpr int TC_M = 128;          // pixels per tile (UMMA M)
-constexpr int TC_NMAX = 128;       // channels per tile (UMMA N <= 128)
+constexpr int TC_M = 128;          // pixels per tile (two wgmma M = 64 halves)
+constexpr int TC_NMAX = 128;       // channels per tile
 constexpr int TC_KC = 8;           // 16-byte k-chunks per stage (K = 32 fp32 per stage)
-constexpr int TC_STAGES = 3;
-constexpr int TC_PRODUCERS = 256;
-constexpr int TC_THREADS = TC_PRODUCERS + 32;
+constexpr int TC_MAX_STAGES = 4;
+constexpr int TC_PRODUCERS = 128;
+constexpr int TC_CONSUMER_WARPS = 8;
+constexpr int TC_THREADS = TC_PRODUCERS + 32 * TC_CONSUMER_WARPS;
 constexpr int TC_MAX_TAPS = 49;
 
 struct TcArgs {
@@ -47,9 +51,6 @@ struct TcArgs {
     int M;                 // B * Hc * Wc
     int act;
     float slope;
-    int three;             // 1: 3xTF32, 0: single TF32
-    int swap_lbo_sbo;      // debug: swap the descriptor strides (layout probe)
-    int swz;               // 0: K-major no-swizzle [chunk][row][16B]; 1: K-major SWIZZLE_128B [row][128B], chunk ^= row&7
     int splits, kt_per_split;          // split-K over k-tiles (grid.z); partials go to `partial`
     float* partial;                    // [splits][numel(out)] raw accumulators (bias/res/act applied by the reduce kernel)
     long long out_numel;
@@ -79,7 +80,7 @@ __device__ __forceinline__ bool mbar_try(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded spin: a protocol bug traps (the launch fails) instead of hanging the GPU box.
+// Bounded spin: a protocol bug traps (the launch fails) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
     while (!mbar_try(bar, parity)) {
@@ -88,41 +89,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
 }
@@ -133,20 +99,85 @@ __device__ __forceinline__ float tf32_hi(float x) {
     return __uint_as_float(r);
 }
 
-// K-major, no-swizzle shared-memory matrix descriptor for a [chunk][rows][16 B] tile (rows = 128)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 0) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;      // descriptor version 1 (Blackwell)
-    d |= (uint64_t)(layout_type & 7) << 61;   // 0 SWIZZLE_NONE, 2 SWIZZLE_128B
-    return d;                    // base_offset 0, lbo_mode 0
+// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B tile: 8-row atoms 1024 B apart (stride byte
+// offset); the leading byte offset is unused by this layout; layout type 1 = 128-byte swizzle.  A k-step of 8 tf32
+// advances the start address by 32 B inside the 128-byte row (the swizzle is a function of the absolute address,
+// so every tile starts on a 1 KB boundary).
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// float4 index of (row, 16-byte chunk) inside one operand tile
-__device__ __forceinline__ int tile_idx(int row, int chunk, int swz) {
-    return swz ? (row * TC_KC + (chunk ^ (row & 7))) : (chunk * TC_M + row);
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+template <int R>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 in, fp32 accumulators in registers (N / 2 per thread)
+__device__ __forceinline__ void wgmma_tf32_n16(float (&d)[8], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db));
+}
+template <int NT>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[NT / 2], uint64_t da, uint64_t db) {
+    if constexpr (NT == 16) wgmma_tf32_n16(d, da, db);
+    else if constexpr (NT == 32) wgmma_tf32_n32(d, da, db);
+    else if constexpr (NT == 64) wgmma_tf32_n64(d, da, db);
+    else wgmma_tf32_n128(d, da, db);
+}
+
+// float4 index of (row, 16-byte chunk) inside one swizzled operand tile
+__device__ __forceinline__ int tile_idx(int row, int chunk) { return row * TC_KC + (chunk ^ (row & 7)); }
 
 __device__ __forceinline__ float tc_act(float v, int act, float slope) {
     switch (act) {
@@ -157,48 +188,74 @@ __device__ __forceinline__ float tc_act(float v, int act, float slope) {
     }
 }
 
-constexpr int TC_TILE_BYTES = TC_KC * TC_M * 16;                   // one operand copy of one stage: 16 KB
-constexpr int TC_STAGE_BYTES = 4 * TC_TILE_BYTES;                  // A hi, A lo, B hi, B lo
-constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 2048;   // + barriers / tmem slot / alignment slack
+constexpr int TC_TILE_BYTES = TC_KC * TC_M * 16;                   // one A operand copy of one stage: 16 KB
+constexpr int TC_SMEM_MAX = 227 * 1024;
 
-template <bool THREE, bool SWZ>
-__global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const TcArgs a) {
+// Consumer side shared by both kernels: for each full stage, 4 k-steps of [(lo*hi) + (hi*lo) +] (hi*hi) on this
+// warpgroup's 64 rows into the scratch registers `part`, then acc += part in fp32 and the stage goes back to the producers.
+template <bool THREE, int NT>
+__device__ __forceinline__ void tc_consume(unsigned char* smem, int stage_bytes, int b_tile_bytes, int NST, int nst,
+                                           uint64_t* full_bar, uint64_t* empty_bar, int wg, int lane,
+                                           float (&acc)[NT / 2], float (&part)[NT / 2]) {
+    for (int it = 0; it < nst; ++it) {
+        const int s = it % NST;
+        mbar_wait(&full_bar[s], (it / NST) & 1);
+        const uint32_t base = smem_u32(smem + s * stage_bytes);
+        const uint32_t a_hi = base + wg * (TC_TILE_BYTES / 2), a_lo = a_hi + TC_TILE_BYTES;
+        const uint32_t b_hi = base + 2 * TC_TILE_BYTES, b_lo = b_hi + b_tile_bytes;
+#pragma unroll
+        for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
+        wg_fence();
+        if (THREE) {
+#pragma unroll
+            for (int ks = 0; ks < TC_KC / 2; ++ks) {
+                const uint32_t koff = (uint32_t)ks * 32u;
+                wgmma_tf32<NT>(part, wg_desc(a_lo + koff), wg_desc(b_hi + koff));
+                wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(b_lo + koff));
+            }
+        }
+#pragma unroll
+        for (int ks = 0; ks < TC_KC / 2; ++ks) {
+            const uint32_t koff = (uint32_t)ks * 32u;
+            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(b_hi + koff));
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_regs(part);
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+        for (int j = 0; j < NT / 2; ++j) acc[j] += part[j];
+    }
+}
+
+template <bool THREE, int NT>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) {
     CCB_PDL_TRIGGER();
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B atoms are 1 KB
     const int NST = a.stages;
     const int stage_bytes = 2 * TC_TILE_BYTES + 2 * a.b_tile_bytes;     // A hi, A lo, B hi, B lo
     uint64_t* full_bar = (uint64_t*)(smem + NST * stage_bytes);
-    uint64_t* empty_bar = full_bar + TC_STAGES;      // (barrier arrays sized for the maximum depth)
-    uint64_t* accum_bar = empty_bar + TC_STAGES;
-    uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
+    uint64_t* empty_bar = full_bar + TC_MAX_STAGES;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
     const int ntile = min(TC_NMAX, a.Ntot - n0);
-    const int umma_n = (ntile + 15) & ~15;
     const int ktiles_all = a.Kp / (TC_KC * 4);
     const int kt_beg = blockIdx.z * a.kt_per_split;
     const int ktiles = max(0, min(ktiles_all, kt_beg + a.kt_per_split) - kt_beg);   // k-tiles of this split
     const long long HWin = (long long)a.Hin * a.Win;
 
     if (tid == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], TC_PRODUCERS / 2); mbar_init(&empty_bar[s], 1); }
-        mbar_init(accum_bar, 1);
+        for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], TC_PRODUCERS); mbar_init(&empty_bar[s], TC_CONSUMER_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 8) tmem_alloc(tmem_slot, 256);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     CCB_PDL_SYNC();                                               // everything above touched no global data
 
-    if (warp < 8) {
-        // ===================== producers =====================
-        // Two groups of 4 warps fill alternating stages, so one group's global-load latency overlaps the
-        // other group's convert + shared-memory store phase.  Within a group: thread == tile row.
-        const int grp = warp >> 2, r = tid & 127;
+    if (warp < TC_PRODUCERS / 32) {
+        // ===================== producers: thread == tile row =====================
+        const int r = tid;
         const int m = m0 + r;
         const bool mvalid = m < a.M;
         int b = 0, oy = 0, ox = 0;
@@ -213,7 +270,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const TcArgs a) 
         const int iy0 = oy * a.in_stride, ix0 = ox * a.in_stride;
         const int cpt = a.cpad >> 2;                 // chunks per tap
         const int nchunks = a.ntaps * cpt;           // real chunks; the rest of Kp is zero padding
-        for (int it = grp; it < ktiles; it += 2) {
+        for (int it = 0; it < ktiles; ++it) {
             const int s = it % NST;
             const int kt = kt_beg + it;                   // global k-tile
             // ---- A: the 8 chunks (32 floats) of this thread's pixel row
@@ -268,13 +325,12 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const TcArgs a) 
                 const int idx = r + j * 128;                      // 0 .. 1023
                 const int c = ((idx >> 8) << 1) | (idx & 1);
                 const int n = (idx >> 1) & 127;
-                if (n < umma_n) {
-                    // rows in [ntile, umma_n) exist in the prepared buffer only if they are < Ntot; clamp to row 0 and
-                    // let the epilogue ignore those columns (their products never reach a stored output)
+                if (n < NT) {
+                    // rows in [ntile, NT) are clamped to row 0: the epilogue ignores those columns
                     const int nn = (n < ntile) ? n : 0;
                     const float* src = a.wp + (long long)(n0 + nn) * a.Kp + kt * (TC_KC * 4) + c * 4;
-                    cp_async16(&b_hi[tile_idx(n, c, SWZ)], src);
-                    if (THREE) cp_async16(&b_lo[tile_idx(n, c, SWZ)], src + (long long)a.Ntot * a.Kp);
+                    cp_async16(&b_hi[tile_idx(n, c)], src);
+                    if (THREE) cp_async16(&b_lo[tile_idx(n, c)], src + (long long)a.Ntot * a.Kp);
                 }
             }
             // ---- A: split + store
@@ -282,52 +338,44 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const TcArgs a) 
             for (int c = 0; c < TC_KC; ++c) {
                 float4 h, l;
                 h.x = tf32_hi(av[c][0]); h.y = tf32_hi(av[c][1]); h.z = tf32_hi(av[c][2]); h.w = tf32_hi(av[c][3]);
-                a_hi[tile_idx(r, c, SWZ)] = h;
+                a_hi[tile_idx(r, c)] = h;
                 if (THREE) {
                     l.x = tf32_hi(av[c][0] - h.x); l.y = tf32_hi(av[c][1] - h.y); l.z = tf32_hi(av[c][2] - h.z); l.w = tf32_hi(av[c][3] - h.w);
-                    a_lo[tile_idx(r, c, SWZ)] = l;
+                    a_lo[tile_idx(r, c)] = l;
                 }
             }
             cp_async_wait_all();
             fence_proxy_async();
             mbar_arrive(&full_bar[s]);
         }
-        // ===================== epilogue =====================
-        if (ktiles > 0) mbar_wait(accum_bar, 0);
-        tc_fence_after();
-        const int q4 = warp & 3, colhalf = warp >> 2;
-        const int em = m0 + q4 * 32 + lane;
-        const bool evalid = em < a.M;
-        long long obase = 0;
-        if (evalid) {
+    } else {
+        // ===================== consumers: MMA + epilogue =====================
+        const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
+        float acc[NT / 2], part[NT / 2];
+#pragma unroll
+        for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;                  // an empty split contributes zeros
+        tc_consume<THREE, NT>(smem, stage_bytes, a.b_tile_bytes, NST, ktiles, full_bar, empty_bar, wg, lane, acc, part);
+        const long long HWout = (long long)a.Hout * a.Wout;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            // accumulator layout of wgmma m64nN: row 16 * warp + lane / 4 (+ 8), columns 8 i + 2 (lane % 4) (+ 1)
+            const int em = m0 + wg * 64 + wq * 16 + (lane >> 2) + half * 8;
+            if (em >= a.M) continue;
             int hw = a.Hc * a.Wc;
             int eb = em / hw;
             int rem = em - eb * hw;
             int eoy = rem / a.Wc, eox = rem - eoy * a.Wc;
-            obase = (long long)eb * a.Ntot * a.Hout * a.Wout + (long long)(eoy * a.out_stride + a.out_oy) * a.Wout +
-                    (eox * a.out_stride + a.out_ox);
-        }
-        const long long HWout = (long long)a.Hout * a.Wout;
-        for (int cg = colhalf; cg * 16 < umma_n; cg += 2) {
-            float v[16];
-            if (ktiles > 0) {
-                tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(cg * 16), v);
-                if (THREE) {
-                    float vl[16];
-                    tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + 128u + (uint32_t)(cg * 16), vl);
+            const long long obase = (long long)eb * a.Ntot * HWout + (long long)(eoy * a.out_stride + a.out_oy) * a.Wout +
+                                    (eox * a.out_stride + a.out_ox);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] += vl[j];
-                }
-            } else {
+            for (int i = 0; i < NT / 8; ++i)
 #pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = 0.f;          // empty split: contributes zeros
-            }
-            if (evalid) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = n0 + cg * 16 + j;
-                    if (n < a.Ntot && cg * 16 + j < ntile) {
-                        float o = v[j];
+                for (int e = 0; e < 2; ++e) {
+                    const int nl = 8 * i + 2 * (lane & 3) + e;
+                    if (nl < ntile) {
+                        const int j = 4 * i + 2 * half + e;
+                        float o = acc[j];
+                        const int n = n0 + nl;
                         const long long off = obase + (long long)n * HWout;
                         if (a.splits > 1) {
                             a.partial[(long long)blockIdx.z * a.out_numel + off] = o;
@@ -338,51 +386,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const TcArgs a) 
                         }
                     }
                 }
-            }
         }
-        tc_fence_before();
-    } else {
-        // ===================== MMA issuer (one thread) =====================
-        // instruction descriptor: D fp32, A/B tf32, both K-major, N = umma_n, M = 128
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(umma_n >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-        uint32_t lbo = SWZ ? 16u : (uint32_t)(TC_M * 16);
-        uint32_t sbo = SWZ ? 1024u : 128u;
-        if (a.swap_lbo_sbo) { uint32_t t = lbo; lbo = sbo; sbo = t; }
-        const uint32_t ltype = SWZ ? 2u : 0u;
-        const uint32_t kstep_bytes = SWZ ? 32u : 2u * (uint32_t)(TC_M * 16);
-        for (int it = 0; it < ktiles; ++it) {
-            const int s = it % NST;
-            mbar_wait(&full_bar[s], (it / NST) & 1);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t base = smem_u32(smem + s * stage_bytes);
-#pragma unroll
-                for (int ks = 0; ks < TC_KC / 2; ++ks) {
-                    const uint32_t koff = (uint32_t)ks * kstep_bytes;
-                    const uint64_t ah = make_desc(base + koff, lbo, sbo, ltype);
-                    const uint64_t al = make_desc(base + TC_TILE_BYTES + koff, lbo, sbo, ltype);
-                    const uint64_t bh = make_desc(base + 2 * TC_TILE_BYTES + koff, lbo, sbo, ltype);
-                    const uint64_t bl = make_desc(base + 2 * TC_TILE_BYTES + a.b_tile_bytes + koff, lbo, sbo, ltype);
-                    // hi*hi goes to columns [0,128); the two small cross terms to [128,256): the tensor core
-                    // truncates on every accumulate, so keeping the small terms out of the big accumulator
-                    // (and summing them in fp32 in the epilogue) cuts the accumulated bias ~3x
-                    umma_tf32(tmem_base, ah, bh, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-                    if (THREE) {
-                        umma_tf32(tmem_base + 128u, al, bh, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-                        umma_tf32(tmem_base + 128u, ah, bl, idesc, 1u);
-                    }
-                }
-                umma_commit(&empty_bar[s]);                 // frees the stage when these MMAs have read it
-                if (it == ktiles - 1) umma_commit(accum_bar);
-            }
-            __syncwarp();
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 8) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 256);
     }
 }
 
@@ -393,13 +397,38 @@ static int roundup(int v, int m) { return (v + m - 1) / m * m; }
 void launch_splitk_reduce(const float* work, float* out, const float* bias, const float* res, long long numel, int splits,
                           int plane, int C, int act, float slope, cudaStream_t st);   // conv_ffma.cu
 
-static int tc_smem_bytes(int stages, int b_tile_bytes) { return stages * (2 * TC_TILE_BYTES + 2 * b_tile_bytes) + 2048; }
+// Operand tile geometry of one launch: the B tile holds the wgmma N (16/32/64/128) rows, and as many stages as fit
+// in shared memory (up to 4: 3 at N = 128 in 3xTF32 layout, 4 below).
+static void tc_geometry(int N, int& nt, int& b_tile_bytes, int& stages, int& smem) {
+    const int ntile_max = N < TC_NMAX ? N : TC_NMAX;
+    nt = 16;
+    while (nt < ntile_max) nt <<= 1;
+    b_tile_bytes = nt * 128;
+    const int stage = 2 * TC_TILE_BYTES + 2 * b_tile_bytes;
+    stages = (TC_SMEM_MAX - 2048) / stage;
+    if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
+    smem = stages * stage + 2048;                     // + barriers / alignment slack
+}
+
+template <typename Args>
+static int tc_launch_kernel(void (*const (&kfns)[2][4])(const Args), const Args& a, int three, int nt, dim3 grid, int smem,
+                            cudaStream_t st, const char* what) {
+    const int ni = nt == 16 ? 0 : nt == 32 ? 1 : nt == 64 ? 2 : 3;
+    auto kfn = kfns[three ? 1 : 0][ni];
+    cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
+    CCB_LAUNCH(kfn, grid, dim3(TC_THREADS), smem, st, a);
+    return check_launch(what);
+}
+
+static void (*const TC_FPROP_KERNELS[2][4])(const TcArgs) = {
+    {conv_tc_kernel<false, 16>, conv_tc_kernel<false, 32>, conv_tc_kernel<false, 64>, conv_tc_kernel<false, 128>},
+    {conv_tc_kernel<true, 16>, conv_tc_kernel<true, 32>, conv_tc_kernel<true, 64>, conv_tc_kernel<true, 128>}};
 
 // Split-K plan shared by all parity classes of one call: enough CTAs for ~2 waves, >= 2 k-tiles per split.
 static int plan_splits(long long M, int N, int max_ktiles, long long out_numel, long long part_floats) {
     const long long tiles = (long long)cdiv((int)M, TC_M) * cdiv(N, TC_NMAX);
-    if (tiles >= 148 || max_ktiles < 4) return 1;
-    long long s = (2 * 148 + tiles - 1) / tiles;
+    if (tiles >= NUM_SMS || max_ktiles < 4) return 1;
+    long long s = (2 * NUM_SMS + tiles - 1) / tiles;
     if (s > max_ktiles / 2) s = max_ktiles / 2;
     if (s > 32) s = 32;
     if (out_numel > 0 && s * out_numel > part_floats) s = part_floats / out_numel;
@@ -408,7 +437,7 @@ static int plan_splits(long long M, int N, int max_ktiles, long long out_numel, 
 
 // One generalised-fprop launch (+ its weight preparation).  `work` = [prepared weights | split-K partials].
 static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK, int Ci, const signed char* tap_index,
-                     float* work, long long work_floats, int splits, float* partial, cudaStream_t st) {
+                     float* work, long long work_floats, int splits, float* partial, int three, cudaStream_t st) {
     a.cpad = roundup(Cc, 4);
     a.Kp = roundup(a.ntaps * a.cpad, TC_KC * 4);
     if (a.Kp == 0) a.Kp = TC_KC * 4;      // a parity class without taps still runs one all-zero k-tile
@@ -428,20 +457,10 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     a.splits = splits;
     a.kt_per_split = cdiv(a.Kp / (TC_KC * 4), splits);
     a.partial = partial ? partial : work + wp_floats;
-    // shared-memory geometry: the B operand only needs the (16-padded) N-tile rows; small tiles run 2 CTAs / SM
-    const int ntile_max = N < TC_NMAX ? N : TC_NMAX;
-    int nalloc = 16;
-    while (nalloc < ntile_max) nalloc <<= 1;
-    if (!a.swz) nalloc = 128;                         // the no-swizzle debug layout is [chunk][128 rows]
-    a.b_tile_bytes = nalloc * 128;
-    a.stages = (nalloc <= 64) ? 2 : TC_STAGES;
-    const int smem = tc_smem_bytes(a.stages, a.b_tile_bytes);
+    int nt, smem;
+    tc_geometry(N, nt, a.b_tile_bytes, a.stages, smem);
     dim3 grid(cdiv(a.M, TC_M), cdiv(N, TC_NMAX), splits);
-    auto kfn = a.swz ? (a.three ? conv_tc_kernel<true, true> : conv_tc_kernel<false, true>)
-                     : (a.three ? conv_tc_kernel<true, false> : conv_tc_kernel<false, false>);
-    cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES);
-    CCB_LAUNCH(kfn, grid, dim3(TC_THREADS), smem, st, a);
-    return check_launch("conv_tc");
+    return tc_launch_kernel(TC_FPROP_KERNELS, a, three, nt, grid, smem, st, "conv_tc");
 }
 
 // ================================================================================================
@@ -458,71 +477,55 @@ struct TcWgradArgs {
     int cpad, Mtot;      // channels padded to 4; Mtot = kh*kw*cpad rows
     int P;               // B*Ho*Wo pixels (Wo % 4 == 0)
     int stages, per_split, splits;
-    int three, swz, swap_lbo_sbo;
     int nstages, b_tile_bytes;   // pipeline depth / bytes of one dY operand copy (Co-tile dependent)
 };
 
-template <bool THREE, bool SWZ>
-__global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_wgrad_kernel(const TcWgradArgs a) {
+template <bool THREE, int NT>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWgradArgs a) {
     CCB_PDL_TRIGGER();
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int NST = a.nstages;
     const int stage_bytes = 2 * TC_TILE_BYTES + 2 * a.b_tile_bytes;
     uint64_t* full_bar = (uint64_t*)(smem + NST * stage_bytes);
-    uint64_t* empty_bar = full_bar + TC_STAGES;
-    uint64_t* accum_bar = empty_bar + TC_STAGES;
-    uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
+    uint64_t* empty_bar = full_bar + TC_MAX_STAGES;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
     const int ntile = min(TC_NMAX, a.Co - n0);
-    const int umma_n = (ntile + 15) & ~15;
     const int st_beg = blockIdx.z * a.per_split, st_end = min(a.stages, st_beg + a.per_split);
     const int nst = st_end - st_beg;          // >= 1 by construction
     const int KK = a.kh * a.kw;
     const int HWo = a.Ho * a.Wo, HWi = a.Hi * a.Wi;
 
     if (tid == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], TC_PRODUCERS / 2); mbar_init(&empty_bar[s], 1); }
-        mbar_init(accum_bar, 1);
+        for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], TC_PRODUCERS); mbar_init(&empty_bar[s], TC_CONSUMER_WARPS); }
         fence_barrier_init();
     }
-    if (warp == 8) tmem_alloc(tmem_slot, 256);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     CCB_PDL_SYNC();                                               // everything above touched no global data
 
-    if (warp < 8) {
-        // two producer groups (4 warps each) fill alternating stages; inside a group 8 consecutive threads
-        // walk the 8 K-chunks (32 consecutive pixels) of one row, rows rbase + 16 j
-        const int grp = warp >> 2;
-        const int c = tid & 7, rbase = (tid & 127) >> 3;
+    if (warp < TC_PRODUCERS / 32) {
+        // 8 consecutive threads walk the 8 K-chunks (32 consecutive pixels) of one row, rows rbase + 16 j
+        const int c = tid & 7, rbase = tid >> 3;
         // per-row constants: x offset of the row's (ci, ky, kx) relative to the pixel base, and its tap shift
         int rowoff[8], dky[8], dkx[8];
+        unsigned rvalid = 0;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             int m = m0 + rbase + 16 * j;
-            rowoff[j] = -1; dky[j] = dkx[j] = 0;
+            rowoff[j] = 0; dky[j] = dkx[j] = 0;
             if (m < a.Mtot) {
                 int tap = m / a.cpad, ci = m - tap * a.cpad;
                 if (ci < a.Ci) {
                     int ky = tap / a.kw, kx = tap - ky * a.kw;
                     dky[j] = ky - a.pad; dkx[j] = kx - a.pad;
-                    rowoff[j] = ci * HWi + dky[j] * a.Wi + dkx[j];       // >= -(pad*Wi+pad): flagged by dky/dkx checks below
-                    if (rowoff[j] < 0) rowoff[j] += 0;                  // (kept as is; validity is tracked by `rvalid`)
+                    rowoff[j] = ci * HWi + dky[j] * a.Wi + dkx[j];       // may be negative: only used where the tap is in bounds
+                    rvalid |= 1u << j;
                 }
             }
         }
-        unsigned rvalid = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            int m = m0 + rbase + 16 * j;
-            if (m < a.Mtot && (m - (m / a.cpad) * a.cpad) < a.Ci) rvalid |= 1u << j;
-        }
-        for (int it = grp; it < nst; it += 2) {
+        for (int it = 0; it < nst; ++it) {
             const int s = it % NST;
             const int p0 = ((st_beg + it) * TC_KC + c) * 4;       // first of this chunk's 4 pixels
             const bool pvalid = p0 < a.P;
@@ -570,92 +573,53 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_wgrad_kernel(const TcWg
                 const int r = rbase + 16 * j;
                 float4 h, l;
                 h.x = tf32_hi(av[j][0]); h.y = tf32_hi(av[j][1]); h.z = tf32_hi(av[j][2]); h.w = tf32_hi(av[j][3]);
-                a_hi[tile_idx(r, c, SWZ)] = h;
+                a_hi[tile_idx(r, c)] = h;
                 if (THREE) {
                     l.x = tf32_hi(av[j][0] - h.x); l.y = tf32_hi(av[j][1] - h.y); l.z = tf32_hi(av[j][2] - h.z); l.w = tf32_hi(av[j][3] - h.w);
-                    a_lo[tile_idx(r, c, SWZ)] = l;
+                    a_lo[tile_idx(r, c)] = l;
                 }
-                if (r < umma_n) {
+                if (r < NT) {
                     h.x = tf32_hi(bv[j].x); h.y = tf32_hi(bv[j].y); h.z = tf32_hi(bv[j].z); h.w = tf32_hi(bv[j].w);
-                    b_hi[tile_idx(r, c, SWZ)] = h;
+                    b_hi[tile_idx(r, c)] = h;
                     if (THREE) {
                         l.x = tf32_hi(bv[j].x - h.x); l.y = tf32_hi(bv[j].y - h.y); l.z = tf32_hi(bv[j].z - h.z); l.w = tf32_hi(bv[j].w - h.w);
-                        b_lo[tile_idx(r, c, SWZ)] = l;
+                        b_lo[tile_idx(r, c)] = l;
                     }
                 }
             }
             fence_proxy_async();
             mbar_arrive(&full_bar[s]);
         }
-        // ---- epilogue: lane == row m = (tap, ci); columns == co
-        mbar_wait(accum_bar, 0);
-        tc_fence_after();
-        const int q4 = warp & 3, colhalf = warp >> 2;
-        const int em = m0 + q4 * 32 + lane;
-        int eci = -1, etap = 0;
-        if (em < a.Mtot) {
-            etap = em / a.cpad;
-            int ci = em - etap * a.cpad;
-            if (ci < a.Ci) eci = ci;
-        }
-        float* outp = a.out + (long long)blockIdx.z * a.Co * a.Ci * KK;
-        for (int cg = colhalf; cg * 16 < umma_n; cg += 2) {
-            float v[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(cg * 16), v);
-            if (THREE) {
-                float vl[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + 128u + (uint32_t)(cg * 16), vl);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] += vl[j];
-            }
-            if (eci >= 0) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = cg * 16 + j;
-                    if (n < ntile) outp[((long long)(n0 + n) * a.Ci + eci) * KK + etap] = v[j];
-                }
-            }
-        }
-        tc_fence_before();
     } else {
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(umma_n >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-        uint32_t lbo = SWZ ? 16u : (uint32_t)(TC_M * 16);
-        uint32_t sbo = SWZ ? 1024u : 128u;
-        if (a.swap_lbo_sbo) { uint32_t t = lbo; lbo = sbo; sbo = t; }
-        const uint32_t ltype = SWZ ? 2u : 0u;
-        const uint32_t kstep_bytes = SWZ ? 32u : 2u * (uint32_t)(TC_M * 16);
-        for (int it = 0; it < nst; ++it) {
-            const int s = it % NST;
-            mbar_wait(&full_bar[s], (it / NST) & 1);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t base = smem_u32(smem + s * stage_bytes);
+        // ---- consumers; epilogue: row m = (tap, ci); columns == co
+        const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
+        float acc[NT / 2], part[NT / 2];
 #pragma unroll
-                for (int ks = 0; ks < TC_KC / 2; ++ks) {
-                    const uint32_t koff = (uint32_t)ks * kstep_bytes;
-                    const uint64_t ah = make_desc(base + koff, lbo, sbo, ltype);
-                    const uint64_t al = make_desc(base + TC_TILE_BYTES + koff, lbo, sbo, ltype);
-                    const uint64_t bh = make_desc(base + 2 * TC_TILE_BYTES + koff, lbo, sbo, ltype);
-                    const uint64_t bl = make_desc(base + 2 * TC_TILE_BYTES + a.b_tile_bytes + koff, lbo, sbo, ltype);
-                    umma_tf32(tmem_base, ah, bh, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-                    if (THREE) {
-                        umma_tf32(tmem_base + 128u, al, bh, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-                        umma_tf32(tmem_base + 128u, ah, bl, idesc, 1u);
-                    }
+        for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
+        tc_consume<THREE, NT>(smem, stage_bytes, a.b_tile_bytes, NST, nst, full_bar, empty_bar, wg, lane, acc, part);
+        float* outp = a.out + (long long)blockIdx.z * a.Co * a.Ci * KK;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const int em = m0 + wg * 64 + wq * 16 + (lane >> 2) + half * 8;
+            if (em >= a.Mtot) continue;
+            const int etap = em / a.cpad;
+            const int eci = em - etap * a.cpad;
+            if (eci >= a.Ci) continue;
+#pragma unroll
+            for (int i = 0; i < NT / 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int nl = 8 * i + 2 * (lane & 3) + e;
+                    const int j = 4 * i + 2 * half + e;
+                    if (nl < ntile) outp[((long long)(n0 + nl) * a.Ci + eci) * KK + etap] = acc[j];
                 }
-                umma_commit(&empty_bar[s]);
-                if (it == nst - 1) umma_commit(accum_bar);
-            }
-            __syncwarp();
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 8) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 256);
     }
 }
+
+static void (*const TC_WGRAD_KERNELS[2][4])(const TcWgradArgs) = {
+    {conv_tc_wgrad_kernel<false, 16>, conv_tc_wgrad_kernel<false, 32>, conv_tc_wgrad_kernel<false, 64>, conv_tc_wgrad_kernel<false, 128>},
+    {conv_tc_wgrad_kernel<true, 16>, conv_tc_wgrad_kernel<true, 32>, conv_tc_wgrad_kernel<true, 64>, conv_tc_wgrad_kernel<true, 128>}};
 
 // out[i] = sum_s work[s][i]
 __global__ void __launch_bounds__(256) tc_splitk_sum_kernel(const float* __restrict__ work, float* __restrict__ out,
@@ -667,9 +631,6 @@ __global__ void __launch_bounds__(256) tc_splitk_sum_kernel(const float* __restr
     for (int s = 0; s < splits; ++s) v += __ldg(work + (long long)s * numel + i);
     out[i] = v;
 }
-
-static int g_tc_swap = 0;
-static int g_tc_swz = 1;     // SWIZZLE_128B by default; the no-swizzle layout stays selectable for the probe
 
 // Shape gate: which problems take the tensor-core path under CCB_CONV_IMPL_AUTO
 bool tc_supported(const ccb_conv_desc* d, int op) {
@@ -693,9 +654,9 @@ static int wgrad_splits(const ccb_conv_desc* d, int& stages, int& per_split) {
     const long long P = (long long)d->B * d->Ho * d->Wo;
     stages = (int)((P + 31) / 32);
     const int tiles = cdiv(d->kh * d->kw * cpad, TC_M) * cdiv(d->Co, TC_NMAX);
-    int splits = cdiv(2 * 148, tiles);
+    int splits = cdiv(2 * NUM_SMS, tiles);
     if (splits > stages / 4) splits = stages / 4;
-    if (splits > 296) splits = 296;
+    if (splits > 2 * NUM_SMS) splits = 2 * NUM_SMS;
     if (splits < 1) splits = 1;
     per_split = cdiv(stages, splits);
     splits = cdiv(stages, per_split);          // no empty split
@@ -714,7 +675,7 @@ long long tc_workspace_floats(const ccb_conv_desc* d, int op) {
     long long out_numel = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Co * d->Ho * d->Wo : (long long)d->B * d->Ci * d->Hi * d->Wi;
     long long M = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Ho * d->Wo : (long long)d->B * d->Hi * d->Wi / (d->stride * d->stride);
     long long tiles = (long long)cdiv((int)M, TC_M) * cdiv(N, TC_NMAX);
-    long long part = (tiles < 148) ? 32 * out_numel : 0;       // room for up to 32 splits when the grid is small
+    long long part = (tiles < NUM_SMS) ? 32 * out_numel : 0;       // room for up to 32 splits when the grid is small
     return wpf + part;
 }
 
@@ -728,7 +689,7 @@ int tc_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float
     a.out_stride = 1; a.out_oy = 0; a.out_ox = 0; a.in_stride = d->stride;
     a.ntaps = d->kh * d->kw;
     a.M = d->B * d->Ho * d->Wo;
-    a.act = d->act; a.slope = d->slope; a.three = three; a.swap_lbo_sbo = g_tc_swap & 1; a.swz = g_tc_swz;
+    a.act = d->act; a.slope = d->slope;
     signed char tix[TC_MAX_TAPS];
     for (int ky = 0; ky < d->kh; ++ky)
         for (int kx = 0; kx < d->kw; ++kx) {
@@ -741,7 +702,7 @@ int tc_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float
     const int Kp = roundup(a.ntaps * roundup(d->Ci, 4), 32);
     const long long wpf = 2ll * d->Co * Kp;
     const int splits = plan_splits(a.M, d->Co, Kp / 32, a.out_numel, work_floats - wpf);
-    int rc = launch_tc(a, w, 0, d->Co, d->Ci, d->kh * d->kw, d->Ci, tix, work, work_floats, splits, nullptr, st);
+    int rc = launch_tc(a, w, 0, d->Co, d->Ci, d->kh * d->kw, d->Ci, tix, work, work_floats, splits, nullptr, three, st);
     if (rc || splits == 1) return rc;
     launch_splitk_reduce(a.partial, y, bias, res, a.out_numel, splits, d->Ho * d->Wo, d->Co, d->act, d->slope, st);
     return check_launch("conv_tc splitk reduce");
@@ -769,7 +730,7 @@ int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const floa
             a.Hc = (d->Hi - py + s - 1) / s; a.Wc = (d->Wi - px + s - 1) / s;
             a.out_stride = s; a.out_oy = py; a.out_ox = px; a.in_stride = 1;
             a.M = d->B * a.Hc * a.Wc;
-            a.act = d->act; a.slope = d->slope; a.three = three; a.swap_lbo_sbo = g_tc_swap & 1; a.swz = g_tc_swz;
+            a.act = d->act; a.slope = d->slope;
             signed char tix[TC_MAX_TAPS];
             int nt = 0;
             for (int ky = 0; ky < d->kh; ++ky) {
@@ -786,7 +747,7 @@ int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const floa
             a.ntaps = nt;
             // every class prepares its own weights at the start of `work`; partials live after the largest prep
             int rc = launch_tc(a, w, 1, d->Ci, d->Co, d->kh * d->kw, d->Ci, tix, work, wpf_max + (splits > 1 ? splits * out_numel : 0),
-                               splits, work + wpf_max, st);
+                               splits, work + wpf_max, three, st);
             if (rc) return rc;
         }
     if (splits > 1) {
@@ -807,7 +768,6 @@ int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
     a.Mtot = d->kh * d->kw * a.cpad;
     a.P = d->B * d->Ho * d->Wo;
     a.splits = wgrad_splits(d, a.stages, a.per_split);
-    a.three = three; a.swz = g_tc_swz; a.swap_lbo_sbo = g_tc_swap & 1;
     const long long numel = (long long)d->Co * d->Ci * d->kh * d->kw;
     if (a.splits > 1) {
         CCB_REQUIRE(work && (long long)a.splits * numel <= work_floats, CCB_ERR_ARG, "conv_tc wgrad: workspace too small");
@@ -815,32 +775,24 @@ int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
     } else {
         a.out = dw;
     }
-    {
-        const int ntile_max = d->Co < TC_NMAX ? d->Co : TC_NMAX;
-        int nalloc = 16;
-        while (nalloc < ntile_max) nalloc <<= 1;
-        if (!a.swz) nalloc = 128;
-        a.b_tile_bytes = nalloc * 128;
-        a.nstages = (nalloc <= 64) ? 2 : TC_STAGES;
-    }
-    const int wsmem = tc_smem_bytes(a.nstages, a.b_tile_bytes);
+    int nt, wsmem;
+    tc_geometry(d->Co, nt, a.b_tile_bytes, a.nstages, wsmem);
     dim3 grid(cdiv(a.Mtot, TC_M), cdiv(d->Co, TC_NMAX), a.splits);
-    auto kfn = a.swz ? (a.three ? conv_tc_wgrad_kernel<true, true> : conv_tc_wgrad_kernel<false, true>)
-                     : (a.three ? conv_tc_wgrad_kernel<true, false> : conv_tc_wgrad_kernel<false, false>);
-    cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES);
-    CCB_LAUNCH(kfn, grid, dim3(TC_THREADS), wsmem, st, a);
-    int rc = check_launch("conv_tc_wgrad");
+    int rc = tc_launch_kernel(TC_WGRAD_KERNELS, a, three, nt, grid, wsmem, st, "conv_tc_wgrad");
     if (rc || a.splits == 1) return rc;
     CCB_LAUNCH(tc_splitk_sum_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), 0, st, (const float*)work, dw, numel, a.splits);
     return check_launch("conv_tc_wgrad_reduce");
 }
 
-void tma_set_enabled(int v);   // conv_tma.cu
-void tc_set_debug_swap(int v) { g_tc_swap = v & 1; g_tc_swz = (v & 4) ? 0 : 1; tma_set_enabled(((v & 8) ? 0 : 1) | ((v & 16) ? 2 : 0)); }
-
 }  // namespace ccb
 
-extern "C" void ccb_debug_tc_swap_strides(int v) { ccb::tc_set_debug_swap(v); }
+// host-side tile geometry of a launch with N output channels (no launch, no GPU needed):
+// out4 = {wgmma N, bytes of one B operand copy, pipeline stages, dynamic shared memory bytes}
+extern "C" int ccb_debug_tc_plan(int N, int* out4) {
+    if (N < 1 || !out4) return CCB_ERR_ARG;
+    ccb::tc_geometry(N, out4[0], out4[1], out4[2], out4[3]);
+    return CCB_OK;
+}
 
 #else   // CCB_CPU_SIM: no tensor cores in the CPU execution-model simulator
 
@@ -856,6 +808,7 @@ int tc_wgrad(const ccb_conv_desc*, const float*, const float*, float*, float*, l
     return CCB_ERR_UNSUPPORTED;
 }
 }  // namespace ccb
-extern "C" void ccb_debug_tc_swap_strides(int) {}
+
+extern "C" int ccb_debug_tc_plan(int, int*) { return CCB_ERR_UNSUPPORTED; }
 
 #endif

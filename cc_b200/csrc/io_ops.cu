@@ -343,7 +343,7 @@ using namespace ccb;
 
 static int grid_for(long long n) {
     long long g = (n + 255) / 256;
-    const long long cap = 148 * 8;
+    const long long cap = NUM_SMS * 8;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

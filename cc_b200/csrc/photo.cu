@@ -7,7 +7,7 @@
 // coordinates), run the separable 13-tap Gaussian moments out of shared memory
 // (rows -> smem, columns -> registers), and finish SSIM / robust-L1 / mask terms in registers.
 //
-// Roofline note (DESIGN.md): with the reference's real 13x13 window the kernel is FP32-FMA bound
+// Roofline note: with the reference's real 13x13 window the kernel is FP32-FMA bound
 // (~1.4 kFMA per level-pixel forward), not HBM bound; with wssim == 0 the SSIM stage is compiled
 // out (template SSIM=false) and the kernel is a pure streaming pass.
 //

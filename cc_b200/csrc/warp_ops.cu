@@ -64,6 +64,7 @@ struct WarpArgs {
     float* d_depth;
     float* d_flow;
     float* d_img;
+    unsigned long long* d_img_fx;   // flow-warp backward: fixed-point accumulators of d_img, then max |grad_out| bits
     float* d_pose;
     float* pose_partials;
     int B, C, h, w, rot, pad;
@@ -179,6 +180,56 @@ __device__ __forceinline__ void warp_coords(const WarpArgs& a, float x, float y,
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// The image gradient of a bilinear sample is a scatter: an arbitrary flow can send any number of output pixels to one
+// source pixel.  Float atomics would make the sum depend on the order the hardware serialises them in, and the training
+// step (DispResNet6's chaotic gradient above all) would not compute the same thing twice.  The scatter therefore adds
+// 64-bit fixed-point integers - integer addition is associative, so the result is independent of the order:
+//   pass 1  max |grad_out| over the finite values (an order-free max, as integer bits)
+//   pass 2  each contribution v -> round(v * 2^s) added to its accumulator, s = 62 - e - c with grad_out < 2^e and
+//           h*w < 2^c: at most h*w contributions of magnitude <= max |grad_out| reach one accumulator, so none overflows,
+//           and the resolution is 2^-(62 - c) of max |grad_out| (2^-44 at 256x832), far below fp32 rounding of the sum
+//   pass 3  d_img += accumulator * 2^-s
+// A non-finite contribution (inf / NaN in grad_out) cannot be held in fixed point: it goes straight into its own d_img
+// element with a float atomic, as an unfixed scatter would put it - an inf / NaN sum does not depend on the order either.
+__device__ __forceinline__ double fx_scale(const WarpArgs& a) {
+    const float gmax = __uint_as_float((unsigned)a.d_img_fx[(long long)a.B * a.C * a.h * a.w]);
+    if (!(gmax > 0.f)) return 1.0;
+    const long long hw = (long long)a.h * a.w;
+    const int e = ilogbf(gmax) + 1, c = 64 - __clzll(hw);
+    return ldexp(1.0, 62 - e - c);
+}
+__device__ __forceinline__ void fx_add(const WarpArgs& a, long long i, float v, double scale) {
+    if (isfinite(v)) atomicAdd(a.d_img_fx + i, (unsigned long long)__double2ll_rn((double)v * scale));
+    else atomicAdd(a.d_img + i, v);
+}
+__device__ __forceinline__ void fx_scatter(const WarpArgs& a, long long plane_off, const Samp& s, float g, double scale) {
+    const long long i = plane_off + (long long)s.y0 * a.w + s.x0;
+    if (s.oky0 && s.okx0) fx_add(a, i, g * s.wy0 * s.wx0, scale);
+    if (s.oky0 && s.okx1) fx_add(a, i + 1, g * s.wy0 * s.wx1, scale);
+    if (s.oky1 && s.okx0) fx_add(a, i + a.w, g * s.wy1 * s.wx0, scale);
+    if (s.oky1 && s.okx1) fx_add(a, i + a.w + 1, g * s.wy1 * s.wx1, scale);
+}
+
+__global__ void __launch_bounds__(WNT) fx_absmax_kernel(const WarpArgs a, long long n) {
+    CCB_PDL_WAIT();
+    unsigned m = 0;
+    for (long long i = (long long)blockIdx.x * WNT + threadIdx.x; i < n; i += (long long)gridDim.x * WNT) {
+        const unsigned bits = __float_as_uint(__ldg(a.grad_out + i)) & 0x7fffffffu;   // |g| as bits: ordered like the values
+        if (bits < 0x7f800000u) m = max(m, bits);                                        // finite only
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(a.d_img_fx + n, (unsigned long long)m);
+}
+
+__global__ void __launch_bounds__(WNT) fx_finish_kernel(const WarpArgs a, long long n) {
+    CCB_PDL_WAIT();
+    const long long i = (long long)blockIdx.x * WNT + threadIdx.x;
+    if (i >= n) return;
+    a.d_img[i] += (float)((double)(long long)a.d_img_fx[i] / fx_scale(a));
+}
+
 // flow_warp (inverse_warp.py:164-192), any channel count
 __global__ void __launch_bounds__(WNT) flow_warp_fwd_kernel(const WarpArgs a) {
     CCB_PDL_WAIT();
@@ -209,6 +260,7 @@ __global__ void __launch_bounds__(WNT) flow_warp_bwd_kernel(const WarpArgs a) {
     Samp s = make_samp(Xn, Yn, a.w, a.h, a.pad);
     const float* im = a.img + (long long)b * a.C * hw;
     float gix = 0.f, giy = 0.f;
+    const double scale = a.d_img ? fx_scale(a) : 1.0;
     for (int c = 0; c < a.C; ++c) {
         float g = __ldg(a.grad_out + (long long)b * a.C * hw + c * hw + idx);
         if (a.d_flow) {
@@ -216,13 +268,7 @@ __global__ void __launch_bounds__(WNT) flow_warp_bwd_kernel(const WarpArgs a) {
             gix += g * interp_dx(cr, s);
             giy += g * interp_dy(cr, s);
         }
-        if (a.d_img) {
-            float* di = a.d_img + (long long)b * a.C * hw + c * hw + (long long)s.y0 * a.w + s.x0;
-            if (s.oky0 && s.okx0) atomicAdd(di, g * s.wy0 * s.wx0);
-            if (s.oky0 && s.okx1) atomicAdd(di + 1, g * s.wy0 * s.wx1);
-            if (s.oky1 && s.okx0) atomicAdd(di + a.w, g * s.wy1 * s.wx0);
-            if (s.oky1 && s.okx1) atomicAdd(di + a.w + 1, g * s.wy1 * s.wx1);
-        }
+        if (a.d_img) fx_scatter(a, (long long)b * a.C * hw + c * hw, s, g, scale);
     }
     if (a.d_flow) {
         a.d_flow[(long long)b * 2 * hw + idx] = gix * s.gmx * (2.f / w1);
@@ -474,6 +520,7 @@ __global__ void __launch_bounds__(WNT) flow_warp_bwd_wpp_kernel(const WarpArgs a
     const Samp s = make_samp(Xn, Yn, a.w, a.h, a.pad);
     const float* im = a.img + (long long)b * a.C * hw;
     float gix = 0.f, giy = 0.f;
+    const double scale = a.d_img ? fx_scale(a) : 1.0;
     for (int c = lane; c < a.C; c += 32) {
         const float g = __ldg(a.grad_out + (long long)b * a.C * hw + c * hw + idx);
         if (a.d_flow) {
@@ -481,13 +528,7 @@ __global__ void __launch_bounds__(WNT) flow_warp_bwd_wpp_kernel(const WarpArgs a
             gix += g * interp_dx(cr, s);
             giy += g * interp_dy(cr, s);
         }
-        if (a.d_img) {
-            float* di = a.d_img + (long long)b * a.C * hw + c * hw + (long long)s.y0 * a.w + s.x0;
-            if (s.oky0 && s.okx0) atomicAdd(di, g * s.wy0 * s.wx0);
-            if (s.oky0 && s.okx1) atomicAdd(di + 1, g * s.wy0 * s.wx1);
-            if (s.oky1 && s.okx0) atomicAdd(di + a.w, g * s.wy1 * s.wx0);
-            if (s.oky1 && s.okx1) atomicAdd(di + a.w + 1, g * s.wy1 * s.wx1);
-        }
+        if (a.d_img) fx_scatter(a, (long long)b * a.C * hw + c * hw, s, g, scale);
     }
     if (a.d_flow) {
         gix = warp_sum(gix);
@@ -501,6 +542,12 @@ __global__ void __launch_bounds__(WNT) flow_warp_bwd_wpp_kernel(const WarpArgs a
 
 static bool warp_per_pixel(int B, int C, int h, int w) { return C >= 16 && (long long)B * h * w < 32768; }
 static void launch_flow_warp(const WarpArgs& a, bool bwd, cudaStream_t st) {
+    const long long n = (long long)a.B * a.C * a.h * a.w;
+    if (bwd && a.d_img) {
+        cudaMemsetAsync(a.d_img_fx, 0, (size_t)(n + 1) * sizeof(unsigned long long), st);
+        const long long nb = (n + WNT - 1) / WNT;
+        CCB_LAUNCH(fx_absmax_kernel, dim3((unsigned)(nb < 4 * NUM_SMS ? nb : 4 * NUM_SMS)), dim3(WNT), 0, st, a, n);
+    }
     if (warp_per_pixel(a.B, a.C, a.h, a.w)) {
         const unsigned nb = (unsigned)cdiv((int)((long long)a.B * a.h * a.w), WNT / 32);
         if (bwd) CCB_LAUNCH(flow_warp_bwd_wpp_kernel, dim3(nb), dim3(WNT), 0, st, a);
@@ -509,6 +556,7 @@ static void launch_flow_warp(const WarpArgs& a, bool bwd, cudaStream_t st) {
         if (bwd) CCB_LAUNCH(flow_warp_bwd_kernel, dim3(cdiv(a.h * a.w, WNT), a.B), dim3(WNT), 0, st, a);
         else CCB_LAUNCH(flow_warp_fwd_kernel, dim3(cdiv(a.h * a.w, WNT), a.B), dim3(WNT), 0, st, a);
     }
+    if (bwd && a.d_img) CCB_LAUNCH(fx_finish_kernel, dim3((unsigned)((n + WNT - 1) / WNT)), dim3(WNT), 0, st, a, n);
 }
 
 extern "C" int ccb_flow_warp_fwd(const float* img, const float* flow, int B, int C, int h, int w,
@@ -524,11 +572,12 @@ extern "C" int ccb_flow_warp_fwd(const float* img, const float* flow, int B, int
 
 extern "C" int ccb_flow_warp_bwd(const float* img, const float* flow, int B, int C, int h, int w,
                                  int padding_mode, const float* grad_out, float* d_flow, float* d_img,
-                                 ccb_stream_t stream) {
+                                 unsigned long long* work, ccb_stream_t stream) {
     CCB_REQUIRE(img && flow && grad_out, CCB_ERR_ARG, "flow_warp_bwd: null pointer");
+    CCB_REQUIRE(!d_img || work, CCB_ERR_ARG, "flow_warp_bwd: d_img needs the fixed-point workspace");
     WarpArgs a;
     memset(&a, 0, sizeof(a));
-    a.img = img; a.flow = flow; a.grad_out = grad_out; a.d_flow = d_flow; a.d_img = d_img;
+    a.img = img; a.flow = flow; a.grad_out = grad_out; a.d_flow = d_flow; a.d_img = d_img; a.d_img_fx = work;
     a.B = B; a.C = C; a.h = h; a.w = w; a.pad = padding_mode;
     launch_flow_warp(a, true, (cudaStream_t)stream);
     return check_launch("flow_warp_bwd");
@@ -546,11 +595,12 @@ extern "C" int ccb_featwarp_fwd(const float* x, const float* flow, int B, int C,
 }
 
 extern "C" int ccb_featwarp_bwd(const float* x, const float* flow, int B, int C, int h, int w, const float* grad_out,
-                                float* d_flow, float* d_x, ccb_stream_t stream) {
+                                float* d_flow, float* d_x, unsigned long long* work, ccb_stream_t stream) {
     CCB_REQUIRE(x && flow && grad_out, CCB_ERR_ARG, "featwarp_bwd: null pointer");
+    CCB_REQUIRE(!d_x || work, CCB_ERR_ARG, "featwarp_bwd: d_x needs the fixed-point workspace");
     WarpArgs a;
     memset(&a, 0, sizeof(a));
-    a.img = x; a.flow = flow; a.grad_out = grad_out; a.d_flow = d_flow; a.d_img = d_x;
+    a.img = x; a.flow = flow; a.grad_out = grad_out; a.d_flow = d_flow; a.d_img = d_x; a.d_img_fx = work;
     a.B = B; a.C = C; a.h = h; a.w = w; a.pad = CCB_PAD_BORDER; a.b2f_norm = 1;
     launch_flow_warp(a, true, (cudaStream_t)stream);
     return check_launch("featwarp_bwd");

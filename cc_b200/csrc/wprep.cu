@@ -11,33 +11,9 @@
 namespace ccb {
 
 __device__ __forceinline__ bool wprep_decode(const WPrepDesc& a, int k, int& slot, int& c) {
-    if (a.layout == WPREP_TC) {                       // k = slot * cpad + c
-        slot = k / a.p0;
-        c = k - slot * a.p0;
-        return slot < a.ntaps && c < a.Cc;
-    }
-    if (a.layout == WPREP_TMA) {                      // k = unit * cb + j, unit = slot * cblocks + channel block
-        const int unit = k / a.p0, j = k - unit * a.p0;
-        if (unit >= a.p2) return false;
-        slot = unit / a.p1;
-        c = (unit - slot * a.p1) * a.p0 + j;
-        return slot < a.ntaps && c < a.Cc;
-    }
-    if (a.layout == WPREP_NHWC) {                     // k-stage = (channel block, slot), 32 channels each (tail zero)
-        const int kt = k >> 5;
-        const int cblock = kt / a.p2;
-        slot = kt - cblock * a.p2;
-        c = cblock * 32 + (k & 31);
-        return cblock < a.p1 && slot < a.ntaps && c < a.Cc;
-    }
-    // WPREP_SLAB: k-stage -> (channel block, flattened (slot, channel) index inside the block)
-    const int kt = k >> 5;
-    const int cblock = min(kt / a.p2, a.p1 - 1);
-    const int kl = (kt - cblock * a.p2) * 32 + (k & 31);
-    const int nch = min(a.p0, a.Cc - cblock * a.p0);
-    slot = kl / nch;
-    c = cblock * a.p0 + (kl - slot * nch);
-    return slot < a.ntaps;
+    slot = k / a.p0;                                  // k = slot * cpad + c
+    c = k - slot * a.p0;
+    return slot < a.ntaps && c < a.Cc;
 }
 
 __device__ __forceinline__ void wprep_block(const WPrepDesc& a, int nb, int block, float* sw) {
@@ -111,7 +87,7 @@ static int wprep_nb(const WPrepDesc& d) {
     if (nb > 8) nb = 8;
     if (nb < 1) nb = 1;
     // keep enough blocks in flight
-    while (nb > 1 && cdiv(d.N, nb) < 148) nb >>= 1;
+    while (nb > 1 && cdiv(d.N, nb) < NUM_SMS) nb >>= 1;
     return nb;
 }
 
@@ -190,7 +166,7 @@ extern "C" long long ccb_wcache_plan_floats(void* h) {
     c->offs.clear();
     for (auto& e : c->entries) {
         c->offs.push_back(tot);
-        tot += (2ll * e.d.N * e.d.Kp + 63) / 64 * 64;          // 256-byte aligned copies (TMA needs 16)
+        tot += (2ll * e.d.N * e.d.Kp + 63) / 64 * 64;          // 256-byte aligned copies
     }
     return tot;
 }

@@ -7,7 +7,7 @@ rank runs the whole step (nets + losses) on its own b/N shard and the only excha
 ncclAllReduce(sum) over the flat fp32 gradient buffer, averaged by the Adam kernel's
 grad_scale = 1/world_size.
 
-Semantics versus the reference (documented deviation, DESIGN.md section 5):
+Semantics versus the reference (documented deviation):
   * BatchNorm batch statistics are per replica in the reference's DataParallel too - identical.
   * The losses are NOT: the reference gathers the net outputs to GPU0 and evaluates every loss over the
     FULL batch, so `oob_normalization_const = numel/valid.sum()` (loss_functions.py:48,103) and every

@@ -1,7 +1,7 @@
 """Drop-in for the reference's ``inverse_warp`` module (inverse_warp.py), backed by libccb200.
 
 Same names, argument meaning and AssertionError text as the reference; every function launches
-hand-written sm_100a kernels (cc_b200/csrc/warp_ops.cu) and supports autograd through
+hand-written sm_90a kernels (cc_b200/csrc/warp_ops.cu) and supports autograd through
 hand-derived backward kernels.  ``train.py:22`` imports inverse_warp, pose2flow, flow2oob, flow_warp."""
 from __future__ import division
 import torch
@@ -101,8 +101,10 @@ class _FlowWarp(torch.autograd.Function):
         g = _f(g)
         d_flow = torch.empty_like(flow) if ctx.needs_input_grad[1] else None
         d_img = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
+        work = _lib.scatter_workspace(img) if d_img is not None else None
         _lib.check(_lib.lib().ccb_flow_warp_bwd(_lib.ptr(img), _lib.ptr(flow), B, Cc, h, w, ctx.pad, _lib.ptr(g),
-                                                _lib.ptr(d_flow), _lib.ptr(d_img), _lib.stream(img)), 'flow_warp_bwd')
+                                                _lib.ptr(d_flow), _lib.ptr(d_img), _lib.ptr(work, 'work', torch.int64),
+                                                _lib.stream(img)), 'flow_warp_bwd')
         return d_img, d_flow, None
 
 

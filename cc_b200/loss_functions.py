@@ -1,11 +1,11 @@
 """Drop-in for the reference's ``loss_functions`` module (loss_functions.py), backed by libccb200.
 
 Every name ``train.py:23-26`` imports exists here with the same signature.  The multi-scale
-photometric / SSIM / smoothness / consensus losses each run as ONE fused sm_100a launch over all
+photometric / SSIM / smoothness / consensus losses each run as ONE fused sm_90a launch over all
 pyramid levels (csrc/photo.cu, csrc/smooth_bce.cu) with hand-derived backward kernels, instead of
 the reference's ~30 k ATen calls per step (SURVEY.md 3.1).
 
-Differences a maintainer should know (DESIGN.md "semantic notes"):
+Differences a maintainer should know:
   * the reference's NaN ``assert(... .item() == 1)`` host syncs (loss_functions.py:60,105,115) are
     not replicated - nothing here synchronises the host;
   * pyramid levels must be exact 2^l reductions of the frame (true for every net in the reference).

@@ -12,7 +12,7 @@ from . import _lib
 
 ACT = {None: _lib.ACT_NONE, 'none': _lib.ACT_NONE, 'relu': _lib.ACT_RELU, 'leaky': _lib.ACT_LEAKY,
        'sigmoid': _lib.ACT_SIGMOID}
-CONV_IMPL = _lib.IMPL_AUTO          # tests flip this to force the FFMA or the tcgen05 path
+CONV_IMPL = _lib.IMPL_AUTO          # tests flip this to force the FFMA or the tensor-core path
 
 _WORK = {}
 _WORK_RETIRED = []          # outgrown buffers a captured CUDA graph may still point into: kept alive, never reused
@@ -430,8 +430,9 @@ class _FeatWarpFn(torch.autograd.Function):
         g = _c(g)
         dx = torch.zeros_like(x) if ctx.needs_input_grad[0] else None
         df = torch.empty_like(flo) if ctx.needs_input_grad[1] else None
+        work = _lib.scatter_workspace(x) if dx is not None else None
         _lib.check(_lib.lib().ccb_featwarp_bwd(_lib.ptr(x), _lib.ptr(flo), B, Cc, h, w, _lib.ptr(g), _lib.ptr(df),
-                                               _lib.ptr(dx), _lib.stream(x)), 'featwarp_bwd')
+                                               _lib.ptr(dx), _lib.ptr(work, 'work', torch.int64), _lib.stream(x)), 'featwarp_bwd')
         return dx, df
 
 

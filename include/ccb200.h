@@ -1,4 +1,4 @@
-/* ccb200.h - C ABI of libccb200.so: the B200 (sm_100a) implementation of the Competitive-Collaboration
+/* ccb200.h - C ABI of libccb200.so: the H100 (sm_90a) implementation of the Competitive-Collaboration
  * training step's dense per-pixel path (anuragranj/cc @ 2b4e362).
  *
  * Conventions (SURVEY.md 8b):
@@ -127,10 +127,11 @@ long long ccb_warp_pose_partials_floats(int B, int h, int w);
 /* flow_warp (inverse_warp.py:164-192): img [B,C,h,w], flow [B,2,h,w]; padding zeros|border. */
 int ccb_flow_warp_fwd(const float* img, const float* flow, int B, int C, int h, int w,
                       int padding_mode, float* out, ccb_stream_t stream);
-/* d_flow [B,2,h,w] (may be NULL), d_img [B,C,h,w] (may be NULL; must be zero-filled by the caller). */
+/* d_flow [B,2,h,w] (may be NULL), d_img [B,C,h,w] (may be NULL; the gradient is ADDED to it).  With d_img, work holds
+ * B*C*h*w + 1 64-bit words: the image gradient is a scatter, summed in fixed point so that it is the same on every run. */
 int ccb_flow_warp_bwd(const float* img, const float* flow, int B, int C, int h, int w,
                       int padding_mode, const float* grad_out, float* d_flow, float* d_img,
-                      ccb_stream_t stream);
+                      unsigned long long* work, ccb_stream_t stream);
 /* pose2flow (inverse_warp.py:195-220): -> flow [B,2,h,w]; padding_mode CCB_PAD_NONE | CCB_PAD_ZEROS. */
 int ccb_pose2flow_fwd(const float* depth, const float* pose, int pose_stride, const float* K,
                       const float* Kinv, int B, int h, int w, int rotation_mode, int padding_mode,
@@ -201,13 +202,13 @@ int ccb_bce_bwd(const ccb_bce_desc* d, ccb_stream_t stream);
  *        (plain data-gradient when bias/res are NULL and act is NONE; with them it is the
  *         nn.ConvTranspose2d forward of a layer whose torch weight [Cin_t,Cout_t,k,k] is this w)
  *   dw = d/dw, db = sum dy                                         ccb_conv2d_wgrad
- * impl: CCB_CONV_IMPL_AUTO picks tcgen05 tensor-core tiles where the shape allows and the FFMA
+ * impl: CCB_CONV_IMPL_AUTO picks wgmma tensor-core tiles where the shape allows and the FFMA
  *       kernels otherwise; _FFMA / _TC force one (tests).
  * ---------------------------------------------------------------------------------------------- */
 enum { CCB_ACT_NONE = 0, CCB_ACT_RELU = 1, CCB_ACT_LEAKY = 2, CCB_ACT_SIGMOID = 3 };
 enum { CCB_CONV_FPROP = 0, CCB_CONV_DGRAD = 1, CCB_CONV_WGRAD = 2 };
-enum { CCB_CONV_IMPL_AUTO = 0, CCB_CONV_IMPL_FFMA = 1, CCB_CONV_IMPL_TC = 2 /* tcgen05 3xTF32 (fp32 parity) */,
-       CCB_CONV_IMPL_TC_TF32 = 3 /* tcgen05 single TF32 (cuDNN's default math for the reference) */ };
+enum { CCB_CONV_IMPL_AUTO = 0, CCB_CONV_IMPL_FFMA = 1, CCB_CONV_IMPL_TC = 2 /* wgmma 3xTF32 (fp32 parity) */,
+       CCB_CONV_IMPL_TC_TF32 = 3 /* wgmma single TF32 (cuDNN's default math for the reference) */ };
 typedef struct ccb_conv_desc {
     int B, Ci, Hi, Wi;      /* input  [B,Ci,Hi,Wi] */
     int Co, Ho, Wo;         /* output [B,Co,Ho,Wo]; Ho = (Hi + 2 pad - kh) / stride + 1 */
@@ -269,9 +270,9 @@ int ccb_corr81_bwd(const float* f1, const float* f2, const float* grad_out, floa
                    int C, int h, int w, int reversed, float* work, ccb_stream_t stream);
 int ccb_featwarp_fwd(const float* x, const float* flow, int B, int C, int h, int w, float* out,
                      ccb_stream_t stream);
-/* d_x must be zero-filled by the caller (scatter-add); d_flow / d_x may be NULL */
+/* d_flow / d_x may be NULL; the gradient is ADDED to d_x; with d_x, work holds B*C*h*w + 1 64-bit words (as flow_warp_bwd) */
 int ccb_featwarp_bwd(const float* x, const float* flow, int B, int C, int h, int w, const float* grad_out,
-                     float* d_flow, float* d_x, ccb_stream_t stream);
+                     float* d_flow, float* d_x, unsigned long long* work, ccb_stream_t stream);
 
 /* BatchNorm2d over [B,C,plane] (DispResNet6.py:45-52).  training: batch statistics, stats[C][2] =
  * {mean, invstd} saved for backward, running stats updated in place (momentum, unbiased var). */

@@ -1,6 +1,5 @@
 /* ccb200_debug.h - bring-up and diagnostic entry points of libccb200.so.  NOT part of the drop-in boundary
- * (include/ccb200.h): probes (tools/*_probe.py), the parity tests that switch kernel families, and bench.py's per-kernel
- * timing use them; a reference-side binding never needs them. */
+ * (include/ccb200.h): bench.py's per-kernel timing and the unit tests use them; a reference-side binding never needs them. */
 #ifndef CCB200_DEBUG_H
 #define CCB200_DEBUG_H
 #include "ccb200.h"
@@ -8,29 +7,12 @@
 extern "C" {
 #endif
 
-/* bring-up aid (layout probe): bit 0 swaps the LBO/SBO strides of the UMMA shared-memory descriptors
- * (must produce wrong results), bit 2 selects the K-major no-swizzle operand layout instead of the
- * default SWIZZLE_128B one (must produce identical results), bit 3 turns the TMA-fed kernels off so that
- * every shape takes the register-gather tensor-core kernels (must produce results within rounding), bit 4 makes
- * a barrier time-out inside the TMA kernels a recorded event instead of a trap */
-void ccb_debug_tc_swap_strides(int swap);
-/* synchronises the device, then returns and clears the first recorded barrier time-out of the TMA conv kernels:
- * out4 = {role (0 = none; 1 producer/empty, 2 mma/tma_full, 3 mma/split_full, 4 split/tma_full, 5 epilogue/accum),
- * k-iteration, blockIdx.x, blockIdx.z} */
-int ccb_debug_tma_status(unsigned int* out4);
-/* which kernel the last convolution call of this thread launched ("conv_nhwc", "conv_slab", "conv_tma", "conv_direct", "conv_tc",
- * "conv_slab_wgrad", "conv_tc_wgrad", "conv2d_fprop" ... for the CUDA-core GEMM): bench.py buckets its per-call timings by it */
+/* which kernel the last convolution call of this thread launched ("conv_tc", "conv_tc_wgrad",
+ * "conv2d_fprop" ... for the CUDA-core GEMM): bench.py buckets its per-call timings by it */
 const char* ccb_debug_last_conv_kernel(void);
-/* bring-up aids of the channels-last slab kernel (conv_nhwc.cu): enabled = 0 routes its problems back to the NCHW kernels
- * (must produce results within rounding), soft = 1 records barrier time-outs instead of trapping, dbg bit 0 sets the
- * descriptor base-offset field (must produce wrong results for taps whose slab offset is not a multiple of 8 pixels),
- * bit 2 sends 1x1 convolutions through it as well.  ccb_debug_nhwc_status: like ccb_debug_tma_status. */
-void ccb_debug_nhwc(int enabled, int soft, int dbg);
-int ccb_debug_nhwc_status(unsigned int* out4);
-/* host-side tiling of the TMA-fed convolution family for one problem (no launch, no driver needed; unit tests):
- * op FPROP / DGRAD (parity class py, px) -> out16 = {kind (2 slab, 3 aligned TMA, 4 direct, -1 none), ...}, WGRAD -> {5, ...};
- * field meaning in conv_tma.cu */
-int ccb_debug_conv_plan(const ccb_conv_desc* d, int op, int py, int px, int* out16);
+/* host-side geometry of the wgmma convolution kernels for N output channels (no launch; unit tests):
+ * out4 = {wgmma N, bytes of one B operand copy, pipeline stages, dynamic shared memory bytes} */
+int ccb_debug_tc_plan(int N, int* out4);
 
 #ifdef __cplusplus
 }

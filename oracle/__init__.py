@@ -8,8 +8,8 @@ reference file:line it follows.
 
 Parity pinning: the reference ships NO golden vectors or unit tests
 (SURVEY.md section 4), so the oracle is pinned against *outputs of the reference
-itself executed in the build container* - ``tests/golden/make_golden.py`` imports
-``/root/reference`` and freezes its outputs (and autograd gradients) into
+itself* - ``tests/golden/make_golden.py`` imports
+a checkout of the reference (``$CC_REFERENCE``) and freezes its outputs (and autograd gradients) into
 ``tests/golden/*.npz``; ``tests/test_oracle_golden.py`` checks this package
 against those fixtures.  The third-party ``spatial_correlation_sampler`` used by
 Back2Future is absent from the tree: that one boundary is "parity unpinned"

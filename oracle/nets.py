@@ -13,7 +13,7 @@ this oracle and the CUDA product.
 PARITY UNPINNED at one boundary: ``correlate`` restates the published behaviour of
 the third-party ``spatial_correlation_sampler`` (PyPI spatial-correlation-sampler,
 version un-pinned in reference requirements.txt:13, upstream
-ClementPinard/Pytorch-Correlation-extension; source absent from /root/reference):
+ClementPinard/Pytorch-Correlation-extension; source absent from the reference repository):
 out[b,ph,pw,y,x] = sum_c in1[b,c,y,x] * in2[b,c,y+ph-4,x+pw-4] (zero outside), with
 kernel_size=1, patch_size=9, stride=1.  It is anchored only by the reference's call
 site and permutation tables (back2future.py:15-25,56-59).

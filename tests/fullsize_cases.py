@@ -1,4 +1,4 @@
-"""Step-level parity of the PRODUCTION path (Trainer.step on IMPL_AUTO = the tcgen05 / TMA kernels) at the
+"""Step-level parity of the PRODUCTION path (Trainer.step on IMPL_AUTO = the wgmma tensor-core kernels) at the
 BASELINE.json configurations: b4, 256x832, 6 pyramid levels, cfg1 / cfg2 / cfg3.
 
 For every configuration the CUDA step is compared with the CPU oracle (oracle/step.py = reference
@@ -12,18 +12,18 @@ carries the *noise floor*: the same oracle code run in fp32 on the GPU (ATen ker
 the same oracle on the CPU - two correct fp32 evaluations of the reference that differ only in summation
 order.  A tensor may exceed its bar only if it stays within FLOOR_FACTOR x its own measured floor.
 
-DispResNet6 is the exception, and the reason is measured, not assumed (profiles/r02_parity_notes.md,
-r02_diag_grads_cfg1.txt, r02_diag_convs_cfg1.txt): its gradient is chaotic - 13 BatchNorms, the deepest over
+DispResNet6 is the exception: its gradient is chaotic - 13 BatchNorms, the deepest over
 56 values, and ReLU masks on 2x7 .. 8x26 maps amplify a 1e-7 forward difference ~1e4 times, so the two torch
 evaluations already disagree by 7e-4 (median) .. 1e-1 (worst tensor).  The amplification is linear in the
-per-op error: the exact-fp32 CUDA-core kernels (IMPL_FFMA) sit at 0.9 x the floor (median), the production
-tensor-core kernels - every single conv call within 5e-6 (fprop/dgrad) / 5e-5 (wgrad) of the FFMA result on the
-real step data - at 2.8 x.  For this net the per-tensor rule is replaced by: median(err / floor) <= CHAOS_MEDIAN,
+per-op error: the production wgmma tensor-core kernels sit at 4.4 x the floor (median; cfg1 4.44, cfg3 4.43 on an H100 SXM
+at a 400 W power limit).  The step is bit-reproducible on a given GPU and build (fixed-order reductions, fixed-point warp
+scatter), so this ratio does not vary from run to run; it moves only when the kernels' summation order changes, and any
+such change is held to the bar here.  For this net the per-tensor rule is replaced by: median(err / floor) <= CHAOS_MEDIAN,
 relative L2 error of every tensor <= CHAOS_L2, and the counts are reported.  Values (losses, disparities) keep
 the strict 1e-4 bar.
 
-The per-tensor table is written to gpurun_out/parity_fullsize_<cfg>.json and summarised on stdout; the
-committed copy lives under profiles/."""
+The per-tensor table is summarised on stdout and, when $CCB_PARITY_REPORT_DIR is set, written there as
+parity_fullsize_<cfg>.json."""
 import json
 import os
 import time
@@ -35,14 +35,13 @@ from oracle import step as OS
 
 OUT_TOL, LOSS_TOL, GRAD_TOL = 1e-4, 1e-4, 1e-3
 FLOOR_FACTOR = 3.0
-GRAD_TOL_HARD = 3e-3               # no gradient tensor of Pose / Mask / Flow may exceed this, whatever its floor says (measured max 1.7e-3)
-BETWEEN_FRAC = 0.05                # share of a net's tensors allowed between the bar and the cap (measured: Flow 4-5 of 192 = 2.6 %)
+GRAD_TOL_HARD = 3e-3               # no gradient tensor of Pose / Mask / Flow may exceed this, whatever its floor says (H100: max 7.8e-4)
+BETWEEN_FRAC = 0.05                # share of a net's tensors allowed between the bar and the cap (H100: none)
 CHAOTIC_NETS = ('disp',)           # see the module docstring
 CHAOS_MEDIAN, CHAOS_L2 = 5.0, 5e-2
 # Pose / Mask / Flow gradients: bar 1e-3 (or 3 x floor); at most 5 % of a net's tensors may sit between the bar and the hard
-# cap (measured at b4 256x832 over six runs: Flow 4-5 of 192 at 1.0-1.7e-3, Pose 0, Mask 0; the margins absorb run-to-run
-# differences of the atomics in the feature-warp backward)
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# cap.  Measured at b4 256x832 on an H100 SXM (400 W power limit), cfg3: every Pose / Mask / Flow tensor under the bar (max
+# 1.6e-5 / 2.7e-4 / 7.8e-4); the cap and the 5 % leave room for other GPUs and compilers, whose summation orders differ
 
 
 def _flatten_aux(aux):
@@ -162,11 +161,12 @@ def run(cfg, device, B=4, H=256, W=832, seed=50, with_floor=True, threads=None, 
                                    ratio_median=ratio[len(rs) // 2], ratio_p90=ratio[int(0.9 * len(rs))], l2_max=max(r['l2'] for r in rs))
     if report:
         summarise(rep)
-        out = os.path.join(ROOT, 'gpurun_out')
-        os.makedirs(out, exist_ok=True)
-        tag = cfg if (B, H, W) == (4, 256, 832) else '%s_b%d_%dx%d' % (cfg, B, H, W)
-        with open(os.path.join(out, 'parity_fullsize_%s.json' % tag), 'w') as f:
-            json.dump(rep, f, indent=1)
+        out = os.environ.get('CCB_PARITY_REPORT_DIR')
+        if out:
+            os.makedirs(out, exist_ok=True)
+            tag = cfg if (B, H, W) == (4, 256, 832) else '%s_b%d_%dx%d' % (cfg, B, H, W)
+            with open(os.path.join(out, 'parity_fullsize_%s.json' % tag), 'w') as f:
+                json.dump(rep, f, indent=1)
     assert not bad, '%d tensors miss the parity bar:\n  ' % len(bad) + '\n  '.join(bad[:40])
     return rep
 

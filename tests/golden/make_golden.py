@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (/root/reference,
-anuragranj/cc @ 2b4e362) on CPU fp32 in the build container.
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (anuragranj/cc @ 2b4e362: a checkout
+named `reference` beside this repository, or the one $CC_REFERENCE names) on CPU fp32.
 
-The reference is Python and cannot travel to the GPU box, so its outputs (and autograd
-gradients) on seeded synthetic inputs are frozen here.  Run:  python tests/golden/make_golden.py
+The tests must not depend on the reference being present, so its outputs (and autograd gradients) on
+seeded synthetic inputs are frozen here.  Run:  python tests/golden/make_golden.py
+Fixtures are kept under 1 MB per file: a larger set is written as <name>.part<i>.npz (tests/util.golden merges them).
 Stubs (reference cannot import/run without them, SURVEY.md F11):
   * spatial_correlation_sampler -> oracle.nets.spatial_correlation_sample (third-party op absent
     from the tree; that boundary stays "parity unpinned")
@@ -17,7 +18,7 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-REF = os.environ.get('CC_REFERENCE', '/root/reference')
+REF = os.environ.get('CC_REFERENCE') or os.path.join(os.path.dirname(ROOT), 'reference')
 sys.path.insert(0, ROOT)
 sys.path.insert(0, REF)
 warnings.filterwarnings('ignore')
@@ -46,10 +47,40 @@ def npy(t):
     return t.detach().cpu().numpy()
 
 
+MAX_FILE = 900 * 1024
+
+
+def save_parts(out_dir, name, arrays, max_file=MAX_FILE):
+    """arrays -> <name>.npz, or <name>.part0.npz, .part1.npz ... each below max_file bytes (compressed size estimated
+    per array, then checked)."""
+    import io
+    for f in os.listdir(out_dir):
+        if f == name + '.npz' or (f.startswith(name + '.part') and f.endswith('.npz')):
+            os.remove(os.path.join(out_dir, f))
+    def csize(k, v):
+        b = io.BytesIO()
+        np.savez_compressed(b, **{k: v})
+        return b.tell()
+    groups, cur, cur_bytes = [], {}, 0
+    for k, v in arrays.items():
+        s = csize(k, v)
+        if cur and cur_bytes + s > max_file:
+            groups.append(cur)
+            cur, cur_bytes = {}, 0
+        cur[k] = v
+        cur_bytes += s
+    groups.append(cur)
+    paths = [os.path.join(out_dir, name + '.npz')] if len(groups) == 1 else \
+        [os.path.join(out_dir, '%s.part%d.npz' % (name, i)) for i in range(len(groups))]
+    for p, g in zip(paths, groups):
+        np.savez_compressed(p, **g)
+        assert os.path.getsize(p) <= max_file + 4096, p
+    return paths
+
+
 def save(name, d):
-    path = os.path.join(OUT, name + '.npz')
-    np.savez_compressed(path, **{k: (npy(v) if torch.is_tensor(v) else np.asarray(v)) for k, v in d.items()})
-    print(name, '%.1f KB' % (os.path.getsize(path) / 1024), len(d), 'arrays')
+    paths = save_parts(OUT, name, {k: (npy(v) if torch.is_tensor(v) else np.asarray(v)) for k, v in d.items()})
+    print(name, '%.1f KB' % (sum(os.path.getsize(p) for p in paths) / 1024), len(d), 'arrays in', len(paths), 'file(s)')
 
 
 def compact(g, limit=40000, stride=61):

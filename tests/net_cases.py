@@ -68,7 +68,7 @@ def case_conv_shapes(device, big=False):
 
 
 def case_conv_tc(device):
-    """tcgen05 path against torch fp64 on real layer shapes: fprop, dgrad (incl. strided parity classes /
+    """wgmma tensor-core path against torch fp64 on real layer shapes: fprop, dgrad (incl. strided parity classes /
     ConvTranspose forward) and wgrad.  IMPL_TC = 3xTF32 (fp32 parity), IMPL_TC_TF32 = single TF32 (what cuDNN
     runs by default for the reference).  GPU only (the simulator has no tensor cores)."""
     from cc_b200 import _lib
@@ -120,26 +120,16 @@ def case_conv_tc(device):
         cnn.CONV_IMPL = saved
 
 
-def case_conv_tma_family(device):
-    """The TMA-fed kernels at sizes that reach every dispatch branch (conv_tma.cu): the CUDA-core direct kernel (thin
-    layers, needs >= 148 K output pixels), stacked slab tiles with a ragged bottom, stride-2 slabs, narrow maps through
-    padded rows, aligned 1x1.  Checked against torch fp64 AND against the register-gather kernels (debug flag 8 turns
-    the whole family off): two independent implementations of the same convolution.  GPU only."""
+def _conv_cross_check(device, shapes, seed, name):
+    """Every shape through both convolution families - the wgmma tensor-core kernels (IMPL_TC, 3xTF32) and the CUDA-core
+    FFMA kernels - each against torch fp64 and against each other: two independent implementations of the same
+    convolution, forward with a fused bias + LeakyReLU epilogue and with a linear one, data / weight / bias gradients."""
     from cc_b200 import _lib
-    g = torch.Generator().manual_seed(11)
-    shapes = [(6, 13, 100, 260, 20, 3, 1, 1),     # direct kernel: fprop + dgrad, ragged channels / rows / columns
-              (4, 15, 256, 832, 16, 7, 2, 3),     # direct kernel, stride 2 (PoseNet conv1)
-              (4, 16, 252, 832, 1, 3, 1, 1),      # direct kernel, one output channel (disparity head)
-              (4, 32, 126, 416, 32, 3, 1, 1),     # slab dgrad with stacked tiles and a ragged bottom; gather fprop
-              (2, 160, 12, 36, 72, 3, 1, 1),      # slab: several channel blocks, column tail
-              (2, 24, 9, 22, 40, 3, 1, 1),        # narrow unaligned map: padded rows (fprop, dgrad, wgrad)
-              (2, 40, 16, 64, 136, 1, 1, 0)]      # aligned 1x1: per-tap TMA boxes, N > 128
+    g = torch.Generator().manual_seed(seed)
     saved = cnn.CONV_IMPL
-    lib = _lib.lib()
     try:
-        cnn.CONV_IMPL = _lib.IMPL_TC
         for (B, Ci, H, W, Co, k, s, p) in shapes:
-            tag = f'tma family {Ci}->{Co} k{k} s{s} {H}x{W}'
+            tag = f'{name} {Ci}->{Co} k{k} s{s} {H}x{W}'
             x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
             w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
             b = torch.randn(Co, generator=g).to(device).requires_grad_(True)
@@ -148,67 +138,45 @@ def case_conv_tma_family(device):
             wt = _wts(zd.shape, 9, device)
             gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
             outs = {}
-            for flag in (0, 8):
-                lib.ccb_debug_tc_swap_strides(flag)
+            for impl in (_lib.IMPL_TC, _lib.IMPL_FFMA):
+                cnn.CONV_IMPL = impl
+                assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(zd, 0.2), 1e-4, f'{tag} impl {impl} fprop+leaky')
                 y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
                 gx, gw, gb = torch.autograd.grad((y * wt).sum(), [x, w, b])
-                outs[flag] = (y.detach(), gx, gw, gb)
-                for got, ref, what in zip(outs[flag], (zd,) + tuple(gd), ('fprop', 'dgrad', 'wgrad', 'bias grad')):
-                    assert_close(got, ref, 1e-4, f'{tag} flag {flag} {what}')
-            for a_, b_, what in zip(outs[0], outs[8], ('fprop', 'dgrad', 'wgrad', 'bias grad')):
-                assert_close(a_, b_, 1e-4, f'{tag} TMA family vs gather kernels {what}')
+                outs[impl] = (y.detach(), gx, gw, gb)
+                for got, ref, what in zip(outs[impl], (zd,) + tuple(gd), ('fprop', 'dgrad', 'wgrad', 'bias grad')):
+                    assert_close(got, ref, 1e-4, f'{tag} impl {impl} {what}')
+            for a_, b_, what in zip(outs[_lib.IMPL_TC], outs[_lib.IMPL_FFMA], ('fprop', 'dgrad', 'wgrad', 'bias grad')):
+                assert_close(a_, b_, 1e-4, f'{tag} tensor-core vs CUDA-core kernels {what}')
     finally:
-        lib.ccb_debug_tc_swap_strides(0)
         cnn.CONV_IMPL = saved
+
+
+def case_conv_tma_family(device):
+    """(Named after the removed TMA-fed Blackwell kernels whose dispatch branches these shapes reached.)  Thin and odd layer
+    geometries: ragged channels / rows / columns, stride-2 thin input (PoseNet conv1), one output
+    channel (disparity head), ragged tile bottoms, several 32-channel K blocks with column tails, narrow maps whose width is
+    not a multiple of 4 (weight gradient through padded rows), 1x1 with N > 128.  GPU only."""
+    _conv_cross_check(device, [(6, 13, 100, 260, 20, 3, 1, 1),
+                               (4, 15, 256, 832, 16, 7, 2, 3),
+                               (4, 16, 252, 832, 1, 3, 1, 1),
+                               (4, 32, 126, 416, 32, 3, 1, 1),
+                               (2, 160, 12, 36, 72, 3, 1, 1),
+                               (2, 24, 9, 22, 40, 3, 1, 1),
+                               (2, 40, 16, 64, 136, 1, 1, 0)], 11, 'thin/odd')
 
 
 def case_conv_nhwc(device):
-    """The channels-last slab kernel (conv_nhwc.cu: NCHW -> NHWC copy, one TMA slab per 32-channel block, filter taps as
-    descriptor offsets into the slab): FPROP, DGRAD (stride 1 and the 4 parity classes of stride 2 / ConvTranspose2d),
-    channel tails (C % 32 != 0), N tails, ragged tile rows / columns, 7x7 and 5x5 halos, split-K over channel blocks.
-    Checked against torch fp64 AND against the NCHW kernels (ccb_debug_nhwc(0, ..) turns the path off).  GPU only."""
-    from cc_b200 import _lib
-    g = torch.Generator().manual_seed(13)
-    shapes = [(2, 64, 32, 40, 64, 3, 1, 1),       # the ResBlock shape: 2 channel blocks
-              (2, 32, 48, 72, 32, 7, 1, 3),       # 7x7 halo (DispResNet6 conv1b), one channel block, N = 32
-              (2, 196, 20, 44, 128, 3, 1, 1),     # Back2Future decoder: channel tail 196 = 6 x 32 + 4, ragged rows / columns
-              (2, 100, 33, 23, 72, 5, 1, 2),      # 5x5, N tail (72), odd sizes
-              (1, 512, 16, 24, 200, 3, 1, 1),     # few tiles, long K: split-K over channel blocks, 2 N tiles
-              (2, 64, 48, 64, 48, 3, 2, 1),       # stride 2: DGRAD parity classes through the kernel (fprop stays NCHW)
-              (2, 96, 40, 56, 64, 4, 2, 1)]       # MaskNet6 deconv geometry (k4 s2 p1) as the conv whose dgrad it is
-    saved = cnn.CONV_IMPL
-    lib = _lib.lib()
-    try:
-        cnn.CONV_IMPL = _lib.IMPL_TC
-        for (B, Ci, H, W, Co, k, s, p) in shapes:
-            tag = f'nhwc {Ci}->{Co} k{k} s{s} {H}x{W}'
-            x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
-            w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
-            b = torch.randn(Co, generator=g).to(device).requires_grad_(True)
-            xd, wd, bd = [t.detach().double().requires_grad_(True) for t in (x, w, b)]
-            zd = F.conv2d(xd, wd, bd, s, p)
-            wt = _wts(zd.shape, 9, device)
-            gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
-            outs = {}
-            for on in (1, 0):
-                lib.ccb_debug_nhwc(on, 0, 0)
-                # fused epilogue (bias + LeakyReLU) in the forward; gradients with a linear epilogue (see case_conv_tc)
-                assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(zd, 0.2), 1e-4, f'{tag} nhwc={on} fprop+leaky')
-                y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
-                gx, gw, gb = torch.autograd.grad((y * wt).sum(), [x, w, b])
-                outs[on] = (y.detach(), gx, gw, gb)
-                for got, ref, what in zip(outs[on], (zd,) + tuple(gd), ('fprop', 'dgrad', 'wgrad', 'bias grad')):
-                    assert_close(got, ref, 1e-4, f'{tag} nhwc={on} {what}')
-            for a_, b_, what in zip(outs[1], outs[0], ('fprop', 'dgrad', 'wgrad', 'bias grad')):
-                assert_close(a_, b_, 1e-4, f'{tag} channels-last vs NCHW kernels {what}')
-            if s == 1:      # the channels-last weight-gradient kernel (MN-major operands; selectable, off by default)
-                lib.ccb_debug_nhwc(1, 0, 128)
-                y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
-                gw, = torch.autograd.grad((y * wt).sum(), [w])
-                assert_close(gw, gd[1], 1e-4, f'{tag} channels-last wgrad kernel')
-    finally:
-        lib.ccb_debug_nhwc(1, 0, 0)
-        cnn.CONV_IMPL = saved
+    """(Named after the removed channels-last Blackwell slab kernel these shapes exercised.)  The layer geometries of the four networks' heavy convolutions: the ResBlock shape, a 7x7 halo (DispResNet6 conv1b),
+    channel tails (196 = 6 x 32 + 4), 5x5 with an N tail, few tiles with a long K (split-K, 2 N tiles), stride-2 DGRAD
+    parity classes, the MaskNet6 deconv geometry (k4 s2 p1).  GPU only."""
+    _conv_cross_check(device, [(2, 64, 32, 40, 64, 3, 1, 1),
+                               (2, 32, 48, 72, 32, 7, 1, 3),
+                               (2, 196, 20, 44, 128, 3, 1, 1),
+                               (2, 100, 33, 23, 72, 5, 1, 2),
+                               (1, 512, 16, 24, 200, 3, 1, 1),
+                               (2, 64, 48, 64, 48, 3, 2, 1),
+                               (2, 96, 40, 56, 64, 4, 2, 1)], 13, 'network')
 
 
 ALT_NETS = [  # mirrors tests/golden/make_golden.py:ALT_NETS (name, kwargs, input size, frozen gradients)
@@ -240,7 +208,7 @@ def case_alt_nets(device, names=None, grads=True):
     reference's own modules (tests/golden/alt_nets_small.npz): weights come from synth.seeded_fill on both sides (state_dict
     key names and shapes must therefore agree), train-mode outputs at 1e-4, a sample of parameter gradients, eval output.
     Gradient bars: 2e-3 for the plain nets; the two residual nets carry BatchNorm over 2-16 values at this toy input size
-    (DispResNetS6's conv7 sees a 1x2 map) and are held to 1e-1 (DESIGN.md section 2: chaotic conditioning, measured on
+    (DispResNetS6's conv7 sees a 1x2 map) and are held to 1e-1 (chaotic conditioning, see tests/fullsize_cases.py; measured on
     DispResNet6; the exact-fp32 simulator run already shows 6e-2 against torch on one tensor)."""
     g = golden('alt_nets_small')
     for k, (name, kw, (B, H, W), pn) in enumerate(ALT_NETS):

@@ -1,6 +1,6 @@
 """Build tests/sim/libccb200_sim.so: the product kernel sources compiled by g++ against the CPU
 execution-model simulator (cusim.h).  TEST TOOL ONLY - lets the GPU-less container check kernel
-indexing / reductions against the oracle.  tcgen05 / TMA kernels are excluded (CCB_CPU_SIM)."""
+indexing / reductions against the oracle.  The wgmma tensor-core kernels are excluded (CCB_CPU_SIM)."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, 'cc_b200', 'csrc')
 OUT = os.path.join(HERE, 'libccb200_sim.so')
-SIM_SOURCES = ['common.cu', 'photo.cu', 'warp_ops.cu', 'smooth_bce.cu', 'conv_ffma.cu', 'conv_tc.cu', 'conv_tma.cu', 'conv_nhwc.cu', 'wprep.cu', 'misc_ops.cu', 'b2f_ops.cu', 'io_ops.cu']
+SIM_SOURCES = ['common.cu', 'photo.cu', 'warp_ops.cu', 'smooth_bce.cu', 'conv_ffma.cu', 'conv_tc.cu', 'wprep.cu', 'misc_ops.cu', 'b2f_ops.cu', 'io_ops.cu']
 
 
 def build(force=False):

@@ -1,6 +1,6 @@
 // cusim.h - a tiny single-threaded CUDA *execution-model* simulator for CPU-side unit tests.
 //
-// TEST TOOL ONLY.  The product library (libccb200.so) is compiled by nvcc for sm_100a and never
+// TEST TOOL ONLY.  The product library (libccb200.so) is compiled by nvcc for sm_90a and never
 // includes this file.  tests/sim/build_sim.py compiles the very same kernel sources with
 // g++ -DCCB_CPU_SIM so that the kernels' indexing / tiling / reduction logic can be checked against
 // the oracle in the GPU-less build container before GPU minutes are spent.
@@ -177,6 +177,11 @@ static inline int __float2int_rd(float f) { return (int)floorf(f); }
 static inline float atomicAdd(float* p, float v) { float o = *p; *p = o + v; return o; }
 static inline int atomicAdd(int* p, int v) { int o = *p; *p = o + v; return o; }
 static inline unsigned atomicAdd(unsigned* p, unsigned v) { unsigned o = *p; *p = o + v; return o; }
+static inline unsigned long long atomicAdd(unsigned long long* p, unsigned long long v) { unsigned long long o = *p; *p = o + v; return o; }
+static inline unsigned long long atomicMax(unsigned long long* p, unsigned long long v) { unsigned long long o = *p; if (v > o) *p = v; return o; }
+static inline long long __double2ll_rn(double x) { return llrint(x); }
+using std::isfinite;
+static inline int __clzll(long long x) { return x == 0 ? 64 : __builtin_clzll((unsigned long long)x); }
 static inline unsigned atomicInc(unsigned* p, unsigned lim) { unsigned o = *p; *p = (o >= lim) ? 0 : o + 1; return o; }
 static inline int min(int a, int b) { return a < b ? a : b; }
 static inline int max(int a, int b) { return a > b ? a : b; }

@@ -1,4 +1,4 @@
-"""-m gpu: the production path (IMPL_AUTO: tcgen05 / TMA conv kernels + fused loss kernels) at the BASELINE.json
+"""-m gpu: the production path (IMPL_AUTO: wgmma conv kernels + fused loss kernels) at the BASELINE.json
 configurations (b4, 256x832, 6 levels) against the CPU oracle, per tensor; and against the step fixture frozen
 from the reference's real train() body.  See tests/fullsize_cases.py for the bars."""
 import pytest
@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 def cuda_lib():
     from cc_b200 import _lib, pyramid, nn as cnn
     _lib._lib = None
-    assert not _lib.is_simulator(), 'GPU tests must run on the sm_100a library'
+    assert not _lib.is_simulator(), 'GPU tests must run on the sm_90a library'
     assert cnn.CONV_IMPL == _lib.IMPL_AUTO, 'full-size parity is defined on the production dispatch'
     pyramid.clear()
     torch.backends.cudnn.allow_tf32 = False       # the noise-floor run (oracle on the GPU) must be fp32

@@ -1,5 +1,5 @@
 """Parity tests proper: the CUDA path (through cc_b200.* and the C ABI of libccb200.so) against the
-oracle and the golden fixtures, on the B200."""
+oracle and the golden fixtures, on the H100."""
 import pytest
 import torch
 from tests import kernel_cases as KC
@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 def cuda_lib():
     from cc_b200 import _lib, pyramid
     _lib._lib = None                      # make sure the real library (not a simulator) is bound
-    assert not _lib.is_simulator(), 'GPU tests must run on the sm_100a library'
+    assert not _lib.is_simulator(), 'GPU tests must run on the sm_90a library'
     pyramid.clear()
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -29,6 +29,37 @@ def test_full_size_rigid_loss_vs_cpu_oracle():
     KC.case_rigid_loss_oracle(torch.device('cuda:0'), B=4, H=256, W=832, NL=6, seed=5, robust=True,
                               oracle_device=torch.device('cpu'))
     KC.case_occlusion_and_valid_masks(torch.device('cuda:0'), B=4, H=256, W=832, NL=6, seed=5)
+
+
+def test_warp_image_gradient_is_reproducible():
+    """The image gradient of flow_warp / Back2Future's feature warp is a scatter; flows that pull many pixels onto a
+    few source pixels make float atomics order-dependent.  Two runs must agree bit for bit (values: the parity cases),
+    on both kernels (a warp per pixel for small many-channel maps, a thread per pixel otherwise); an inf in grad_out
+    reaches only the source pixels it is scattered to."""
+    from cc_b200 import inverse_warp as CW, nn as cnn
+    dev = torch.device('cuda:0')
+    g = torch.Generator().manual_seed(21)
+    for (B, C, H, W) in ((2, 64, 48, 160), (2, 3, 128, 416)):
+        img = torch.randn(B, C, H, W, generator=g).to(dev)
+        ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float32), torch.arange(W, dtype=torch.float32), indexing='ij')
+        # every pixel is pulled to within ~1.5 px of one of a few centres: thousands of contributions per source pixel
+        flow = torch.stack([(xs // 40) * 40 + 20 - xs, (ys // 24) * 24 + 12 - ys])[None].repeat(B, 1, 1, 1)
+        flow = (flow + 1.5 * torch.rand(B, 2, H, W, generator=g)).to(dev)
+        gout = torch.randn(B, C, H, W, generator=g).to(dev)
+        for warp in (lambda x: CW.flow_warp(x, flow), lambda x: cnn.feat_warp(x, flow)):
+            grads = []
+            for _ in range(2):
+                x = img.clone().requires_grad_(True)
+                (warp(x) * gout).sum().backward()
+                grads.append(x.grad)
+            assert torch.equal(grads[0], grads[1]), (B, C, H, W)
+            assert bool(torch.isfinite(grads[0]).all())
+            ginf = gout.clone()
+            ginf[0, 0, H // 2, W // 2] = float('inf')
+            x = img.clone().requires_grad_(True)
+            (warp(x) * ginf).sum().backward()
+            bad = ~torch.isfinite(x.grad)
+            assert 1 <= int(bad.sum()) <= 4 and bool(bad[0, 0].any()), int(bad.sum())
 
 
 def test_full_size_properties():
@@ -94,6 +125,8 @@ def test_conv_tensor_core_path():
 
 
 def test_conv_tma_family():
+    """Named after the TMA-fed kernel family it was written for; those Blackwell kernels are gone, and the same thin / odd
+    shapes now cross-check the wgmma kernels against the CUDA-core kernels and fp64 torch (net_cases.case_conv_tma_family)."""
     NC.case_conv_tma_family(torch.device('cuda:0'))
 
 
@@ -103,6 +136,8 @@ def test_alternate_nets():
 
 
 def test_conv_nhwc_slab():
+    """Named after the channels-last slab kernel it was written for; that Blackwell kernel is gone, and the same network
+    layer shapes now cross-check the wgmma kernels against the CUDA-core kernels and fp64 torch (net_cases.case_conv_nhwc)."""
     NC.case_conv_nhwc(torch.device('cuda:0'))
 
 

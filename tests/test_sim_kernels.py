@@ -1,6 +1,6 @@
 """The product kernel sources, compiled by g++ against the CPU execution-model simulator
 (tests/sim), checked against the oracle and the golden fixtures - so that indexing / reduction /
-derivation bugs are caught in the GPU-less container.  The same cases run on the real B200 in
+derivation bugs are caught in the GPU-less container.  The same cases run on the real H100 in
 tests/test_gpu_parity.py."""
 import os
 import sys

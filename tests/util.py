@@ -8,9 +8,17 @@ _cache = {}
 
 
 def golden(name):
+    """The arrays of tests/golden/<name>.npz, or merged from <name>.part<i>.npz when the set is split (files < 1 MB)."""
     if name not in _cache:
-        with np.load(os.path.join(GOLDEN, name + '.npz')) as z:
-            _cache[name] = {k: z[k] for k in z.files}
+        whole = os.path.join(GOLDEN, name + '.npz')
+        parts = [whole] if os.path.exists(whole) else \
+            sorted(os.path.join(GOLDEN, f) for f in os.listdir(GOLDEN) if f.startswith(name + '.part') and f.endswith('.npz'))
+        assert parts, 'golden fixture %s is missing' % name
+        d = {}
+        for p in parts:
+            with np.load(p) as z:
+                d.update({k: z[k] for k in z.files})
+        _cache[name] = d
     return _cache[name]
 
 
@@ -50,8 +58,8 @@ def pick(g, stride):
 def assert_close_robust(a, b, tol=1e-4, max_outlier_frac=2e-4, what=''):
     """Full-size variant: the gradient of a bilinear sample is discontinuous where a coordinate lands on
     an integer pixel, so 1-ulp coordinate differences flip a handful of pixels' gradients - the oracle
-    run on CPU and on GPU disagree with EACH OTHER at ~1e-4 of the level-0 pixels (gpurun diag_masks
-    log, profiles/r01_parity_notes.md).  Require <= tol everywhere except a vanishing fraction."""
+    run on CPU and on GPU disagree with EACH OTHER at ~1e-4 of the level-0 pixels (tools/diag_masks.py
+    log).  Require <= tol everywhere except a vanishing fraction."""
     a = torch.as_tensor(a, dtype=torch.float64).cpu()
     b = torch.as_tensor(b, dtype=torch.float64).cpu()
     assert a.shape == b.shape, (a.shape, b.shape)
