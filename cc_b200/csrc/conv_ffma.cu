@@ -404,12 +404,22 @@ static int pick_splits(int tiles, int ktiles, int max_splits) {
     return s < 1 ? 1 : s;
 }
 
+// Split-K partials a call may use: room for 64 splits, capped at 64 MiB.  The split count is planned from this, never
+// from a larger buffer the caller happens to pass, so that a call sums in the same order whatever ran before it.
+static long long ffma_work_floats(long long out_numel) {
+    const long long cap = 16ll * 1024 * 1024;
+    long long want = out_numel * 64;
+    if (want > cap) want = (cap / out_numel) * out_numel;
+    return want < out_numel ? 0 : want;
+}
+
 template <int MODE>
 static int launch_gemm(ConvArgs& a, long long out_numel, long long work_floats, cudaStream_t st, const char* what) {
     const bool narrow = a.N <= 16;
     const int BM = narrow ? 128 : 64, BN = narrow ? 16 : 64;
     const int mt = cdiv(a.M, BM), nt = cdiv(a.N, BN), ktiles = cdiv(a.K, 16);
-    int max_splits = (a.work && out_numel > 0) ? (int)(work_floats / out_numel) : 1;
+    const long long plan_floats = work_floats < ffma_work_floats(out_numel) ? work_floats : ffma_work_floats(out_numel);
+    int max_splits = (a.work && out_numel > 0) ? (int)(plan_floats / out_numel) : 1;
     if (max_splits > 64) max_splits = 64;
     a.splits = pick_splits(mt * nt, ktiles, max_splits);
     // make sure no split is empty
@@ -528,11 +538,7 @@ extern "C" long long ccb_conv_workspace_floats(const ccb_conv_desc* d, int op) {
     long long numel = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Co * d->Ho * d->Wo
                     : (op == CCB_CONV_DGRAD) ? (long long)d->B * d->Ci * d->Hi * d->Wi
                                              : (long long)d->Co * d->Ci * d->kh * d->kw;
-    // enough for up to 16 splits, capped at 64 MiB of floats
-    long long cap = 16ll * 1024 * 1024;
-    long long want = numel * 16;
-    if (want > cap) want = (cap / numel) * numel;
-    if (want < numel) want = 0;
+    const long long want = ffma_work_floats(numel);
     return want > bias_need ? want : bias_need;
 }
 

@@ -179,6 +179,131 @@ def case_conv_nhwc(device):
                                (2, 96, 40, 56, 64, 4, 2, 1)], 13, 'network')
 
 
+# Layers whose prepared weights cover the paths of the weight cache's one-launch preparation (wprep_all_kernel):
+# kind, B, Cin, H, W (input), Cout, k, stride, pad, output_padding.  nb = output channels staged per block (wprep_nb).
+WCACHE_LAYERS = [
+    ('conv', 1, 512, 8, 8, 512, 3, 1, 1, 0),     # 18 KB per channel row: nb = 3 (54 KB of dynamic shared memory), 512 = 3 x 170 + 2
+    ('conv', 2, 32, 12, 16, 275, 3, 1, 1, 0),    # N = 275: nb = 2 with a one-channel last block, three wgmma N tiles
+    ('conv', 2, 64, 8, 12, 136, 1, 1, 0, 0),     # 1x1, N > 128
+    ('conv', 2, 32, 16, 24, 32, 7, 1, 3, 0),     # 7x7: 49 taps
+    ('conv', 2, 64, 16, 24, 128, 3, 2, 1, 0),    # stride 2: the data gradient runs 4 parity classes of 1, 2, 2, 4 taps
+    ('conv', 2, 64, 16, 24, 128, 1, 2, 0, 0),    # 1x1 stride 2: one class with a tap, three without (one shared layout)
+    ('convT', 2, 96, 8, 12, 32, 4, 2, 1, 0),     # MaskNet6 deconvolution k4 s2 p1: 4 classes of 4 taps
+    ('convT', 2, 64, 8, 12, 32, 3, 2, 1, 1),     # k3 s2 p1 output_padding 1: classes of 1, 2, 2, 4 taps
+]
+# fprop layout + one per data-gradient parity class (each requested once per forward + backward); the three tap-less
+# classes of the 1x1 stride-2 layer share one layout
+WCACHE_REQUESTS = 2 + 2 + 2 + 2 + 5 + 5 + 5 + 5
+WCACHE_LAYOUTS = WCACHE_REQUESTS - 2
+
+
+def case_conv_weight_cache(device):
+    """Convolutions reading their prepared (tf32 hi / lo) weights from a committed cnn.WeightCache - one table of 26
+    layouts re-prepared by ONE launch of wprep_all_kernel - against the same calls preparing their weights per call
+    (wprep_staged_kernel), and against fp64 torch.  Both kernels compute the same cvt.rna split, so outputs and
+    gradients must be bit-identical: after commit(), and after an in-place weight update followed by refresh().  The
+    cache statistics prove the cached path ran: every layout hit, none missed.  GPU only (tensor-core path)."""
+    from cc_b200 import _lib
+    g = torch.Generator().manual_seed(17)
+    layers = []
+    for (kind, B, Ci, H, W, Co, k, s, p, op) in WCACHE_LAYERS:
+        wshape = (Co, Ci, k, k) if kind == 'conv' else (Ci, Co, k, k)
+        x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
+        w = (torch.randn(wshape, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
+        b = torch.randn(Co, generator=g).to(device).requires_grad_(True)
+        layers.append((kind, s, p, op, x, w, b))
+
+    def fwd(kind, s, p, op, x, w, b, f64=False):
+        if kind == 'conv':
+            return F.conv2d(x, w, b, s, p) if f64 else cnn.conv2d(x, w, b, None, s, p, None)
+        return F.conv_transpose2d(x, w, b, s, p, op) if f64 else cnn.conv_transpose2d(x, w, b, s, p, op, None)
+
+    def run(handle):
+        """Forward + all gradients of every layer, with cnn.WCACHE = handle."""
+        out = []
+        cnn.WCACHE = handle
+        try:
+            for i, (kind, s, p, op, x, w, b) in enumerate(layers):
+                y = fwd(kind, s, p, op, x, w, b)
+                out.append((y.detach(),) + torch.autograd.grad((y * _wts(y.shape, 30 + i, device)).sum(), [x, w, b]))
+        finally:
+            cnn.WCACHE = None
+        return out
+
+    def check(got, ref, what):
+        for i, (a, r) in enumerate(zip(got, ref)):
+            tag = f'{what}: {WCACHE_LAYERS[i]}'
+            xd, wd, bd = [t.detach().double().requires_grad_(True) for t in layers[i][4:]]
+            zd = fwd(*layers[i][:4], xd, wd, bd, f64=True)
+            gd = torch.autograd.grad((zd * _wts(zd.shape, 30 + i, device).double()).sum(), [xd, wd, bd])
+            for a_, r_, d_, nm in zip(a, r, (zd,) + tuple(gd), ('output', 'dx', 'dw', 'db')):
+                assert torch.equal(a_, r_), f'{tag} {nm}: cached weights differ from per-call preparation by ' \
+                                            f'{(a_ - r_).abs().max().item():.3e}'
+                assert_close(a_, d_, 1e-4, f'{tag} {nm} vs fp64')
+
+    saved = cnn.CONV_IMPL
+    try:
+        cnn.CONV_IMPL = _lib.IMPL_TC
+        cache = cnn.WeightCache(device)
+        ref = run(None)
+        rec = run(cache.h)                      # recording: layouts noted, weights still prepared per call
+        st = cache.stats()
+        assert st == dict(layouts=WCACHE_LAYOUTS, hits=0, misses=0, committed=False), st
+        for a, r in zip(rec, ref):
+            assert all(torch.equal(a_, r_) for a_, r_ in zip(a, r)), 'recording changed a result'
+        cache.commit()                          # allocates the cache and prepares every layout in one launch
+        check(run(cache.h), ref, 'committed')
+        st = cache.stats()
+        assert st == dict(layouts=WCACHE_LAYOUTS, hits=WCACHE_REQUESTS, misses=0, committed=True), st
+        with torch.no_grad():                   # an optimiser step: weights change in place, then one refresh
+            for i, (_, _, _, _, _, w, _) in enumerate(layers):
+                w.add_(_wts(w.shape, 60 + i, device) * (0.1 * w.abs().max()))
+        cache.refresh()
+        check(run(cache.h), run(None), 'refreshed')
+        st = cache.stats()
+        assert st == dict(layouts=WCACHE_LAYOUTS, hits=2 * WCACHE_REQUESTS, misses=0, committed=True), st
+    finally:
+        cnn.CONV_IMPL = saved
+        cnn.WCACHE = None
+
+
+def case_conv_plan_ignores_workspace(device):
+    """A convolution's split-K plan is a function of its shape alone: the same call given the workspace it asks for
+    (ccb_conv_workspace_floats) and given a much larger one - as the grow-only workspace in cc_b200.nn is once a bigger
+    layer has run - sums in the same order, so the results are bit-identical.  Small maps under long reductions, where
+    both convolution families split K: fprop / stride-1 dgrad with 4 output pixels and 2304-deep K, wgrad over 2048
+    pixels into a 16 x 144 weight."""
+    import ctypes as C
+    from cc_b200 import _lib
+    lib = _lib.lib()
+    g = torch.Generator().manual_seed(23)
+    impls = (_lib.IMPL_FFMA,) if _lib.is_simulator() else (_lib.IMPL_FFMA, _lib.IMPL_TC, _lib.IMPL_AUTO)
+    for (B, Ci, H, W, Co, k, s, p) in ((2, 256, 1, 2, 256, 3, 1, 1), (2, 16, 32, 32, 16, 3, 1, 1)):
+        Ho, Wo = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
+        x = torch.randn(B, Ci, H, W, generator=g).to(device)
+        w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device)
+        dy = torch.randn(B, Co, Ho, Wo, generator=g).to(device)
+        for impl in impls:
+            d = _lib.ConvDesc()
+            d.B, d.Ci, d.Hi, d.Wi, d.Co, d.Ho, d.Wo = B, Ci, H, W, Co, Ho, Wo
+            d.kh = d.kw = k
+            d.stride, d.pad, d.act, d.slope, d.impl, d.wcache = s, p, _lib.ACT_NONE, 0.0, impl, None
+            for op, ins, out in ((_lib.CONV_FPROP, (x, w, None, None), dy), (_lib.CONV_DGRAD, (dy, w, None, None), x),
+                                 (_lib.CONV_WGRAD, (x, dy), w)):
+                fn = (lib.ccb_conv2d_fprop, lib.ccb_conv2d_dgrad, lib.ccb_conv2d_wgrad)[op]
+                need = lib.ccb_conv_workspace_floats(C.byref(d), op)
+                res = []
+                for wf in (need, 8 * need + 4096):
+                    work = torch.full((max(wf, 1),), float('nan'), device=device)
+                    y = torch.empty_like(out)
+                    args = [_lib.ptr(t) for t in ins] + [y.data_ptr()] + ([None] if op == _lib.CONV_WGRAD else [])
+                    _lib.check(fn(C.byref(d), *args, work.data_ptr() if wf else None, wf, _lib.stream(x)), 'conv op %d' % op)
+                    res.append(y)
+                tag = f'impl {impl} op {op} {Ci}->{Co} {H}x{W}: workspace of {need} vs {8 * need + 4096} floats'
+                assert bool(torch.isfinite(res[0]).all()), tag
+                assert torch.equal(res[0], res[1]), f'{tag} changes the result by {(res[0] - res[1]).abs().max().item():.3e}'
+
+
 ALT_NETS = [  # mirrors tests/golden/make_golden.py:ALT_NETS (name, kwargs, input size, frozen gradients)
     ('DispNetS', {}, (2, 64, 128), ['conv1.0.weight', 'conv7.2.bias', 'upconv4.0.weight', 'iconv3.0.weight', 'predict_disp4.0.weight']),
     ('DispNetS6', {}, (2, 64, 128), ['conv1.2.weight', 'conv5.0.bias', 'upconv7.0.weight', 'iconv1.0.weight', 'predict_disp6.0.bias']),
@@ -406,4 +531,5 @@ def smoke_case(device):
     case_conv_shapes(device)
 
 
-NET_CASES = [case_conv_shapes, case_bn_upsample, case_disp_pose_golden, case_mask_golden, case_flow_golden, case_alt_pose_nets]
+NET_CASES = [case_conv_shapes, case_bn_upsample, case_disp_pose_golden, case_mask_golden, case_flow_golden, case_alt_pose_nets,
+             case_conv_plan_ignores_workspace]

@@ -1,11 +1,108 @@
 """Step-level parity: cc_b200.train_step.Trainer (nets + fused losses + flat Adam) vs the oracle's
 train_step (reference train.py:445-568 restated) on identical seeded inputs / weights."""
+import math
 import torch
-from tests.util import assert_close
-from cc_b200 import synth, nn as cnn
+from tests.util import assert_close, rel_err
+from cc_b200 import synth, nn as cnn, pyramid, _lib
 from cc_b200.optim import FlatAdam
 from cc_b200.train_step import Trainer, HP
 from oracle import step as OS, nets as ON
+
+U32 = 2.0 ** -24           # fp32 unit roundoff
+TINY32 = 1e-44             # a few fp32 subnormal steps: the absolute error of a product that underflows
+
+
+def f32(x):
+    """A Python float rounded to fp32: FlatAdam hands lr, betas and eps to its kernel as fp32 arguments."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def adam_reference(p, m, v, g, t, lr, betas, eps, grad_scale=1.0):
+    """One torch.optim.Adam step (weight decay 0, step count t after the step) in fp64 from the fp32 state before it
+    (oracle/step.Adam's update), and per-element bounds on what an fp32 evaluation of that step may differ by.
+    Returns ((p, m, v), (bound_p, bound_m, bound_v)), all fp64.  Pass lr / betas / eps as the kernel receives them (f32).
+
+    The bounds are error analysis of one fp32 step, u = 2^-24, |.| elementwise, g' = grad_scale * g:
+      m:  4u (b1 |m| + (1 - b1) |g'|)              - relative to the summands, not to m: m cancels when g changes sign
+      v:  6u v                                     - every term is non-negative
+      p:  2u |p| + 8u |upd| + |upd| dd / denom + (lr / bc1) bound_m / denom
+          fl(p - upd) rounds once (2u |p|: about an ulp of p); the update itself takes ~6 roundings, including the fp32
+          bias corrections kept in the optimiser state (8u |upd|); the error allowed in m and in v (dd: the change of
+          denom when v moves by bound_v) passes into the update through m / denom.
+    TINY32 is added to every bound, for squares and products of gradients that underflow fp32."""
+    p, m, v, g = (x.double() for x in (p, m, v, g))
+    b1, b2 = betas
+    g = g * grad_scale
+    m1 = b1 * m + (1 - b1) * g
+    v1 = b2 * v + (1 - b2) * g * g
+    bc1, bc2s = 1 - b1 ** t, math.sqrt(1 - b2 ** t)
+    denom = v1.sqrt() / bc2s + eps
+    upd = (lr / bc1) * m1 / denom
+    p1 = p - upd
+    bm = 4 * U32 * (b1 * m.abs() + (1 - b1) * g.abs()) + TINY32
+    bv = 6 * U32 * v1 + TINY32
+    dd = ((v1 + bv).sqrt() - v1.sqrt()) / bc2s
+    bp = 2 * U32 * p1.abs() + 8 * U32 * upd.abs() + upd.abs() * dd / denom + (lr / bc1) * bm / denom + TINY32
+    return (p1, m1, v1), (bp, bm, bv)
+
+
+def assert_adam_step(before, after, g, t, lr, betas, eps, grad_scale, what):
+    """`after` = (flat_p, exp_avg, exp_avg_sq, state) of a FlatAdam right after its t-th step from `before` (the same
+    fp32 buffers, state excluded) with gradient g: every element within adam_reference's bound, state[:3] = the step
+    count and the bias corrections 1 - b1^t, sqrt(1 - b2^t) of step t."""
+    lr, betas, eps = f32(lr), (f32(betas[0]), f32(betas[1])), f32(eps)
+    n, chunk = g.numel(), 1 << 23               # fp64 temporaries of a full-size model, a slice at a time
+    for c0 in range(0, n, chunk):
+        sl = slice(c0, min(n, c0 + chunk))
+        ref, bound = adam_reference(before[0][sl], before[1][sl], before[2][sl], g[sl], t, lr, betas, eps, grad_scale)
+        for got, r, b, nm in zip(after[:3], ref, bound, ('flat_p', 'exp_avg', 'exp_avg_sq')):
+            got = got[sl]
+            err = (got.double() - r).abs()
+            bad = err > b
+            if bool(bad.any()):
+                i = int((err / b).argmax())
+                raise AssertionError(f'{what}: {nm}: {int(bad.sum())} of {err.numel()} elements from {c0} outside the fp32 '
+                                     f'bound; worst [{c0 + i}] {got[i].item():.9g} vs fp64 {r[i].item():.9g} (bound {b[i].item():.3g})')
+    st = after[3].double().cpu()
+    want = torch.tensor([float(t), 1 - betas[0] ** t, math.sqrt(1 - betas[1] ** t)], dtype=torch.float64)
+    assert st[0].item() == t and bool(((st[1:3] - want[1:]).abs() <= 2 * U32 * want[1:]).all()), \
+        f'{what}: optimiser state {st[:3].tolist()}, want {want.tolist()}'
+
+
+def case_adam_fp64(device, steps=5):
+    """FlatAdam (ccb_adam_step) over three parameters for 5 steps against the fp64 reference, element by element, on
+    synthetic gradients: exact zeros (every step, or every other step), values near eps (1e-9 .. 1e-7), large values
+    (1e4), ordinary ones, with random signs that change from step to step, and one step with grad_scale = 0.5.
+    Parameters span 1 .. 1e-4 with exact zeros, so the updates are not hidden under the parameters' ulp.  Each step
+    starts from the optimiser's own previous buffers; the bounds are adam_reference's."""
+    gen = torch.Generator().manual_seed(5)
+    shapes = [(16, 3, 3, 3), (257,), (1000,)]
+    params = []
+    for s in shapes:
+        p0 = torch.randn(s, generator=gen) * 10.0 ** (-4 * torch.rand(s, generator=gen))
+        p0.view(-1)[::7] = 0.0
+        params.append(torch.nn.Parameter(p0.to(device)))
+    opt = FlatAdam(params, lr=1e-3)
+    n = opt.numel
+    cls = torch.arange(n) % 5
+    mag = torch.where(cls == 1, 10.0 ** (-9 + 2 * torch.rand(n, generator=gen)),        # near eps
+                      torch.where(cls == 2, 1e4 * (0.5 + torch.rand(n, generator=gen)),  # large
+                                  torch.randn(n, generator=gen).abs() * 1e-2))           # ordinary
+    mag[cls == 0] = 0.0                                                                   # zero at every step
+    for t in range(1, steps + 1):
+        sign = torch.where(torch.rand(n, generator=gen) < 0.5, -1.0, 1.0)
+        g = mag * sign
+        if t % 2 == 1:
+            g[cls == 4] = 0.0                                                             # zero every other step
+        gs = 0.5 if t == 3 else 1.0
+        before = (opt.flat_p.clone(), opt.exp_avg.clone(), opt.exp_avg_sq.clone())
+        opt.flat_g.copy_(g.to(device))
+        opt.grad_scale = gs
+        opt.step()
+        after = (opt.flat_p.clone(), opt.exp_avg.clone(), opt.exp_avg_sq.clone(), opt.state.clone())
+        assert_adam_step(before, after, g.to(device), t, opt.lr, opt.betas, opt.eps, gs, f'FlatAdam step {t}')
+        assert torch.equal(after[0][cls.to(device) == 0], before[0][cls.to(device) == 0]), 'a parameter without gradient moved'
+    opt.grad_scale = 1.0
 
 
 def case_flat_adam(device):
@@ -90,4 +187,106 @@ def case_step_cfg3(device, B=2, H=64, W=128):
         assert_close(gc, go, 5e-2, f'cfg3 grad norm {net}')
 
 
-STEP_CASES_SIM = [case_flat_adam]
+def _record(tr, loss=None):
+    """Device copies of everything one training step changes: loss, flat gradient / parameter / Adam buffers, optimiser
+    state, every BatchNorm buffer (running statistics and batch counters)."""
+    o = tr.opt
+    rec = dict(flat_g=o.flat_g.clone(), flat_p=o.flat_p.clone(), exp_avg=o.exp_avg.clone(), exp_avg_sq=o.exp_avg_sq.clone(),
+               state=o.state.clone())
+    rec.update(('%s.%s' % (n, k), b.clone()) for n, net in tr.nets.items() for k, b in net.named_buffers())
+    if loss is not None:
+        rec['loss'] = loss.detach().clone()
+    return rec
+
+
+def _assert_same(got, want, what, skip=()):
+    for k in want:
+        if k in skip:
+            continue
+        a, b = got[k], want[k]
+        if not torch.equal(a, b):
+            d = (a.double() - b.double()).abs()
+            raise AssertionError(f'{what}: {k} differs in {int((a != b).sum())} of {a.numel()} elements (max {d.max().item():.3e})')
+
+
+def case_step_graph_vs_eager(device, cfg, B=2, H=64, W=128, loss_tol=None, seed=70):
+    """The step the benchmark times - Trainer.capture() + replay(): a CUDA graph whose convolutions read a committed
+    weight cache and whose Adam keeps its step count on the device - against Trainer.step() run eagerly, over three
+    steps on three different seeded batches, both trainers built from the same oracle weights.
+
+      * replay i equals eager step i BIT FOR BIT: loss, flat gradient / parameters / Adam moments, optimiser state,
+        BatchNorm buffers.  (Eager step 0 prepares weights per call while recording the cache; every later step and
+        every replay reads what wprep_all_kernel prepared.  Different batches: the replay reads the static inputs.)
+      * capture() runs real warm-up steps; afterwards parameters, moments, state and BatchNorm buffers equal the
+        snapshot taken before it, bit for bit (the flat gradient still holds warm-up gradients; the graph zeroes it).
+        capture() restores the snapshot after the warm-up and again after capturing, which executes nothing, so this
+        fails only when neither restore runs.
+      * each replay's parameters / moments / state against the fp64 Adam reference (adam_reference) applied to that
+        replay's own gradient, from the state recorded before it.
+      * loss_tol: eager losses against oracle.step.train_step run on the CPU for the same three steps.
+      * replay() refuses a graph whose learning rate is stale.
+    The trainers run one after the other (full size: one set of activations at a time)."""
+    batches = []
+    for i in range(3):
+        tgt, refs = synth.frames(B, H, W, seed=seed + i)
+        batches.append([tgt] + refs + list(synth.intrinsics(B, H, W)))
+    P = OS.make_params(cfg)
+    sd = _oracle_params_as_state_dicts(P)
+    saved = (cnn.GRAPH_LIVE, cnn.CONV_IMPL)
+    tr = None
+    try:
+        cnn.CONV_IMPL = _lib.IMPL_AUTO
+        tr = Trainer(cfg, device, state_dicts=sd)
+        eager = []
+        for b in batches:
+            d = [t.to(device) for t in b]
+            loss, _ = tr.step(d[0], d[1:5], d[5], d[6])
+            eager.append(_record(tr, loss))
+        del tr, loss, d
+        tr = None
+        torch.cuda.empty_cache()
+
+        tr = Trainer(cfg, device, state_dicts=sd)
+        static = [t.to(device) for t in batches[0]]
+        snap = _record(tr)
+        tr.capture(static[0], static[1:5], static[5], static[6])
+        _assert_same(_record(tr), snap, f'{cfg}: state after capture()', skip=('flat_g',))
+        prev = snap
+        o = tr.opt
+        for i, b in enumerate(batches):
+            for s, h in zip(static, b):
+                s.copy_(h)
+            cur = _record(tr, tr.replay())
+            _assert_same(cur, eager[i], f'{cfg}: replay {i} vs eager step {i}')
+            assert_adam_step((prev['flat_p'], prev['exp_avg'], prev['exp_avg_sq']),
+                             (cur['flat_p'], cur['exp_avg'], cur['exp_avg_sq'], cur['state']), cur['flat_g'], i + 1,
+                             o.lr, o.betas, o.eps, o.grad_scale, f'{cfg}: Adam of replay {i}')
+            prev = cur
+        lr = o.lr
+        o.lr = lr * 0.5
+        try:
+            tr.replay()
+            raise RuntimeError('replay() ran a graph captured with another learning rate')
+        except AssertionError:
+            pass
+        finally:
+            o.lr = lr
+    finally:
+        if tr is not None:
+            tr.graph = None
+        tr = None
+        torch.cuda.synchronize()
+        cnn.GRAPH_LIVE, cnn.CONV_IMPL = saved
+        pyramid.clear()
+    if loss_tol is not None:
+        oopt = OS.Adam(OS.all_params(P), HP['lr'], HP['beta1'], HP['beta2'])
+        errs = []
+        for i, b in enumerate(batches):
+            lo, _ = OS.train_step(cfg, P, oopt, b[0], b[1:5], b[5], b[6])
+            errs.append(rel_err(eager[i]['loss'], lo))
+        assert max(errs) <= loss_tol, f'{cfg} {B}x{H}x{W}: relative loss errors of steps 0-2 vs the oracle ' \
+                                      f'{["%.2e" % e for e in errs]}, bar {loss_tol:.0e}'
+        print(f'{cfg} {B}x{H}x{W}: loss vs oracle {["%.2e" % e for e in errs]}')
+
+
+STEP_CASES_SIM = [case_flat_adam, case_adam_fp64]
