@@ -22,6 +22,12 @@ such change is held to the bar here.  For this net the per-tensor rule is replac
 relative L2 error of every tensor <= CHAOS_L2, and the counts are reported.  Values (losses, disparities) keep
 the strict 1e-4 bar.
 
+Per-layer correctness at this size, DispResNet6's layers included, is established by the layer audit (audit_step below,
+tests/layer_audit.py): every convolution, BatchNorm, upsample, cost-volume and feature-warp call of the timed cfg3 step is
+checked against fp64 element by element, on its real inputs, within a derived per-element bound.  A per-op error of a
+few per cent confined to one layer, which the chaos bar could not see, fails there.  The chaos bar stays as the
+end-to-end check of the step against the oracle.
+
 The per-tensor table is summarised on stdout and, when $CCB_PARITY_REPORT_DIR is set, written there as
 parity_fullsize_<cfg>.json."""
 import json
@@ -29,7 +35,7 @@ import os
 import time
 import torch
 from tests.util import rel_err
-from cc_b200 import synth
+from cc_b200 import synth, nn as cnn
 from cc_b200.train_step import Trainer
 from oracle import step as OS
 
@@ -184,6 +190,61 @@ def summarise(rep):
         print('   %-5s %-44s err %.2e  floor %s  bar %.0e %s' % (r['kind'], r['name'], r['err'],
                                                                  'n/a     ' if r['floor'] is None else '%.2e' % r['floor'], r['bar'],
                                                                  '' if r['ok'] else 'FAIL'))
+
+
+def audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
+    """The layer audit (tests/layer_audit.py) of the step the benchmark times: Trainer(cfg) from the oracle's weights, one
+    eager step (it records the weight-cache layouts, which then commit), then the SECOND eager step - committed cache,
+    production IMPL_AUTO dispatch - with every layer call checked against fp64 element by element.
+      * completeness: every Conv2d / ConvTranspose2d / BatchNorm2d module of the nets is audited forward and backward
+        (the occlusion decoders do not run in training, see build_nets), and Back2Future's ten cost volumes and eight
+        feature warps;
+      * non-interference: the audited step's loss and flat gradient equal, bit for bit, an unaudited second step from
+        the same snapshot;
+      * coverage: the coarsest cost volume (C = 192 on a 4x13 map: one tile per sample) runs corr_chunks = 32 channel
+        chunks, and the BatchNorm of DispResNet6's iconv1 shortcut reduces its 851968 values per channel in 104 splits.
+    Returns the audit summary."""
+    from tests import layer_audit as LA
+    tgt, refs = synth.frames(B, H, W, seed=seed)
+    K, Kinv = synth.intrinsics(B, H, W)
+    P = OS.make_params(cfg)
+    sd = {n: {k: v.detach().clone() for k, v in d.items()} for n, d in P.items()}
+    tr = Trainer(cfg, device, state_dicts=sd)
+    args = (tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device))
+    tr.step(*args)
+    assert tr.wcache is not None and tr.wcache.committed
+    snap = tr._snapshot()
+    loss_ref = tr.step(*args)[0].clone()
+    grad_ref = tr.opt.flat_g.clone()
+    tr._restore(snap)
+    torch.cuda.synchronize(device)
+    t0 = time.perf_counter()
+    audit = LA.LayerAudit(nets=tr.nets, tag='%s_b%d_%dx%d' % (cfg, B, H, W))
+    with audit:
+        loss = tr.step(*args)[0]
+    torch.cuda.synchronize(device)
+    print('   audited step: %.1f s (fp64 references included)' % (time.perf_counter() - t0))
+    assert torch.equal(loss, loss_ref), (loss.item(), loss_ref.item())
+    assert torch.equal(tr.opt.flat_g, grad_ref), 'the audit changed the flat gradient by %.3e' % (tr.opt.flat_g - grad_ref).abs().max().item()
+    st = tr.wcache.stats()
+    assert st['misses'] == 0 and st['hits'] > 0, st
+
+    rows = audit.rows
+    want = {'%s.%s' % (n, k) for n, net in tr.nets.items() for k, m in net.named_modules()
+            if isinstance(m, (cnn.Conv2d, cnn.ConvTranspose2d, cnn.BatchNorm2d)) and not k.startswith('decoder_occ')}
+    for phase in ('fwd', 'bwd'):
+        got = {r['name'] for r in rows if r['phase'] == phase and r['op'] in ('conv', 'convT', 'bn')}
+        assert got == want, (phase, sorted(want - got)[:10], sorted(got - want)[:10])
+    for op, n in (('corr81', 10), ('featwarp', 8)):
+        for phase in ('fwd', 'bwd'):
+            k = sum(r['op'] == op and r['phase'] == phase and r['name'].startswith('flow') for r in rows)
+            assert k == n, (op, phase, k)
+    h6, w6 = H // 64, W // 64
+    assert LA.corr_chunks(B, 192, h6, w6) == 32
+    assert {r['phase'] for r in rows if r['op'] == 'corr81' and r['shape'] == [B, 192, h6, w6] and r['chunks'] == 32} == {'fwd', 'bwd'}
+    assert LA.bn_splits(B, H * W) == 104
+    assert {r['phase'] for r in rows if r['op'] == 'bn' and r['name'] == 'disp.iconv1.0.downsample.1' and r['splits'] == 104} == {'fwd', 'bwd'}
+    return audit.summary()
 
 
 def _golden_rows(g, losses3, grads3, losses1, grads1):
