@@ -247,6 +247,54 @@ def audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
     return audit.summary()
 
 
+def loss_audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
+    """The loss audit (tests/loss_audit.py) of the step the benchmark times, set up as audit_step: one eager step, then
+    the second step with the weight cache committed, every loss-layer call checked against fp64 element by element.
+      * completeness: one rigid and one flow photometric call (forward and backward), four smoothness and two BCE calls
+        (forward and backward), one consensus-target call, twelve pose2flow forwards; every level has partial tiles;
+      * non-interference: the audited step's loss and flat gradient equal, bit for bit, an unaudited second step;
+      * detectability: one dropped level-0 tile would put d_pose over its bound (the audit's tile_drop_r).
+    Returns the audit summary."""
+    from tests import loss_audit as LSA
+    tgt, refs = synth.frames(B, H, W, seed=seed)
+    K, Kinv = synth.intrinsics(B, H, W)
+    P = OS.make_params(cfg)
+    sd = {n: {k: v.detach().clone() for k, v in d.items()} for n, d in P.items()}
+    tr = Trainer(cfg, device, state_dicts=sd)
+    args = (tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device))
+    tr.step(*args)
+    assert tr.wcache is not None and tr.wcache.committed
+    snap = tr._snapshot()
+    loss_ref = tr.step(*args)[0].clone()
+    grad_ref = tr.opt.flat_g.clone()
+    tr._restore(snap)
+    torch.cuda.synchronize(device)
+    t0 = time.perf_counter()
+    audit = LSA.LossAudit(tag='%s_b%d_%dx%d' % (cfg, B, H, W))
+    with audit:
+        loss = tr.step(*args)[0]
+    torch.cuda.synchronize(device)
+    print('   audited step: %.1f s (fp64 references included)' % (time.perf_counter() - t0))
+    assert torch.equal(loss, loss_ref), (loss.item(), loss_ref.item())
+    assert torch.equal(tr.opt.flat_g, grad_ref), 'the audit changed the flat gradient by %.3e' % (tr.opt.flat_g - grad_ref).abs().max().item()
+    n = {}
+    for r in audit.rows:
+        n[(r['op'], r['phase'])] = n.get((r['op'], r['phase']), 0) + 1
+    want = {('photo_rigid', 'fwd'): 1, ('photo_rigid', 'bwd'): 1, ('photo_flow', 'fwd'): 1, ('photo_flow', 'bwd'): 1,
+            ('smooth', 'fwd'): 4, ('smooth', 'bwd'): 4, ('bce', 'fwd'): 2, ('bce', 'bwd'): 2, ('consensus', 'fwd'): 1,
+            ('pose2flow', 'fwd'): 12}
+    assert {k: v for k, v in n.items() if k[0] != 'pyramid'} == want, n
+    assert n.get(('pyramid', 'fwd'), 0) > 0
+    for r in audit.rows:
+        if r['op'].startswith('photo') and r['phase'] == 'fwd':
+            assert len(r['partial_tiles']) == 6 and all(r['partial_tiles']), r['partial_tiles']
+    summ = audit.summary()
+    # one dropped 64x20 tile of level 0, at the real proportion of a tile to ~2.1e5 pixels per (b, ref), is detected
+    assert summ['photo_rigid']['tile_drop_r'] > LSA.R_OUT[('photo_rigid', 'd_pose')], summ['photo_rigid']['tile_drop_r']
+    print('   audited calls: %d' % len(audit.rows))
+    return summ
+
+
 def _golden_rows(g, losses3, grads3, losses1, grads1):
     """rows (name, err, bar) of one implementation against tests/golden/step_small.npz.
     grads*: {net: {param name: grad}}."""

@@ -479,8 +479,9 @@ def measure(got, ref, s, tie=None):
     return rmax, rel, int(tie.sum()) if tie is not None else 0
 
 
-def evaluate(op, checks):
-    """checks of one call -> {what: (r, rel, ties)}, worst r, and the list of failures against R[op] / REL_BAR."""
+def evaluate(op, checks, R=R):
+    """checks of one call -> {what: (r, rel, ties)}, worst r, and the list of failures against R[op] / REL_BAR (R: the
+    bound table of the audit the call belongs to)."""
     res, bad = {}, []
     for what, got, ref, s, tie in checks:
         assert got.shape == ref.shape, (op, what, tuple(got.shape), tuple(ref.shape))

@@ -30,6 +30,11 @@ def test_layer_audit_cfg3_second_step():
     FC.audit_step(torch.device('cuda:0'))
 
 
+def test_loss_audit_cfg3_second_step():
+    """Every loss-layer call of the timed step (cfg3 b4 256x832, committed weight cache) against fp64, element by element."""
+    FC.loss_audit_step(torch.device('cuda:0'))
+
+
 def test_step_vs_reference_fixture():
     """step_small.npz (reference train.py:454-509 on the reference modules) vs the CUDA step, per-parameter gradients."""
     rows = FC.golden_step_small(torch.device('cuda:0'))

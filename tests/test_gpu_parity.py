@@ -203,3 +203,17 @@ from tests import eval_cases as EC   # noqa: E402
 def test_eval_case(case):
     """Evaluation cores (SURVEY N3: test_disp / test_pose / test_flow sample loops) against the oracle restatement."""
     case(torch.device('cuda:0'))
+
+
+from tests import loss_audit as LSA   # noqa: E402
+
+
+@pytest.mark.parametrize('opts', [{}] + LSA.SWEEP, ids=lambda o: '-'.join('%s=%s' % kv for kv in o.items()) or 'cfg3')
+def test_loss_audit_options(opts):
+    """The loss audit on the sm_90a build: the cfg3 loss layer at b2 64x128 and the template paths the step never takes
+    (SSIM compiled out, powf, the oob term, border padding, quaternion poses, no masks, an 84x136 frame with 3 levels)."""
+    o = dict(opts)
+    kw = {k: o.pop(k) for k in ('H', 'W', 'NL') if k in o}
+    with LSA.LossAudit(tag='gpu_' + ('_'.join(map(str, opts.values())) or 'cfg3')):
+        LSA.cfg3_losses(torch.device('cuda:0'), opts=o, **kw)
+    torch.cuda.synchronize()
