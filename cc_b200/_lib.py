@@ -119,6 +119,8 @@ _SIGS = {
     'ccb_corr81_fwd_workspace_floats': (_LL, [_I, _I, _I, _I]),
     'ccb_corr81_fwd': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _LL, _P]),
     'ccb_corr81_bwd': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    'ccb_corr441d_fwd': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    'ccb_corr441d_bwd': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'ccb_featwarp_fwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
     'ccb_featwarp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     'ccb_bn_workspace_floats': (_LL, [_I, _I, _I]),

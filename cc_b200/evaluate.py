@@ -12,7 +12,7 @@ reference - they are a few hundred flops per sample."""
 import numpy as np
 import torch
 from .inverse_warp import pose2flow, pose_vec2mat
-from . import loss_functions as LF
+from . import loss_functions as LF, models
 
 
 def _to_net_input(img_hwc, device):
@@ -103,7 +103,8 @@ def flow_sample_errors(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kin
     depth = 1 / disp
     pose = pose_net(tgt, refs)
     emask = mask_net(tgt, refs)
-    flow_fwd = flow_net(tgt, refs[1:3])[0]
+    # test_flow.py:122-125: Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
+    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
     flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
     rigidity = (1 - (1 - emask[:, 1]) * (1 - emask[:, 2])).unsqueeze(1) > 0.5
     soft = (flow_cam - flow_fwd).abs()

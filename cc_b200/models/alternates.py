@@ -9,8 +9,7 @@ state_dict keys as the reference, so its checkpoints load; ReLU / sigmoid / resi
   PoseExpNet    models/PoseExpNet.py:18-94     SfMLearner's pose + explainability net (4 mask scales)
   MaskResNet6   models/MaskResNet6.py:67-160   residual encoder + MaskNet6's decoder
 
-Not built: FlowNetC6 (models/FlowNetC6.py) - its 21x21 dilated correlation (kernel 1, patch 21, dilation_patch 2) is a
-different operator from Back2Future's 9x9 cost volume and no configuration of BASELINE.json uses it."""
+The alternate flow net, FlowNetC6 (--flownet, train.py:90), has its own module: FlowNetC6.py."""
 import torch
 import torch.nn as nn
 from .. import nn as cnn

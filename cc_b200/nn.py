@@ -412,6 +412,33 @@ class _Corr81Fn(torch.autograd.Function):
         return d1, d2, None
 
 
+class _Corr441dFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, f1, f2):
+        f1, f2 = _c(f1), _c(f2)
+        if f1.shape != f2.shape or f1.dim() != 4:
+            raise ValueError('cc_b200: corr441d needs two [B,C,h,w] maps of one shape, got %s and %s'
+                             % (tuple(f1.shape), tuple(f2.shape)))
+        B, Cc, h, w = f1.shape
+        out = torch.empty(B, 441, h, w, device=f1.device, dtype=torch.float32)
+        _lib.check(_lib.lib().ccb_corr441d_fwd(_lib.ptr(f1), _lib.ptr(f2), _lib.ptr(out), B, Cc, h, w, _lib.stream(f1)),
+                   'corr441d_fwd')
+        ctx.save_for_backward(f1, f2, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        f1, f2, out = ctx.saved_tensors
+        B, Cc, h, w = f1.shape
+        g = _c(g)
+        d1 = torch.empty_like(f1) if ctx.needs_input_grad[0] else None
+        d2 = torch.empty_like(f2) if ctx.needs_input_grad[1] else None
+        if d1 is not None or d2 is not None:
+            _lib.check(_lib.lib().ccb_corr441d_bwd(_lib.ptr(f1), _lib.ptr(f2), _lib.ptr(out), _lib.ptr(g), _lib.ptr(d1),
+                                                   _lib.ptr(d2), B, Cc, h, w, _lib.stream(f1)), 'corr441d_bwd')
+        return d1, d2
+
+
 class _FeatWarpFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, flo):
@@ -439,6 +466,11 @@ class _FeatWarpFn(torch.autograd.Function):
 def corr81(f1, f2, reversed_=False):
     """correlate(f1, f2).index_select(1, idx_fwd | idx_bwd) of back2future.py:15-25,173-176."""
     return _Corr81Fn.apply(f1, f2, reversed_)
+
+
+def corr441d(f1, f2):
+    """LeakyReLU(0.1)(correlate(f1, f2)) of FlowNetC6.py:18-30,111-112: the 21x21 cost volume at dilation 2, [B,441,h,w]."""
+    return _Corr441dFn.apply(f1, f2)
 
 
 def feat_warp(x, flo):

@@ -5,6 +5,8 @@
   cfg2  Back2Future flow + flow photometric/SSIM + smoothness
   cfg3  full joint step (Disp + Pose + Mask + Flow, all five losses)
 
+The flow net is Back2Future unless `flownet='FlowNetC6'` is chosen, as the reference's --flownet (train.py:90,252-255).
+
 Hyper-parameters default to the README command line (README.md:59-65; train.py:120-130)."""
 import torch
 from . import models, loss_functions as LF, dist as cdist
@@ -14,10 +16,13 @@ from .optim import FlatAdam
 HP = dict(w1=1.0, w2=0.1, w3=0.1, w4=0.5, w5=0.3, wssim=0.997, qch=0.5, lambda_oob=0.0,
           THRESH=0.01, wbce=0.5, wrig=1.0, lr=1e-4, beta1=0.9, beta2=0.999, smoothness='edgeaware')
 NETS_OF = {'cfg1': ('disp', 'pose'), 'cfg2': ('flow',), 'cfg3': ('disp', 'pose', 'mask', 'flow')}
+FLOWNETS = ('Back2Future', 'FlowNetC6')          # the choices of --flownet, train.py:90
 
 
-def build_nets(cfg, device, state_dicts=None, seed=0):
+def build_nets(cfg, device, state_dicts=None, seed=0, flownet='Back2Future'):
     """Instantiate the nets of a configuration (reference constructor arguments, train.py:245-255)."""
+    if flownet not in FLOWNETS:
+        raise ValueError('flownet must be one of %s, got %r' % (FLOWNETS, flownet))
     torch.manual_seed(seed)
     nets = {}
     for name in NETS_OF[cfg]:
@@ -27,6 +32,8 @@ def build_nets(cfg, device, state_dicts=None, seed=0):
             net = models.PoseNetB6(nb_ref_imgs=4)
         elif name == 'mask':
             net = models.MaskNet6(nb_ref_imgs=4, output_exp=True)
+        elif flownet == 'FlowNetC6':
+            net = models.FlowNetC6(nlevels=6)
         else:
             # the five occlusion decoders are dead work in training: train.py:463 discards `occ` and they get no
             # gradient (SURVEY.md F9); their parameters stay in the module (checkpoint contract) and in the optimiser
@@ -44,6 +51,15 @@ def _smooth(hp, tgt, preds):
     return LF.smooth_loss(preds)
 
 
+def flow_pair(flow_net, tgt, refs):
+    """(flow_fwd, flow_bwd) of the training step, train.py:462-466: Back2Future sees both neighbours in one call,
+    another flow net is called once per direction (the target tower is recomputed in each call, as in the reference)."""
+    if isinstance(flow_net, models.Back2Future):
+        ff, fb, _ = flow_net(tgt, refs[1:3])
+        return ff, fb
+    return flow_net(tgt, refs[2]), flow_net(tgt, refs[1])
+
+
 def loss_cfg1(nets, tgt, refs, K, Kinv, hp=HP):
     disp = nets['disp'](tgt)
     depth = [1 / d for d in disp]
@@ -55,7 +71,7 @@ def loss_cfg1(nets, tgt, refs, K, Kinv, hp=HP):
 
 
 def loss_cfg2(nets, tgt, refs, K, Kinv, hp=HP):
-    ff, fb, _ = nets['flow'](tgt, refs[1:3])
+    ff, fb = flow_pair(nets['flow'], tgt, refs)
     l4 = LF.photometric_flow_loss(tgt, refs[1:3], [fb, ff], [None] * len(ff),
                                   lambda_oob=hp['lambda_oob'], qch=hp['qch'], wssim=hp['wssim'])
     l3 = _smooth(hp, tgt, ff) + _smooth(hp, tgt, fb)
@@ -68,7 +84,7 @@ def loss_cfg3(nets, tgt, refs, K, Kinv, hp=HP):
     depth = [1 / d for d in disp]
     pose = nets['pose'](tgt, refs)
     emask = nets['mask'](tgt, refs)
-    ff, fb, _ = nets['flow'](tgt, refs[1:3])
+    ff, fb = flow_pair(nets['flow'], tgt, refs)
     cam_f = [pose2flow(d.squeeze(1), pose[:, 2], K, Kinv) for d in depth]
     cam_b = [pose2flow(d.squeeze(1), pose[:, 1], K, Kinv) for d in depth]
     tgt_masks = LF.consensus_exp_masks(cam_f, cam_b, ff, fb, tgt, refs[2], refs[1],
@@ -95,9 +111,9 @@ class Trainer:
     """Nets + one flat Adam + (optionally) one NCCL gradient all-reduce; `step()` is
     optimizer.zero_grad(); loss.backward(); optimizer.step() of train.py:566-568."""
 
-    def __init__(self, cfg, device, hp=HP, state_dicts=None, seed=0):
-        self.cfg, self.hp, self.device = cfg, dict(hp), device
-        self.nets = build_nets(cfg, device, state_dicts, seed)
+    def __init__(self, cfg, device, hp=HP, state_dicts=None, seed=0, flownet='Back2Future'):
+        self.cfg, self.hp, self.device, self.flownet = cfg, dict(hp), device, flownet
+        self.nets = build_nets(cfg, device, state_dicts, seed, flownet)
         params = [p for n in NETS_OF[cfg] for p in self.nets[n].parameters()]
         self.opt = FlatAdam(params, lr=hp['lr'], betas=(hp['beta1'], hp['beta2']))
         cdist.broadcast_params(self.opt)

@@ -268,6 +268,15 @@ int ccb_corr81_fwd(const float* f1, const float* f2, float* out, int B, int C, i
 /* work: B*81*h*w floats (the mirrored gradient planes), required when d_f2 != NULL */
 int ccb_corr81_bwd(const float* f1, const float* f2, const float* grad_out, float* d_f1, float* d_f2, int B,
                    int C, int h, int w, int reversed, float* work, ccb_stream_t stream);
+/* FlowNetC6 operator (models/FlowNetC6.py).
+ * corr441d: correlate() :18-30 (third-party spatial_correlation_sample, kernel 1, patch 21, stride 1, padding 0,
+ * dilation_patch 2, divided by C) with corr_activation LeakyReLU(0.1) :54,112 fused:
+ *   out[b, 21 i + j, y, x] = leaky((1/C) sum_c f1[b,c,y,x] f2[b,c,y + 2(i-10), x + 2(j-10)]), zero outside the map.
+ * f1,f2 [B,C,h,w] -> out [B,441,h,w].  Backward takes the forward's `out` (the activation derivative comes from its sign);
+ * d_f1 / d_f2 may be NULL (not both).  No workspace: every element is summed in a fixed order by one thread. */
+int ccb_corr441d_fwd(const float* f1, const float* f2, float* out, int B, int C, int h, int w, ccb_stream_t stream);
+int ccb_corr441d_bwd(const float* f1, const float* f2, const float* out, const float* grad_out, float* d_f1, float* d_f2,
+                     int B, int C, int h, int w, ccb_stream_t stream);
 int ccb_featwarp_fwd(const float* x, const float* flow, int B, int C, int h, int w, float* out,
                      ccb_stream_t stream);
 /* d_flow / d_x may be NULL; the gradient is ADDED to d_x; with d_x, work holds B*C*h*w + 1 64-bit words (as flow_warp_bwd) */

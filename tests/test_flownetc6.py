@@ -1,0 +1,123 @@
+"""FlowNetC6 without a GPU: the oracle restatement against the fixture frozen from the reference module, the mirrored
+module's state_dict contract, and the dilated cost-volume kernels compiled for the CPU simulator (tests/sim) against
+fp64, including planted defects the bound must catch.  The whole network runs on the H100 in
+tests/test_gpu_flownetc6.py (on the simulator it would take far longer than the rest of this suite)."""
+import os
+import sys
+import time
+import pytest
+import torch
+import torch.nn.functional as F
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'sim'))
+
+from cc_b200 import models as CM          # noqa: E402
+from cc_b200.train_step import build_nets  # noqa: E402
+from oracle import nets as ON              # noqa: E402
+from tests import flownetc6_cases as FC, flownetc6_oracle as O6   # noqa: E402
+from tests.util import golden              # noqa: E402
+
+NTOL = 2e-5        # tests/test_oracle_golden.py: module vs functional conv algorithms
+
+
+@pytest.fixture(scope='module')
+def sim_lib():
+    import build_sim
+    from cc_b200 import _lib
+    prev = (_lib._lib, _lib._is_sim)
+    _lib.use_library(build_sim.build())
+    assert _lib.is_simulator()
+    yield
+    _lib._lib, _lib._is_sim = prev
+
+
+def test_oracle_matches_fixture():
+    P = {k: v.detach().clone().requires_grad_(True) for k, v in FC.fixture_weights().items()}
+    assert sum(v.numel() for v in P.values()) == O6.NPARAMS == int(golden(FC.FIXTURE)['nparams'])
+    tgt, ref = FC.fixture_inputs('cpu')
+    outs = O6.flownetc6_forward(P, tgt, ref)
+    loss = sum((x * FC._wts(x.shape, FC.WTS_SEED + i, 'cpu')).sum() for i, x in enumerate(outs))
+    names = FC.grad_names()
+    grads = dict(zip(names, torch.autograd.grad(loss, [P[n] for n in names])))
+    with torch.no_grad():
+        ev = O6.flownetc6_forward(P, tgt, ref, training=False)
+    FC.check_against_fixture(outs, grads, ev, NTOL, NTOL)
+
+
+def test_init_weights_is_the_references():
+    """FlowNetC6.py:84-94: xavier_uniform weights, U[0,1) biases on every conv and transposed conv."""
+    torch.manual_seed(0)
+    net = CM.FlowNetC6()
+    net.init_weights()
+    for k, v in net.state_dict().items():
+        if k.endswith('bias'):
+            assert 0 <= v.min() and 0 < v.max() < 1, k
+        else:
+            bound = (6.0 / ((v.shape[0] + v.shape[1]) * v[0, 0].numel())) ** 0.5
+            assert v.abs().max() <= bound and v.abs().max() > 0.9 * bound, k
+
+
+def test_module_state_dict_matches_reference():
+    net = CM.FlowNetC6()
+    assert {k: tuple(v.shape) for k, v in net.state_dict().items()} == FC.fixture_state_dict_keys()
+    assert list(net.state_dict()) == list(FC.fixture_state_dict_keys())
+    assert sum(p.numel() for p in net.parameters()) == O6.NPARAMS
+    with pytest.raises(NotImplementedError):
+        CM.FlowNetC6(batchNorm=True)
+    with pytest.raises(NotImplementedError):
+        CM.FlowNetC6(full_res=False)
+
+
+def test_build_nets_flownet_choice():
+    nets = build_nets('cfg2', 'cpu', flownet='FlowNetC6')
+    assert isinstance(nets['flow'], CM.FlowNetC6) and nets['flow'].training
+    assert isinstance(build_nets('cfg2', 'cpu')['flow'], CM.Back2Future)
+    with pytest.raises(ValueError):
+        build_nets('cfg2', 'cpu', flownet='SpyNet')
+
+
+def test_correlation_restatement_at_dilation_1_is_back2futures():
+    g = torch.Generator().manual_seed(3)
+    a, b = torch.randn(2, 5, 7, 11, generator=g), torch.randn(2, 5, 7, 11, generator=g)
+    assert torch.equal(O6.spatial_correlation_sample(a, b, 9, 1), ON.spatial_correlation_sample(a, b, 9))
+
+
+def test_corr441d_sim_vs_fp64(sim_lib):
+    t0 = time.time()
+    worst = FC.case_corr441d(torch.device('cpu'))
+    print('corr441d on the simulator: %.1f s; worst r per shape %s' % (time.time() - t0, {
+        s: {k: round(v, 3) for k, v in r.items()} for s, r in worst.items()}))
+
+
+def _flagged_fwd(f1, f2, bad):
+    return FC.corr441d_fwd_ratio(f1, f2, bad) > FC.R_CORR441D
+
+
+def test_corr441d_planted_defects_fail_the_bound(sim_lib):
+    B, C, h, w = 3, 13, 8, 16
+    f1, f2, go = FC._inputs(B, C, h, w, 'cpu', 5)
+    out, d1, d2 = FC.run_corr441d(f1, f2, go)
+    assert FC.corr441d_fwd_ratio(f1, f2, out) <= FC.R_CORR441D
+    j0 = 13
+    # forward: one horizontal displacement skipped by the j loop (its 21 channels never accumulate)
+    bad = out.clone()
+    bad[:, j0::FC.N] = 0
+    assert _flagged_fwd(f1, f2, bad)
+    # forward: the second staged channel group (channels 8..12) missing from every sum
+    part = O6.spatial_correlation_sample(f1[:, :8], f2[:, :8]).reshape(B, FC.N * FC.N, h, w) / C
+    assert _flagged_fwd(f1, f2, F.leaky_relu(part, 0.1))
+    # d f1: the terms of displacement column j0 dropped for every i
+    dz = torch.where(out > 0, go, go * FC.SLOPE32)
+    col = torch.zeros_like(dz)
+    col[:, j0::FC.N] = dz[:, j0::FC.N]
+    miss1, _ = FC.corr441d_adjoint(col, f1, f2)
+    r = FC.corr441d_bwd_ratios(f1, f2, out, go, d1=d1 - miss1 / C)['d_f1']
+    assert r > FC.R_CORR441D, r
+    # d f2: one channel chunk never written (left at zero)
+    bad2 = d2.clone()
+    bad2[:, 8:] = 0
+    r = FC.corr441d_bwd_ratios(f1, f2, out, go, d2=bad2)['d_f2']
+    assert r > FC.R_CORR441D, r
+    # and the correct results pass
+    rs = FC.corr441d_bwd_ratios(f1, f2, out, go, d1=d1, d2=d2)
+    assert max(rs.values()) <= FC.R_CORR441D, rs
