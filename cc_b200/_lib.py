@@ -66,7 +66,7 @@ class ConvDesc(C.Structure):
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SIGMOID = 0, 1, 2, 3
 CONV_FPROP, CONV_DGRAD, CONV_WGRAD = 0, 1, 2
-IMPL_AUTO, IMPL_FFMA, IMPL_TC, IMPL_TC_TF32 = 0, 1, 2, 3
+IMPL_AUTO, IMPL_FFMA, IMPL_TC = 0, 1, 2
 
 _lib = None
 _is_sim = False
@@ -101,12 +101,9 @@ _SIGS = {
     'ccb_conv_workspace_floats': (_LL, [C.POINTER(ConvDesc), _I]),
     'ccb_conv2d_fprop': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _LL, _P]),
     'ccb_conv2d_dgrad': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _LL, _P]),
-    'ccb_conv2d_wgrad': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _LL, _P]),
-    'ccb_act_bwd': (_I, [_P, _P, _P, _LL, _I, _F, _P]),
+    'ccb_conv2d_wgrad': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _LL, _P]),
     'ccb_act_bwd_bias_workspace_floats': (_LL, [_I, _I, _I]),
     'ccb_act_bwd_bias': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, _LL, _P]),
-    'ccb_bias_grad_workspace_floats': (_LL, [_I, _I, _I]),
-    'ccb_bias_grad': (_I, [_P, _P, _I, _I, _I, _P, _LL, _P]),
     'ccb_debug_last_conv_kernel': (C.c_char_p, []),
     'ccb_debug_tc_plan': (_I, [_I, C.POINTER(_I)]),
     'ccb_wcache_create': (C.c_void_p, []),

@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(CD_TX * CD_TY) corr441d_fwd_kernel(const float
 }
 
 // Backward, both inputs with one kernel: d[c](y,x) = (1/C) sum_{i,j} G[i,j](y,x) F[c](y + 2(i-10), x + 2(j-10)), summed
-// over i then j, with dz = g * leaky'(out) (the sign of the stored output, as ccb_act_bwd).
+// over i then j, with dz = g * leaky'(out) (the sign of the stored output, as ccb_act_bwd_bias).
 //   d f1: F = f2, G[i,j](y,x) = dz[21 i + j](y,x).
 //   d f2: F = f1 and the mirrored gradient G[i,j](y,x) = dz[21 (20-i) + (20-j)](y + 2(i-10), x + 2(j-10)) (zero outside the
 //         map), gathered in place: corr(f1,f2)[i,j](y,x) reads f2 at the pixel that corr(f2,f1)[20-i,20-j] maps back to.

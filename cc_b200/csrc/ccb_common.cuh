@@ -55,6 +55,8 @@ namespace ccb {
 // ---- error plumbing (C ABI never throws; reference raises AssertionError in Python instead) ----
 void set_error(const char* fmt, ...);
 int check_launch(const char* what);
+// kernel family of this thread's last convolution call (ccb_debug_last_conv_kernel): set by the dispatcher from its plan
+extern thread_local const char* g_last_conv;
 
 #define CCB_REQUIRE(cond, code, ...)            \
     do {                                        \

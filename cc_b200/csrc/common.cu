@@ -7,7 +7,7 @@ namespace ccb {
 
 static thread_local char g_err[512] = "";
 long long g_launches = 0;
-static thread_local const char* g_last_conv = "";    // main kernel of the last convolution call (bench.py kernel shares)
+thread_local const char* g_last_conv = "";
 
 int pdl_enabled() {
     static int v = -1;
@@ -26,7 +26,6 @@ void set_error(const char* fmt, ...) {
 }
 
 int check_launch(const char* what) {
-    if (strncmp(what, "conv_", 5) == 0 && !strstr(what, "reduce") && !strstr(what, "pad")) g_last_conv = what;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
         set_error("%s: CUDA error: %s", what, cudaGetErrorString(e));

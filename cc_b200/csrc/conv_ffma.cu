@@ -249,63 +249,6 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
     out[i] = apply_act(v, act, slope);
 }
 
-// dz = dy * act'(y)  (in terms of the activation OUTPUT y), optionally accumulating a second grad
-__global__ void __launch_bounds__(256) act_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y,
-                                                      float* __restrict__ dz, long long numel, int act, float slope) {
-    CCB_PDL_WAIT();
-    long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-    if (i >= numel) return;
-    float g = __ldg(dy + i), yv = __ldg(y + i);
-    switch (act) {
-        case CCB_ACT_RELU: g = (yv > 0.f) ? g : 0.f; break;
-        case CCB_ACT_LEAKY: g = (yv > 0.f) ? g : g * slope; break;
-        case CCB_ACT_SIGMOID: g = g * yv * (1.f - yv); break;
-        default: break;
-    }
-    dz[i] = g;
-}
-
-// db[c] = sum_{b,y,x} dy[b,c,y,x] : one CTA per channel, fixed-order two-level sum
-__global__ void __launch_bounds__(256) bias_grad_kernel(const float* __restrict__ dy, float* __restrict__ db, int B,
-                                                        int C, int plane) {
-    CCB_PDL_WAIT();
-    __shared__ float s_red[32];
-    const int c = blockIdx.x;
-    float v[1] = {0.f};
-    for (int b = 0; b < B; ++b) {
-        const float* p = dy + ((long long)b * C + c) * plane;
-        for (int i = threadIdx.x; i < plane; i += 256) v[0] += __ldg(p + i);
-    }
-    block_sum<1>(v, s_red);
-    if (threadIdx.x == 0) db[c] = v[0];
-}
-
-// parallel variant for few channels x large planes: grid (C, nsplit) partials, then a per-channel merge
-constexpr int BG_CHUNK = 16384;
-__global__ void __launch_bounds__(256) bias_grad_partial_kernel(const float* __restrict__ dy, float* __restrict__ part, int B,
-                                                                int C, int plane, int nsplit) {
-    CCB_PDL_WAIT();
-    __shared__ float s_red[32];
-    const int c = blockIdx.x, sp = blockIdx.y;
-    const long long per = (long long)B * plane;
-    const long long beg = (long long)sp * BG_CHUNK, end = min(per, beg + (long long)BG_CHUNK);
-    float v[1] = {0.f};
-    for (long long i = beg + threadIdx.x; i < end; i += 256) {
-        int b = (int)(i / plane), o = (int)(i - (long long)b * plane);
-        v[0] += __ldg(dy + ((long long)b * C + c) * plane + o);
-    }
-    block_sum<1>(v, s_red);
-    if (threadIdx.x == 0) part[(long long)c * nsplit + sp] = v[0];
-}
-__global__ void bias_grad_merge_kernel(const float* __restrict__ part, float* __restrict__ db, int C, int nsplit) {
-    CCB_PDL_WAIT();
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    float a = 0.f;
-    for (int s = 0; s < nsplit; ++s) a += part[(long long)c * nsplit + s];
-    db[c] = a;
-}
-
 // dz = dy * act'(y) and db[c] = sum_{b,px} dz in ONE pass over the gradient (act_bwd + bias_grad read it twice and cost
 // ~200 launches per step).  Large planes: grid (chunks, B, C), 256 threads x float4, per-CTA partial -> abb_merge_kernel;
 // small planes (B * plane <= ABB_SMALL): one CTA per channel does everything.  Fixed summation order.
@@ -375,19 +318,6 @@ __global__ void __launch_bounds__(256) abb_small_kernel(const float* __restrict_
     if (threadIdx.x == 0) db[c] = v[0];
 }
 
-static int launch_bias_grad(const float* dy, float* db, int B, int C, int plane, float* work, long long work_floats,
-                            cudaStream_t st) {
-    const long long per = (long long)B * plane;
-    const int nsplit = (int)((per + BG_CHUNK - 1) / BG_CHUNK);
-    if (nsplit > 1 && work && (long long)C * nsplit <= work_floats) {
-        CCB_LAUNCH(bias_grad_partial_kernel, dim3(C, nsplit), dim3(256), 0, st, dy, work, B, C, plane, nsplit);
-        CCB_LAUNCH(bias_grad_merge_kernel, dim3(cdiv(C, 128)), dim3(128), 0, st, (const float*)work, db, C, nsplit);
-    } else {
-        CCB_LAUNCH(bias_grad_kernel, dim3(C), dim3(256), 0, st, dy, db, B, C, plane);
-    }
-    return check_launch("bias_grad");
-}
-
 void launch_splitk_reduce(const float* work, float* out, const float* bias, const float* res, long long numel, int splits,
                           int plane, int C, int act, float slope, cudaStream_t st) {
     CCB_LAUNCH(splitk_reduce_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), 0, st, work, out, bias, res, numel, splits,
@@ -395,36 +325,10 @@ void launch_splitk_reduce(const float* work, float* out, const float* bias, cons
 }
 
 // ------------------------------------------------------------------------------------------------
-static int pick_splits(int tiles, int ktiles, int max_splits) {
-    const int target = NUM_SMS * 4;
-    if (tiles >= target || ktiles <= 2) return 1;
-    int s = target / tiles;
-    if (s > ktiles / 2) s = ktiles / 2;
-    if (s > max_splits) s = max_splits;
-    return s < 1 ? 1 : s;
-}
-
-// Split-K partials a call may use: room for 64 splits, capped at 64 MiB.  The split count is planned from this, never
-// from a larger buffer the caller happens to pass, so that a call sums in the same order whatever ran before it.
-static long long ffma_work_floats(long long out_numel) {
-    const long long cap = 16ll * 1024 * 1024;
-    long long want = out_numel * 64;
-    if (want > cap) want = (cap / out_numel) * out_numel;
-    return want < out_numel ? 0 : want;
-}
-
 template <int MODE>
-static int launch_gemm(ConvArgs& a, long long out_numel, long long work_floats, cudaStream_t st, const char* what) {
+static int launch_gemm(const ConvArgs& a, long long out_numel, cudaStream_t st, const char* what) {
     const bool narrow = a.N <= 16;
-    const int BM = narrow ? 128 : 64, BN = narrow ? 16 : 64;
-    const int mt = cdiv(a.M, BM), nt = cdiv(a.N, BN), ktiles = cdiv(a.K, 16);
-    const long long plan_floats = work_floats < ffma_work_floats(out_numel) ? work_floats : ffma_work_floats(out_numel);
-    int max_splits = (a.work && out_numel > 0) ? (int)(plan_floats / out_numel) : 1;
-    if (max_splits > 64) max_splits = 64;
-    a.splits = pick_splits(mt * nt, ktiles, max_splits);
-    // make sure no split is empty
-    while (a.splits > 1 && cdiv(ktiles, a.splits) * (a.splits - 1) >= ktiles) --a.splits;
-    dim3 grid(mt, nt, a.splits);
+    dim3 grid(cdiv(a.M, narrow ? 128 : 64), cdiv(a.N, narrow ? 16 : 64), a.splits);
     auto k_narrow = conv_gemm_kernel<MODE, Cfg<128, 16, 8, 1>>;
     auto k_wide = conv_gemm_kernel<MODE, Cfg<64, 64, 4, 4>>;
     if (narrow) CCB_LAUNCH(k_narrow, grid, dim3(256), 0, st, a);
@@ -442,7 +346,27 @@ static int launch_gemm(ConvArgs& a, long long out_numel, long long work_floats, 
     return rc;
 }
 
-static int fill_conv(ConvArgs& a, const ccb_conv_desc* d) {
+// Split-K count of an FFMA call: about 4 CTAs per SM (launch_gemm's tiles), at least 2 k-tiles per split and none empty,
+// at most 64 splits and 64 MiB of partials.  The strided data gradient never splits: its parity classes would share the
+// partials.
+static int ffma_splits(const ccb_conv_desc* d, int op, long long out_numel) {
+    if (op == CCB_CONV_DGRAD && d->stride > 1) return 1;
+    const int kk = d->kh * d->kw;
+    const int M = op == CCB_CONV_FPROP ? d->B * d->Ho * d->Wo : op == CCB_CONV_DGRAD ? d->B * d->Hi * d->Wi : d->Ci * kk;
+    const int N = op == CCB_CONV_DGRAD ? d->Ci : d->Co;
+    const int K = op == CCB_CONV_FPROP ? d->Ci * kk : op == CCB_CONV_DGRAD ? d->Co * kk : d->B * d->Ho * d->Wo;
+    const bool narrow = N <= 16;
+    const int tiles = cdiv(M, narrow ? 128 : 64) * cdiv(N, narrow ? 16 : 64), ktiles = cdiv(K, 16);
+    if (tiles >= 4 * NUM_SMS || ktiles <= 2) return 1;
+    long long s = 4 * NUM_SMS / tiles;
+    if (s > ktiles / 2) s = ktiles / 2;
+    if (s > 64) s = 64;
+    if (s > (16ll << 20) / out_numel) s = (16ll << 20) / out_numel;
+    while (s > 1 && cdiv(ktiles, (int)s) * (s - 1) >= ktiles) --s;
+    return s < 1 ? 1 : (int)s;
+}
+
+static int check_desc(const ccb_conv_desc* d) {
     CCB_REQUIRE(d != nullptr, CCB_ERR_ARG, "conv: null descriptor");
     CCB_REQUIRE(d->B >= 1 && d->Ci >= 1 && d->Co >= 1 && d->Hi >= 1 && d->Wi >= 1, CCB_ERR_ARG, "conv: bad sizes");
     CCB_REQUIRE(d->kh >= 1 && d->kw >= 1 && d->stride >= 1 && d->pad >= 0, CCB_ERR_ARG, "conv: bad kernel/stride/pad");
@@ -451,24 +375,28 @@ static int fill_conv(ConvArgs& a, const ccb_conv_desc* d) {
     CCB_REQUIRE((d->Hi + 2 * d->pad - d->kh) / d->stride + 1 == d->Ho && (d->Wi + 2 * d->pad - d->kw) / d->stride + 1 == d->Wo,
                 CCB_ERR_ARG, "conv: Ho/Wo inconsistent with Hi/Wi (%d,%d -> %d,%d, k %d s %d p %d)", d->Hi, d->Wi, d->Ho,
                 d->Wo, d->kh, d->stride, d->pad);
+    CCB_REQUIRE(d->impl >= CCB_CONV_IMPL_AUTO && d->impl <= CCB_CONV_IMPL_TC, CCB_ERR_ARG, "conv: unknown impl %d", d->impl);
+    return CCB_OK;
+}
+
+static ConvArgs ffma_args(const ccb_conv_desc* d, int splits, float* work) {
+    ConvArgs a;
     memset(&a, 0, sizeof(a));
     a.B = d->B; a.Ci = d->Ci; a.Hi = d->Hi; a.Wi = d->Wi; a.Co = d->Co; a.Ho = d->Ho; a.Wo = d->Wo;
     a.kh = d->kh; a.kw = d->kw; a.stride = d->stride; a.pad = d->pad;
-    a.act = d->act; a.slope = d->slope; a.splits = 1;
-    return CCB_OK;
+    a.act = d->act; a.slope = d->slope; a.splits = splits; a.work = work;
+    return a;
 }
 
 // tensor-core path (conv_tc.cu)
 bool tc_supported(const ccb_conv_desc* d, int op);
 bool tc_profitable(const ccb_conv_desc* d, int op);
-long long tc_workspace_floats(const ccb_conv_desc* d, int op);
+int tc_plan(const ccb_conv_desc* d, int op, long long& panel_floats);
 int tc_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias, const float* res, float* y,
-             float* work, long long work_floats, int three, cudaStream_t st);
+             float* wp, float* partial, int splits, cudaStream_t st);
 int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const float* bias, const float* res, float* dx,
-             float* work, long long work_floats, int three, cudaStream_t st);
-
-int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* work, long long work_floats,
-             int three, cudaStream_t st);
+             float* wp, float* partial, int splits, cudaStream_t st);
+int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* partial, int splits, cudaStream_t st);
 
 // the weight cache of the conv call in flight (wprep_get looks it up); sim builds have none
 struct WCacheScope {
@@ -479,17 +407,6 @@ struct WCacheScope {
     explicit WCacheScope(void*) {}
 #endif
 };
-
-// 0: FFMA, 1: wgmma 3xTF32, 2: wgmma single TF32
-static int pick_impl(const ccb_conv_desc* d, int op) {
-    switch (d->impl) {
-        case CCB_CONV_IMPL_FFMA: return 0;
-        // forcing the tensor-core path falls back to FFMA only for shapes it cannot express at all
-        case CCB_CONV_IMPL_TC: return tc_supported(d, op) ? 1 : 0;
-        case CCB_CONV_IMPL_TC_TF32: return tc_supported(d, op) ? 2 : 0;
-        default: return tc_profitable(d, op) ? 1 : 0;
-    }
-}
 
 // rows of W floats -> rows of Wp >= W floats, zero tail
 __global__ void __launch_bounds__(256) pad_rows_kernel(const float* __restrict__ src, float* __restrict__ dst, long long rows, int W,
@@ -505,15 +422,65 @@ __global__ void __launch_bounds__(256) pad_rows_kernel(const float* __restrict__
 // WGRAD on small feature maps whose width is not a multiple of 4 (26, 13, 7 ...): the tensor-core kernel reads
 // 16-byte pixel chunks, so x and dy are first copied into rows padded to a multiple of 4 with zeros - a zero dy
 // column contributes nothing and a zero x column is exactly what the convolution's own zero padding would read.
-static bool wgrad_pad_desc(const ccb_conv_desc* d, ccb_conv_desc& dp, long long& xpf, long long& dypf) {
-    if (d->impl == CCB_CONV_IMPL_FFMA || (d->Wo % 4) == 0) return false;
+// dp: the padded call; xpf, dypf: floats of the padded copies of x and dy.
+static void wgrad_pad_desc(const ccb_conv_desc* d, ccb_conv_desc& dp, long long& xpf, long long& dypf) {
     dp = *d;
     dp.Wo = (d->Wo + 3) & ~3;
     dp.Wi = (d->Wi + 3) & ~3;
     xpf = (long long)d->B * d->Ci * d->Hi * dp.Wi;
     dypf = (long long)d->B * d->Co * d->Ho * dp.Wo;
-    if (xpf + dypf > (8ll << 20)) return false;                    // small maps only (<= 32 MiB of copies)
-    return tc_profitable(&dp, CCB_CONV_WGRAD);
+}
+
+enum { PATH_FFMA, PATH_TC, PATH_TC_PADDED };
+struct ConvPlan {
+    int path;               // PATH_*
+    int splits;             // split-K count (the data gradient's parity classes share it)
+    long long head_floats;  // workspace ahead of the split-K partials: the prepared weights (tensor-core fprop / dgrad)
+                            // or the padded copies of x and dy (PATH_TC_PADDED)
+    long long work_floats;  // head + partials: the workspace the call needs
+    const char* kernel;     // what ccb_debug_last_conv_kernel() reports after the call
+};
+static const char* const CONV_OP_NAME[3] = {"conv2d_fprop", "conv2d_dgrad", "conv2d_wgrad"};
+
+// How one call runs, from the descriptor alone (shape + impl) and never from the workspace the caller passes, so that a
+// call sums in the same order whatever ran before it.  AUTO takes the tensor cores where they pay off, TC wherever the
+// kernels can express the shape, both take them for the weight gradient of a small map whose width is not a multiple
+// of 4 through padded rows; everything else runs on the FFMA kernels.
+static ConvPlan conv_plan(const ccb_conv_desc* d, int op) {
+    ConvPlan p = {PATH_FFMA, 1, 0, 0, CONV_OP_NAME[op]};
+    const long long numel = op == CCB_CONV_FPROP ? (long long)d->B * d->Co * d->Ho * d->Wo
+                          : op == CCB_CONV_DGRAD ? (long long)d->B * d->Ci * d->Hi * d->Wi
+                                                 : (long long)d->Co * d->Ci * d->kh * d->kw;
+    if (d->impl == CCB_CONV_IMPL_TC ? tc_supported(d, op) : d->impl == CCB_CONV_IMPL_AUTO && tc_profitable(d, op)) {
+        p.path = PATH_TC;
+        p.splits = tc_plan(d, op, p.head_floats);
+        p.kernel = op == CCB_CONV_WGRAD ? "conv_tc_wgrad" : "conv_tc";
+    } else if (op == CCB_CONV_WGRAD && d->impl != CCB_CONV_IMPL_FFMA && d->Wo % 4 != 0) {
+        ccb_conv_desc dp;
+        long long xpf, dypf;
+        wgrad_pad_desc(d, dp, xpf, dypf);
+        if (xpf + dypf <= (8ll << 20) && tc_profitable(&dp, op)) {     // small maps only (<= 32 MiB of copies)
+            p.path = PATH_TC_PADDED;
+            p.splits = tc_plan(&dp, op, p.head_floats);
+            p.head_floats = xpf + dypf;
+            p.kernel = "conv_tc_wgrad";
+        }
+    }
+    if (p.path == PATH_FFMA) p.splits = ffma_splits(d, op, numel);
+    p.work_floats = p.head_floats + (p.splits > 1 ? p.splits * numel : 0);
+    return p;
+}
+
+// Checks the call and its workspace against its plan; from then on the call is labelled with the plan's kernel.
+static int start_conv(const ccb_conv_desc* d, int op, const float* work, long long work_floats, ConvPlan& p) {
+    int rc = check_desc(d);
+    if (rc) return rc;
+    p = conv_plan(d, op);
+    const long long have = work ? work_floats : 0;
+    CCB_REQUIRE(have >= p.work_floats, CCB_ERR_ARG, "%s: workspace of %lld floats, the call needs %lld (ccb_conv_workspace_floats)",
+                CONV_OP_NAME[op], have, p.work_floats);
+    g_last_conv = p.kernel;
+    return CCB_OK;
 }
 
 }  // namespace ccb
@@ -521,58 +488,35 @@ static bool wgrad_pad_desc(const ccb_conv_desc* d, ccb_conv_desc& dp, long long&
 using namespace ccb;
 
 extern "C" long long ccb_conv_workspace_floats(const ccb_conv_desc* d, int op) {
-    if (!d) return -1;
-    const long long bias_need = (op == CCB_CONV_WGRAD) ? (long long)d->Co * (((long long)d->B * d->Ho * d->Wo + BG_CHUNK - 1) / BG_CHUNK) : 0;
-    if (op == CCB_CONV_WGRAD) {
-        ccb_conv_desc dp;
-        long long xpf, dypf;
-        if (wgrad_pad_desc(d, dp, xpf, dypf)) {
-            const long long t = xpf + dypf + tc_workspace_floats(&dp, op);
-            return t > bias_need ? t : bias_need;
-        }
-    }
-    if (d->impl != CCB_CONV_IMPL_FFMA && tc_supported(d, op) && pick_impl(d, op) > 0) {
-        const long long t = tc_workspace_floats(d, op);
-        return t > bias_need ? t : bias_need;
-    }
-    long long numel = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Co * d->Ho * d->Wo
-                    : (op == CCB_CONV_DGRAD) ? (long long)d->B * d->Ci * d->Hi * d->Wi
-                                             : (long long)d->Co * d->Ci * d->kh * d->kw;
-    const long long want = ffma_work_floats(numel);
-    return want > bias_need ? want : bias_need;
+    if (op < CCB_CONV_FPROP || op > CCB_CONV_WGRAD || check_desc(d)) return -1;
+    return conv_plan(d, op).work_floats;
 }
 
 extern "C" int ccb_conv2d_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias,
                                 const float* res, float* y, float* work, long long work_floats, ccb_stream_t stream) {
-    ConvArgs a;
-    int rc = fill_conv(a, d);
-    if (rc) return rc;
     CCB_REQUIRE(x && w && y, CCB_ERR_ARG, "conv2d_fprop: null pointer");
+    ConvPlan p;
+    int rc = start_conv(d, CCB_CONV_FPROP, work, work_floats, p);
+    if (rc) return rc;
     WCacheScope wc_scope(d->wcache);
-    {
-        int impl = pick_impl(d, CCB_CONV_FPROP);
-        CCB_REQUIRE(impl >= 0, CCB_ERR_UNSUPPORTED, "conv2d_fprop: shape not supported by the tensor-core path");
-        if (impl > 0) return tc_fprop(d, x, w, bias, res, y, work, work_floats, impl == 1, (cudaStream_t)stream);
-    }
-    a.x = x; a.w = w; a.bias = bias; a.res = res; a.out = y; a.work = work;
+    if (p.path == PATH_TC) return tc_fprop(d, x, w, bias, res, y, work, work + p.head_floats, p.splits, (cudaStream_t)stream);
+    ConvArgs a = ffma_args(d, p.splits, work);
+    a.x = x; a.w = w; a.bias = bias; a.res = res; a.out = y;
     a.M = a.B * a.Ho * a.Wo; a.N = a.Co; a.K = a.Ci * a.kh * a.kw;
-    return launch_gemm<MODE_FPROP>(a, (long long)a.M * a.N, work_floats, (cudaStream_t)stream, "conv2d_fprop");
+    return launch_gemm<MODE_FPROP>(a, (long long)a.M * a.N, (cudaStream_t)stream, p.kernel);
 }
 
 // dx[B,Ci,Hi,Wi] = conv_transpose(dy, w); with bias/res/act this is the ConvTranspose2d forward.
 extern "C" int ccb_conv2d_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const float* bias,
                                 const float* res, float* dx, float* work, long long work_floats, ccb_stream_t stream) {
-    ConvArgs a;
-    int rc = fill_conv(a, d);
-    if (rc) return rc;
     CCB_REQUIRE(dy && w && dx, CCB_ERR_ARG, "conv2d_dgrad: null pointer");
+    ConvPlan p;
+    int rc = start_conv(d, CCB_CONV_DGRAD, work, work_floats, p);
+    if (rc) return rc;
     WCacheScope wc_scope(d->wcache);
-    {
-        int impl = pick_impl(d, CCB_CONV_DGRAD);
-        CCB_REQUIRE(impl >= 0, CCB_ERR_UNSUPPORTED, "conv2d_dgrad: shape not supported by the tensor-core path");
-        if (impl > 0) return tc_dgrad(d, dy, w, bias, res, dx, work, work_floats, impl == 1, (cudaStream_t)stream);
-    }
-    a.dy = dy; a.w = w; a.bias = bias; a.res = res; a.out = dx; a.work = work;
+    if (p.path == PATH_TC) return tc_dgrad(d, dy, w, bias, res, dx, work, work + p.head_floats, p.splits, (cudaStream_t)stream);
+    ConvArgs a = ffma_args(d, p.splits, work);
+    a.dy = dy; a.w = w; a.bias = bias; a.res = res; a.out = dx;
     const int s = a.stride;
     for (int py = 0; py < s && py < a.Hi; ++py)
         for (int px = 0; px < s && px < a.Wi; ++px) {
@@ -584,67 +528,37 @@ extern "C" int ccb_conv2d_dgrad(const ccb_conv_desc* d, const float* dy, const f
             c.nkx = (a.kw > c.kx0) ? (a.kw - c.kx0 + s - 1) / s : 0;
             c.M = a.B * c.Hc * c.Wc; c.N = a.Ci; c.K = a.Co * c.nky * c.nkx;
             if (c.K == 0) { c.K = 1; c.nky = c.nkx = 1; c.ky0 = a.kh; c.kx0 = a.kw; }   // no tap hits: output = epilogue(0)
-            // split-K partials of different parity classes must not alias: no split-K for strided dgrad
-            float* wk = (s == 1) ? work : nullptr;
-            c.work = wk;
-            rc = launch_gemm<MODE_DGRAD>(c, (long long)a.B * a.Ci * a.Hi * a.Wi, wk ? work_floats : 0, (cudaStream_t)stream,
-                                         "conv2d_dgrad");
+            rc = launch_gemm<MODE_DGRAD>(c, (long long)a.B * a.Ci * a.Hi * a.Wi, (cudaStream_t)stream, p.kernel);
             if (rc) return rc;
         }
     return CCB_OK;
 }
 
-extern "C" int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* db,
-                                float* work, long long work_floats, ccb_stream_t stream) {
-    ConvArgs a;
-    int rc = fill_conv(a, d);
-    if (rc) return rc;
+extern "C" int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* work,
+                                long long work_floats, ccb_stream_t stream) {
     CCB_REQUIRE(x && dy && dw, CCB_ERR_ARG, "conv2d_wgrad: null pointer");
-    {
-        int impl = pick_impl(d, CCB_CONV_WGRAD);
-        CCB_REQUIRE(impl >= 0, CCB_ERR_UNSUPPORTED, "conv2d_wgrad: shape not supported by the tensor-core path");
-        if (impl > 0) {
-            rc = tc_wgrad(d, x, dy, dw, work, work_floats, impl == 1, (cudaStream_t)stream);
-            if (rc) return rc;
-            if (db) rc = launch_bias_grad(dy, db, d->B, d->Co, d->Ho * d->Wo, work, work_floats, (cudaStream_t)stream);
-            return rc;
-        }
-    }
-    {
+    ConvPlan p;
+    int rc = start_conv(d, CCB_CONV_WGRAD, work, work_floats, p);
+    if (rc) return rc;
+    if (p.path == PATH_TC) return tc_wgrad(d, x, dy, dw, work, p.splits, (cudaStream_t)stream);
+    if (p.path == PATH_TC_PADDED) {
         ccb_conv_desc dp;
         long long xpf, dypf;
-        const bool padded = wgrad_pad_desc(d, dp, xpf, dypf);
-        const long long inner = padded ? tc_workspace_floats(&dp, CCB_CONV_WGRAD) : 0;
-        if (padded && work && xpf + dypf + inner <= work_floats) {
-            float* xp = work;
-            float* dyp = work + xpf;
-            CCB_LAUNCH(pad_rows_kernel, dim3((unsigned)((xpf + 255) / 256)), dim3(256), 0, stream, x, xp, (long long)d->B * d->Ci * d->Hi,
-                       d->Wi, dp.Wi);
-            CCB_LAUNCH(pad_rows_kernel, dim3((unsigned)((dypf + 255) / 256)), dim3(256), 0, stream, dy, dyp, (long long)d->B * d->Co * d->Ho,
-                       d->Wo, dp.Wo);
-            rc = check_launch("conv2d_wgrad pad");
-            if (rc) return rc;
-            rc = tc_wgrad(&dp, xp, dyp, dw, work + xpf + dypf, work_floats - xpf - dypf, d->impl != CCB_CONV_IMPL_TC_TF32,
-                          (cudaStream_t)stream);
-            if (rc) return rc;
-            if (db) rc = launch_bias_grad(dy, db, d->B, d->Co, d->Ho * d->Wo, work, work_floats, (cudaStream_t)stream);
-            return rc;
-        }
+        wgrad_pad_desc(d, dp, xpf, dypf);
+        float* xp = work;
+        float* dyp = work + xpf;
+        CCB_LAUNCH(pad_rows_kernel, dim3((unsigned)((xpf + 255) / 256)), dim3(256), 0, stream, x, xp, (long long)d->B * d->Ci * d->Hi,
+                   d->Wi, dp.Wi);
+        CCB_LAUNCH(pad_rows_kernel, dim3((unsigned)((dypf + 255) / 256)), dim3(256), 0, stream, dy, dyp, (long long)d->B * d->Co * d->Ho,
+                   d->Wo, dp.Wo);
+        rc = check_launch("conv2d_wgrad pad");
+        if (rc) return rc;
+        return tc_wgrad(&dp, xp, dyp, dw, work + p.head_floats, p.splits, (cudaStream_t)stream);
     }
-    a.x = x; a.dy = dy; a.out = dw; a.work = work; a.act = CCB_ACT_NONE;
+    ConvArgs a = ffma_args(d, p.splits, work);
+    a.x = x; a.dy = dy; a.out = dw; a.act = CCB_ACT_NONE;
     a.M = a.Ci * a.kh * a.kw; a.N = a.Co; a.K = a.B * a.Ho * a.Wo;
-    rc = launch_gemm<MODE_WGRAD>(a, (long long)a.M * a.N, work_floats, (cudaStream_t)stream, "conv2d_wgrad");
-    if (rc) return rc;
-    if (db) rc = launch_bias_grad(dy, db, a.B, a.Co, a.Ho * a.Wo, work, work_floats, (cudaStream_t)stream);
-    return rc;
-}
-
-extern "C" int ccb_act_bwd(const float* dy, const float* y, float* dz, long long numel, int act, float slope,
-                           ccb_stream_t stream) {
-    CCB_REQUIRE(dy && y && dz && numel >= 0, CCB_ERR_ARG, "act_bwd: null pointer");
-    if (numel == 0) return CCB_OK;
-    CCB_LAUNCH(act_bwd_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), 0, stream, dy, y, dz, numel, act, slope);
-    return check_launch("act_bwd");
+    return launch_gemm<MODE_WGRAD>(a, (long long)a.M * a.N, (cudaStream_t)stream, p.kernel);
 }
 
 extern "C" long long ccb_act_bwd_bias_workspace_floats(int B, int C, int plane) {
@@ -667,14 +581,4 @@ extern "C" int ccb_act_bwd_bias(const float* dy, const float* y, float* dz, floa
     CCB_LAUNCH(abb_large_kernel, dim3(nchunk, B, C), dim3(256), 0, stream, dy, y, dz, db ? work : nullptr, C, plane, nchunk, act, slope);
     if (db) CCB_LAUNCH(abb_merge_kernel, dim3(cdiv(C, 128)), dim3(128), 0, stream, (const float*)work, db, C, B * nchunk);
     return check_launch("act_bwd_bias");
-}
-
-extern "C" long long ccb_bias_grad_workspace_floats(int B, int C, int plane) {
-    const long long nsplit = ((long long)B * plane + BG_CHUNK - 1) / BG_CHUNK;
-    return nsplit > 1 ? (long long)C * nsplit : 0;
-}
-extern "C" int ccb_bias_grad(const float* dy, float* db, int B, int C, int plane, float* work, long long work_floats,
-                             ccb_stream_t stream) {
-    CCB_REQUIRE(dy && db, CCB_ERR_ARG, "bias_grad: null pointer");
-    return launch_bias_grad(dy, db, B, C, plane, work, work_floats, (cudaStream_t)stream);
 }

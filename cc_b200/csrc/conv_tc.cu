@@ -13,7 +13,6 @@
 //   tf32 MMAs (hi*hi + lo*hi + hi*lo) ("3xTF32", error ~2^-21).  The tensor core only sums one 32-deep stage (small
 //   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
 //   fp32 adds, so no long accumulation chain runs through the tensor core's own rounding;
-//   CCB_CONV_IMPL_TC_TF32 issues hi*hi only (what cuDNN does by default for the reference on Ampere+);
 // * mbarrier pipeline of up to 4 stages: producers -> full[s] -> consumers (wgmma, commit group, wait, fp32 add)
 //   -> empty[s];
 //   the epilogue adds bias / residual, applies the activation and stores NCHW straight from the accumulators.
@@ -191,9 +190,9 @@ __device__ __forceinline__ float tc_act(float v, int act, float slope) {
 constexpr int TC_TILE_BYTES = TC_KC * TC_M * 16;                   // one A operand copy of one stage: 16 KB
 constexpr int TC_SMEM_MAX = 227 * 1024;
 
-// Consumer side shared by both kernels: for each full stage, 4 k-steps of [(lo*hi) + (hi*lo) +] (hi*hi) on this
+// Consumer side shared by both kernels: for each full stage, 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this
 // warpgroup's 64 rows into the scratch registers `part`, then acc += part in fp32 and the stage goes back to the producers.
-template <bool THREE, int NT>
+template <int NT>
 __device__ __forceinline__ void tc_consume(unsigned char* smem, int stage_bytes, int b_tile_bytes, int NST, int nst,
                                            uint64_t* full_bar, uint64_t* empty_bar, int wg, int lane,
                                            float (&acc)[NT / 2], float (&part)[NT / 2]) {
@@ -206,13 +205,11 @@ __device__ __forceinline__ void tc_consume(unsigned char* smem, int stage_bytes,
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
         wg_fence();
-        if (THREE) {
 #pragma unroll
-            for (int ks = 0; ks < TC_KC / 2; ++ks) {
-                const uint32_t koff = (uint32_t)ks * 32u;
-                wgmma_tf32<NT>(part, wg_desc(a_lo + koff), wg_desc(b_hi + koff));
-                wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(b_lo + koff));
-            }
+        for (int ks = 0; ks < TC_KC / 2; ++ks) {
+            const uint32_t koff = (uint32_t)ks * 32u;
+            wgmma_tf32<NT>(part, wg_desc(a_lo + koff), wg_desc(b_hi + koff));
+            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(b_lo + koff));
         }
 #pragma unroll
         for (int ks = 0; ks < TC_KC / 2; ++ks) {
@@ -228,7 +225,7 @@ __device__ __forceinline__ void tc_consume(unsigned char* smem, int stage_bytes,
     }
 }
 
-template <bool THREE, int NT>
+template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) {
     CCB_PDL_TRIGGER();
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -330,7 +327,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
                     const int nn = (n < ntile) ? n : 0;
                     const float* src = a.wp + (long long)(n0 + nn) * a.Kp + kt * (TC_KC * 4) + c * 4;
                     cp_async16(&b_hi[tile_idx(n, c)], src);
-                    if (THREE) cp_async16(&b_lo[tile_idx(n, c)], src + (long long)a.Ntot * a.Kp);
+                    cp_async16(&b_lo[tile_idx(n, c)], src + (long long)a.Ntot * a.Kp);
                 }
             }
             // ---- A: split + store
@@ -339,10 +336,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
                 float4 h, l;
                 h.x = tf32_hi(av[c][0]); h.y = tf32_hi(av[c][1]); h.z = tf32_hi(av[c][2]); h.w = tf32_hi(av[c][3]);
                 a_hi[tile_idx(r, c)] = h;
-                if (THREE) {
-                    l.x = tf32_hi(av[c][0] - h.x); l.y = tf32_hi(av[c][1] - h.y); l.z = tf32_hi(av[c][2] - h.z); l.w = tf32_hi(av[c][3] - h.w);
-                    a_lo[tile_idx(r, c)] = l;
-                }
+                l.x = tf32_hi(av[c][0] - h.x); l.y = tf32_hi(av[c][1] - h.y); l.z = tf32_hi(av[c][2] - h.z); l.w = tf32_hi(av[c][3] - h.w);
+                a_lo[tile_idx(r, c)] = l;
             }
             cp_async_wait_all();
             fence_proxy_async();
@@ -354,7 +349,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
         float acc[NT / 2], part[NT / 2];
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;                  // an empty split contributes zeros
-        tc_consume<THREE, NT>(smem, stage_bytes, a.b_tile_bytes, NST, ktiles, full_bar, empty_bar, wg, lane, acc, part);
+        tc_consume<NT>(smem, stage_bytes, a.b_tile_bytes, NST, ktiles, full_bar, empty_bar, wg, lane, acc, part);
         const long long HWout = (long long)a.Hout * a.Wout;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -393,6 +388,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
 // Weight re-layout: wp[n][t*cpad + c] = w[(co,ci) by mode][tap(t)], zero padded to Kp.
 //   mode 0 (fprop): n = co, c = ci : w[n][c][tap]        mode 1 (dgrad): n = ci, c = co : w[c][n][tap]
 static int roundup(int v, int m) { return (v + m - 1) / m * m; }
+// Kp of `ntaps` taps of Cc channels: whole k-tiles; a parity class without taps still runs one all-zero k-tile
+static int tc_kp(int ntaps, int Cc) { return ntaps > 0 ? roundup(ntaps * roundup(Cc, 4), TC_KC * 4) : TC_KC * 4; }
 
 void launch_splitk_reduce(const float* work, float* out, const float* bias, const float* res, long long numel, int splits,
                           int plane, int C, int act, float slope, cudaStream_t st);   // conv_ffma.cu
@@ -411,42 +408,25 @@ static void tc_geometry(int N, int& nt, int& b_tile_bytes, int& stages, int& sme
 }
 
 template <typename Args>
-static int tc_launch_kernel(void (*const (&kfns)[2][4])(const Args), const Args& a, int three, int nt, dim3 grid, int smem,
-                            cudaStream_t st, const char* what) {
-    const int ni = nt == 16 ? 0 : nt == 32 ? 1 : nt == 64 ? 2 : 3;
-    auto kfn = kfns[three ? 1 : 0][ni];
+static int tc_launch_kernel(void (*const (&kfns)[4])(const Args), const Args& a, int nt, dim3 grid, int smem, cudaStream_t st,
+                            const char* what) {
+    auto kfn = kfns[nt == 16 ? 0 : nt == 32 ? 1 : nt == 64 ? 2 : 3];
     cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
     CCB_LAUNCH(kfn, grid, dim3(TC_THREADS), smem, st, a);
     return check_launch(what);
 }
 
-static void (*const TC_FPROP_KERNELS[2][4])(const TcArgs) = {
-    {conv_tc_kernel<false, 16>, conv_tc_kernel<false, 32>, conv_tc_kernel<false, 64>, conv_tc_kernel<false, 128>},
-    {conv_tc_kernel<true, 16>, conv_tc_kernel<true, 32>, conv_tc_kernel<true, 64>, conv_tc_kernel<true, 128>}};
+static void (*const TC_FPROP_KERNELS[4])(const TcArgs) = {conv_tc_kernel<16>, conv_tc_kernel<32>, conv_tc_kernel<64>,
+                                                          conv_tc_kernel<128>};
 
-// Split-K plan shared by all parity classes of one call: enough CTAs for ~2 waves, >= 2 k-tiles per split.
-static int plan_splits(long long M, int N, int max_ktiles, long long out_numel, long long part_floats) {
-    const long long tiles = (long long)cdiv((int)M, TC_M) * cdiv(N, TC_NMAX);
-    if (tiles >= NUM_SMS || max_ktiles < 4) return 1;
-    long long s = (2 * NUM_SMS + tiles - 1) / tiles;
-    if (s > max_ktiles / 2) s = max_ktiles / 2;
-    if (s > 32) s = 32;
-    if (out_numel > 0 && s * out_numel > part_floats) s = part_floats / out_numel;
-    return s < 2 ? 1 : (int)s;
-}
-
-// One generalised-fprop launch (+ its weight preparation).  `work` = [prepared weights | split-K partials].
+// One generalised-fprop launch (+ its weight preparation into `wp`, tf32 hi copy + lo copy).
 static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK, int Ci, const signed char* tap_index,
-                     float* work, long long work_floats, int splits, float* partial, int three, cudaStream_t st) {
+                     float* wp, float* partial, int splits, cudaStream_t st) {
     a.cpad = roundup(Cc, 4);
-    a.Kp = roundup(a.ntaps * a.cpad, TC_KC * 4);
-    if (a.Kp == 0) a.Kp = TC_KC * 4;      // a parity class without taps still runs one all-zero k-tile
-    const long long wp_floats = 2ll * N * a.Kp;                  // tf32 hi copy + lo copy
-    CCB_REQUIRE(wp_floats + (splits > 1 ? (long long)splits * a.out_numel : 0) <= work_floats, CCB_ERR_ARG,
-                "conv_tc: workspace too small (%lld floats)", work_floats);
+    a.Kp = tc_kp(a.ntaps, Cc);
     WPrepDesc p;
     memset(&p, 0, sizeof(p));
-    p.w = w; p.wp = work; p.N = N; p.Cc = Cc; p.KK = KK; p.ntaps = a.ntaps; p.Kp = a.Kp; p.mode = mode; p.Ci = Ci;
+    p.w = w; p.wp = wp; p.N = N; p.Cc = Cc; p.KK = KK; p.ntaps = a.ntaps; p.Kp = a.Kp; p.mode = mode; p.Ci = Ci;
     p.layout = WPREP_TC; p.p0 = a.cpad;
     for (int t = 0; t < a.ntaps; ++t) p.tap_index[t] = tap_index[t];
     const float* wpp = nullptr;
@@ -456,11 +436,11 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     a.Ntot = N;
     a.splits = splits;
     a.kt_per_split = cdiv(a.Kp / (TC_KC * 4), splits);
-    a.partial = partial ? partial : work + wp_floats;
+    a.partial = partial;
     int nt, smem;
     tc_geometry(N, nt, a.b_tile_bytes, a.stages, smem);
     dim3 grid(cdiv(a.M, TC_M), cdiv(N, TC_NMAX), splits);
-    return tc_launch_kernel(TC_FPROP_KERNELS, a, three, nt, grid, smem, st, "conv_tc");
+    return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, grid, smem, st, "conv_tc");
 }
 
 // ================================================================================================
@@ -480,7 +460,7 @@ struct TcWgradArgs {
     int nstages, b_tile_bytes;   // pipeline depth / bytes of one dY operand copy (Co-tile dependent)
 };
 
-template <bool THREE, int NT>
+template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWgradArgs a) {
     CCB_PDL_TRIGGER();
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -574,17 +554,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
                 float4 h, l;
                 h.x = tf32_hi(av[j][0]); h.y = tf32_hi(av[j][1]); h.z = tf32_hi(av[j][2]); h.w = tf32_hi(av[j][3]);
                 a_hi[tile_idx(r, c)] = h;
-                if (THREE) {
-                    l.x = tf32_hi(av[j][0] - h.x); l.y = tf32_hi(av[j][1] - h.y); l.z = tf32_hi(av[j][2] - h.z); l.w = tf32_hi(av[j][3] - h.w);
-                    a_lo[tile_idx(r, c)] = l;
-                }
+                l.x = tf32_hi(av[j][0] - h.x); l.y = tf32_hi(av[j][1] - h.y); l.z = tf32_hi(av[j][2] - h.z); l.w = tf32_hi(av[j][3] - h.w);
+                a_lo[tile_idx(r, c)] = l;
                 if (r < NT) {
                     h.x = tf32_hi(bv[j].x); h.y = tf32_hi(bv[j].y); h.z = tf32_hi(bv[j].z); h.w = tf32_hi(bv[j].w);
                     b_hi[tile_idx(r, c)] = h;
-                    if (THREE) {
-                        l.x = tf32_hi(bv[j].x - h.x); l.y = tf32_hi(bv[j].y - h.y); l.z = tf32_hi(bv[j].z - h.z); l.w = tf32_hi(bv[j].w - h.w);
-                        b_lo[tile_idx(r, c)] = l;
-                    }
+                    l.x = tf32_hi(bv[j].x - h.x); l.y = tf32_hi(bv[j].y - h.y); l.z = tf32_hi(bv[j].z - h.z); l.w = tf32_hi(bv[j].w - h.w);
+                    b_lo[tile_idx(r, c)] = l;
                 }
             }
             fence_proxy_async();
@@ -596,7 +572,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
         float acc[NT / 2], part[NT / 2];
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
-        tc_consume<THREE, NT>(smem, stage_bytes, a.b_tile_bytes, NST, nst, full_bar, empty_bar, wg, lane, acc, part);
+        tc_consume<NT>(smem, stage_bytes, a.b_tile_bytes, NST, nst, full_bar, empty_bar, wg, lane, acc, part);
         float* outp = a.out + (long long)blockIdx.z * a.Co * a.Ci * KK;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -617,9 +593,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
     }
 }
 
-static void (*const TC_WGRAD_KERNELS[2][4])(const TcWgradArgs) = {
-    {conv_tc_wgrad_kernel<false, 16>, conv_tc_wgrad_kernel<false, 32>, conv_tc_wgrad_kernel<false, 64>, conv_tc_wgrad_kernel<false, 128>},
-    {conv_tc_wgrad_kernel<true, 16>, conv_tc_wgrad_kernel<true, 32>, conv_tc_wgrad_kernel<true, 64>, conv_tc_wgrad_kernel<true, 128>}};
+static void (*const TC_WGRAD_KERNELS[4])(const TcWgradArgs) = {conv_tc_wgrad_kernel<16>, conv_tc_wgrad_kernel<32>,
+                                                                conv_tc_wgrad_kernel<64>, conv_tc_wgrad_kernel<128>};
 
 // out[i] = sum_s work[s][i]
 __global__ void __launch_bounds__(256) tc_splitk_sum_kernel(const float* __restrict__ work, float* __restrict__ out,
@@ -632,7 +607,7 @@ __global__ void __launch_bounds__(256) tc_splitk_sum_kernel(const float* __restr
     out[i] = v;
 }
 
-// Shape gate: which problems take the tensor-core path under CCB_CONV_IMPL_AUTO
+// Shapes the kernels can express, and those where they pay off (CCB_CONV_IMPL_AUTO)
 bool tc_supported(const ccb_conv_desc* d, int op) {
     if (d->kh != d->kw || d->kh * d->kw > TC_MAX_TAPS) return false;
     if (op == CCB_CONV_WGRAD) return (d->Wo % 4 == 0);      // 16-byte pixel chunks must not straddle rows
@@ -640,47 +615,44 @@ bool tc_supported(const ccb_conv_desc* d, int op) {
 }
 bool tc_profitable(const ccb_conv_desc* d, int op) {
     if (!tc_supported(d, op)) return false;
-    long long M = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Ho * d->Wo : (long long)d->B * d->Hi * d->Wi;
-    int N = (op == CCB_CONV_FPROP) ? d->Co : d->Ci;
-    int Cc = (op == CCB_CONV_FPROP) ? d->Ci : d->Co;
-    (void)N; (void)Cc;
+    const long long M = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Ho * d->Wo : (long long)d->B * d->Hi * d->Wi;
     const long long wsize = (long long)d->Ci * d->Co * d->kh * d->kw;
     // tiny feature maps (2x7, 4x13 ...) under a large weight matrix are split-K problems: one M tile, many k-tiles
     return (M >= 128 && wsize >= 64) || (M >= 8 && wsize >= 65536);
 }
 
-static int wgrad_splits(const ccb_conv_desc* d, int& stages, int& per_split) {
-    const int cpad = roundup(d->Ci, 4);
-    const long long P = (long long)d->B * d->Ho * d->Wo;
-    stages = (int)((P + 31) / 32);
-    const int tiles = cdiv(d->kh * d->kw * cpad, TC_M) * cdiv(d->Co, TC_NMAX);
-    int splits = cdiv(2 * NUM_SMS, tiles);
-    if (splits > stages / 4) splits = stages / 4;
-    if (splits > 2 * NUM_SMS) splits = 2 * NUM_SMS;
-    if (splits < 1) splits = 1;
-    per_split = cdiv(stages, splits);
-    splits = cdiv(stages, per_split);          // no empty split
-    return splits;
-}
-
-long long tc_workspace_floats(const ccb_conv_desc* d, int op) {
+// Split-K count of a tensor-core call, and the prepared weights (tf32 hi + lo copies) a fprop / dgrad keeps at the start of
+// its workspace, in floats.  fprop / dgrad: enough CTAs for ~2 waves, >= 2 k-tiles per split, <= 32 splits; the data
+// gradient plans once for all its parity classes (they share the partials, each writes its own pixels), sized by the
+// class with the most taps.  wgrad: ~2 waves of (tap, channel) x Co tiles, >= 4 pixel stages per split.
+int tc_plan(const ccb_conv_desc* d, int op, long long& panel_floats) {
+    panel_floats = 0;
     if (op == CCB_CONV_WGRAD) {
-        int stages, per;
-        int splits = wgrad_splits(d, stages, per);
-        return splits > 1 ? (long long)splits * d->Co * d->Ci * d->kh * d->kw : 0;
+        const int stages = cdiv(d->B * d->Ho * d->Wo, 32);
+        const int tiles = cdiv(d->kh * d->kw * roundup(d->Ci, 4), TC_M) * cdiv(d->Co, TC_NMAX);
+        int splits = cdiv(2 * NUM_SMS, tiles);
+        if (splits > stages / 4) splits = stages / 4;
+        if (splits > 2 * NUM_SMS) splits = 2 * NUM_SMS;
+        if (splits < 1) splits = 1;
+        return cdiv(stages, cdiv(stages, splits));          // no empty split
     }
-    int N = (op == CCB_CONV_FPROP) ? d->Co : d->Ci;
-    int Cc = (op == CCB_CONV_FPROP) ? d->Ci : d->Co;
-    long long wpf = 2ll * N * roundup(d->kh * d->kw * roundup(Cc, 4), 32);
-    long long out_numel = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Co * d->Ho * d->Wo : (long long)d->B * d->Ci * d->Hi * d->Wi;
-    long long M = (op == CCB_CONV_FPROP) ? (long long)d->B * d->Ho * d->Wo : (long long)d->B * d->Hi * d->Wi / (d->stride * d->stride);
-    long long tiles = (long long)cdiv((int)M, TC_M) * cdiv(N, TC_NMAX);
-    long long part = (tiles < NUM_SMS) ? 32 * out_numel : 0;       // room for up to 32 splits when the grid is small
-    return wpf + part;
+    const bool fp = op == CCB_CONV_FPROP;
+    const int s = fp ? 1 : d->stride, N = fp ? d->Co : d->Ci;
+    const int Kp = tc_kp(cdiv(d->kh, s) * cdiv(d->kw, s), fp ? d->Ci : d->Co);
+    panel_floats = 2ll * N * Kp;
+    const long long M = fp ? (long long)d->B * d->Ho * d->Wo : (long long)d->B * cdiv(d->Hi, s) * cdiv(d->Wi, s);
+    const long long tiles = (long long)cdiv((int)M, TC_M) * cdiv(N, TC_NMAX);
+    const int ktiles = Kp / (TC_KC * 4);
+    if (tiles >= NUM_SMS || ktiles < 4) return 1;
+    long long splits = (2 * NUM_SMS + tiles - 1) / tiles;
+    if (splits > ktiles / 2) splits = ktiles / 2;
+    if (splits > 32) splits = 32;
+    return splits < 2 ? 1 : (int)splits;
 }
 
+// y = act(conv(x, w) + bias + res): weights prepared into `wp`, split-K partials in `partial`
 int tc_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias, const float* res, float* y,
-             float* work, long long work_floats, int three, cudaStream_t st) {
+             float* wp, float* partial, int splits, cudaStream_t st) {
     TcArgs a;
     memset(&a, 0, sizeof(a));
     a.x = x; a.bias = bias; a.res = res; a.out = y;
@@ -699,26 +671,18 @@ int tc_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float
             tix[t] = (signed char)t;
         }
     a.out_numel = (long long)d->B * d->Co * d->Ho * d->Wo;
-    const int Kp = roundup(a.ntaps * roundup(d->Ci, 4), 32);
-    const long long wpf = 2ll * d->Co * Kp;
-    const int splits = plan_splits(a.M, d->Co, Kp / 32, a.out_numel, work_floats - wpf);
-    int rc = launch_tc(a, w, 0, d->Co, d->Ci, d->kh * d->kw, d->Ci, tix, work, work_floats, splits, nullptr, three, st);
+    int rc = launch_tc(a, w, 0, d->Co, d->Ci, d->kh * d->kw, d->Ci, tix, wp, partial, splits, st);
     if (rc || splits == 1) return rc;
-    launch_splitk_reduce(a.partial, y, bias, res, a.out_numel, splits, d->Ho * d->Wo, d->Co, d->act, d->slope, st);
+    launch_splitk_reduce(partial, y, bias, res, a.out_numel, splits, d->Ho * d->Wo, d->Co, d->act, d->slope, st);
     return check_launch("conv_tc splitk reduce");
 }
 
-// dx[b,ci,iy,ix] = sum_{co,ky,kx} dy[b,co,(iy+p-ky)/s,(ix+p-kx)/s] w[co,ci,ky,kx]   (one launch per parity class)
+// dx[b,ci,iy,ix] = sum_{co,ky,kx} dy[b,co,(iy+p-ky)/s,(ix+p-kx)/s] w[co,ci,ky,kx]   (one launch per parity class; every
+// class prepares its own weights into `wp`, all share the split-K partials in `partial`)
 int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const float* bias, const float* res, float* dx,
-             float* work, long long work_floats, int three, cudaStream_t st) {
+             float* wp, float* partial, int splits, cudaStream_t st) {
     const int s = d->stride;
-    // one split-K plan for every parity class (they share the partial buffers; each writes its own pixels)
     const long long out_numel = (long long)d->B * d->Ci * d->Hi * d->Wi;
-    const int max_taps = cdiv(d->kh, s) * cdiv(d->kw, s);
-    const int Kp_max = roundup(max_taps * roundup(d->Co, 4), 32);
-    const long long wpf_max = 2ll * d->Ci * Kp_max;
-    const long long Mclass = (long long)d->B * cdiv(d->Hi, s) * cdiv(d->Wi, s);
-    const int splits = plan_splits(Mclass, d->Ci, Kp_max / 32, out_numel, work_floats - wpf_max);
     for (int py = 0; py < s && py < d->Hi; ++py)
         for (int px = 0; px < s && px < d->Wi; ++px) {
             TcArgs a;
@@ -745,20 +709,18 @@ int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const floa
                 }
             }
             a.ntaps = nt;
-            // every class prepares its own weights at the start of `work`; partials live after the largest prep
-            int rc = launch_tc(a, w, 1, d->Ci, d->Co, d->kh * d->kw, d->Ci, tix, work, wpf_max + (splits > 1 ? splits * out_numel : 0),
-                               splits, work + wpf_max, three, st);
+            int rc = launch_tc(a, w, 1, d->Ci, d->Co, d->kh * d->kw, d->Ci, tix, wp, partial, splits, st);
             if (rc) return rc;
         }
     if (splits > 1) {
-        launch_splitk_reduce(work + wpf_max, dx, bias, res, out_numel, splits, d->Hi * d->Wi, d->Ci, d->act, d->slope, st);
+        launch_splitk_reduce(partial, dx, bias, res, out_numel, splits, d->Hi * d->Wi, d->Ci, d->act, d->slope, st);
         return check_launch("conv_tc dgrad splitk reduce");
     }
     return CCB_OK;
 }
 
-int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* work, long long work_floats,
-             int three, cudaStream_t st) {
+// dw; split-K partials in `partial`
+int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* partial, int splits, cudaStream_t st) {
     TcWgradArgs a;
     memset(&a, 0, sizeof(a));
     a.x = x; a.dy = dy;
@@ -767,20 +729,17 @@ int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
     a.cpad = roundup(d->Ci, 4);
     a.Mtot = d->kh * d->kw * a.cpad;
     a.P = d->B * d->Ho * d->Wo;
-    a.splits = wgrad_splits(d, a.stages, a.per_split);
+    a.stages = cdiv(a.P, 32);
+    a.per_split = cdiv(a.stages, splits);
+    a.splits = splits;
+    a.out = splits > 1 ? partial : dw;
     const long long numel = (long long)d->Co * d->Ci * d->kh * d->kw;
-    if (a.splits > 1) {
-        CCB_REQUIRE(work && (long long)a.splits * numel <= work_floats, CCB_ERR_ARG, "conv_tc wgrad: workspace too small");
-        a.out = work;
-    } else {
-        a.out = dw;
-    }
     int nt, wsmem;
     tc_geometry(d->Co, nt, a.b_tile_bytes, a.nstages, wsmem);
     dim3 grid(cdiv(a.Mtot, TC_M), cdiv(d->Co, TC_NMAX), a.splits);
-    int rc = tc_launch_kernel(TC_WGRAD_KERNELS, a, three, nt, grid, wsmem, st, "conv_tc_wgrad");
+    int rc = tc_launch_kernel(TC_WGRAD_KERNELS, a, nt, grid, wsmem, st, "conv_tc_wgrad");
     if (rc || a.splits == 1) return rc;
-    CCB_LAUNCH(tc_splitk_sum_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), 0, st, (const float*)work, dw, numel, a.splits);
+    CCB_LAUNCH(tc_splitk_sum_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), 0, st, (const float*)partial, dw, numel, a.splits);
     return check_launch("conv_tc_wgrad_reduce");
 }
 
@@ -799,14 +758,12 @@ extern "C" int ccb_debug_tc_plan(int N, int* out4) {
 namespace ccb {
 bool tc_supported(const ccb_conv_desc*, int) { return false; }
 bool tc_profitable(const ccb_conv_desc*, int) { return false; }
-long long tc_workspace_floats(const ccb_conv_desc*, int) { return 0; }
-int tc_fprop(const ccb_conv_desc*, const float*, const float*, const float*, const float*, float*, float*, long long, int,
+int tc_plan(const ccb_conv_desc*, int, long long& panel_floats) { panel_floats = 0; return 1; }
+int tc_fprop(const ccb_conv_desc*, const float*, const float*, const float*, const float*, float*, float*, float*, int,
              cudaStream_t) { return CCB_ERR_UNSUPPORTED; }
-int tc_dgrad(const ccb_conv_desc*, const float*, const float*, const float*, const float*, float*, float*, long long, int,
+int tc_dgrad(const ccb_conv_desc*, const float*, const float*, const float*, const float*, float*, float*, float*, int,
              cudaStream_t) { return CCB_ERR_UNSUPPORTED; }
-int tc_wgrad(const ccb_conv_desc*, const float*, const float*, float*, float*, long long, int, cudaStream_t) {
-    return CCB_ERR_UNSUPPORTED;
-}
+int tc_wgrad(const ccb_conv_desc*, const float*, const float*, float*, float*, int, cudaStream_t) { return CCB_ERR_UNSUPPORTED; }
 }  // namespace ccb
 
 extern "C" int ccb_debug_tc_plan(int, int*) { return CCB_ERR_UNSUPPORTED; }

@@ -119,15 +119,6 @@ def _grad_done(*params):
             cb.note(p)
 
 
-def _act_bwd(g, y, act, slope):
-    if act == _lib.ACT_NONE:
-        return g
-    dz = torch.empty_like(g)
-    _lib.check(_lib.lib().ccb_act_bwd(_lib.ptr(g), _lib.ptr(y), _lib.ptr(dz), g.numel(), act, slope, _lib.stream(g)),
-               'act_bwd')
-    return dz
-
-
 def _act_bwd_bias(g, y, act, slope, db):
     """dz = g * act'(y) and (db given) db[c] = sum dz, one pass (ccb_act_bwd_bias)."""
     if act == _lib.ACT_NONE and db is None:
@@ -179,7 +170,7 @@ class _Conv2dFn(torch.autograd.Function):
             _run(_lib.CONV_DGRAD, d, dz, w, None, None, dx)
         if want_w:
             dw, w_direct = _grad_slot(ctx.params[0], w)
-            _run(_lib.CONV_WGRAD, d, x, dz, dw, None)
+            _run(_lib.CONV_WGRAD, d, x, dz, dw)
             _grad_done(ctx.params[0] if w_direct else None, ctx.params[1] if b_direct else None)
             dw = None if w_direct else dw
             db = None if b_direct else db
@@ -226,7 +217,7 @@ class _ConvT2dFn(torch.autograd.Function):
             _run(_lib.CONV_FPROP, d, dz, w, None, None, dx)
         if ctx.needs_input_grad[1]:
             dw, direct = _grad_slot(ctx.params[0], w)
-            _run(_lib.CONV_WGRAD, d, dz, x, dw, None)        # roles swapped: activations = dz, grads = x
+            _run(_lib.CONV_WGRAD, d, dz, x, dw)              # roles swapped: activations = dz, grads = x
             _grad_done(ctx.params[0] if direct else None)
             dw = None if direct else dw
         return dx, dw, db, None, None, None, None, None

@@ -201,14 +201,14 @@ int ccb_bce_bwd(const ccb_bce_desc* d, ccb_stream_t stream);
  *   dx = act(conv_transpose(dy, w) + bias + res)                   ccb_conv2d_dgrad
  *        (plain data-gradient when bias/res are NULL and act is NONE; with them it is the
  *         nn.ConvTranspose2d forward of a layer whose torch weight [Cin_t,Cout_t,k,k] is this w)
- *   dw = d/dw, db = sum dy                                         ccb_conv2d_wgrad
- * impl: CCB_CONV_IMPL_AUTO picks wgmma tensor-core tiles where the shape allows and the FFMA
- *       kernels otherwise; _FFMA / _TC force one (tests).
+ *   dw = d/dw                                                      ccb_conv2d_wgrad
+ *        (the bias gradient comes with the activation backward: ccb_act_bwd_bias)
+ * impl: CCB_CONV_IMPL_AUTO picks the wgmma tensor-core kernels (3xTF32: fp32 parity) where they pay off
+ *       and the FFMA kernels otherwise; _FFMA / _TC force one (tests).
  * ---------------------------------------------------------------------------------------------- */
 enum { CCB_ACT_NONE = 0, CCB_ACT_RELU = 1, CCB_ACT_LEAKY = 2, CCB_ACT_SIGMOID = 3 };
 enum { CCB_CONV_FPROP = 0, CCB_CONV_DGRAD = 1, CCB_CONV_WGRAD = 2 };
-enum { CCB_CONV_IMPL_AUTO = 0, CCB_CONV_IMPL_FFMA = 1, CCB_CONV_IMPL_TC = 2 /* wgmma 3xTF32 (fp32 parity) */,
-       CCB_CONV_IMPL_TC_TF32 = 3 /* wgmma single TF32 (cuDNN's default math for the reference) */ };
+enum { CCB_CONV_IMPL_AUTO = 0, CCB_CONV_IMPL_FFMA = 1, CCB_CONV_IMPL_TC = 2 };
 typedef struct ccb_conv_desc {
     int B, Ci, Hi, Wi;      /* input  [B,Ci,Hi,Wi] */
     int Co, Ho, Wo;         /* output [B,Co,Ho,Wo]; Ho = (Hi + 2 pad - kh) / stride + 1 */
@@ -233,26 +233,20 @@ int ccb_wcache_commit(void* cache, float* buf, long long buf_floats, void* table
 int ccb_wcache_refresh(void* cache, ccb_stream_t stream);
 /* out4 = {recorded layouts, cache hits, misses after commit, state (0 recording, 1 committed)} */
 void ccb_wcache_stats(void* cache, long long* out4);
+/* Each call is planned from the descriptor alone (kernels, split-K, hence the summation order): `work` must hold at least
+ * ccb_conv_workspace_floats() floats (else CCB_ERR_ARG, nothing launched); a larger one changes nothing.  -1: bad descriptor. */
 long long ccb_conv_workspace_floats(const ccb_conv_desc* d, int op);
 int ccb_conv2d_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias,
                      const float* res, float* y, float* work, long long work_floats, ccb_stream_t stream);
 int ccb_conv2d_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const float* bias,
                      const float* res, float* dx, float* work, long long work_floats, ccb_stream_t stream);
-int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* db,
+int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
                      float* work, long long work_floats, ccb_stream_t stream);
-/* dz = dy * act'(.) expressed through the activation OUTPUT y (in place allowed: dz == dy). */
-int ccb_act_bwd(const float* dy, const float* y, float* dz, long long numel, int act, float slope,
-                ccb_stream_t stream);
 /* fused: dz = dy * act'(y) (not touched when act == CCB_ACT_NONE; in place allowed) and, when db != NULL,
  * db[c] = sum over (b, pixel) of dz - one pass over the gradient.  work: ccb_act_bwd_bias_workspace_floats() floats. */
 long long ccb_act_bwd_bias_workspace_floats(int B, int C, int plane);
 int ccb_act_bwd_bias(const float* dy, const float* y, float* dz, float* db, int B, int C, int plane, int act, float slope,
                      float* work, long long work_floats, ccb_stream_t stream);
-/* db[c] = sum over (b, pixel) of dy; `work` (ccb_bias_grad_workspace_floats) lets large planes be reduced in two
- * deterministic stages, without it one block per channel does the whole sum */
-long long ccb_bias_grad_workspace_floats(int B, int C, int plane);
-int ccb_bias_grad(const float* dy, float* db, int B, int C, int plane, float* work, long long work_floats,
-                  ccb_stream_t stream);
 /* bring-up / diagnostic entry points (ccb_debug_*): include/ccb200_debug.h - not part of the drop-in boundary */
 
 /* Back2Future operators (models/back2future.py).

@@ -7,8 +7,8 @@
 extern "C" {
 #endif
 
-/* which kernel the last convolution call of this thread launched ("conv_tc", "conv_tc_wgrad",
- * "conv2d_fprop" ... for the CUDA-core GEMM): bench.py buckets its per-call timings by it */
+/* which kernel the last convolution call of this thread launched ("conv_tc", "conv_tc_wgrad", or
+ * "conv2d_fprop" / "conv2d_dgrad" / "conv2d_wgrad" for the CUDA-core GEMM): bench.py buckets its per-call timings by it */
 const char* ccb_debug_last_conv_kernel(void);
 /* host-side geometry of the wgmma convolution kernels for N output channels (no launch; unit tests):
  * out4 = {wgmma N, bytes of one B operand copy, pipeline stages, dynamic shared memory bytes} */

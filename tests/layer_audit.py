@@ -142,7 +142,7 @@ def _act64(z, act, slope):
 
 
 def _act_bwd64(g, y, act, slope):
-    """dz = g * act'(y) from the kernel's fp32 output y, as ccb_act_bwd computes it; and its rounding count."""
+    """dz = g * act'(y) from the kernel's fp32 output y, as ccb_act_bwd_bias computes it; and its rounding count."""
     if act == _lib.ACT_RELU:
         return g * (y > 0), 0
     if act == _lib.ACT_LEAKY:

@@ -68,9 +68,8 @@ def case_conv_shapes(device, big=False):
 
 
 def case_conv_tc(device):
-    """wgmma tensor-core path against torch fp64 on real layer shapes: fprop, dgrad (incl. strided parity classes /
-    ConvTranspose forward) and wgrad.  IMPL_TC = 3xTF32 (fp32 parity), IMPL_TC_TF32 = single TF32 (what cuDNN
-    runs by default for the reference).  GPU only (the simulator has no tensor cores)."""
+    """wgmma tensor-core path (IMPL_TC, 3xTF32) against torch fp64 on real layer shapes: fprop, dgrad (incl. strided parity
+    classes / ConvTranspose forward) and wgrad.  GPU only (the simulator has no tensor cores)."""
     from cc_b200 import _lib
     g = torch.Generator().manual_seed(7)
     shapes = [(2, 32, 16, 24, 64, 3, 1, 1), (2, 17, 13, 20, 40, 3, 2, 1), (4, 128, 32, 104, 128, 3, 1, 1),
@@ -79,32 +78,30 @@ def case_conv_tc(device):
               (4, 512, 8, 26, 512, 3, 1, 1), (4, 256, 16, 52, 512, 3, 2, 1)]      # small-M layers: split-K
     saved = cnn.CONV_IMPL
     try:
+        cnn.CONV_IMPL = _lib.IMPL_TC
         for (B, Ci, H, W, Co, k, s, p) in shapes:
             x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
             w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
             b = torch.randn(Co, generator=g).to(device).requires_grad_(True)
             xd, wd, bd = [t.detach().double().requires_grad_(True) for t in (x, w, b)]
-            for impl, tol in ((_lib.IMPL_TC, 1e-4), (_lib.IMPL_TC_TF32, 5e-3)):
-                tag = f'tc impl {impl} {Ci}->{Co} k{k} s{s}'
-                cnn.CONV_IMPL = impl
-                # fused epilogue (bias + LeakyReLU) in the forward ...
-                assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(F.conv2d(xd, wd, bd, s, p), 0.2), tol,
-                             tag + ' fprop+leaky')
-                # ... gradients with a linear epilogue: a forward difference of 1e-6 flips LeakyReLU masks of
-                # near-zero pre-activations, which changes dx by ~1e-2 for ANY two implementations
-                zd = F.conv2d(xd, wd, bd, s, p)
-                wt = _wts(zd.shape, 5, device)
-                gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
-                y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
-                assert_close(y, zd, tol, tag + ' fprop')
-                gx, gw, gb = torch.autograd.grad((y * wt).sum(), [x, w, b])
-                assert_close(gx, gd[0], tol, tag + ' dgrad')
-                assert_close(gw, gd[1], tol, tag + ' wgrad')
-                assert_close(gb, gd[2], tol, tag + ' bias grad')
+            tag = f'tc {Ci}->{Co} k{k} s{s}'
+            # fused epilogue (bias + LeakyReLU) in the forward ...
+            assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(F.conv2d(xd, wd, bd, s, p), 0.2), 1e-4,
+                         tag + ' fprop+leaky')
+            # ... gradients with a linear epilogue: a forward difference of 1e-6 flips LeakyReLU masks of
+            # near-zero pre-activations, which changes dx by ~1e-2 for ANY two implementations
+            zd = F.conv2d(xd, wd, bd, s, p)
+            wt = _wts(zd.shape, 5, device)
+            gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
+            y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
+            assert_close(y, zd, 1e-4, tag + ' fprop')
+            gx, gw, gb = torch.autograd.grad((y * wt).sum(), [x, w, b])
+            assert_close(gx, gd[0], 1e-4, tag + ' dgrad')
+            assert_close(gw, gd[1], 1e-4, tag + ' wgrad')
+            assert_close(gb, gd[2], 1e-4, tag + ' bias grad')
         # ConvTranspose2d forward == strided dgrad parity classes
         x = torch.randn(4, 96, 8, 28, generator=g).to(device).requires_grad_(True)      # small M per parity class: split-K
         b = torch.randn(32, generator=g).to(device)
-        cnn.CONV_IMPL = _lib.IMPL_TC
         for (k, op) in ((4, 0), (3, 1)):
             w = (torch.randn(96, 32, k, k, generator=g) * 0.05).to(device).requires_grad_(True)
             xd, wd = x.detach().double().requires_grad_(True), w.detach().double().requires_grad_(True)
@@ -267,23 +264,28 @@ def case_conv_weight_cache(device):
         cnn.WCACHE = None
 
 
-def case_conv_plan_ignores_workspace(device):
-    """A convolution's split-K plan is a function of its shape alone: the same call given the workspace it asks for
+def case_conv_plan_from_shape(device):
+    """A convolution's plan is a function of its shape alone: the same call given the workspace it asks for
     (ccb_conv_workspace_floats) and given a much larger one - as the grow-only workspace in cc_b200.nn is once a bigger
-    layer has run - sums in the same order, so the results are bit-identical.  Small maps under long reductions, where
-    both convolution families split K: fprop / stride-1 dgrad with 4 output pixels and 2304-deep K, wgrad over 2048
-    pixels into a 16 x 144 weight."""
+    layer has run - sums in the same order, so the results are bit-identical; given one float less it fails with an
+    error naming the workspace and writes nothing.  After each call ccb_debug_last_conv_kernel() names the kernel family
+    that ran.  Small maps under long reductions, where both convolution families split K: fprop / stride-1 dgrad with 4
+    output pixels and 2304-deep K (AUTO leaves them to the FFMA kernels; the weight gradient of the 2-wide map runs on
+    the tensor cores through padded rows), wgrad over 2048 pixels into a 16 x 144 weight."""
     import ctypes as C
     from cc_b200 import _lib
     lib = _lib.lib()
     g = torch.Generator().manual_seed(23)
     impls = (_lib.IMPL_FFMA,) if _lib.is_simulator() else (_lib.IMPL_FFMA, _lib.IMPL_TC, _lib.IMPL_AUTO)
-    for (B, Ci, H, W, Co, k, s, p) in ((2, 256, 1, 2, 256, 3, 1, 1), (2, 16, 32, 32, 16, 3, 1, 1)):
+    ffma = ('conv2d_fprop', 'conv2d_dgrad', 'conv2d_wgrad')
+    tc = ('conv_tc', 'conv_tc', 'conv_tc_wgrad')
+    for (B, Ci, H, W, Co, k, s, p), auto in (((2, 256, 1, 2, 256, 3, 1, 1), ffma[:2] + tc[2:]), ((2, 16, 32, 32, 16, 3, 1, 1), tc)):
         Ho, Wo = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
         x = torch.randn(B, Ci, H, W, generator=g).to(device)
         w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device)
         dy = torch.randn(B, Co, Ho, Wo, generator=g).to(device)
         for impl in impls:
+            kernels = {_lib.IMPL_FFMA: ffma, _lib.IMPL_TC: tc, _lib.IMPL_AUTO: auto}[impl]
             d = _lib.ConvDesc()
             d.B, d.Ci, d.Hi, d.Wi, d.Co, d.Ho, d.Wo = B, Ci, H, W, Co, Ho, Wo
             d.kh = d.kw = k
@@ -292,16 +294,27 @@ def case_conv_plan_ignores_workspace(device):
                                  (_lib.CONV_WGRAD, (x, dy), w)):
                 fn = (lib.ccb_conv2d_fprop, lib.ccb_conv2d_dgrad, lib.ccb_conv2d_wgrad)[op]
                 need = lib.ccb_conv_workspace_floats(C.byref(d), op)
+                tag = f'impl {impl} op {op} {Ci}->{Co} {H}x{W}'
+                assert need >= 0, tag
                 res = []
                 for wf in (need, 8 * need + 4096):
                     work = torch.full((max(wf, 1),), float('nan'), device=device)
                     y = torch.empty_like(out)
-                    args = [_lib.ptr(t) for t in ins] + [y.data_ptr()] + ([None] if op == _lib.CONV_WGRAD else [])
+                    args = [_lib.ptr(t) for t in ins] + [y.data_ptr()]
                     _lib.check(fn(C.byref(d), *args, work.data_ptr() if wf else None, wf, _lib.stream(x)), 'conv op %d' % op)
+                    got = lib.ccb_debug_last_conv_kernel().decode()
+                    assert got == kernels[op], f'{tag}: the call ran {kernels[op]}, labelled {got!r}'
                     res.append(y)
-                tag = f'impl {impl} op {op} {Ci}->{Co} {H}x{W}: workspace of {need} vs {8 * need + 4096} floats'
                 assert bool(torch.isfinite(res[0]).all()), tag
-                assert torch.equal(res[0], res[1]), f'{tag} changes the result by {(res[0] - res[1]).abs().max().item():.3e}'
+                assert torch.equal(res[0], res[1]), \
+                    f'{tag}: workspace of {need} vs {8 * need + 4096} floats changes the result by {(res[0] - res[1]).abs().max().item():.3e}'
+                if need > 0:
+                    work = torch.full((max(need - 1, 1),), float('nan'), device=device)
+                    y = torch.full_like(out, 7.0)
+                    rc = fn(C.byref(d), *[_lib.ptr(t) for t in ins], y.data_ptr(), work.data_ptr() if need > 1 else None, need - 1,
+                            _lib.stream(x))
+                    assert rc == -1 and b'workspace' in lib.ccb_last_error_string(), f'{tag}: {need - 1} floats accepted ({rc})'
+                    assert bool((y == 7.0).all()), f'{tag}: a call refused for its workspace wrote its output'
 
 
 ALT_NETS = [  # mirrors tests/golden/make_golden.py:ALT_NETS (name, kwargs, input size, frozen gradients)
@@ -532,4 +545,4 @@ def smoke_case(device):
 
 
 NET_CASES = [case_conv_shapes, case_bn_upsample, case_disp_pose_golden, case_mask_golden, case_flow_golden, case_alt_pose_nets,
-             case_conv_plan_ignores_workspace]
+             case_conv_plan_from_shape]

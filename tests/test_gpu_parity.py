@@ -143,7 +143,7 @@ def test_train_step_cfg1_vs_oracle():
         cnn.CONV_IMPL = saved
 
 
-def test_conv_tensor_core_path():
+def test_conv_tensor_core_3xtf32():
     NC.case_conv_tc(torch.device('cuda:0'))
 
 

@@ -43,7 +43,8 @@ def timeit(fn, iters=5):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--impl', type=int, default=_lib.IMPL_AUTO)
+    ap.add_argument('--impl', type=int, default=_lib.IMPL_AUTO, choices=(_lib.IMPL_AUTO, _lib.IMPL_FFMA, _lib.IMPL_TC),
+                    help='0 auto, 1 FFMA kernels, 2 tensor-core kernels')
     ap.add_argument('--nets', default='disp,pose')
     args = ap.parse_args()
     cnn.CONV_IMPL = args.impl
