@@ -126,6 +126,7 @@ _SIGS = {
     'ccb_upsample2x_fwd': (_I, [_P, _P, _I, _I, _I, _P]),
     'ccb_upsample2x_bwd': (_I, [_P, _P, _I, _I, _I, _P]),
     'ccb_adam_step': (_I, [_P, _P, _P, _P, _LL, _P, _F, _F, _F, _F, _F, _P]),
+    'ccb_adam_step_ranges': (_I, [_P, _P, _P, _P, _P, _I, _LL, _P, _I, _P, _F, _F, _F, _F, _F, _P]),
     'ccb_launch_count': (_LL, []),
     'ccb_flow_metrics_workspace_bytes': (_LL, [_I, _I, _I]),
     'ccb_flow_metrics': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _F, _P, _P, _P, _P]),

@@ -200,26 +200,48 @@ __global__ void __launch_bounds__(256) upsample2x_bwd_kernel(const float* __rest
 }
 
 // ---- Adam over a flat parameter / gradient buffer (torch.optim.Adam semantics, no weight decay) ----
-// The step counter and bias corrections live in device memory (state[0..2] = step, 1-b1^t, sqrt(1-b2^t))
-// so that the whole training step can be captured once in a CUDA graph and replayed.
-__global__ void adam_prep_kernel(float* __restrict__ state, float b1, float b2) {
+// The step counters and bias corrections live in device memory (group g: state[4g..4g+2] = step, 1-b1^t, sqrt(1-b2^t))
+// so that the whole training step can be captured once in a CUDA graph and replayed.  One thread per group; groups
+// whose `active` flag is zero (a fixed network) keep their count.
+__global__ void adam_prep_kernel(float* __restrict__ state, const int* __restrict__ active, int ngroups, float b1, float b2) {
     CCB_PDL_WAIT();
-    if (threadIdx.x == 0 && blockIdx.x == 0) {
-        float t = state[0] + 1.f;
-        state[0] = t;
-        state[1] = (float)(1.0 - pow((double)b1, (double)t));
-        state[2] = (float)sqrt(1.0 - pow((double)b2, (double)t));
+    const int grp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (grp < ngroups && (active == nullptr || __ldg(active + grp) != 0)) {
+        float* s = state + 4 * grp;
+        float t = s[0] + 1.f;
+        s[0] = t;
+        s[1] = (float)(1.0 - pow((double)b1, (double)t));
+        s[2] = (float)sqrt(1.0 - pow((double)b2, (double)t));
     }
 }
 
 // grad_scale multiplies the gradient first (1/world_size after the NCCL sum).
+// Block -> range: the largest entry whose first_block <= blockIdx.x (binary search over the table; one range and no
+// table when ranges == nullptr).  The range decides only which elements and which group's bias corrections a thread
+// uses, never the per-element arithmetic.
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                                   float* __restrict__ v, long long n, const float* __restrict__ state,
+                                                   float* __restrict__ v, long long n, const long long* __restrict__ ranges,
+                                                   int nranges, const float* __restrict__ state,
                                                    float lr, float b1, float b2, float eps, float grad_scale) {
     CCB_PDL_WAIT();
-    long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-    if (i >= n) return;
-    const float bc1 = __ldg(state + 1), bc2_sqrt = __ldg(state + 2);
+    long long off = 0, cnt = n, blk = blockIdx.x;
+    int grp = 0;
+    if (ranges != nullptr) {
+        int lo = 0, hi = nranges - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (__ldg(ranges + 4 * mid + 3) <= blk) lo = mid;
+            else hi = mid - 1;
+        }
+        off = __ldg(ranges + 4 * lo);
+        cnt = __ldg(ranges + 4 * lo + 1);
+        grp = (int)__ldg(ranges + 4 * lo + 2);
+        blk -= __ldg(ranges + 4 * lo + 3);
+    }
+    const long long j = blk * 256 + threadIdx.x;
+    if (j >= cnt) return;
+    const long long i = off + j;
+    const float bc1 = __ldg(state + 4 * grp + 1), bc2_sqrt = __ldg(state + 4 * grp + 2);
     float gi = __ldg(g + i) * grad_scale;
     float mi = b1 * m[i] + (1.f - b1) * gi;
     float vi = b2 * v[i] + (1.f - b2) * gi * gi;
@@ -290,10 +312,26 @@ extern "C" int ccb_adam_step(float* params, const float* grads, float* exp_avg, 
                              float* state, float lr, float beta1, float beta2, float eps, float grad_scale,
                              ccb_stream_t stream) {
     CCB_REQUIRE(params && grads && exp_avg && exp_avg_sq && state && n >= 0, CCB_ERR_ARG, "adam_step: bad argument");
-    CCB_LAUNCH(adam_prep_kernel, dim3(1), dim3(32), 0, stream, state, beta1, beta2);
+    CCB_LAUNCH(adam_prep_kernel, dim3(1), dim3(32), 0, stream, state, (const int*)nullptr, 1, beta1, beta2);
     int rc = check_launch("adam_prep");
     if (rc || n == 0) return rc;
     CCB_LAUNCH(adam_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, params, grads, exp_avg, exp_avg_sq, n,
-               (const float*)state, lr, beta1, beta2, eps, grad_scale);
+               (const long long*)nullptr, 1, (const float*)state, lr, beta1, beta2, eps, grad_scale);
     return check_launch("adam_step");
+}
+
+extern "C" int ccb_adam_step_ranges(float* params, const float* grads, float* exp_avg, float* exp_avg_sq,
+                                    const long long* ranges, int nranges, long long nblocks, const int* group_active,
+                                    int ngroups, float* group_state, float lr, float beta1, float beta2, float eps,
+                                    float grad_scale, ccb_stream_t stream) {
+    CCB_REQUIRE(params && grads && exp_avg && exp_avg_sq && group_state && ngroups >= 1 && nranges >= 0 && nblocks >= 0,
+                CCB_ERR_ARG, "adam_step_ranges: bad argument");
+    CCB_REQUIRE(nranges == 0 || (ranges != nullptr && nblocks >= 1), CCB_ERR_ARG, "adam_step_ranges: empty range table");
+    CCB_REQUIRE(nblocks < (1LL << 31), CCB_ERR_ARG, "adam_step_ranges: %lld blocks", nblocks);
+    CCB_LAUNCH(adam_prep_kernel, dim3(cdiv(ngroups, 32)), dim3(32), 0, stream, group_state, group_active, ngroups, beta1, beta2);
+    int rc = check_launch("adam_prep");
+    if (rc || nranges == 0) return rc;
+    CCB_LAUNCH(adam_kernel, dim3((unsigned)nblocks), dim3(256), 0, stream, params, grads, exp_avg, exp_avg_sq, 0LL, ranges,
+               nranges, (const float*)group_state, lr, beta1, beta2, eps, grad_scale);
+    return check_launch("adam_step_ranges");
 }

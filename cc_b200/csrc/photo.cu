@@ -50,7 +50,10 @@ __device__ __noinline__ float2 rigid_occ_pairs(const Cam* cams, float x, float y
 
 // ================================================================================================
 // Forward.  MODE: CCB_PHOTO_RIGID / FLOW / CONSENSUS.  SSIM=false compiles the 13x13 stage out.
-template <int MODE, bool SSIM>
+// SAVE=false is the value-only forward (no backward will run): the saved-for-backward maps dmaps / vo / gmask are not
+// written, so the SSIM derivatives are dead code.  GMASK=false (the mask needs no gradient) skips gmask only.  Neither
+// flag touches the terms of the loss value: its sums and their order are those of the full forward.
+template <int MODE, bool SSIM, bool SAVE = true, bool GMASK = true>
 __global__ void __launch_bounds__(NT, 2) photo_fwd_kernel(const PhotoArgs a) {
     CCB_PDL_WAIT();
     constexpr int HALO = SSIM ? 6 : 0;
@@ -203,8 +206,8 @@ __global__ void __launch_bounds__(NT, 2) photo_fwd_kernel(const PhotoArgs a) {
                     s_l1 += rl1(df, d.qch);
                     float sl = (1.f - S * valid[j]) * om[j];
                     s_ss += sl * mk[j];
-                    if (d.has_mask) gm[j] += rl1_d(df, d.qch) * e + d.wssim * sl;
-                    if (SSIM) {
+                    if (SAVE && GMASK && d.has_mask) gm[j] += rl1_d(df, d.qch) * e + d.wssim * sl;
+                    if (SSIM && SAVE) {
                         float gam = -valid[j] * om[j] * mk[j];
                         int off = (y0 + rg * PXT + j) * w + (x0 + col);
                         float* dm = d.dmaps[l] + ((b * R + i) * 9 + c * 3) * hw + off;
@@ -240,8 +243,8 @@ __global__ void __launch_bounds__(NT, 2) photo_fwd_kernel(const PhotoArgs a) {
                 int off = (b * R + i) * hw + (y0 + rg * PXT + j) * w + (x0 + col);
                 s_va += valid[j];
                 s_ob += rl1(1.f - valid[j], d.qch);
-                d.vo[l][off] = valid[j] * om[j];
-                if (d.has_mask) d.gmask[l][off] = gm[j];
+                if (SAVE) d.vo[l][off] = valid[j] * om[j];
+                if (SAVE && GMASK && d.has_mask) d.gmask[l][off] = gm[j];
             }
             float red[4] = {s_l1, s_ss, s_va, s_ob};
             block_sum<4>(red, s_red);
@@ -296,8 +299,9 @@ __global__ void __launch_bounds__(1024) photo_fwd_finalize(const PhotoArgs a) {
 
 // ================================================================================================
 // Backward.  Blurs the saved gamma*dS maps (halo 6), recomputes the centre-pixel warp, and chains to
-// depth / pose (rigid) or flow; mask gradient is a scale of the saved unscaled term.
-template <int MODE, bool SSIM>
+// depth / pose (rigid) or flow; mask gradient is a scale of the saved unscaled term.  GMASK=false: the mask (still read
+// as a factor) needs no gradient and d_mask is not written.
+template <int MODE, bool SSIM, bool GMASK = true>
 __global__ void __launch_bounds__(NT, 2) photo_bwd_kernel(const PhotoArgs a) {
     CCB_PDL_WAIT();
     using T = Tile<6>;
@@ -402,7 +406,7 @@ __global__ void __launch_bounds__(NT, 2) photo_bwd_kernel(const PhotoArgs a) {
                     df[0] = gXn * (2.f / w1);
                     df[hw] = gYn * (2.f / h1);
                 }
-                if (d.has_mask) d.d_mask[l][moff] = c_l * __ldg(d.gmask[l] + moff);
+                if (GMASK && d.has_mask) d.d_mask[l][moff] = c_l * __ldg(d.gmask[l] + moff);
             }
         }
         if (MODE == CCB_PHOTO_RIGID) {
@@ -478,21 +482,35 @@ template <int HALO>
 static size_t fwd_smem() { return (size_t)(6 * Tile<HALO>::PLANE + (HALO ? 3 * Tile<HALO>::RH * HP : 0)) * sizeof(float); }
 static size_t bwd_smem() { return (size_t)(3 * Tile<6>::PLANE + 3 * Tile<6>::RH * HP) * sizeof(float); }
 
-template <int MODE, bool SSIM>
+template <int MODE, bool SSIM, bool SAVE = true, bool GMASK = true>
 static int launch_fwd(const PhotoArgs& a, cudaStream_t st) {
-    auto k = photo_fwd_kernel<MODE, SSIM>;
+    auto k = photo_fwd_kernel<MODE, SSIM, SAVE, GMASK>;
     size_t sm = SSIM ? fwd_smem<6>() : fwd_smem<0>();
     { static bool once = false; if (!once) { cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); once = true; } }
     CCB_LAUNCH(k, dim3(a.blk_off[a.d.nlevels]), dim3(NT), sm, st, a);
     return check_launch("photo_fwd");
 }
-template <int MODE, bool SSIM>
+template <int MODE, bool SSIM, bool GMASK>
 static int launch_bwd(const PhotoArgs& a, cudaStream_t st) {
-    auto k = photo_bwd_kernel<MODE, SSIM>;
+    auto k = photo_bwd_kernel<MODE, SSIM, GMASK>;
     size_t sm = bwd_smem();
     { static bool once = false; if (!once) { cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); once = true; } }
     CCB_LAUNCH(k, dim3(a.blk_off[a.d.nlevels]), dim3(NT), sm, st, a);
     return check_launch("photo_bwd");
+}
+
+// full forward <SAVE, GMASK> = <true, true> (also without a mask); the mask needs no gradient <true, false>;
+// value-only <false, false>
+template <int MODE>
+static int launch_fwd_saving(const PhotoArgs& a, bool ss, bool save, bool gmask, cudaStream_t st) {
+    if (!save) return ss ? launch_fwd<MODE, true, false, false>(a, st) : launch_fwd<MODE, false, false, false>(a, st);
+    if (!gmask) return ss ? launch_fwd<MODE, true, true, false>(a, st) : launch_fwd<MODE, false, true, false>(a, st);
+    return ss ? launch_fwd<MODE, true>(a, st) : launch_fwd<MODE, false>(a, st);
+}
+template <int MODE>
+static int launch_bwd_masking(const PhotoArgs& a, bool ss, bool gmask, cudaStream_t st) {
+    if (!gmask) return ss ? launch_bwd<MODE, true, false>(a, st) : launch_bwd<MODE, false, false>(a, st);
+    return ss ? launch_bwd<MODE, true, true>(a, st) : launch_bwd<MODE, false, true>(a, st);
 }
 
 }  // namespace ccb
@@ -510,7 +528,18 @@ extern "C" long long ccb_photo_pose_partials_floats(const ccb_photo_desc* d) {
     return (long long)a.blk_off[d->nlevels] * d->R * 12;
 }
 
+// Which saved-for-backward maps a call uses.  Forward: vo NULL = value-only (dmaps / gmask NULL too); gmask NULL with a
+// mask = the mask needs no gradient.  Backward: d_mask NULL with a mask = no mask gradient (gmask unused).
+struct SaveFlags { bool save, gmask; };
+static SaveFlags save_flags(const ccb_photo_desc* d, bool bwd) {
+    if (d->mode == CCB_PHOTO_CONSENSUS) return {true, true};
+    if (bwd) return {true, d->has_mask && d->d_mask[0] != nullptr};
+    const bool save = d->vo[0] != nullptr;
+    return {save, save && d->has_mask && d->gmask[0] != nullptr};
+}
+
 static int check_common(const ccb_photo_desc* d, bool bwd) {
+    const SaveFlags sf = save_flags(d, bwd);
     for (int l = 0; l < d->nlevels; ++l) {
         CCB_REQUIRE(d->tgt[l] != nullptr, CCB_ERR_ARG, "photo: tgt[%d] is null", l);
         for (int i = 0; i < d->R; ++i) {
@@ -519,10 +548,13 @@ static int check_common(const ccb_photo_desc* d, bool bwd) {
         }
         if (d->mode == CCB_PHOTO_RIGID) CCB_REQUIRE(d->depth[l] != nullptr, CCB_ERR_ARG, "photo: depth[%d] is null", l);
         if (d->has_mask) CCB_REQUIRE(d->mask[l] != nullptr, CCB_ERR_ARG, "photo: mask[%d] is null", l);
-        if (d->mode != CCB_PHOTO_CONSENSUS) {
+        if (d->mode != CCB_PHOTO_CONSENSUS && sf.save) {
             CCB_REQUIRE(d->vo[l] != nullptr, CCB_ERR_ARG, "photo: vo[%d] is null", l);
             if (d->wssim != 0.f) CCB_REQUIRE(d->dmaps[l] != nullptr, CCB_ERR_ARG, "photo: dmaps[%d] is null", l);
-            if (d->has_mask) CCB_REQUIRE(d->gmask[l] != nullptr, CCB_ERR_ARG, "photo: gmask[%d] is null", l);
+            if (sf.gmask) CCB_REQUIRE(d->gmask[l] != nullptr, CCB_ERR_ARG, "photo: gmask[%d] is null", l);
+        } else if (d->mode != CCB_PHOTO_CONSENSUS) {
+            CCB_REQUIRE(d->vo[l] == nullptr && d->dmaps[l] == nullptr && d->gmask[l] == nullptr, CCB_ERR_ARG,
+                        "photo: value-only forward (vo[0] null) with saved maps at level %d", l);
         }
     }
     if (d->mode == CCB_PHOTO_RIGID) {
@@ -546,8 +578,10 @@ extern "C" int ccb_photo_loss_fwd(const ccb_photo_desc* d, ccb_stream_t stream) 
     CCB_REQUIRE(d->partials && d->scal && d->loss, CCB_ERR_ARG, "photo_loss_fwd: partials/scal/loss null");
     cudaStream_t st = (cudaStream_t)stream;
     const bool ss = d->wssim != 0.f;
-    if (d->mode == CCB_PHOTO_RIGID) rc = ss ? launch_fwd<CCB_PHOTO_RIGID, true>(a, st) : launch_fwd<CCB_PHOTO_RIGID, false>(a, st);
-    else rc = ss ? launch_fwd<CCB_PHOTO_FLOW, true>(a, st) : launch_fwd<CCB_PHOTO_FLOW, false>(a, st);
+    const SaveFlags sf = save_flags(d, false);
+    const bool gm = sf.gmask || !d->has_mask;
+    if (d->mode == CCB_PHOTO_RIGID) rc = launch_fwd_saving<CCB_PHOTO_RIGID>(a, ss, sf.save, gm, st);
+    else rc = launch_fwd_saving<CCB_PHOTO_FLOW>(a, ss, sf.save, gm, st);
     if (rc) return rc;
     CCB_LAUNCH(photo_fwd_finalize, dim3(1), dim3(1024), 0, st, a);
     return check_launch("photo_fwd_finalize");
@@ -561,22 +595,23 @@ extern "C" int ccb_photo_loss_bwd(const ccb_photo_desc* d, ccb_stream_t stream) 
     rc = check_common(d, true);
     if (rc) return rc;
     CCB_REQUIRE(d->grad_out && d->scal, CCB_ERR_ARG, "photo_loss_bwd: grad_out/scal null");
+    const SaveFlags sf = save_flags(d, true);
     for (int l = 0; l < d->nlevels; ++l) {
         if (d->mode == CCB_PHOTO_RIGID) CCB_REQUIRE(d->d_depth[l] != nullptr, CCB_ERR_ARG, "photo_loss_bwd: d_depth[%d] null", l);
         else for (int i = 0; i < d->R; ++i) CCB_REQUIRE(d->d_flow[l][i] != nullptr, CCB_ERR_ARG, "photo_loss_bwd: d_flow[%d][%d] null", l, i);
-        if (d->has_mask) CCB_REQUIRE(d->d_mask[l] != nullptr, CCB_ERR_ARG, "photo_loss_bwd: d_mask[%d] null", l);
+        if (sf.gmask) CCB_REQUIRE(d->d_mask[l] != nullptr, CCB_ERR_ARG, "photo_loss_bwd: d_mask[%d] null", l);
     }
     cudaStream_t st = (cudaStream_t)stream;
     const bool ss = d->wssim != 0.f;
     if (d->mode == CCB_PHOTO_RIGID) {
         CCB_REQUIRE(d->d_pose && d->pose_partials, CCB_ERR_ARG, "photo_loss_bwd: d_pose/pose_partials null");
-        rc = ss ? launch_bwd<CCB_PHOTO_RIGID, true>(a, st) : launch_bwd<CCB_PHOTO_RIGID, false>(a, st);
+        rc = launch_bwd_masking<CCB_PHOTO_RIGID>(a, ss, sf.gmask || !d->has_mask, st);
         if (rc) return rc;
         int nw = d->B * d->R;
         CCB_LAUNCH(photo_pose_finalize, dim3(cdiv(nw * 32, 128)), dim3(128), 0, st, a);
         return check_launch("photo_pose_finalize");
     }
-    return ss ? launch_bwd<CCB_PHOTO_FLOW, true>(a, st) : launch_bwd<CCB_PHOTO_FLOW, false>(a, st);
+    return launch_bwd_masking<CCB_PHOTO_FLOW>(a, ss, sf.gmask || !d->has_mask, st);
 }
 
 extern "C" int ccb_consensus_targets(const ccb_photo_desc* d, ccb_stream_t stream) {

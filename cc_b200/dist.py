@@ -135,8 +135,11 @@ class GradBuckets:
             if id(p) not in seen and not getattr(p, '_ccb_indirect', False):
                 seen.add(id(p))
                 done.append(p)
-        rest = [p for p in opt.params if id(p) not in seen]           # no direct gradient (unused / torch-accumulated): tail
-        opt.relayout(done + rest)
+        fixed = {id(p) for p in opt.params if opt.group_of[id(p)] in opt.frozen}    # frozen groups: never exchanged
+        done = [p for p in done if id(p) not in fixed]
+        rest = [p for p in opt.params if id(p) not in seen and id(p) not in fixed]  # no direct gradient (unused /
+        opt.relayout(done + rest + [p for p in opt.params if id(p) in fixed])       # torch-accumulated): tail
+        end = sum(p.numel() for p in done + rest)                                    # the fixed parameters follow
         self.buckets = []
         lo, cnt, cur = 0, 0, 0
         for p in done:
@@ -148,7 +151,7 @@ class GradBuckets:
         if cnt:
             self.buckets.append(_Bucket(self, lo, cur, cnt))
             lo = cur
-        self.tail = (lo, opt.numel) if lo < opt.numel else None     # reduced in finish(): zero or late gradients
+        self.tail = (lo, end) if lo < end else None                 # reduced in finish(): zero or late gradients
         bi = 0
         for p in opt.params:
             p._ccb_bucket = None
@@ -179,8 +182,11 @@ class GradBuckets:
             return
         opt = self.opt
         if self.learning:
-            if self.world > 1:
+            if self.world > 1 and not opt.frozen:
                 dist.all_reduce(opt.flat_g, op=dist.ReduceOp.SUM)
+            elif self.world > 1:
+                for off, k, _ in opt.ranges():          # the ranges Adam updates: frozen groups are not exchanged
+                    dist.all_reduce(opt.flat_g[off:off + k], op=dist.ReduceOp.SUM)
             self.plan()
             return
         for b in self.buckets:

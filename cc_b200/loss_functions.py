@@ -74,11 +74,14 @@ class _PhotoLoss(torch.autograd.Function):
                     d.flow[l][i] = _lib.ptr(flows[l * R + i], 'flow')
         if masks is not None:
             _set_levels(d.mask, masks, 'mask')
+        # saved-for-backward maps only where a backward will read them: none for a value-only call, no gmask when the
+        # mask needs no gradient (the loss value is the same either way)
+        save, mask_grad = cfg.get('save', True), cfg.get('mask_grad', cfg['has_mask'])
         use_ssim = cfg['wssim'] != 0
-        dm = [torch.empty(B, R, 9, h, w, device=dev) for (h, w) in sizes] if use_ssim else []
-        vo = [torch.empty(B, R, h, w, device=dev) for (h, w) in sizes]
-        gm = [torch.empty(B, R, h, w, device=dev) for (h, w) in sizes] if cfg['has_mask'] else []
-        if use_ssim:
+        dm = [torch.empty(B, R, 9, h, w, device=dev) for (h, w) in sizes] if (use_ssim and save) else []
+        vo = [torch.empty(B, R, h, w, device=dev) for (h, w) in sizes] if save else []
+        gm = [torch.empty(B, R, h, w, device=dev) for (h, w) in sizes] if (mask_grad and save) else []
+        if dm:
             _set_levels(d.dmaps, dm, 'dmaps')
         _set_levels(d.vo, vo, 'vo')
         if gm:
@@ -117,12 +120,23 @@ class _PhotoLoss(torch.autograd.Function):
                 for i in range(R):
                     d.d_flow[l][i] = _lib.ptr(d_flow[l * R + i])
             grads = d_flow
-        if cfg['has_mask']:
+        if cfg['has_mask'] and cfg.get('mask_grad', True):
             d_mask = [torch.empty(B, R, h, w, device=dev) for (h, w) in sizes]
             _set_levels(d.d_mask, d_mask, 'd_mask')
             grads = grads + d_mask
+        elif cfg['has_mask']:
+            grads = grads + [None] * L
         _lib.check(lib.ccb_photo_loss_bwd(C.byref(d), _lib.stream(g)), 'photo_loss_bwd')
         return (None,) + tuple(grads)
+
+
+def _photo_apply(cfg, args, masks):
+    """_PhotoLoss on `args`, told whether autograd will call its backward (grad mode on and an input that requires a
+    gradient) and whether the masks need a gradient (a fixed MaskNet's output does not)."""
+    grad = torch.is_grad_enabled()
+    cfg['save'] = grad and any(t.requires_grad for t in args)
+    cfg['mask_grad'] = cfg['save'] and cfg['has_mask'] and any(m.requires_grad for m in masks)
+    return _PhotoLoss.apply(cfg, *args)
 
 
 def _level_sizes(preds):
@@ -152,7 +166,7 @@ def photometric_reconstruction_loss(tgt_img, ref_imgs, intrinsics, intrinsics_in
                lambda_oob=float(lambda_oob), K=intrinsics, Kinv=intrinsics_inv,
                tgt=pyramid.levels_for(tgt_img, sizes), refs=[pyramid.levels_for(r, sizes) for r in ref_imgs])
     args = [pose] + list(depth) + (list(masks) if has_mask else [])
-    return _PhotoLoss.apply(cfg, *args)
+    return _photo_apply(cfg, args, masks if has_mask else [])
 
 
 def photometric_flow_loss(tgt_img, ref_imgs, flows, explainability_mask, lambda_oob=0, qch=0.5, wssim=0.5):
@@ -175,7 +189,7 @@ def photometric_flow_loss(tgt_img, ref_imgs, flows, explainability_mask, lambda_
                sizes=sizes, has_mask=has_mask, wssim=float(wssim), qch=float(qch), lambda_oob=float(lambda_oob),
                tgt=pyramid.levels_for(tgt_img, sizes), refs=[pyramid.levels_for(r, sizes) for r in ref_imgs])
     args = [flows[i][l] for l in range(L) for i in range(R)] + (list(masks) if has_mask else [])
-    return _PhotoLoss.apply(cfg, *args)
+    return _photo_apply(cfg, args, masks if has_mask else [])
 
 
 def consensus_exp_masks(cam_flows_fwd, cam_flows_bwd, flows_fwd, flows_bwd, tgt_img, ref_img_fwd, ref_img_bwd,

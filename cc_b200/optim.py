@@ -10,13 +10,21 @@ buffer (cc_b200/dist.py).
 The order of the parameters inside the flat buffers is an internal detail (`relayout()` re-packs them in
 gradient-completion order so that the data-parallel buckets are contiguous); checkpoints therefore use
 torch.optim.Adam's own per-parameter `state_dict()` format, indexed by the order of the `params` argument
-(= the reference's chain(disp, pose, mask, flow) order, train.py:307-310), and load either way."""
+(= the reference's chain(disp, pose, mask, flow) order, train.py:307-310), and load either way.
+
+Step groups (`groups=`, one per network) give each network its own step counter, as torch.optim.Adam's per-parameter
+counts do when a network is fixed for a phase of training (train.py --fix-*: requires_grad = False, so Adam skips it).
+`freeze()` names the groups the step skips: their parameters, moments and counters are not touched.  The step is then
+one `ccb_adam_step_ranges` launch over the maximal runs of active groups in the current flat layout; the device range
+table is rebuilt when the layout or the frozen set changes, never per step."""
 import torch
 from . import _lib
 
+ADAM_BLOCK = 256            # elements per block of the Adam kernel (misc_ops.cu)
+
 
 class FlatAdam:
-    def __init__(self, params, lr=2e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0):
+    def __init__(self, params, lr=2e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, groups=None):
         if weight_decay != 0:
             raise NotImplementedError('cc_b200.FlatAdam: weight_decay is 0 in the reference command line')
         self.params = [p for p in params if p.requires_grad]     # constructor order: the checkpoint index
@@ -25,7 +33,19 @@ class FlatAdam:
         self.numel = sum(p.numel() for p in self.params)
         self.grad_scale = 1.0
         self.flat_p = self.flat_g = self.exp_avg = self.exp_avg_sq = None
-        self.state = torch.zeros(4, device=self.params[0].device, dtype=torch.float32)   # step, 1-b1^t, sqrt(1-b2^t)
+        if groups is None:
+            self.groups = [list(self.params)]
+        else:
+            mine = {id(p) for p in self.params}
+            self.groups = [[p for p in g if id(p) in mine] for g in groups]
+            seen = [id(p) for g in self.groups for p in g]
+            if len(seen) != len(set(seen)) or set(seen) != mine:
+                raise ValueError('FlatAdam: groups must partition the parameters')
+        self.group_of = {id(p): gi for gi, g in enumerate(self.groups) for p in g}
+        self.frozen = frozenset()
+        dev = self.params[0].device
+        # group g: state[4g:4g+4] = step, 1-b1^t, sqrt(1-b2^t), unused
+        self.state = torch.zeros(4 * len(self.groups), device=dev, dtype=torch.float32)
         self._pack(list(self.params), None)
 
     # ---- flat layout -------------------------------------------------------------------------------
@@ -56,6 +76,7 @@ class FlatAdam:
                 off += k
         self.order = list(order)
         self.flat_p, self.flat_g, self.exp_avg, self.exp_avg_sq = flat_p, flat_g, exp_avg, exp_avg_sq
+        self._build_ranges()
 
     def _views(self, buf, p):
         off, k = self.offset[p]
@@ -68,6 +89,43 @@ class FlatAdam:
         old = {p: (self._views(self.exp_avg, p).clone(), self._views(self.exp_avg_sq, p).clone(),
                    self._views(self.flat_g, p).clone()) for p in self.params}
         self._pack(list(order), old)
+
+    # ---- step groups ---------------------------------------------------------------------------------
+    def freeze(self, group_indices):
+        """Set the groups step() skips (replacing the previous set).  Rebuilds the device range table: call it between
+        steps, not inside a CUDA-graph capture."""
+        frozen = frozenset(int(g) for g in group_indices)
+        if not all(0 <= g < len(self.groups) for g in frozen):
+            raise ValueError('FlatAdam.freeze: group indices %s out of range 0..%d' % (sorted(frozen), len(self.groups) - 1))
+        if frozen != self.frozen:
+            self.frozen = frozen
+            self._build_ranges()
+
+    def ranges(self):
+        """[(offset, count, group)]: the maximal runs of one active group in the current flat layout."""
+        runs = []
+        for p in self.order:
+            gi = self.group_of[id(p)]
+            if gi in self.frozen:
+                continue
+            off, k = self.offset[p]
+            if runs and runs[-1][2] == gi and runs[-1][0] + runs[-1][1] == off:
+                runs[-1][1] += k
+            else:
+                runs.append([off, k, gi])
+        return [tuple(r) for r in runs]
+
+    def _build_ranges(self):
+        """Device tables of ccb_adam_step_ranges: {offset, count, group, first_block} per range, active flag per group."""
+        dev = self.flat_p.device
+        table, nb = [], 0
+        for off, k, gi in self.ranges():
+            table += [off, k, gi, nb]
+            nb += (k + ADAM_BLOCK - 1) // ADAM_BLOCK
+        self._nranges, self._nblocks = len(table) // 4, nb
+        self._range_table = torch.tensor(table or [0, 0, 0, 0], dtype=torch.int64).to(dev)
+        self._active = torch.tensor([0 if g in self.frozen else 1 for g in range(len(self.groups))],
+                                    dtype=torch.int32).to(dev)
 
     # ---- step ----------------------------------------------------------------------------------------
     def zero_grad(self, set_to_none=False):
@@ -87,17 +145,30 @@ class FlatAdam:
             if g is not None and g.data_ptr() != p._ccb_grad.data_ptr():
                 p._ccb_grad.add_(g)
                 p.grad = p._ccb_grad
-        _lib.check(_lib.lib().ccb_adam_step(_lib.ptr(self.flat_p), _lib.ptr(self.flat_g), _lib.ptr(self.exp_avg),
-                                            _lib.ptr(self.exp_avg_sq), self.numel, _lib.ptr(self.state), self.lr,
-                                            self.betas[0], self.betas[1], self.eps, self.grad_scale,
-                                            _lib.stream(self.flat_p)), 'adam_step')
+        lib = _lib.lib()
+        if len(self.groups) == 1 and not self.frozen:
+            _lib.check(lib.ccb_adam_step(_lib.ptr(self.flat_p), _lib.ptr(self.flat_g), _lib.ptr(self.exp_avg),
+                                         _lib.ptr(self.exp_avg_sq), self.numel, _lib.ptr(self.state), self.lr,
+                                         self.betas[0], self.betas[1], self.eps, self.grad_scale,
+                                         _lib.stream(self.flat_p)), 'adam_step')
+            return
+        _lib.check(lib.ccb_adam_step_ranges(_lib.ptr(self.flat_p), _lib.ptr(self.flat_g), _lib.ptr(self.exp_avg),
+                                            _lib.ptr(self.exp_avg_sq), _lib.ptr(self._range_table, 'ranges', torch.int64),
+                                            self._nranges, self._nblocks, _lib.ptr(self._active, 'group_active', torch.int32),
+                                            len(self.groups), _lib.ptr(self.state), self.lr, self.betas[0], self.betas[1],
+                                            self.eps, self.grad_scale, _lib.stream(self.flat_p)), 'adam_step_ranges')
+
+    def group_steps(self):
+        """Step count of every group (host copy)."""
+        return [int(x) for x in self.state.view(-1, 4)[:, 0].tolist()]
 
     # ---- checkpoint: torch.optim.Adam's state_dict format (reference utils.py:55-63 saves optimizer.state_dict()) ----
     def state_dict(self):
-        step = torch.tensor(float(self.state[0].item()))
+        steps = self.state.view(-1, 4)[:, 0].cpu()
         state = {}
-        if float(step) > 0:
-            for i, p in enumerate(self.params):
+        for i, p in enumerate(self.params):
+            step = steps[self.group_of[id(p)]]
+            if float(step) > 0:                # a group that never stepped has no state, as in torch
                 state[i] = {'step': step.clone(), 'exp_avg': self._views(self.exp_avg, p).detach().clone(),
                             'exp_avg_sq': self._views(self.exp_avg_sq, p).detach().clone()}
         group = {'lr': self.lr, 'betas': tuple(self.betas), 'eps': self.eps, 'weight_decay': 0, 'amsgrad': False,
@@ -106,16 +177,17 @@ class FlatAdam:
         return {'state': state, 'param_groups': [group]}
 
     def load_state_dict(self, sd):
+        """A group's counter is the largest step among its parameters that have state (0 when none has)."""
+        steps = [0.0] * len(self.groups)
         if 'flat' in sd:                       # round-1 format of this class
             assert self.order == self.params, 'flat optimizer checkpoints predate relayout()'
             self.exp_avg.copy_(sd['exp_avg'])
             self.exp_avg_sq.copy_(sd['exp_avg_sq'])
-            step, g = sd['step'], sd
+            steps, g = [float(sd['step'])] * len(self.groups), sd
         else:
             g = sd['param_groups'][0]
             assert len(g['params']) == len(self.params), 'optimizer checkpoint has %d parameters, this model %d' % (
                 len(g['params']), len(self.params))
-            step = 0.0
             with torch.no_grad():
                 for i, p in enumerate(self.params):
                     st = sd['state'].get(g['params'][i])
@@ -125,9 +197,10 @@ class FlatAdam:
                     else:
                         self._views(self.exp_avg, p).copy_(st['exp_avg'])
                         self._views(self.exp_avg_sq, p).copy_(st['exp_avg_sq'])
-                        step = max(step, float(st['step']))
+                        gi = self.group_of[id(p)]
+                        steps[gi] = max(steps[gi], float(st['step']))
         self.state.zero_()
-        self.state[0] = float(step)
+        self.state.view(-1, 4)[:, 0] = torch.tensor(steps, dtype=torch.float32)
         self.lr, self.betas, self.eps = g['lr'], tuple(g['betas']), g['eps']
 
     # ---- snapshot / restore (Trainer.capture warms up on real steps and must not train) --------------------------

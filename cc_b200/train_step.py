@@ -109,19 +109,53 @@ LOSS_FNS = {'cfg1': loss_cfg1, 'cfg2': loss_cfg2, 'cfg3': loss_cfg3}
 
 class Trainer:
     """Nets + one flat Adam + (optionally) one NCCL gradient all-reduce; `step()` is
-    optimizer.zero_grad(); loss.backward(); optimizer.step() of train.py:566-568."""
+    optimizer.zero_grad(); loss.backward(); optimizer.step() of train.py:566-568.
 
-    def __init__(self, cfg, device, hp=HP, state_dicts=None, seed=0, flownet='Back2Future'):
+    `fixed` names nets of the configuration that are not trained, as the reference's --fix-dispnet / --fix-posenet /
+    --fix-masknet / --fix-flownet (train.py:332-346): their parameters get requires_grad = False, so no gradient reaches
+    them, and their Adam group keeps its step count.  They stay in train mode (a fixed DispResNet6 still updates its
+    BatchNorm running statistics, train.py:438-441).  The README's command is Trainer('cfg3', dev, fixed=('mask', 'flow'))."""
+
+    def __init__(self, cfg, device, hp=HP, state_dicts=None, seed=0, flownet='Back2Future', fixed=()):
         self.cfg, self.hp, self.device, self.flownet = cfg, dict(hp), device, flownet
         self.nets = build_nets(cfg, device, state_dicts, seed, flownet)
-        params = [p for n in NETS_OF[cfg] for p in self.nets[n].parameters()]
-        self.opt = FlatAdam(params, lr=hp['lr'], betas=(hp['beta1'], hp['beta2']))
+        # one Adam group per net, in the reference's chain(disp, pose, mask, flow) order (train.py:307)
+        groups = [list(self.nets[n].parameters()) for n in NETS_OF[cfg]]
+        self.opt = FlatAdam([p for g in groups for p in g], lr=hp['lr'], betas=(hp['beta1'], hp['beta2']), groups=groups)
         cdist.broadcast_params(self.opt)
         self.buckets = cdist.GradBuckets(self.opt)          # overlapped gradient exchange (no-op at world size 1)
         self.graph = None
+        self.fixed = ()
         # prepared conv weights are refreshed once per optimiser step (one launch), not once per conv call
         from . import nn as cnn, _lib
         self.wcache = None if (_lib.is_simulator() or torch.device(device).type != 'cuda') else cnn.WeightCache(torch.device(device))
+        self.set_fixed(fixed)
+
+    def set_fixed(self, fixed):
+        """Change the set of fixed nets (between epochs or phases of training).  Drops any captured graph and the learned
+        gradient buckets (re-learned on the next step)."""
+        names = NETS_OF[self.cfg]
+        want = (fixed,) if isinstance(fixed, str) else tuple(fixed)
+        bad = [n for n in want if n not in names]
+        if bad:
+            raise ValueError('fixed nets %s are not nets of %s %s' % (bad, self.cfg, names))
+        fixed = tuple(n for n in names if n in want)
+        if len(fixed) == len(names):
+            raise ValueError('every net of %s is fixed: there is nothing to train' % self.cfg)
+        for n, group in zip(names, self.opt.groups):
+            for p in group:
+                p.requires_grad_(n not in fixed)
+        self.opt.freeze([i for i, n in enumerate(names) if n in fixed])
+        if fixed != self.fixed:
+            self.graph = None
+            if self.buckets.enabled and self.buckets.buckets is not None:
+                # the next step re-learns the buckets and re-packs the flat buffers; the weight cache keys its copies by
+                # parameter address, so it records its layouts again after that
+                self.buckets.buckets = None
+                if self.wcache is not None:
+                    from . import nn as cnn
+                    self.wcache = cnn.WeightCache(self.wcache.device)
+        self.fixed = fixed
 
     def refresh_weights(self):
         """Call after changing parameters behind the trainer's back (load_state_dict, manual edits)."""
@@ -186,7 +220,7 @@ class Trainer:
         self._restore(snap)
         pyramid.clear()
         cnn.GRAPH_LIVE = True                                # conv workspaces referenced by the graph are never freed
-        self._captured = dict(lr=self.opt.lr, grad_scale=self.opt.grad_scale)
+        self._captured = dict(lr=self.opt.lr, grad_scale=self.opt.grad_scale, fixed=self.fixed)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.static_loss, _ = self.step(tgt, refs, K, Kinv)
@@ -198,6 +232,9 @@ class Trainer:
         # lr and grad_scale are kernel arguments baked into the graph: refuse to replay a stale one
         assert self.opt.lr == self._captured['lr'] and self.opt.grad_scale == self._captured['grad_scale'], \
             'learning rate / world size changed after capture(): re-capture the step'
+        # the fixed set decides which gradients and Adam ranges the graph computes (set_fixed() drops the graph)
+        assert self.graph is not None and self.fixed == self._captured['fixed'], \
+            'the fixed nets changed after capture(): re-capture the step'
         self.graph.replay()
         return self.static_loss
 

@@ -86,7 +86,9 @@ typedef struct ccb_photo_desc {
     const float* pose;                                /* rigid: [B,R,6] */
     const float* K;                                   /* rigid: [B,3,3] full-res intrinsics */
     const float* Kinv;                                /* rigid: [B,3,3] */
-    /* saved for backward (written by fwd, read by bwd) */
+    /* saved for backward (written by fwd, read by bwd).  Forward with vo[0] == NULL: value-only (no backward will run;
+     * dmaps / vo / gmask all NULL, none written).  gmask[0] == NULL with has_mask: the mask needs no gradient (not
+     * computed); then the backward takes d_mask == NULL.  The loss value is the same in every case. */
     float* dmaps[CCB_MAX_LEVELS];    /* [B,R,9,h,w] gamma * dS/d(mu2,Eyy,Exy); unused when wssim == 0 */
     float* gmask[CCB_MAX_LEVELS];    /* [B,R,h,w]  unscaled d loss / d mask (has_mask only) */
     float* vo[CCB_MAX_LEVELS];       /* [B,R,h,w]  valid * (1 - occ) */
@@ -295,6 +297,17 @@ int ccb_upsample2x_bwd(const float* dy, float* dx, int planes, int h, int w, ccb
 int ccb_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
                   float* state, float lr, float beta1, float beta2, float eps, float grad_scale,
                   ccb_stream_t stream);
+/* The same Adam over listed ranges of the flat buffers, each range belonging to one parameter group with its own
+ * step counter (torch.optim.Adam keeps one per parameter; a network that is fixed for a phase of training, train.py
+ * --fix-*, keeps its count).  ranges: device table of nranges entries {offset, count, group, first_block}, where
+ * first_block is the number of 256-element blocks of the entries before it; nblocks is that number over all entries.
+ * Elements outside the listed ranges are neither read nor written.  group_state: 4*ngroups device floats, group g at
+ * [4g, 4g+4) laid out as ccb_adam_step's state; group_active: ngroups device ints, the prep step advances the counter
+ * and bias corrections of the groups that are non-zero there (NULL: all).  ccb_adam_step is the call with one range
+ * {0, n, 0, 0} and one active group. */
+int ccb_adam_step_ranges(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const long long* ranges,
+                         int nranges, long long nblocks, const int* group_active, int ngroups, float* group_state,
+                         float lr, float beta1, float beta2, float eps, float grad_scale, ccb_stream_t stream);
 /* ---- callers either side of the step (SURVEY.md 8f N2 / N1) -------------------------------------------------------
  * Validation metrics, reference loss_functions.py:355-467, as fused masked reductions (deterministic, no host sync).
  * ccb_flow_metrics: gt [B,nc,Hg,Wg] (nc 3: third channel = valid mask; nc 2: plain mean), predictions [B,2,hp,wp]
