@@ -133,6 +133,12 @@ _SIGS = {
     'ccb_depth_errors_workspace_bytes': (_LL, [_I, _I, _I]),
     'ccb_depth_errors': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     'ccb_prep_frames': (_I, [_P, C.POINTER(_P), _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    'ccb_prep_frames_unit': (_I, [_P, C.POINTER(_P), _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    'ccb_rotate_frames_u8': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    'ccb_resize_u8_workspace_bytes': (_LL, [_I, _I, _I, _I, _I]),
+    'ccb_resize_u8': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _LL, _P]),
+    'ccb_normalize_local_workspace_bytes': (_LL, [_I, _I, _I]),
+    'ccb_normalize_local': (_I, [C.POINTER(_P), _I, _I, _I, _I, _P, _P, _LL, _P]),
 }
 # entry points added by later translation units register themselves here (conv, nets, optimiser ...)
 EXTRA_SIGS = {}

@@ -7,9 +7,21 @@
 //       augmentations (ArrayToTensor /255, Normalize mean .5 std .5, RandomHorizontalFlip, RandomScaleCrop;
 //       custom_transforms.py:21-30,47-118) applied per sample from host-drawn parameters, plus the matching
 //       intrinsics update.  H2D traffic drops 4x (uint8 instead of fp32).
+//       The reference's other transforms, bit-exact with Pillow (behind scipy.misc.imrotate / imresize):
+//       RandomRotate (:75-85) as Pillow's bilinear affine transform, Scale (:120-137) as Pillow's 8-bit resampler,
+//       NormalizeLocally (:33-44) as per-sample channel statistics.
 //
 // All reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize).
 #include "ccb_common.cuh"
+
+#ifdef CCB_CPU_SIM
+// The fp64 round-to-nearest intrinsics the Pillow restatements below use, for the host build of this file: one IEEE
+// operation each, kept apart by the volatile store so that the host compiler cannot fuse them either.
+static inline double __dadd_rn(double a, double b) { volatile double r = a + b; return r; }
+static inline double __dsub_rn(double a, double b) { volatile double r = a - b; return r; }
+static inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
+static inline double __ddiv_rn(double a, double b) { volatile double r = a / b; return r; }
+#endif
 
 namespace ccb {
 
@@ -307,6 +319,8 @@ struct PrepArgs {
     int B, F, Hs, Ws, H, W;
 };
 
+// UNIT: ArrayToTensor alone (v / 255), for NormalizeLocally to follow; otherwise Normalize(.5, .5) as well.
+template <bool UNIT>
 __global__ void __launch_bounds__(256) prep_frames_kernel(const PrepArgs a) {
     CCB_PDL_WAIT();
     const long long n = (long long)a.B * a.F * a.H * a.W;
@@ -332,8 +346,207 @@ __global__ void __launch_bounds__(256) prep_frames_kernel(const PrepArgs a) {
             const float v00 = (float)s[((long long)y0 * a.Ws + xa) * 3 + c], v01 = (float)s[((long long)y0 * a.Ws + xb) * 3 + c];
             const float v10 = (float)s[((long long)y1 * a.Ws + xa) * 3 + c], v11 = (float)s[((long long)y1 * a.Ws + xb) * 3 + c];
             const float v = (1.f - wy) * ((1.f - wx) * v00 + wx * v01) + wy * ((1.f - wx) * v10 + wx * v11);
-            d[(long long)c * a.H * a.W] = (v / 255.f - 0.5f) / 0.5f;
+            d[(long long)c * a.H * a.W] = UNIT ? v / 255.f : (v / 255.f - 0.5f) / 0.5f;
         }
+    }
+}
+
+// ================================================================================================
+// RandomRotate (custom_transforms.py:75-85) = scipy.misc.imrotate = Pillow Image.rotate(angle, BILINEAR), restated from
+// Pillow's ImagingGenericTransform with affine_transform and bilinear_filter32RGB.  affine [B][6] maps an output pixel
+// centre to an input point (the host builds it as Pillow does, with cos / sin rounded to 15 decimals; the identity leaves a
+// frame unchanged).  Every operation is an explicit _rn intrinsic: Pillow's x86-64 build does not fuse multiply-adds, and
+// a fused one moves some samples across a uint8 truncation step.
+struct RotArgs {
+    const unsigned char* src;   // [B][F][H][W][3]
+    const double* affine;       // [B][6]
+    unsigned char* dst;         // [B][F][H][W][3]
+    int B, F, H, W;
+};
+
+__global__ void __launch_bounds__(256) rotate_frames_kernel(const RotArgs a) {
+    CCB_PDL_WAIT();
+    const long long n = (long long)a.B * a.F * a.H * a.W;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const int x = (int)(i % a.W);
+        const int y = (int)((i / a.W) % a.H);
+        const long long bf = i / ((long long)a.W * a.H);
+        const double* m = a.affine + (bf / a.F) * 6;
+        const double xo = (double)x + 0.5, yo = (double)y + 0.5;
+        double xin = __dadd_rn(__dadd_rn(__dmul_rn(__ldg(m + 0), xo), __dmul_rn(__ldg(m + 1), yo)), __ldg(m + 2));
+        double yin = __dadd_rn(__dadd_rn(__dmul_rn(__ldg(m + 3), xo), __dmul_rn(__ldg(m + 4), yo)), __ldg(m + 5));
+        unsigned char* d = a.dst + i * 3;
+        if (xin < 0.0 || xin >= (double)a.W || yin < 0.0 || yin >= (double)a.H) {   // outside: the fill colour 0
+            d[0] = 0; d[1] = 0; d[2] = 0;
+            continue;
+        }
+        xin = __dsub_rn(xin, 0.5);
+        yin = __dsub_rn(yin, 0.5);
+        const int xf = (int)floor(xin), yf = (int)floor(yin);
+        const double dx = __dsub_rn(xin, (double)xf), dy = __dsub_rn(yin, (double)yf);
+        const int x0 = min(max(xf, 0), a.W - 1), x1 = min(max(xf + 1, 0), a.W - 1);
+        const bool row2 = (yf + 1 >= 0) && (yf + 1 < a.H);          // first row clamped; a missing second row repeats it
+        const unsigned char* r0 = a.src + (bf * a.H + min(max(yf, 0), a.H - 1)) * (long long)a.W * 3;
+        const unsigned char* r1 = row2 ? a.src + (bf * a.H + yf + 1) * (long long)a.W * 3 : r0;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const int p0 = r0[x0 * 3 + c], p1 = r0[x1 * 3 + c];
+            const double v1 = __dadd_rn((double)p0, __dmul_rn((double)(p1 - p0), dx));
+            double v2 = v1;
+            if (row2) {
+                const int q0 = r1[x0 * 3 + c], q1 = r1[x1 * 3 + c];
+                v2 = __dadd_rn((double)q0, __dmul_rn((double)(q1 - q0), dx));
+            }
+            d[c] = (unsigned char)(int)__dadd_rn(v1, __dmul_rn(__dsub_rn(v2, v1), dy));   // truncated, as Pillow's (UINT8) cast
+        }
+    }
+}
+
+// ================================================================================================
+// Scale (custom_transforms.py:120-137) / RandomScaleCrop's resize = scipy.misc.imresize = Pillow resize(BILINEAR):
+// ImagingResample with 8-bit precision.  Per axis, output index i takes input samples [xmin, xmin + cnt) with the
+// triangle filter widened by the scale factor on a downscale (antialiasing), normalised, in 22-bit fixed point
+// (precompute_coeffs / normalize_coeffs_8bpc).  The horizontal pass runs first and is rounded back to uint8; a pass whose
+// size does not change is skipped.
+constexpr int RESAMPLE_BITS = 22;
+
+struct CoeffArgs {
+    int in_x, out_x, ks_x, in_y, out_y, ks_y;
+    int* kk_x; int* bounds_x;     // [out_x][ks_x] weights, [out_x][2] = {xmin, count}
+    int* kk_y; int* bounds_y;
+};
+
+__device__ __forceinline__ double tri_filter(double t) {
+    if (t < 0.0) t = -t;
+    return (t < 1.0) ? __dsub_rn(1.0, t) : 0.0;
+}
+
+// one thread per output index of either axis (threads [0, out_x) the horizontal one), fp64 in Pillow's operation order
+__global__ void resample_coeffs_kernel(const CoeffArgs a) {
+    CCB_PDL_WAIT();
+    int t = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool hx = t < a.out_x;
+    if (!hx) t -= a.out_x;
+    const int in_size = hx ? a.in_x : a.in_y, out_size = hx ? a.out_x : a.out_y, ksize = hx ? a.ks_x : a.ks_y;
+    if (t >= out_size) return;
+    int* k = (hx ? a.kk_x : a.kk_y) + (long long)t * ksize;
+    int* bounds = (hx ? a.bounds_x : a.bounds_y) + 2 * t;
+    const double scale = __ddiv_rn((double)in_size, (double)out_size);
+    const double support = scale < 1.0 ? 1.0 : scale;           // the triangle's support 1, times the filter scale
+    const double ss = __ddiv_rn(1.0, support);
+    const double center = __dmul_rn(__dadd_rn((double)t, 0.5), scale);
+    const int xmin = max((int)__dadd_rn(__dsub_rn(center, support), 0.5), 0);
+    const int cnt = min((int)__dadd_rn(__dadd_rn(center, support), 0.5), in_size) - xmin;
+    double ww = 0.0;
+    for (int x = 0; x < cnt; ++x)
+        ww = __dadd_rn(ww, tri_filter(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss)));
+    for (int x = 0; x < ksize; ++x) {
+        int q = 0;
+        if (x < cnt) {
+            double w = tri_filter(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss));
+            if (ww != 0.0) w = __ddiv_rn(w, ww);
+            q = (int)__dadd_rn(0.5, __dmul_rn(w, (double)(1 << RESAMPLE_BITS)));
+        }
+        k[x] = q;
+    }
+    bounds[0] = xmin;
+    bounds[1] = cnt;
+}
+
+// One pass over [outer][len][inner][3] uint8 along `len` (horizontal: inner 1; vertical: inner = row width).
+struct ResampleArgs {
+    const unsigned char* src;   // [outer][in_len][inner][3]
+    unsigned char* dst;         // [outer][out_len][inner][3]
+    const int* kk;              // [out_len][ksize]
+    const int* bounds;          // [out_len][2]
+    long long outer;
+    int in_len, out_len, inner, ksize;
+};
+
+__device__ __forceinline__ unsigned char clip8(int v) {
+    return (unsigned char)min(max(v >> RESAMPLE_BITS, 0), 255);
+}
+
+__global__ void __launch_bounds__(256) resample_pass_kernel(const ResampleArgs a) {
+    CCB_PDL_WAIT();
+    const long long n = a.outer * a.out_len * a.inner;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const int ii = (int)(i % a.inner);
+        const int l = (int)((i / a.inner) % a.out_len);
+        const long long o = i / ((long long)a.inner * a.out_len);
+        const int xmin = __ldg(a.bounds + 2 * l), cnt = __ldg(a.bounds + 2 * l + 1);
+        const int* k = a.kk + (long long)l * a.ksize;
+        const long long step = (long long)a.inner * 3;
+        const unsigned char* s = a.src + ((o * a.in_len + xmin) * a.inner + ii) * 3;
+        int s0 = 1 << (RESAMPLE_BITS - 1), s1 = s0, s2 = s0;
+        for (int j = 0; j < cnt; ++j) {
+            const int kj = __ldg(k + j);
+            s0 += (int)s[0] * kj;
+            s1 += (int)s[1] * kj;
+            s2 += (int)s[2] * kj;
+            s += step;
+        }
+        unsigned char* d = a.dst + i * 3;
+        d[0] = clip8(s0); d[1] = clip8(s1); d[2] = clip8(s2);
+    }
+}
+
+// ================================================================================================
+// NormalizeLocally (custom_transforms.py:33-44): per sample b and channel c, mean and unbiased std over the F frames'
+// H x W values (fp64 block partials, fixed-order finalize: the same bits on every run), rounded to fp32; then
+// x = (x - m) / s in fp32 (t.sub_(m).div_(s)).  A zero std gives inf / nan, as in the reference.
+struct NormLocalArgs {
+    float* x[8];                // F frames [B][3][H][W], normalised in place
+    double* partials;           // [B*3][nblk][2]
+    float* stats;               // [B][3][2] = {mean, std}
+    int B, F;
+    long long hw;
+};
+
+__global__ void __launch_bounds__(256) normlocal_partials_kernel(const NormLocalArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ double scratch[2 * 32];
+    const int bc = blockIdx.y;
+    double acc[2] = {0.0, 0.0};
+    for (int f = 0; f < a.F; ++f) {
+        const float* p = a.x[f] + bc * a.hw;
+        for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < a.hw; i += (long long)gridDim.x * 256) {
+            const double v = (double)__ldg(p + i);
+            acc[0] += v;
+            acc[1] += v * v;
+        }
+    }
+    block_sum_d<2>(acc, scratch);
+    if (threadIdx.x == 0) {
+        a.partials[((long long)bc * gridDim.x + blockIdx.x) * 2 + 0] = acc[0];
+        a.partials[((long long)bc * gridDim.x + blockIdx.x) * 2 + 1] = acc[1];
+    }
+}
+
+__global__ void normlocal_finalize_kernel(const NormLocalArgs a, int nblk) {
+    CCB_PDL_WAIT();
+    const int bc = blockIdx.x * blockDim.x + threadIdx.x;
+    if (bc >= a.B * 3) return;
+    double s1 = 0.0, s2 = 0.0;
+    for (int k = 0; k < nblk; ++k) {
+        s1 += a.partials[((long long)bc * nblk + k) * 2 + 0];
+        s2 += a.partials[((long long)bc * nblk + k) * 2 + 1];
+    }
+    const double n = (double)a.F * (double)a.hw;
+    const double mean = s1 / n;
+    const double var = (s2 - s1 * mean) / (n - 1.0);
+    a.stats[bc * 2 + 0] = (float)mean;
+    a.stats[bc * 2 + 1] = (float)sqrt(var);
+}
+
+__global__ void __launch_bounds__(256) normlocal_apply_kernel(const NormLocalArgs a) {
+    CCB_PDL_WAIT();
+    const int bc = blockIdx.y;
+    const float m = a.stats[bc * 2 + 0], s = a.stats[bc * 2 + 1];
+    for (int f = 0; f < a.F; ++f) {
+        float* p = a.x[f] + bc * a.hw;
+        for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < a.hw; i += (long long)gridDim.x * 256)
+            p[i] = __fdiv_rn(__fsub_rn(p[i], m), s);
     }
 }
 
@@ -408,15 +621,134 @@ extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H
     return check_launch("depth_errors");
 }
 
-extern "C" int ccb_prep_frames(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B, int F,
-                               int Hs, int Ws, int H, int W, ccb_stream_t stream) {
-    CCB_REQUIRE(src_u8 && dst && params && offs, CCB_ERR_ARG, "prep_frames: null pointer");
-    CCB_REQUIRE(F >= 1 && F <= 8, CCB_ERR_ARG, "prep_frames: 1..8 frames per sample, got %d", F);
-    CCB_REQUIRE(B > 0 && Hs > 0 && Ws > 0 && H > 0 && W > 0, CCB_ERR_ARG, "prep_frames: bad sizes");
+template <bool UNIT>
+static int prep_frames_launch(const char* what, const unsigned char* src_u8, float* const* dst, const float* params, const int* offs,
+                              int B, int F, int Hs, int Ws, int H, int W, ccb_stream_t stream) {
+    CCB_REQUIRE(src_u8 && dst && params && offs, CCB_ERR_ARG, "%s: null pointer", what);
+    CCB_REQUIRE(F >= 1 && F <= 8, CCB_ERR_ARG, "%s: 1..8 frames per sample, got %d", what, F);
+    CCB_REQUIRE(B > 0 && Hs > 0 && Ws > 0 && H > 0 && W > 0, CCB_ERR_ARG, "%s: bad sizes", what);
     PrepArgs a;
     a.src = src_u8; a.params = params; a.offs = offs; a.B = B; a.F = F; a.Hs = Hs; a.Ws = Ws; a.H = H; a.W = W;
     for (int f = 0; f < 8; ++f) a.dst[f] = (f < F) ? dst[f] : nullptr;
-    for (int f = 0; f < F; ++f) CCB_REQUIRE(a.dst[f] != nullptr, CCB_ERR_ARG, "prep_frames: dst[%d] is null", f);
-    CCB_LAUNCH(prep_frames_kernel, dim3(grid_for((long long)B * F * H * W)), dim3(256), 0, stream, a);
-    return check_launch("prep_frames");
+    for (int f = 0; f < F; ++f) CCB_REQUIRE(a.dst[f] != nullptr, CCB_ERR_ARG, "%s: dst[%d] is null", what, f);
+    CCB_LAUNCH(prep_frames_kernel<UNIT>, dim3(grid_for((long long)B * F * H * W)), dim3(256), 0, stream, a);
+    return check_launch(what);
+}
+
+extern "C" int ccb_prep_frames(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B, int F,
+                               int Hs, int Ws, int H, int W, ccb_stream_t stream) {
+    return prep_frames_launch<false>("prep_frames", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
+}
+
+extern "C" int ccb_prep_frames_unit(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B,
+                                    int F, int Hs, int Ws, int H, int W, ccb_stream_t stream) {
+    return prep_frames_launch<true>("prep_frames_unit", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
+}
+
+extern "C" int ccb_rotate_frames_u8(const unsigned char* src, const double* affine, unsigned char* dst, int B, int F, int H, int W,
+                                    ccb_stream_t stream) {
+    CCB_REQUIRE(src && affine && dst, CCB_ERR_ARG, "rotate_frames_u8: null pointer");
+    CCB_REQUIRE(src != dst, CCB_ERR_ARG, "rotate_frames_u8: cannot rotate in place");
+    CCB_REQUIRE(B > 0 && F > 0 && H > 0 && W > 0, CCB_ERR_ARG, "rotate_frames_u8: bad sizes");
+    RotArgs a;
+    a.src = src; a.affine = affine; a.dst = dst; a.B = B; a.F = F; a.H = H; a.W = W;
+    CCB_LAUNCH(rotate_frames_kernel, dim3(grid_for((long long)B * F * H * W)), dim3(256), 0, stream, a);
+    return check_launch("rotate_frames_u8");
+}
+
+// Workspace of ccb_resize_u8: both coefficient tables, then (when both passes run) the uint8 intermediate.
+struct ResizePlan {
+    int ks_x, ks_y;
+    long long kk_x, bounds_x, kk_y, bounds_y, tmp, bytes;   // byte offsets; bytes = total
+};
+
+static int resample_ksize(int in_size, int out_size) {
+    const double scale = (double)in_size / (double)out_size;
+    return (int)ceil(scale < 1.0 ? 1.0 : scale) * 2 + 1;
+}
+
+static ResizePlan resize_plan(int N, int Hs, int Ws, int H, int W) {
+    auto up = [](long long v) { return (v + 255) / 256 * 256; };
+    ResizePlan p;
+    p.ks_x = resample_ksize(Ws, W);
+    p.ks_y = resample_ksize(Hs, H);
+    p.kk_x = 0;
+    p.bounds_x = up(p.kk_x + 4LL * W * p.ks_x);
+    p.kk_y = up(p.bounds_x + 8LL * W);
+    p.bounds_y = up(p.kk_y + 4LL * H * p.ks_y);
+    p.tmp = up(p.bounds_y + 8LL * H);
+    p.bytes = p.tmp + ((W != Ws && H != Hs) ? up((long long)N * Hs * W * 3) : 0);
+    return p;
+}
+
+extern "C" long long ccb_resize_u8_workspace_bytes(int N, int Hs, int Ws, int H, int W) {
+    if (N <= 0 || Hs <= 0 || Ws <= 0 || H <= 0 || W <= 0) return -1;
+    return resize_plan(N, Hs, Ws, H, W).bytes;
+}
+
+extern "C" int ccb_resize_u8(const unsigned char* src, unsigned char* dst, int N, int Hs, int Ws, int H, int W, void* work,
+                             long long work_bytes, ccb_stream_t stream) {
+    CCB_REQUIRE(src && dst, CCB_ERR_ARG, "resize_u8: null pointer");
+    CCB_REQUIRE(src != dst, CCB_ERR_ARG, "resize_u8: cannot resize in place");
+    CCB_REQUIRE(N > 0 && Hs > 0 && Ws > 0 && H > 0 && W > 0, CCB_ERR_ARG, "resize_u8: bad sizes");
+    const ResizePlan p = resize_plan(N, Hs, Ws, H, W);
+    CCB_REQUIRE(work && work_bytes >= p.bytes, CCB_ERR_ARG, "resize_u8: workspace of %lld bytes, %lld needed", work_bytes, p.bytes);
+    const bool hpass = W != Ws, vpass = H != Hs;
+    if (!hpass && !vpass) {
+#ifdef CCB_CPU_SIM
+        memcpy(dst, src, (size_t)N * H * W * 3);
+#else
+        cudaMemcpyAsync(dst, src, (size_t)N * H * W * 3, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
+#endif
+        return check_launch("resize_u8");
+    }
+    char* w = (char*)work;
+    CoeffArgs c;
+    c.in_x = Ws; c.out_x = W; c.ks_x = p.ks_x; c.in_y = Hs; c.out_y = H; c.ks_y = p.ks_y;
+    c.kk_x = (int*)(w + p.kk_x); c.bounds_x = (int*)(w + p.bounds_x); c.kk_y = (int*)(w + p.kk_y); c.bounds_y = (int*)(w + p.bounds_y);
+    CCB_LAUNCH(resample_coeffs_kernel, dim3((W + H + 127) / 128), dim3(128), 0, stream, c);
+    unsigned char* mid = (hpass && vpass) ? (unsigned char*)(w + p.tmp) : dst;
+    if (hpass) {
+        ResampleArgs r;
+        r.src = src; r.dst = mid; r.kk = c.kk_x; r.bounds = c.bounds_x;
+        r.outer = (long long)N * Hs; r.in_len = Ws; r.out_len = W; r.inner = 1; r.ksize = p.ks_x;
+        CCB_LAUNCH(resample_pass_kernel, dim3(grid_for((long long)N * Hs * W)), dim3(256), 0, stream, r);
+    }
+    if (vpass) {
+        ResampleArgs r;
+        r.src = hpass ? mid : src; r.dst = dst; r.kk = c.kk_y; r.bounds = c.bounds_y;
+        r.outer = N; r.in_len = Hs; r.out_len = H; r.inner = W; r.ksize = p.ks_y;
+        CCB_LAUNCH(resample_pass_kernel, dim3(grid_for((long long)N * H * W)), dim3(256), 0, stream, r);
+    }
+    return check_launch("resize_u8");
+}
+
+static int normlocal_blocks(int H, int W) {
+    const long long g = ((long long)H * W + 2047) / 2048;
+    return (int)(g < 1 ? 1 : (g > 64 ? 64 : g));
+}
+
+extern "C" long long ccb_normalize_local_workspace_bytes(int B, int H, int W) {
+    if (B <= 0 || H <= 0 || W <= 0) return -1;
+    return (long long)B * 3 * normlocal_blocks(H, W) * 2 * (long long)sizeof(double) + (long long)B * 3 * 2 * (long long)sizeof(float);
+}
+
+extern "C" int ccb_normalize_local(float* const* frames, int B, int F, int H, int W, float* stats, void* work, long long work_bytes,
+                                   ccb_stream_t stream) {
+    CCB_REQUIRE(frames, CCB_ERR_ARG, "normalize_local: null pointer");
+    CCB_REQUIRE(F >= 1 && F <= 8, CCB_ERR_ARG, "normalize_local: 1..8 frames per sample, got %d", F);
+    CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "normalize_local: bad sizes");
+    const long long need = ccb_normalize_local_workspace_bytes(B, H, W);
+    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "normalize_local: workspace of %lld bytes, %lld needed", work_bytes, need);
+    NormLocalArgs a;
+    for (int f = 0; f < 8; ++f) a.x[f] = (f < F) ? frames[f] : nullptr;
+    for (int f = 0; f < F; ++f) CCB_REQUIRE(a.x[f] != nullptr, CCB_ERR_ARG, "normalize_local: frames[%d] is null", f);
+    const int nblk = normlocal_blocks(H, W);
+    a.partials = (double*)work;
+    a.stats = stats ? stats : (float*)((char*)work + (long long)B * 3 * nblk * 2 * sizeof(double));
+    a.B = B; a.F = F; a.hw = (long long)H * W;
+    CCB_LAUNCH(normlocal_partials_kernel, dim3(nblk, B * 3), dim3(256), 0, stream, a);
+    CCB_LAUNCH(normlocal_finalize_kernel, dim3((B * 3 + 63) / 64), dim3(64), 0, stream, a, nblk);
+    CCB_LAUNCH(normlocal_apply_kernel, dim3(nblk, B * 3), dim3(256), 0, stream, a);
+    return check_launch("normalize_local");
 }

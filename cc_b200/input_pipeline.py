@@ -11,20 +11,35 @@ augmentation decisions as the reference loader.
 Documented deviation: the reference resizes with scipy.misc.imresize (PIL BILINEAR on uint8: fixed-point, the
 horizontally and vertically resampled images are each rounded back to uint8); here the same half-pixel-centre
 bilinear lookup is evaluated in fp32 without re-quantisation, so a pixel differs from the reference by at most
-one uint8 step per pass (<= 2/255 before normalisation); with scale 1 the result is identical."""
+one uint8 step per pass (<= 2/255 before normalisation); with scale 1 the result is identical.
+
+The reference's other transforms run on the device as well, bit-exact with Pillow (the library behind scipy.misc):
+  * RandomRotate (custom_transforms.py:75-85, first in the train transform whenever the flow net trains, train.py:178-185):
+    DeviceAugment(rotate=True) rotates the uint8 frames (csrc/io_ops.cu: ccb_rotate_frames_u8) before flip / scale-crop;
+  * NormalizeLocally (custom_transforms.py:33-44, --data-normalization local): normalization='local' writes v/255
+    (ccb_prep_frames_unit) and normalises each sample by its own per-channel mean and unbiased std over all its frames
+    (ccb_normalize_local);
+  * Scale(h, w) (custom_transforms.py:120-137, the validation-flow transform, train.py:189-190): DeviceScale resamples
+    the uint8 frames as Pillow's BILINEAR resize does (ccb_resize_u8, antialiased on a downscale), then normalises.
+The reference's loaders hand scipy.misc float32 copies of the uint8 frames (load_as_float), and scipy.misc byte-scales a
+float image to its own [min, max] before resampling; this pipeline takes the uint8 frames as they are, which is the
+same whenever a frame spans 0..255."""
 import ctypes as C
+import math
 import random
 import numpy as np
 import torch
 from . import _lib
 
 
-def draw_params(B, Hs, Ws, H=None, W=None, rng_random=random, rng_np=np.random, flip=True, scale_crop=True):
+def draw_params(B, Hs, Ws, H=None, W=None, rng_random=random, rng_np=np.random, flip=True, scale_crop=True, rotate=False):
     """Per-sample augmentation decisions, reference generators and order.  Returns a dict of numpy arrays."""
     H, W = H or Hs, W or Ws
     out = dict(flip=np.zeros(B, np.float32), x_scaling=np.ones(B), y_scaling=np.ones(B), scaled_h=np.full(B, Hs), scaled_w=np.full(B, Ws),
-               offset_x=np.zeros(B, np.int32), offset_y=np.zeros(B, np.int32))
+               offset_x=np.zeros(B, np.int32), offset_y=np.zeros(B, np.int32), rotate=np.zeros(B, bool), angle=np.zeros(B))
     for b in range(B):
+        if rotate and not rng_np.random() > 0.5:                          # custom_transforms.py:78
+            out['rotate'][b], out['angle'][b] = True, rng_np.uniform(0, 10)   # :82
         if flip and rng_random.random() < 0.5:                       # custom_transforms.py:52
             out['flip'][b] = 1.0
         if scale_crop:
@@ -34,6 +49,22 @@ def draw_params(B, Hs, Ws, H=None, W=None, rng_random=random, rng_np=np.random, 
             out['offset_y'][b] = rng_np.randint(sh - H + 1)             # :117
             out['offset_x'][b] = rng_np.randint(sw - W + 1)             # :118
     return out
+
+
+def pil_rotate_affine(angle, W, H):
+    """The 6 coefficients Pillow's Image.rotate(angle) (no expand, centre (W/2, H/2)) hands its affine transform: output
+    pixel centre (x, y) -> input point (a0 x + a1 y + a2, a3 x + a4 y + a5).  Restated from Pillow, including its
+    rounding of cos / sin to 15 decimals, so that the device rotation samples the same points."""
+    t = -math.radians(float(angle) % 360.0)
+    m = [round(math.cos(t), 15), round(math.sin(t), 15), 0.0, round(-math.sin(t), 15), round(math.cos(t), 15), 0.0]
+    cx, cy = W / 2, H / 2
+    m[2], m[5] = m[0] * -cx + m[1] * -cy + m[2], m[3] * -cx + m[4] * -cy + m[5]
+    m[2] += cx
+    m[5] += cy
+    return m
+
+
+IDENTITY_AFFINE = [1.0, 0.0, 0.0, 0.0, 1.0, 0.0]
 
 
 def augment_intrinsics(K, p, Ws):
@@ -49,27 +80,130 @@ def augment_intrinsics(K, p, Ws):
     return K
 
 
-class DeviceAugment:
-    """frames_u8 [B,F,Hs,Ws,3] uint8 (pinned host or device) + intrinsics [B,3,3] -> (tgt, refs, K, Kinv) on `device`."""
+NORMALIZATIONS = ('global', 'local')
 
-    def __init__(self, device, H=None, W=None, flip=True, scale_crop=True):
+
+def rotate_affines(p, B, Hs, Ws):
+    """[B,6] fp64: Pillow's rotation matrix for the rotated samples of `p`, the identity for the others."""
+    rot, ang = p.get('rotate', np.zeros(B, bool)), p.get('angle', np.zeros(B))
+    return np.array([pil_rotate_affine(ang[b], Ws, Hs) if rot[b] else IDENTITY_AFFINE for b in range(B)], np.float64)
+
+
+def rotate_frames(src, affine):
+    """src [B,F,H,W,3] uint8 on the device, affine [B,6] fp64 (host or device) -> rotated copy (ccb_rotate_frames_u8)."""
+    B, F, H, W, _ = src.shape
+    aff = torch.as_tensor(affine, dtype=torch.float64).to(src.device, non_blocking=True).contiguous()
+    assert aff.shape == (B, 6)
+    dst = torch.empty_like(src)
+    _lib.check(_lib.lib().ccb_rotate_frames_u8(_lib.ptr(src, 'frames', torch.uint8), _lib.ptr(aff, 'affine', torch.float64),
+                                               _lib.ptr(dst, 'dst', torch.uint8), B, F, H, W, _lib.stream(src)), 'rotate_frames_u8')
+    return dst
+
+
+def resize_frames(src, h, w):
+    """src [..., Hs, Ws, 3] uint8 on the device -> [..., h, w, 3] uint8 resampled as Pillow's BILINEAR resize (ccb_resize_u8)."""
+    Hs, Ws = src.shape[-3], src.shape[-2]
+    N = src.numel() // (Hs * Ws * 3)
+    dst = torch.empty(tuple(src.shape[:-3]) + (h, w, 3), dtype=torch.uint8, device=src.device)
+    nb = _lib.lib().ccb_resize_u8_workspace_bytes(N, Hs, Ws, h, w)
+    assert nb >= 0, 'resize_frames: bad sizes'
+    work = torch.empty(max(nb, 1), dtype=torch.uint8, device=src.device)
+    _lib.check(_lib.lib().ccb_resize_u8(_lib.ptr(src, 'frames', torch.uint8), _lib.ptr(dst, 'dst', torch.uint8), N, Hs, Ws, h, w,
+                                        _lib.ptr(work, 'work', torch.uint8), nb, _lib.stream(src)), 'resize_u8')
+    return dst
+
+
+def normalize_local(frames):
+    """NormalizeLocally (custom_transforms.py:33-44) in place on F tensors [B,3,H,W] (sample b's frames are frames[f][b]);
+    returns the statistics [B,3,2] = {mean, unbiased std} per sample and channel (ccb_normalize_local)."""
+    B, _, H, W = frames[0].shape
+    F = len(frames)
+    stats = torch.empty(B, 3, 2, device=frames[0].device)
+    nb = _lib.lib().ccb_normalize_local_workspace_bytes(B, H, W)
+    work = torch.empty(nb, dtype=torch.uint8, device=frames[0].device)
+    arr = (C.c_void_p * F)(*[_lib.ptr(f) for f in frames])
+    _lib.check(_lib.lib().ccb_normalize_local(arr, B, F, H, W, _lib.ptr(stats), _lib.ptr(work, 'work', torch.uint8), nb,
+                                              _lib.stream(frames[0])), 'normalize_local')
+    return stats
+
+
+def _prep(src, par, offs, B, F, Hs, Ws, H, W, normalization):
+    """uint8 [B,F,Hs,Ws,3] on the device -> F tensors [B,3,H,W]: flip / scale-crop lookup, ArrayToTensor, then Normalize(.5,
+    .5) (global) or NormalizeLocally (local; returns its statistics, else None)."""
+    outs = [torch.empty(B, 3, H, W, device=src.device) for _ in range(F)]
+    arr = (C.c_void_p * F)(*[_lib.ptr(o) for o in outs])
+    fn, name = ('ccb_prep_frames', 'prep_frames') if normalization == 'global' else ('ccb_prep_frames_unit', 'prep_frames_unit')
+    _lib.check(getattr(_lib.lib(), fn)(_lib.ptr(src, 'frames', torch.uint8), arr, _lib.ptr(par), _lib.ptr(offs, 'offs', torch.int32),
+                                       B, F, Hs, Ws, H, W, _lib.stream(src)), name)
+    return outs, (normalize_local(outs) if normalization == 'local' else None)
+
+
+class DeviceAugment:
+    """frames_u8 [B,F,Hs,Ws,3] uint8 (pinned host or device) + intrinsics [B,3,3] -> (tgt, refs, K, Kinv) on `device`.
+
+    The reference's train transform (train.py:165-185) with
+      rotate        RandomRotate first (the flow net trains: no --fix-flownet): the uint8 frames are rotated into a device
+                    scratch buffer, then flipped / scale-cropped.  As in the reference, rotation leaves the intrinsics
+                    unchanged (custom_transforms.py:85 returns them as they came), although the rotated image no longer
+                    fits them;
+      normalization 'global' Normalize(.5, .5) or 'local' NormalizeLocally (--data-normalization); the statistics of the
+                    last 'local' call are kept in `self.stats` ([B,3,2] = {mean, std}).
+    With the defaults the launches and the output are those of the plain flip / scale-crop transform."""
+
+    def __init__(self, device, H=None, W=None, flip=True, scale_crop=True, rotate=False, normalization='global'):
+        assert normalization in NORMALIZATIONS, normalization
         self.device, self.H, self.W, self.flip, self.scale_crop = torch.device(device), H, W, flip, scale_crop
+        self.rotate, self.normalization, self.stats = rotate, normalization, None
 
     def __call__(self, frames_u8, intrinsics, params=None, tgt_index=None):
         assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 5 and frames_u8.size(4) == 3
         B, F, Hs, Ws, _ = frames_u8.shape
         H, W = self.H or Hs, self.W or Ws
-        p = params if params is not None else draw_params(B, Hs, Ws, H, W, flip=self.flip, scale_crop=self.scale_crop)
+        p = params if params is not None else draw_params(B, Hs, Ws, H, W, flip=self.flip, scale_crop=self.scale_crop,
+                                                          rotate=self.rotate)
         src = frames_u8.to(self.device, non_blocking=True).contiguous()
+        if self.rotate:
+            src = rotate_frames(src, rotate_affines(p, B, Hs, Ws))
         par = torch.from_numpy(np.stack([p['flip'], (p['scaled_w'] / Ws).astype(np.float32), (p['scaled_h'] / Hs).astype(np.float32),
                                          np.zeros(B, np.float32)], 1).astype(np.float32)).to(self.device, non_blocking=True)
         offs = torch.from_numpy(np.stack([p['offset_x'], p['offset_y']], 1).astype(np.int32)).to(self.device, non_blocking=True)
-        outs = [torch.empty(B, 3, H, W, device=self.device) for _ in range(F)]
-        arr = (C.c_void_p * F)(*[_lib.ptr(o) for o in outs])
-        _lib.check(_lib.lib().ccb_prep_frames(_lib.ptr(src, 'frames', torch.uint8), arr, _lib.ptr(par), _lib.ptr(offs, 'offs', torch.int32), B, F, Hs, Ws, H, W,
-                                              _lib.stream(src)), 'prep_frames')
+        outs, self.stats = _prep(src, par, offs, B, F, Hs, Ws, H, W, self.normalization)
         K = augment_intrinsics(intrinsics.cpu().numpy() if torch.is_tensor(intrinsics) else intrinsics, p, Ws)
         Kinv = np.linalg.inv(K).astype(np.float32)                     # sequence_folders.py:61
         t = F // 2 if tgt_index is None else tgt_index                # sequence_folders.py:16-21: the target is the middle frame
         refs = [o for i, o in enumerate(outs) if i != t]
         return outs[t], refs, torch.from_numpy(K).to(self.device), torch.from_numpy(Kinv).to(self.device)
+
+
+def scale_intrinsics(K, Hs, Ws, h, w):
+    """K [B,3,3] -> Scale's intrinsics (custom_transforms.py:133-134): rows 0 / 1 times w/Ws, h/Hs in float32."""
+    K = np.array(K, dtype=np.float32, copy=True)
+    K[:, 0] *= np.float32(w / Ws)
+    K[:, 1] *= np.float32(h / Hs)
+    return K
+
+
+class DeviceScale:
+    """The validation-flow transform Compose([Scale(h, w), ArrayToTensor(), normalize]) (train.py:189-190):
+    frames_u8 [B,F,Hs,Ws,3] uint8 + intrinsics [B,3,3] -> (tgt, refs, K, Kinv) on `device`.  The frames are resampled as
+    Pillow's BILINEAR resize (antialiased when shrinking, as KITTI's ~375x1242 frames are to 256x832), then normalised
+    ('global' or 'local', as DeviceAugment).  K and K^-1 in float32 as custom_transforms.py:133-134 and
+    datasets/validation_flow.py:137 compute them.  The target is frame 0: validation_flow.py:130-133 orders the frames
+    [tgt] + refs."""
+
+    def __init__(self, device, h=256, w=832, normalization='global'):
+        assert normalization in NORMALIZATIONS, normalization
+        self.device, self.h, self.w, self.normalization, self.stats = torch.device(device), h, w, normalization, None
+
+    def __call__(self, frames_u8, intrinsics, tgt_index=0):
+        assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 5 and frames_u8.size(4) == 3
+        B, F, Hs, Ws, _ = frames_u8.shape
+        h, w = self.h, self.w
+        src = resize_frames(frames_u8.to(self.device, non_blocking=True).contiguous(), h, w)
+        par = torch.tensor([[0.0, 1.0, 1.0, 0.0]] * B, device=self.device)
+        offs = torch.zeros(B, 2, dtype=torch.int32, device=self.device)
+        outs, self.stats = _prep(src, par, offs, B, F, h, w, h, w, self.normalization)
+        K = scale_intrinsics(intrinsics.cpu().numpy() if torch.is_tensor(intrinsics) else intrinsics, Hs, Ws, h, w)
+        Kinv = np.linalg.inv(K).astype(np.float32)                     # validation_flow.py:137
+        refs = [o for i, o in enumerate(outs) if i != tgt_index]
+        return outs[tgt_index], refs, torch.from_numpy(K).to(self.device), torch.from_numpy(Kinv).to(self.device)

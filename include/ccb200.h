@@ -334,6 +334,29 @@ int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, in
  * device memory; dst = host array of F device pointers. */
 int ccb_prep_frames(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B, int F,
                     int Hs, int Ws, int H, int W, ccb_stream_t stream);
+/* The same lookup writing v/255 only (ArrayToTensor without Normalize), for ccb_normalize_local to follow. */
+int ccb_prep_frames_unit(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B, int F,
+                         int Hs, int Ws, int H, int W, ccb_stream_t stream);
+/* RandomRotate (custom_transforms.py:75-85) = scipy.misc.imrotate = Pillow Image.rotate(angle, BILINEAR), bit-exact:
+ * src, dst [B,F,H,W,3] uint8 (not in place); affine [B,6] fp64 maps an output pixel centre (x+.5, y+.5) to the input point
+ * (a0 x + a1 y + a2, a3 x + a4 y + a5), as Pillow builds it (cc_b200.input_pipeline.pil_rotate_affine); the identity
+ * leaves a sample's frames unchanged.  Points outside the frame give 0. */
+int ccb_rotate_frames_u8(const unsigned char* src, const double* affine, unsigned char* dst, int B, int F, int H, int W,
+                         ccb_stream_t stream);
+/* Scale (custom_transforms.py:120-137) = scipy.misc.imresize = Pillow resize((W, H), BILINEAR), bit-exact (8-bit
+ * ImagingResample: antialiased on a downscale, 22-bit fixed-point weights, horizontal pass first, each pass rounded to
+ * uint8): src [N,Hs,Ws,3] -> dst [N,H,W,3] uint8.  The weights are computed on the device into `work`
+ * (ccb_resize_u8_workspace_bytes, -1 for bad sizes), so the call is asynchronous and can be captured in a graph. */
+long long ccb_resize_u8_workspace_bytes(int N, int Hs, int Ws, int H, int W);
+int ccb_resize_u8(const unsigned char* src, unsigned char* dst, int N, int Hs, int Ws, int H, int W, void* work,
+                  long long work_bytes, ccb_stream_t stream);
+/* NormalizeLocally (custom_transforms.py:33-44) in place on F frames[f] [B,3,H,W]: per sample and channel, the mean and
+ * unbiased std over all F*H*W values (fp64, deterministic), rounded to fp32, then x = (x - m) / s in fp32.  stats
+ * ([B,3,2] = {mean, std}) may be NULL.  A zero std gives inf / nan, as in the reference.
+ * work: ccb_normalize_local_workspace_bytes(B, H, W) bytes, 8-byte aligned. */
+long long ccb_normalize_local_workspace_bytes(int B, int H, int W);
+int ccb_normalize_local(float* const* frames, int B, int F, int H, int W, float* stats, void* work, long long work_bytes,
+                        ccb_stream_t stream);
 /* number of kernel launches issued through this library by the calling process so far */
 long long ccb_launch_count(void);
 

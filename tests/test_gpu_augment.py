@@ -1,0 +1,29 @@
+"""The reference's remaining data transforms (RandomRotate, NormalizeLocally, Scale) on the H100: the fixture cases of
+tests/augment_cases.py and full-size runs against the numpy restatements of Pillow (tests/augment_oracle.py)."""
+import pytest
+import torch
+from cc_b200 import _lib
+from tests import augment_cases as AC
+
+pytestmark = pytest.mark.gpu
+DEV = torch.device('cuda:0')
+
+
+@pytest.fixture(scope='module', autouse=True)
+def cuda_lib():
+    _lib._lib = None                      # the real library, not a simulator build
+    assert not _lib.is_simulator(), 'GPU tests must run on the sm_90a library'
+    yield
+
+
+@pytest.mark.parametrize('case', AC.AUGMENT_CASES, ids=lambda f: f.__name__)
+def test_augment_case(case):
+    case(DEV)
+
+
+def test_rotate_train_transform_full_size():
+    AC.case_rotate_fullsize(DEV)
+
+
+def test_scale_kitti_full_size():
+    AC.case_scale_fullsize(DEV)
