@@ -75,14 +75,14 @@ def pose_snippet_errors(Pp, imgs, gt_poses, rotation_mode='euler'):
     return compute_pose_error(gt_poses, final) + (final,)
 
 
-def flow_sample_errors(P, tgt, refs, K, Kinv, flow_gt, obj_map_gt, THRESH=0.01):
-    """test_flow.py:112-140 for one sample; P = {'disp','pose','mask','flow'} parameter dicts."""
+def flow_sample_errors(P, tgt, refs, K, Kinv, flow_gt, obj_map_gt, THRESH=0.01, flownet='Back2Future'):
+    """test_flow.py:112-140 for one sample; P = {'disp','pose','mask','flow'} parameter dicts, P['flow'] of `flownet`."""
     with torch.no_grad():
         disp = ON.disp_forward(P['disp'], tgt, training=False)
         depth = 1 / disp
         pose = ON.pose_forward(P['pose'], tgt, refs)
         emask = ON.mask_forward(P['mask'], tgt, refs, training=False)
-        flow_fwd = ON.flow_forward(P['flow'], tgt, refs[1:3], training=False)[0]
+        flow_fwd = ON.flow_eval(P['flow'], tgt, refs, flownet)
         flow_cam = OG.pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
         rigidity_mask = 1 - (1 - emask[:, 1]) * (1 - emask[:, 2]).unsqueeze(1) > 0.5
         soft = (flow_cam - flow_fwd).abs()

@@ -1,4 +1,4 @@
-"""Oracle: the four hot-path CNNs as *functional* fp32 forwards over a state_dict.
+"""Oracle: the hot-path CNNs as *functional* fp32 forwards over a state_dict.
 TEST INFRASTRUCTURE.
 
 Key names and shapes equal the reference modules' ``state_dict()`` (checkpoint
@@ -9,14 +9,17 @@ this oracle and the CUDA product.
 * PoseNetB6   : reference models/PoseNetB6.py:24-83
 * MaskNet6    : reference models/MaskNet6.py:19-123
 * Back2Future : reference models/back2future.py:51-321
+* FlowNetC6   : reference models/FlowNetC6.py:32-164 (+ submodules.py:5-39); the flow net of --flownet FlowNetC6
 
-PARITY UNPINNED at one boundary: ``correlate`` restates the published behaviour of
-the third-party ``spatial_correlation_sampler`` (PyPI spatial-correlation-sampler,
+PARITY UNPINNED at one boundary: ``spatial_correlation_sample`` restates the published
+behaviour of the third-party ``spatial_correlation_sampler`` (PyPI spatial-correlation-sampler,
 version un-pinned in reference requirements.txt:13, upstream
 ClementPinard/Pytorch-Correlation-extension; source absent from the reference repository):
-out[b,ph,pw,y,x] = sum_c in1[b,c,y,x] * in2[b,c,y+ph-4,x+pw-4] (zero outside), with
-kernel_size=1, patch_size=9, stride=1.  It is anchored only by the reference's call
-site and permutation tables (back2future.py:15-25,56-59).
+out[b,ph,pw,y,x] = sum_c in1[b,c,y,x] * in2[b,c,y+d(ph-P//2),x+d(pw-P//2)] (zero outside), with
+kernel_size=1, stride=1, padding=0; the first patch index is the vertical displacement.
+Back2Future calls it with patch_size P=9, dilation_patch d=1, FlowNetC6 with P=21, d=2.  It is
+anchored only by the reference's call sites and Back2Future's permutation tables
+(back2future.py:15-25,56-59, FlowNetC6.py:18-30).
 """
 import math
 import numpy as np
@@ -254,17 +257,15 @@ IDX_FWD = [int(i) for i in _IDX]              # back2future.py:56-58
 IDX_BWD = [int(i) for i in reversed(_IDX)]    # back2future.py:59
 
 
-def spatial_correlation_sample(in1, in2, patch=9):
+def spatial_correlation_sample(in1, in2, patch=9, dilation=1):
     """Restated third-party op (see module docstring): [B,C,H,W]x2 -> [B,patch,patch,H,W]."""
     B, C, H, W = in1.shape
-    r = patch // 2
+    r = (patch // 2) * dilation
     pad = F.pad(in2, (r, r, r, r))
     rows = []
     for ph in range(patch):
-        cols = []
-        for pw in range(patch):
-            cols.append((in1 * pad[:, :, ph:ph + H, pw:pw + W]).sum(1))
-        rows.append(torch.stack(cols, 1))
+        y = ph * dilation
+        rows.append(torch.stack([(in1 * pad[:, :, y:y + H, pw * dilation:pw * dilation + W]).sum(1) for pw in range(patch)], 1))
     return torch.stack(rows, 1)
 
 
@@ -360,3 +361,77 @@ def flow_forward(p, im_tar, im_refs, nlevels=6, training=True, with_occ=True):
         if with_occ:
             oc.append(F.interpolate(occs[6], scale_factor=2, mode='nearest'))
     return ff, fbw, oc
+
+
+# ----------------------------------------------------------------------------- FlowNetC6
+C6_SLOPE = 0.1
+C6_NPARAMS = 39276490
+# (name, in, out, kernel, stride) of the conv blocks (Conv2d + bias + LeakyReLU 0.1), registration order
+C6_CONVS = [('conv1', 3, 64, 7, 2), ('conv2', 64, 128, 5, 2), ('conv3', 128, 256, 5, 2), ('conv_redir', 256, 32, 1, 1),
+            ('conv3_1', 473, 256, 3, 1), ('conv4', 256, 512, 3, 2), ('conv4_1', 512, 512, 3, 1), ('conv5', 512, 512, 3, 2),
+            ('conv5_1', 512, 512, 3, 1), ('conv6', 512, 1024, 3, 2), ('conv6_1', 1024, 1024, 3, 1)]
+C6_DECONVS = [(5, 1024, 512), (4, 1026, 256), (3, 770, 128), (2, 386, 64), (1, 194, 32)]   # ConvT k4 s2 p1 + LeakyReLU
+C6_PREDICT_IN = {6: 1024, 5: 1026, 4: 770, 3: 386, 2: 194, 1: 98}                          # 3x3 -> 2, no activation
+
+
+def flownetc6_correlate(in1, in2):
+    """Reference models/FlowNetC6.py:18-30: [B,441,H,W], divided by C (no activation)."""
+    out = spatial_correlation_sample(in1, in2, patch=21, dilation=2)
+    b, ph, pw, h, w = out.size()
+    return out.view(b, ph * pw, h, w) / in1.size(1)
+
+
+def flownetc6_forward(p, x1, x2, training=True, div_flow=20):
+    """Train mode: (flow1, ..., flow6), each div_flow * bilinear x2 of the head (full_res=True); eval mode: flow1."""
+    spec = {name: (k, s) for name, _, _, k, s in C6_CONVS}
+
+    def conv(name, x):
+        k, s = spec[name]
+        return F.leaky_relu(F.conv2d(x, p[name + '.0.weight'], p[name + '.0.bias'], s, (k - 1) // 2), C6_SLOPE)
+
+    def tower(x):
+        c1 = conv('conv1', x)
+        c2 = conv('conv2', c1)
+        return c1, c2, conv('conv3', c2)
+
+    c1a, c2a, c3a = tower(x1)
+    c3b = tower(x2)[2]
+    corr = F.leaky_relu(flownetc6_correlate(c3a, c3b), C6_SLOPE)
+    c3_1 = conv('conv3_1', torch.cat((conv('conv_redir', c3a), corr), 1))
+    c4 = conv('conv4_1', conv('conv4', c3_1))
+    c5 = conv('conv5_1', conv('conv5', c4))
+    c6 = conv('conv6_1', conv('conv6', c5))
+    skips = {5: c5, 4: c4, 3: c3_1, 2: c2a, 1: c1a}
+    pred = lambda n, t: F.conv2d(t, p['predict_flow%d.weight' % n], p['predict_flow%d.bias' % n], 1, 1)      # noqa: E731
+    flows = {6: pred(6, c6)}
+    feat = c6
+    for n in range(5, 0, -1):
+        dec = F.leaky_relu(F.conv_transpose2d(feat, p['deconv%d.0.weight' % n], p['deconv%d.0.bias' % n], stride=2, padding=1),
+                           C6_SLOPE)
+        up = F.conv_transpose2d(flows[n + 1], p['upsampled_flow%d_to_%d.weight' % (n + 1, n)],
+                                p['upsampled_flow%d_to_%d.bias' % (n + 1, n)], stride=2, padding=1)
+        feat = torch.cat((skips[n], dec, up), 1)
+        flows[n] = pred(n, feat)
+    outs = [div_flow * F.interpolate(flows[n], scale_factor=2, mode='bilinear', align_corners=False) for n in range(1, 7)]
+    return tuple(outs) if training else outs[0]
+
+
+# ----------------------------------------------------------------------------- the flow net of a step
+def flow_pair(p, tgt, refs, flownet='Back2Future'):
+    """(flow_fwd, flow_bwd) of the training step, train mode (reference train.py:462-466): Back2Future sees both
+    neighbours in one call (no occlusion decoders), FlowNetC6 is called once per direction."""
+    if flownet == 'Back2Future':
+        ff, fb, _ = flow_forward(p, tgt, refs[1:3], training=True, with_occ=False)
+        return ff, fb
+    if flownet == 'FlowNetC6':
+        return list(flownetc6_forward(p, tgt, refs[2])), list(flownetc6_forward(p, tgt, refs[1]))
+    raise ValueError('unknown flow net %r' % (flownet,))
+
+
+def flow_eval(p, tgt, refs, flownet='Back2Future'):
+    """flow_fwd of the flow evaluation, eval mode (reference test_flow.py:122-125)."""
+    if flownet == 'Back2Future':
+        return flow_forward(p, tgt, refs[1:3], training=False)[0]
+    if flownet == 'FlowNetC6':
+        return flownetc6_forward(p, tgt, refs[2], training=False)
+    raise ValueError('unknown flow net %r' % (flownet,))

@@ -30,9 +30,9 @@ def loss_cfg1(P, tgt, refs, K, Kinv, hp=HP):
     return loss, dict(loss_1=l1, loss_3=l3, disp=disp, pose=pose)
 
 
-def loss_cfg2(P, tgt, refs, K, Kinv, hp=HP):
-    """Back2Future flow + flow photometric(+SSIM) + smoothness (cfg2)."""
-    ff, fb, _ = nets.flow_forward(P['flow'], tgt, refs[1:3], training=True, with_occ=False)
+def loss_cfg2(P, tgt, refs, K, Kinv, hp=HP, flownet='Back2Future'):
+    """Flow net (Back2Future by default) + flow photometric(+SSIM) + smoothness (cfg2)."""
+    ff, fb = nets.flow_pair(P['flow'], tgt, refs, flownet)
     l4 = L.photometric_flow_loss(tgt, refs[1:3], [fb, ff], [None] * len(ff),
                                  lambda_oob=hp['lambda_oob'], qch=hp['qch'], wssim=hp['wssim'])
     l3 = _smooth(hp, tgt, ff) + _smooth(hp, tgt, fb)
@@ -40,13 +40,13 @@ def loss_cfg2(P, tgt, refs, K, Kinv, hp=HP):
     return loss, dict(loss_4=l4, loss_3=l3, flow_fwd=ff, flow_bwd=fb)
 
 
-def loss_cfg3(P, tgt, refs, K, Kinv, hp=HP):
+def loss_cfg3(P, tgt, refs, K, Kinv, hp=HP, flownet='Back2Future'):
     """Full joint step body.  Reference train.py:454-509."""
     disp = nets.disp_forward(P['disp'], tgt, training=True)
     depth = [1 / d for d in disp]
     pose = nets.pose_forward(P['pose'], tgt, refs)
     emask = nets.mask_forward(P['mask'], tgt, refs, training=True)
-    ff, fb, _ = nets.flow_forward(P['flow'], tgt, refs[1:3], training=True, with_occ=False)
+    ff, fb = nets.flow_pair(P['flow'], tgt, refs, flownet)
     cam_f = [pose2flow(d.squeeze(1), pose[:, 2], K, Kinv) for d in depth]
     cam_b = [pose2flow(d.squeeze(1), pose[:, 1], K, Kinv) for d in depth]
     tgt_masks = L.consensus_exp_masks(cam_f, cam_b, ff, fb, tgt, refs[2], refs[1],
@@ -106,10 +106,12 @@ class Adam:
             p.addcdiv_(m, denom, value=-self.lr / bc1)
 
 
-def train_step(cfg, P, opt, tgt, refs, K, Kinv, hp=HP):
-    """zero_grad -> forward -> backward -> Adam (reference train.py:566-568)."""
+def train_step(cfg, P, opt, tgt, refs, K, Kinv, hp=HP, flownet='Back2Future'):
+    """zero_grad -> forward -> backward -> Adam (reference train.py:566-568).  flownet: the net P['flow'] holds
+    (cfg2 / cfg3)."""
     opt.zero_grad()
-    loss, aux = LOSS_FNS[cfg](P, tgt, refs, K, Kinv, hp)
+    fn = LOSS_FNS[cfg]
+    loss, aux = fn(P, tgt, refs, K, Kinv, hp) if cfg == 'cfg1' else fn(P, tgt, refs, K, Kinv, hp, flownet)
     loss.backward()
     opt.step()
     return loss.detach(), aux

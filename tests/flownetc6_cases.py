@@ -14,7 +14,7 @@ import torch
 import torch.nn.functional as F
 from cc_b200 import nn as cnn, models as CM, synth
 from tests.util import golden, assert_close, key_with_stride, pick
-from tests import flownetc6_oracle as O6
+from oracle import nets as ON
 from tests.layer_audit import U, C_PROD, TINY32
 
 R_CORR441D = 6.0
@@ -24,12 +24,18 @@ SLOPE32 = float(torch.tensor(0.1, dtype=torch.float32))
 CORR_SHAPES = [(1, 1, 3, 5), (3, 13, 3, 5), (3, 13, 8, 16), (1, 256, 8, 16), (3, 13, 45, 50), (1, 256, 32, 104)]
 
 
+def corr441d_sample(a, b):
+    """The restated third-party correlation at FlowNetC6's call (patch 21, dilation 2) as [B,441,h,w], not divided by C."""
+    B, _, h, w = a.shape
+    return ON.spatial_correlation_sample(a, b, patch=N, dilation=2).reshape(B, N * N, h, w)
+
+
 def corr441d_ref(f1, f2):
     """fp64 pre-activation z [B,441,h,w] and ||t||_2 / C of its terms."""
     a, b = f1.double(), f2.double()
     B, C, h, w = a.shape
-    z = O6.spatial_correlation_sample(a, b).reshape(B, N * N, h, w) / C
-    tn = O6.spatial_correlation_sample(a * a, b * b).reshape(B, N * N, h, w).sqrt() / C
+    z = corr441d_sample(a, b) / C
+    tn = corr441d_sample(a * a, b * b).sqrt() / C
     return z, tn
 
 
@@ -144,3 +150,16 @@ def fixture_inputs(device):
 def grad_names():
     g = golden(FIXTURE)
     return [k[2:].split('@')[0] for k in g if k.startswith('g_')]
+
+
+def step_flow_params(seed=320, head_scale=0.05):
+    """FlowNetC6 weights for step tests: synth.seeded_fill, the six predict_flow heads scaled by head_scale.
+    Every output is 20 x a head upsampled, so the flows of the reference init (xavier, U[0,1) biases) or of seeded_fill
+    alone are several pixels even on the 2x4 coarsest level of a 64x128 frame: every pixel of that level then samples
+    outside the frame and the flow photometric loss is inf (in the reference as here).  Scaled heads keep the flows
+    below a pixel there."""
+    sd = synth.seeded_fill(CM.FlowNetC6(), seed).state_dict()
+    for k in sd:
+        if k.startswith('predict_flow'):
+            sd[k] = sd[k] * head_scale
+    return sd

@@ -4,7 +4,7 @@ the photometric loss without the outputs autograd would throw away.  Shared by t
 import itertools
 import torch
 from tests.util import assert_close
-from tests.step_cases import assert_adam_step, f32, _record, _assert_same
+from tests.step_cases import assert_adam_step, assert_groups_step, group_range, oracle_state_dicts, _record
 from tests import kernel_cases as KC
 from cc_b200 import _lib, synth, pyramid, nn as cnn, loss_functions as CL
 from cc_b200.optim import FlatAdam, ADAM_BLOCK
@@ -288,37 +288,6 @@ def case_photo_value_only(device, B=2, H=40, W=72, NL=3, seed=31):
 
 
 # ---- the Trainer with fixed nets (GPU) --------------------------------------------------------------------------------
-def group_range(opt, gi):
-    """(lo, hi) of group gi in the flat buffers (contiguous in the constructor layout)."""
-    offs = sorted(opt.offset[p] for p in opt.groups[gi])
-    lo, hi = offs[0][0], offs[-1][0] + offs[-1][1]
-    assert hi - lo == sum(k for _, k in offs), 'group %d is not contiguous' % gi
-    return lo, hi
-
-
-def assert_groups_step(tr, before, after, want_t, what):
-    """Per net of the trainer: an active group's range within assert_adam_step's bound for its own t (want_t[name]); a
-    frozen group's parameters, moments and counter bit-unchanged and its gradient range exactly zero."""
-    o = tr.opt
-    for gi, name in enumerate(NETS_OF[tr.cfg]):
-        lo, hi = group_range(o, gi)
-        sl = slice(lo, hi)
-        st = slice(4 * gi, 4 * gi + 4)
-        if name in tr.fixed:
-            for k in ('flat_p', 'exp_avg', 'exp_avg_sq'):
-                assert torch.equal(after[k][sl], before[k][sl]), f'{what}: fixed {name}: {k} changed'
-            assert torch.equal(after['state'][st], before['state'][st]), f'{what}: fixed {name}: step counter changed'
-            assert not bool(after['flat_g'][sl].any()), f'{what}: fixed {name} received a gradient'
-        else:
-            assert_adam_step((before['flat_p'][sl], before['exp_avg'][sl], before['exp_avg_sq'][sl]),
-                             (after['flat_p'][sl], after['exp_avg'][sl], after['exp_avg_sq'][sl], after['state'][st]),
-                             after['flat_g'][sl], want_t[name], o.lr, o.betas, o.eps, o.grad_scale, f'{what}: {name}')
-
-
-def _oracle_sd(P):
-    return {n: {k: v.detach().clone() for k, v in d.items()} for n, d in P.items()}
-
-
 def _oracle_params(P, names):
     """The oracle's parameters of `names` in chain order (BatchNorm buffers excluded)."""
     return [t for n in names for k, t in P[n].items() if t.is_floating_point() and 'running_' not in k]
@@ -331,7 +300,7 @@ def case_canonical_vs_oracle(device, B=2, H=64, W=128, steps=3):
     of the step's own gradient.  The eager step issues fewer launches than the cfg3 step."""
     from oracle import step as OS
     P = OS.make_params('cfg3')
-    sd = _oracle_sd(P)
+    sd = oracle_state_dicts(P)
     for n in ('mask', 'flow'):
         for t in P[n].values():
             t.requires_grad_(False)
@@ -365,55 +334,6 @@ def case_canonical_vs_oracle(device, B=2, H=64, W=128, steps=3):
     n_full = _lib.lib().ccb_launch_count() - c0
     assert launches[-1] < n_full, (launches, n_full)
     print(f'canonical step: {launches[-1]} launches, cfg3 step: {n_full}')
-
-
-def case_canonical_graph_vs_eager(device, B=2, H=64, W=128, seed=70):
-    """capture() + three replay()s of the canonical step equal three eager steps bit for bit; replay() refuses after
-    set_fixed()."""
-    from oracle import step as OS
-    batches = []
-    for i in range(3):
-        tgt, refs = synth.frames(B, H, W, seed=seed + i)
-        batches.append([tgt] + refs + list(synth.intrinsics(B, H, W)))
-    sd = _oracle_sd(OS.make_params('cfg3'))
-    saved = cnn.GRAPH_LIVE
-    tr = None
-    try:
-        tr = Trainer('cfg3', device, state_dicts=sd, fixed=('mask', 'flow'))
-        eager = []
-        for b in batches:
-            d = [t.to(device) for t in b]
-            loss, _ = tr.step(d[0], d[1:5], d[5], d[6])
-            eager.append(_record(tr, loss))
-        del tr, loss, d
-        tr = None
-        torch.cuda.empty_cache()
-        tr = Trainer('cfg3', device, state_dicts=sd, fixed=('mask', 'flow'))
-        static = [t.to(device) for t in batches[0]]
-        snap = _record(tr)
-        tr.capture(static[0], static[1:5], static[5], static[6])
-        _assert_same(_record(tr), snap, 'canonical: state after capture()', skip=('flat_g',))
-        prev = snap
-        for i, b in enumerate(batches):
-            for s_, h in zip(static, b):
-                s_.copy_(h)
-            cur = _record(tr, tr.replay())
-            _assert_same(cur, eager[i], f'canonical {B}x{H}x{W}: replay {i} vs eager step {i}')
-            assert_groups_step(tr, prev, cur, dict(disp=i + 1, pose=i + 1), f'canonical replay {i}')
-            prev = cur
-        tr.set_fixed(('mask',))
-        try:
-            tr.replay()
-            raise RuntimeError('replay() ran a graph captured under another fixed set')
-        except AssertionError:
-            pass
-    finally:
-        if tr is not None:
-            tr.graph = None
-        tr = None
-        torch.cuda.synchronize()
-        cnn.GRAPH_LIVE = saved
-        pyramid.clear()
 
 
 def case_phase_switch(device, B=2, H=64, W=128):
@@ -464,7 +384,7 @@ def case_fixed_dispnet_batchnorm(device, B=2, H=128, W=416, steps=2):
     (reference train.py:438-441), while its parameters do not move."""
     from oracle import step as OS
     P = OS.make_params('cfg1')
-    sd = _oracle_sd(P)
+    sd = oracle_state_dicts(P)
     for t in P['disp'].values():
         t.requires_grad_(False)
     topt = torch.optim.Adam(_oracle_params(P, ('disp', 'pose')), lr=OS.HP['lr'], betas=(OS.HP['beta1'], OS.HP['beta2']))

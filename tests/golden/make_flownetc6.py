@@ -5,7 +5,7 @@ fixtures are not touched).
 
 make_golden.py's correlation stub takes Back2Future's arguments only.  FlowNetC6 calls spatial_correlation_sample with
 patch_size=21, padding=0 and dilation_patch=2, so its module gets a stub with the full signature, computing the
-restated semantics of tests/flownetc6_oracle.py (the third-party op stays parity unpinned).
+restated semantics of oracle.nets.spatial_correlation_sample (the third-party op stays parity unpinned).
 
 Contents: weights from synth.seeded_fill(FlowNetC6(), 310); B=2 64x128 frames (synth.frames seed 196), called as
 train.py:465 does, flow_net(tgt, ref+): the six train-mode outputs, gradients of sum_i out_i * wts(500 + i) for a sample of
@@ -17,14 +17,14 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import make_golden as MG                      # noqa: E402  (reference import path, stubs, save helpers)
-from tests import flownetc6_oracle as O6      # noqa: E402
+from oracle import nets as ON                 # noqa: E402
 
 RF = sys.modules['models.FlowNetC6']          # the reference's module (imported by make_golden; `models.FlowNetC6` is the class)
 
 
 def _corr_stub(in1, in2, kernel_size=1, patch_size=1, stride=1, padding=0, dilation_patch=1):
     assert kernel_size == 1 and stride == 1 and padding == 0, 'stub restates kernel_size=1, stride=1, padding=0 only'
-    return O6.spatial_correlation_sample(in1, in2, patch_size, dilation_patch)
+    return ON.spatial_correlation_sample(in1, in2, patch_size, dilation_patch)
 
 
 RF.spatial_correlation_sample = _corr_stub

@@ -2,7 +2,7 @@
 GPU tests): product modules vs the golden fixtures frozen from the reference and vs the oracle."""
 import torch
 import torch.nn.functional as F
-from tests.util import golden, T, assert_close, key_with_stride, pick
+from tests.util import golden, T, assert_close, key_with_stride, pick, conv_impl
 from cc_b200 import synth, nn as cnn, models as CM
 from oracle import nets as ON
 
@@ -76,9 +76,7 @@ def case_conv_tc(device):
               (4, 32, 64, 208, 32, 7, 1, 3), (4, 65, 32, 104, 32, 1, 1, 0), (2, 256, 16, 52, 160, 3, 1, 1),
               (2, 16, 64, 208, 1, 3, 1, 1), (4, 3, 64, 208, 32, 7, 2, 3),
               (4, 512, 8, 26, 512, 3, 1, 1), (4, 256, 16, 52, 512, 3, 2, 1)]      # small-M layers: split-K
-    saved = cnn.CONV_IMPL
-    try:
-        cnn.CONV_IMPL = _lib.IMPL_TC
+    with conv_impl(_lib.IMPL_TC):
         for (B, Ci, H, W, Co, k, s, p) in shapes:
             x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
             w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
@@ -113,8 +111,6 @@ def case_conv_tc(device):
             gb_ = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd])
             assert_close(ga[0], gb_[0], 1e-4, f'tc convT k{k} dx')
             assert_close(ga[1], gb_[1], 1e-4, f'tc convT k{k} dw')
-    finally:
-        cnn.CONV_IMPL = saved
 
 
 def _conv_cross_check(device, shapes, seed, name):
@@ -123,30 +119,26 @@ def _conv_cross_check(device, shapes, seed, name):
     convolution, forward with a fused bias + LeakyReLU epilogue and with a linear one, data / weight / bias gradients."""
     from cc_b200 import _lib
     g = torch.Generator().manual_seed(seed)
-    saved = cnn.CONV_IMPL
-    try:
-        for (B, Ci, H, W, Co, k, s, p) in shapes:
-            tag = f'{name} {Ci}->{Co} k{k} s{s} {H}x{W}'
-            x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
-            w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
-            b = torch.randn(Co, generator=g).to(device).requires_grad_(True)
-            xd, wd, bd = [t.detach().double().requires_grad_(True) for t in (x, w, b)]
-            zd = F.conv2d(xd, wd, bd, s, p)
-            wt = _wts(zd.shape, 9, device)
-            gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
-            outs = {}
-            for impl in (_lib.IMPL_TC, _lib.IMPL_FFMA):
-                cnn.CONV_IMPL = impl
+    for (B, Ci, H, W, Co, k, s, p) in shapes:
+        tag = f'{name} {Ci}->{Co} k{k} s{s} {H}x{W}'
+        x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
+        w = (torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5).to(device).requires_grad_(True)
+        b = torch.randn(Co, generator=g).to(device).requires_grad_(True)
+        xd, wd, bd = [t.detach().double().requires_grad_(True) for t in (x, w, b)]
+        zd = F.conv2d(xd, wd, bd, s, p)
+        wt = _wts(zd.shape, 9, device)
+        gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
+        outs = {}
+        for impl in (_lib.IMPL_TC, _lib.IMPL_FFMA):
+            with conv_impl(impl):
                 assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(zd, 0.2), 1e-4, f'{tag} impl {impl} fprop+leaky')
                 y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
                 gx, gw, gb = torch.autograd.grad((y * wt).sum(), [x, w, b])
-                outs[impl] = (y.detach(), gx, gw, gb)
-                for got, ref, what in zip(outs[impl], (zd,) + tuple(gd), ('fprop', 'dgrad', 'wgrad', 'bias grad')):
-                    assert_close(got, ref, 1e-4, f'{tag} impl {impl} {what}')
-            for a_, b_, what in zip(outs[_lib.IMPL_TC], outs[_lib.IMPL_FFMA], ('fprop', 'dgrad', 'wgrad', 'bias grad')):
-                assert_close(a_, b_, 1e-4, f'{tag} tensor-core vs CUDA-core kernels {what}')
-    finally:
-        cnn.CONV_IMPL = saved
+            outs[impl] = (y.detach(), gx, gw, gb)
+            for got, ref, what in zip(outs[impl], (zd,) + tuple(gd), ('fprop', 'dgrad', 'wgrad', 'bias grad')):
+                assert_close(got, ref, 1e-4, f'{tag} impl {impl} {what}')
+        for a_, b_, what in zip(outs[_lib.IMPL_TC], outs[_lib.IMPL_FFMA], ('fprop', 'dgrad', 'wgrad', 'bias grad')):
+            assert_close(a_, b_, 1e-4, f'{tag} tensor-core vs CUDA-core kernels {what}')
 
 
 def case_conv_tma_family(device):
@@ -238,30 +230,28 @@ def case_conv_weight_cache(device):
                                             f'{(a_ - r_).abs().max().item():.3e}'
                 assert_close(a_, d_, 1e-4, f'{tag} {nm} vs fp64')
 
-    saved = cnn.CONV_IMPL
-    try:
-        cnn.CONV_IMPL = _lib.IMPL_TC
-        cache = cnn.WeightCache(device)
-        ref = run(None)
-        rec = run(cache.h)                      # recording: layouts noted, weights still prepared per call
-        st = cache.stats()
-        assert st == dict(layouts=WCACHE_LAYOUTS, hits=0, misses=0, committed=False), st
-        for a, r in zip(rec, ref):
-            assert all(torch.equal(a_, r_) for a_, r_ in zip(a, r)), 'recording changed a result'
-        cache.commit()                          # allocates the cache and prepares every layout in one launch
-        check(run(cache.h), ref, 'committed')
-        st = cache.stats()
-        assert st == dict(layouts=WCACHE_LAYOUTS, hits=WCACHE_REQUESTS, misses=0, committed=True), st
-        with torch.no_grad():                   # an optimiser step: weights change in place, then one refresh
-            for i, (_, _, _, _, _, w, _) in enumerate(layers):
-                w.add_(_wts(w.shape, 60 + i, device) * (0.1 * w.abs().max()))
-        cache.refresh()
-        check(run(cache.h), run(None), 'refreshed')
-        st = cache.stats()
-        assert st == dict(layouts=WCACHE_LAYOUTS, hits=2 * WCACHE_REQUESTS, misses=0, committed=True), st
-    finally:
-        cnn.CONV_IMPL = saved
-        cnn.WCACHE = None
+    with conv_impl(_lib.IMPL_TC):
+        try:
+            cache = cnn.WeightCache(device)
+            ref = run(None)
+            rec = run(cache.h)                      # recording: layouts noted, weights still prepared per call
+            st = cache.stats()
+            assert st == dict(layouts=WCACHE_LAYOUTS, hits=0, misses=0, committed=False), st
+            for a, r in zip(rec, ref):
+                assert all(torch.equal(a_, r_) for a_, r_ in zip(a, r)), 'recording changed a result'
+            cache.commit()                          # allocates the cache and prepares every layout in one launch
+            check(run(cache.h), ref, 'committed')
+            st = cache.stats()
+            assert st == dict(layouts=WCACHE_LAYOUTS, hits=WCACHE_REQUESTS, misses=0, committed=True), st
+            with torch.no_grad():                   # an optimiser step: weights change in place, then one refresh
+                for i, (_, _, _, _, _, w, _) in enumerate(layers):
+                    w.add_(_wts(w.shape, 60 + i, device) * (0.1 * w.abs().max()))
+            cache.refresh()
+            check(run(cache.h), run(None), 'refreshed')
+            st = cache.stats()
+            assert st == dict(layouts=WCACHE_LAYOUTS, hits=2 * WCACHE_REQUESTS, misses=0, committed=True), st
+        finally:
+            cnn.WCACHE = None
 
 
 def case_conv_plan_from_shape(device):
@@ -436,15 +426,11 @@ def case_disp_pose_golden(device):
     deepest BatchNorms normalise over 2-8 values and amplify the ~1e-5 tensor-core accumulation error ~500x
     (same net at 128x416 and up: see tests/step_cases.py)."""
     from cc_b200 import _lib
-    saved = cnn.CONV_IMPL
-    try:
-        cnn.CONV_IMPL = _lib.IMPL_FFMA
+    with conv_impl(_lib.IMPL_FFMA):
         _disp_pose_golden(device, 5e-4)
-        if device.type == 'cuda':
-            cnn.CONV_IMPL = _lib.IMPL_AUTO
+    if device.type == 'cuda':
+        with conv_impl(_lib.IMPL_AUTO):
             _disp_pose_golden(device, 5e-2)
-    finally:
-        cnn.CONV_IMPL = saved
 
 
 def _disp_pose_golden(device, gtol):

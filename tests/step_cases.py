@@ -2,11 +2,12 @@
 train_step (reference train.py:445-568 restated) on identical seeded inputs / weights."""
 import math
 import torch
-from tests.util import assert_close, rel_err
-from cc_b200 import synth, nn as cnn, pyramid, _lib
+from tests.util import assert_close, rel_err, conv_impl
+from cc_b200 import synth, nn as cnn, pyramid, _lib, models as CM
 from cc_b200.optim import FlatAdam
-from cc_b200.train_step import Trainer, HP
+from cc_b200.train_step import Trainer, HP, NETS_OF
 from oracle import step as OS, nets as ON
+from tests import flownetc6_cases as FC6
 
 U32 = 2.0 ** -24           # fp32 unit roundoff
 TINY32 = 1e-44             # a few fp32 subnormal steps: the absolute error of a product that underflows
@@ -131,7 +132,8 @@ def case_flat_adam(device):
     assert abs(opt.state[0].item() - 3.0) < 1e-6
 
 
-def _oracle_params_as_state_dicts(P):
+def oracle_state_dicts(P):
+    """The oracle's parameter dicts as state dicts for Trainer / build_nets: detached copies."""
     return {n: {k: v.detach().clone() for k, v in d.items()} for n, d in P.items()}
 
 
@@ -142,7 +144,7 @@ def case_step_cfg1(device, B=2, H=128, W=416, steps=2, gtol=4e-3):
     tgt, refs = synth.frames(B, H, W, seed=50)
     K, Kinv = synth.intrinsics(B, H, W)
     P = OS.make_params('cfg1')
-    tr = Trainer('cfg1', device, state_dicts=_oracle_params_as_state_dicts(P))
+    tr = Trainer('cfg1', device, state_dicts=oracle_state_dicts(P))
     oopt = OS.Adam(OS.all_params(P), HP['lr'], HP['beta1'], HP['beta2'])
     dt, dr, dK, dKi = tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device)
     for s in range(steps):
@@ -170,7 +172,7 @@ def case_step_cfg3(device, B=2, H=64, W=128):
     P = OS.make_params('cfg3')
     lo, auxo = OS.loss_cfg3(P, tgt, refs, K, Kinv)
     lo.backward()
-    nets = build_nets('cfg3', device, state_dicts=_oracle_params_as_state_dicts(P))
+    nets = build_nets('cfg3', device, state_dicts=oracle_state_dicts(P))
     dt, dr, dK, dKi = tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device)
     lc, auxc = loss_cfg3(nets, dt, dr, dK, dKi)
     lc.backward()
@@ -209,10 +211,38 @@ def _assert_same(got, want, what, skip=()):
             raise AssertionError(f'{what}: {k} differs in {int((a != b).sum())} of {a.numel()} elements (max {d.max().item():.3e})')
 
 
-def case_step_graph_vs_eager(device, cfg, B=2, H=64, W=128, loss_tol=None, seed=70):
+def group_range(opt, gi):
+    """(lo, hi) of group gi in the flat buffers (contiguous in the constructor layout)."""
+    offs = sorted(opt.offset[p] for p in opt.groups[gi])
+    lo, hi = offs[0][0], offs[-1][0] + offs[-1][1]
+    assert hi - lo == sum(k for _, k in offs), 'group %d is not contiguous' % gi
+    return lo, hi
+
+
+def assert_groups_step(tr, before, after, want_t, what):
+    """Per net of the trainer: an active group's range within assert_adam_step's bound for its own t (want_t[name]); a
+    frozen group's parameters, moments and counter bit-unchanged and its gradient range exactly zero."""
+    o = tr.opt
+    for gi, name in enumerate(NETS_OF[tr.cfg]):
+        lo, hi = group_range(o, gi)
+        sl = slice(lo, hi)
+        st = slice(4 * gi, 4 * gi + 4)
+        if name in tr.fixed:
+            for k in ('flat_p', 'exp_avg', 'exp_avg_sq'):
+                assert torch.equal(after[k][sl], before[k][sl]), f'{what}: fixed {name}: {k} changed'
+            assert torch.equal(after['state'][st], before['state'][st]), f'{what}: fixed {name}: step counter changed'
+            assert not bool(after['flat_g'][sl].any()), f'{what}: fixed {name} received a gradient'
+        else:
+            assert_adam_step((before['flat_p'][sl], before['exp_avg'][sl], before['exp_avg_sq'][sl]),
+                             (after['flat_p'][sl], after['exp_avg'][sl], after['exp_avg_sq'][sl], after['state'][st]),
+                             after['flat_g'][sl], want_t[name], o.lr, o.betas, o.eps, o.grad_scale, f'{what}: {name}')
+
+
+def case_step_graph_vs_eager(device, cfg, B=2, H=64, W=128, loss_tol=None, seed=70, flownet='Back2Future', fixed=()):
     """The step the benchmark times - Trainer.capture() + replay(): a CUDA graph whose convolutions read a committed
-    weight cache and whose Adam keeps its step count on the device - against Trainer.step() run eagerly, over three
-    steps on three different seeded batches, both trainers built from the same oracle weights.
+    weight cache and whose Adam keeps its step counts on the device - against Trainer.step() run eagerly, over three
+    steps on three different seeded batches, both trainers Trainer(cfg, flownet=flownet, fixed=fixed) built from the same
+    oracle weights (FlowNetC6: flownetc6_cases.step_flow_params).
 
       * replay i equals eager step i BIT FOR BIT: loss, flat gradient / parameters / Adam moments, optimiser state,
         BatchNorm buffers.  (Eager step 0 prepares weights per call while recording the cache; every later step and
@@ -221,72 +251,91 @@ def case_step_graph_vs_eager(device, cfg, B=2, H=64, W=128, loss_tol=None, seed=
         snapshot taken before it, bit for bit (the flat gradient still holds warm-up gradients; the graph zeroes it).
         capture() restores the snapshot after the warm-up and again after capturing, which executes nothing, so this
         fails only when neither restore runs.
-      * each replay's parameters / moments / state against the fp64 Adam reference (adam_reference) applied to that
-        replay's own gradient, from the state recorded before it.
-      * loss_tol: eager losses against oracle.step.train_step run on the CPU for the same three steps.
-      * replay() refuses a graph whose learning rate is stale.
+      * each replay, per Adam group (assert_groups_step): a trained net's parameters / moments / step counter against
+        the fp64 Adam reference (adam_reference) applied to that replay's own gradient, from the state recorded before
+        it; a fixed net bit-unchanged with an exactly zero gradient.
+      * the weight cache is committed, hit, and never missed; the flow net is the one asked for.
+      * loss_tol: eager losses against oracle.step.train_step run on the CPU for the same three steps, the fixed nets'
+        oracle parameters excluded from its Adam.
+      * replay() refuses a graph whose learning rate is stale, and with `fixed`, one captured under another fixed set.
     The trainers run one after the other (full size: one set of activations at a time)."""
     batches = []
     for i in range(3):
         tgt, refs = synth.frames(B, H, W, seed=seed + i)
         batches.append([tgt] + refs + list(synth.intrinsics(B, H, W)))
     P = OS.make_params(cfg)
-    sd = _oracle_params_as_state_dicts(P)
-    saved = (cnn.GRAPH_LIVE, cnn.CONV_IMPL)
+    if flownet == 'FlowNetC6':
+        P['flow'] = ON.clone_params(FC6.step_flow_params(), requires_grad=True)
+    sd = oracle_state_dicts(P)
+    tag = f'{cfg} {B}x{H}x{W}' + ('' if flownet == 'Back2Future' else ' ' + flownet) + (f' fixed={fixed}' if fixed else '')
+    saved = cnn.GRAPH_LIVE
     tr = None
     try:
-        cnn.CONV_IMPL = _lib.IMPL_AUTO
-        tr = Trainer(cfg, device, state_dicts=sd)
-        eager = []
-        for b in batches:
-            d = [t.to(device) for t in b]
-            loss, _ = tr.step(d[0], d[1:5], d[5], d[6])
-            eager.append(_record(tr, loss))
-        del tr, loss, d
-        tr = None
-        torch.cuda.empty_cache()
+        with conv_impl(_lib.IMPL_AUTO):
+            tr = Trainer(cfg, device, state_dicts=sd, flownet=flownet, fixed=fixed)
+            eager = []
+            for b in batches:
+                d = [t.to(device) for t in b]
+                loss, _ = tr.step(d[0], d[1:5], d[5], d[6])
+                eager.append(_record(tr, loss))
+            del tr, loss, d
+            tr = None
+            torch.cuda.empty_cache()
 
-        tr = Trainer(cfg, device, state_dicts=sd)
-        static = [t.to(device) for t in batches[0]]
-        snap = _record(tr)
-        tr.capture(static[0], static[1:5], static[5], static[6])
-        _assert_same(_record(tr), snap, f'{cfg}: state after capture()', skip=('flat_g',))
-        prev = snap
-        o = tr.opt
-        for i, b in enumerate(batches):
-            for s, h in zip(static, b):
-                s.copy_(h)
-            cur = _record(tr, tr.replay())
-            _assert_same(cur, eager[i], f'{cfg}: replay {i} vs eager step {i}')
-            assert_adam_step((prev['flat_p'], prev['exp_avg'], prev['exp_avg_sq']),
-                             (cur['flat_p'], cur['exp_avg'], cur['exp_avg_sq'], cur['state']), cur['flat_g'], i + 1,
-                             o.lr, o.betas, o.eps, o.grad_scale, f'{cfg}: Adam of replay {i}')
-            prev = cur
-        lr = o.lr
-        o.lr = lr * 0.5
-        try:
-            tr.replay()
-            raise RuntimeError('replay() ran a graph captured with another learning rate')
-        except AssertionError:
-            pass
-        finally:
-            o.lr = lr
+            tr = Trainer(cfg, device, state_dicts=sd, flownet=flownet, fixed=fixed)
+            if 'flow' in tr.nets:
+                assert isinstance(tr.nets['flow'], getattr(CM, flownet)), type(tr.nets['flow'])
+            static = [t.to(device) for t in batches[0]]
+            snap = _record(tr)
+            tr.capture(static[0], static[1:5], static[5], static[6])
+            _assert_same(_record(tr), snap, f'{tag}: state after capture()', skip=('flat_g',))
+            assert tr.wcache is not None and tr.wcache.committed
+            prev = snap
+            for i, b in enumerate(batches):
+                for s, h in zip(static, b):
+                    s.copy_(h)
+                cur = _record(tr, tr.replay())
+                _assert_same(cur, eager[i], f'{tag}: replay {i} vs eager step {i}')
+                assert_groups_step(tr, prev, cur, {n: i + 1 for n in NETS_OF[cfg]}, f'{tag}: Adam of replay {i}')
+                prev = cur
+            stats = tr.wcache.stats()
+            assert stats['hits'] > 0 and stats['misses'] == 0, stats
+            o = tr.opt
+            lr = o.lr
+            o.lr = lr * 0.5
+            try:
+                tr.replay()
+                raise RuntimeError('replay() ran a graph captured with another learning rate')
+            except AssertionError:
+                pass
+            finally:
+                o.lr = lr
+            if fixed:
+                tr.set_fixed(fixed[:-1])
+                try:
+                    tr.replay()
+                    raise RuntimeError('replay() ran a graph captured under another fixed set')
+                except AssertionError:
+                    pass
     finally:
         if tr is not None:
             tr.graph = None
         tr = None
         torch.cuda.synchronize()
-        cnn.GRAPH_LIVE, cnn.CONV_IMPL = saved
+        cnn.GRAPH_LIVE = saved
         pyramid.clear()
     if loss_tol is not None:
+        for n in fixed:
+            for t in P[n].values():
+                t.requires_grad_(False)
         oopt = OS.Adam(OS.all_params(P), HP['lr'], HP['beta1'], HP['beta2'])
         errs = []
         for i, b in enumerate(batches):
-            lo, _ = OS.train_step(cfg, P, oopt, b[0], b[1:5], b[5], b[6])
+            lo, _ = OS.train_step(cfg, P, oopt, b[0], b[1:5], b[5], b[6], flownet=flownet)
             errs.append(rel_err(eager[i]['loss'], lo))
-        assert max(errs) <= loss_tol, f'{cfg} {B}x{H}x{W}: relative loss errors of steps 0-2 vs the oracle ' \
+        assert max(errs) <= loss_tol, f'{tag}: relative loss errors of steps 0-2 vs the oracle ' \
                                       f'{["%.2e" % e for e in errs]}, bar {loss_tol:.0e}'
-        print(f'{cfg} {B}x{H}x{W}: loss vs oracle {["%.2e" % e for e in errs]}')
+        print(f'{tag}: loss vs oracle {["%.2e" % e for e in errs]}')
 
 
 STEP_CASES_SIM = [case_flat_adam, case_adam_fp64]

@@ -2,33 +2,19 @@
 compiled for the CPU simulator (tests/sim) against the fixture frozen from the reference and against Pillow itself on
 random images, the numpy restatements of Pillow against Pillow, and the host-side parameter draw.  The same fixture cases
 and the full-size ones run on the H100 in tests/test_gpu_augment.py."""
-import os
 import random
-import sys
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'sim'))
-
-from cc_b200 import input_pipeline as CI               # noqa: E402
-from tests import augment_cases as AC, augment_oracle as AO   # noqa: E402
+from cc_b200 import input_pipeline as CI
+from tests import augment_cases as AC, augment_oracle as AO
+from tests.util import sim_lib      # noqa: F401  (module fixture: the simulator library)
 
 CPU = torch.device('cpu')
 ROTATE_CASES = [((23, 37), a) for a in (0.2, 1.5, 4.4, 8.05, 9.9)] + [((12, 9), 6.1), ((1, 5), 3.0)]
 RESIZE_CASES = [((30, 50), (20, 34)), ((19, 23), (31, 40)), ((16, 40), (16, 27)), ((20, 20), (13, 20)), ((9, 11), (9, 11)),
                 ((40, 7), (6, 3)), ((5, 6), (17, 29))]
-
-
-@pytest.fixture(scope='module')
-def sim_lib():
-    import build_sim
-    from cc_b200 import _lib
-    prev = (_lib._lib, _lib._is_sim)
-    _lib.use_library(build_sim.build())
-    assert _lib.is_simulator()
-    yield
-    _lib._lib, _lib._is_sim = prev
 
 
 @pytest.mark.parametrize('case', AC.AUGMENT_CASES, ids=lambda f: f.__name__)

@@ -4,6 +4,7 @@ import os
 import sys
 import torch
 import torch.multiprocessing as mp
+from tests.util import sim_lib      # noqa: F401  (module fixture: the simulator library)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -131,40 +132,33 @@ def test_two_rank_overlapped_buckets_match_single_allreduce():
     assert all(torch.equal(ret[0][2][k], ret[1][2][k]) for k in ret[0][2] if 'running' not in k and 'num_batches' not in k)
 
 
-def test_flat_adam_checkpoint_roundtrip_with_torch_adam():
+def test_flat_adam_checkpoint_roundtrip_with_torch_adam(sim_lib):
     """FlatAdam.state_dict() loads into torch.optim.Adam and back (reference utils.py:55-63 saves optimizer.state_dict())."""
-    sys.path.insert(0, os.path.join(ROOT, 'tests', 'sim'))
-    import build_sim
-    from cc_b200 import _lib, nn as cnn
+    from cc_b200 import nn as cnn
     from cc_b200.optim import FlatAdam
-    prev = (_lib._lib, _lib._is_sim)
-    _lib.use_library(build_sim.build())
-    try:
-        torch.manual_seed(1)
-        net = torch.nn.Sequential(cnn.Conv2d(3, 4, 3, padding=1, act='relu'), cnn.Conv2d(4, 2, 3, padding=1))
-        opt = FlatAdam(net.parameters(), lr=1e-2)
-        x = torch.randn(2, 3, 5, 6)
-        for _ in range(2):
-            opt.zero_grad(); (net(x) ** 2).mean().backward(); opt.step()
-        sd = opt.state_dict()
-        ref = torch.optim.Adam([torch.nn.Parameter(p.detach().clone()) for p in net.parameters()], lr=1e-2)
-        ref.load_state_dict(sd)                                      # torch accepts it
-        opt.relayout(list(reversed(opt.params)))                       # layout change must not change the checkpoint
-        sd2 = opt.state_dict()
-        for i in sd['state']:
-            assert torch.equal(sd['state'][i]['exp_avg_sq'], sd2['state'][i]['exp_avg_sq'])
-        opt3 = FlatAdam([torch.nn.Parameter(p.detach().clone()) for p in net.parameters()], lr=5e-3)
-        opt3.load_state_dict(ref.state_dict())                        # and back from torch
-        assert opt3.lr == 1e-2 and abs(float(opt3.state[0]) - 2.0) < 1e-6
-        for i, p in enumerate(opt3.params):
-            assert torch.allclose(opt3._views(opt3.exp_avg, p), sd['state'][i]['exp_avg'])
-        # a stray gradient installed by net.zero_grad(set_to_none=True) + a torch-produced grad is folded in, not dropped
-        opt.zero_grad()
-        p0 = opt.params[0]
-        p0.grad = None
-        p0.grad = torch.ones_like(p0)
-        before = p0.detach().clone()
-        opt.step()
-        assert not torch.equal(before, p0.detach()) and p0.grad.data_ptr() == p0._ccb_grad.data_ptr()
-    finally:
-        _lib._lib, _lib._is_sim = prev
+    torch.manual_seed(1)
+    net = torch.nn.Sequential(cnn.Conv2d(3, 4, 3, padding=1, act='relu'), cnn.Conv2d(4, 2, 3, padding=1))
+    opt = FlatAdam(net.parameters(), lr=1e-2)
+    x = torch.randn(2, 3, 5, 6)
+    for _ in range(2):
+        opt.zero_grad(); (net(x) ** 2).mean().backward(); opt.step()
+    sd = opt.state_dict()
+    ref = torch.optim.Adam([torch.nn.Parameter(p.detach().clone()) for p in net.parameters()], lr=1e-2)
+    ref.load_state_dict(sd)                                      # torch accepts it
+    opt.relayout(list(reversed(opt.params)))                       # layout change must not change the checkpoint
+    sd2 = opt.state_dict()
+    for i in sd['state']:
+        assert torch.equal(sd['state'][i]['exp_avg_sq'], sd2['state'][i]['exp_avg_sq'])
+    opt3 = FlatAdam([torch.nn.Parameter(p.detach().clone()) for p in net.parameters()], lr=5e-3)
+    opt3.load_state_dict(ref.state_dict())                        # and back from torch
+    assert opt3.lr == 1e-2 and abs(float(opt3.state[0]) - 2.0) < 1e-6
+    for i, p in enumerate(opt3.params):
+        assert torch.allclose(opt3._views(opt3.exp_avg, p), sd['state'][i]['exp_avg'])
+    # a stray gradient installed by net.zero_grad(set_to_none=True) + a torch-produced grad is folded in, not dropped
+    opt.zero_grad()
+    p0 = opt.params[0]
+    p0.grad = None
+    p0.grad = torch.ones_like(p0)
+    before = p0.detach().clone()
+    opt.step()
+    assert not torch.equal(before, p0.detach()) and p0.grad.data_ptr() == p0._ccb_grad.data_ptr()

@@ -2,45 +2,30 @@
 module's state_dict contract, and the dilated cost-volume kernels compiled for the CPU simulator (tests/sim) against
 fp64, including planted defects the bound must catch.  The whole network runs on the H100 in
 tests/test_gpu_flownetc6.py (on the simulator it would take far longer than the rest of this suite)."""
-import os
-import sys
 import time
 import pytest
 import torch
 import torch.nn.functional as F
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'sim'))
-
-from cc_b200 import models as CM          # noqa: E402
-from cc_b200.train_step import build_nets  # noqa: E402
-from oracle import nets as ON              # noqa: E402
-from tests import flownetc6_cases as FC, flownetc6_oracle as O6   # noqa: E402
-from tests.util import golden              # noqa: E402
+from cc_b200 import models as CM
+from cc_b200.train_step import build_nets
+from oracle import nets as ON
+from tests import flownetc6_cases as FC
+from tests.util import golden, sim_lib    # noqa: F401  (sim_lib: module fixture, the simulator library)
 
 NTOL = 2e-5        # tests/test_oracle_golden.py: module vs functional conv algorithms
 
 
-@pytest.fixture(scope='module')
-def sim_lib():
-    import build_sim
-    from cc_b200 import _lib
-    prev = (_lib._lib, _lib._is_sim)
-    _lib.use_library(build_sim.build())
-    assert _lib.is_simulator()
-    yield
-    _lib._lib, _lib._is_sim = prev
-
-
 def test_oracle_matches_fixture():
     P = {k: v.detach().clone().requires_grad_(True) for k, v in FC.fixture_weights().items()}
-    assert sum(v.numel() for v in P.values()) == O6.NPARAMS == int(golden(FC.FIXTURE)['nparams'])
+    assert sum(v.numel() for v in P.values()) == ON.C6_NPARAMS == int(golden(FC.FIXTURE)['nparams'])
     tgt, ref = FC.fixture_inputs('cpu')
-    outs = O6.flownetc6_forward(P, tgt, ref)
+    outs = ON.flownetc6_forward(P, tgt, ref)
     loss = sum((x * FC._wts(x.shape, FC.WTS_SEED + i, 'cpu')).sum() for i, x in enumerate(outs))
     names = FC.grad_names()
     grads = dict(zip(names, torch.autograd.grad(loss, [P[n] for n in names])))
     with torch.no_grad():
-        ev = O6.flownetc6_forward(P, tgt, ref, training=False)
+        ev = ON.flownetc6_forward(P, tgt, ref, training=False)
     FC.check_against_fixture(outs, grads, ev, NTOL, NTOL)
 
 
@@ -61,7 +46,7 @@ def test_module_state_dict_matches_reference():
     net = CM.FlowNetC6()
     assert {k: tuple(v.shape) for k, v in net.state_dict().items()} == FC.fixture_state_dict_keys()
     assert list(net.state_dict()) == list(FC.fixture_state_dict_keys())
-    assert sum(p.numel() for p in net.parameters()) == O6.NPARAMS
+    assert sum(p.numel() for p in net.parameters()) == ON.C6_NPARAMS
     with pytest.raises(NotImplementedError):
         CM.FlowNetC6(batchNorm=True)
     with pytest.raises(NotImplementedError):
@@ -74,12 +59,6 @@ def test_build_nets_flownet_choice():
     assert isinstance(build_nets('cfg2', 'cpu')['flow'], CM.Back2Future)
     with pytest.raises(ValueError):
         build_nets('cfg2', 'cpu', flownet='SpyNet')
-
-
-def test_correlation_restatement_at_dilation_1_is_back2futures():
-    g = torch.Generator().manual_seed(3)
-    a, b = torch.randn(2, 5, 7, 11, generator=g), torch.randn(2, 5, 7, 11, generator=g)
-    assert torch.equal(O6.spatial_correlation_sample(a, b, 9, 1), ON.spatial_correlation_sample(a, b, 9))
 
 
 def test_corr441d_sim_vs_fp64(sim_lib):
@@ -104,7 +83,7 @@ def test_corr441d_planted_defects_fail_the_bound(sim_lib):
     bad[:, j0::FC.N] = 0
     assert _flagged_fwd(f1, f2, bad)
     # forward: the second staged channel group (channels 8..12) missing from every sum
-    part = O6.spatial_correlation_sample(f1[:, :8], f2[:, :8]).reshape(B, FC.N * FC.N, h, w) / C
+    part = FC.corr441d_sample(f1[:, :8], f2[:, :8]) / C
     assert _flagged_fwd(f1, f2, F.leaky_relu(part, 0.1))
     # d f1: the terms of displacement column j0 dropped for every i
     dz = torch.where(out > 0, go, go * FC.SLOPE32)

@@ -7,24 +7,11 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
+from tests import frozen_cases as FC
+from tests.util import sim_lib      # noqa: F401  (module fixture: the simulator library)
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, 'tests', 'sim'))
-
-
-@pytest.fixture(scope='module', autouse=True)
-def sim_lib():
-    import build_sim
-    from cc_b200 import _lib, pyramid
-    prev = (_lib._lib, _lib._is_sim)
-    _lib.use_library(build_sim.build())
-    assert _lib.is_simulator()
-    pyramid.clear()
-    yield
-    _lib._lib, _lib._is_sim = prev
-    pyramid.clear()
-
-
-from tests import frozen_cases as FC   # noqa: E402
+pytestmark = pytest.mark.usefixtures('sim_lib')
 
 
 @pytest.mark.parametrize('case', [FC.case_adam_ranges_fp64, FC.case_adam_one_range_is_adam_step, FC.case_flat_adam_phases,

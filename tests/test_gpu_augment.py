@@ -2,18 +2,11 @@
 tests/augment_cases.py and full-size runs against the numpy restatements of Pillow (tests/augment_oracle.py)."""
 import pytest
 import torch
-from cc_b200 import _lib
 from tests import augment_cases as AC
+from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library)
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 DEV = torch.device('cuda:0')
-
-
-@pytest.fixture(scope='module', autouse=True)
-def cuda_lib():
-    _lib._lib = None                      # the real library, not a simulator build
-    assert not _lib.is_simulator(), 'GPU tests must run on the sm_90a library'
-    yield
 
 
 @pytest.mark.parametrize('case', AC.AUGMENT_CASES, ids=lambda f: f.__name__)

@@ -3,9 +3,10 @@ against the oracle, its CUDA-graph replay, phase switches with checkpoints, a fi
 and the photometric loss's value-only paths at full size."""
 import pytest
 import torch
-from tests import frozen_cases as FC
+from tests import frozen_cases as FC, step_cases as SC
+from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library)
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 DEV = torch.device('cuda:0')
 
 
@@ -15,8 +16,10 @@ def test_canonical_step_vs_oracle():
 
 @pytest.mark.parametrize('size', [(2, 64, 128), (4, 256, 832)], ids=lambda s: 'b%d_%dx%d' % s)
 def test_canonical_graph_replay(size):
+    """capture() + three replay()s of the canonical step equal three eager steps bit for bit; replay() refuses after
+    set_fixed()."""
     B, H, W = size
-    FC.case_canonical_graph_vs_eager(DEV, B, H, W)
+    SC.case_step_graph_vs_eager(DEV, 'cfg3', B, H, W, fixed=('mask', 'flow'))
 
 
 def test_phase_switch_and_checkpoints():

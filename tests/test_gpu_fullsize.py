@@ -4,20 +4,15 @@ from the reference's real train() body.  See tests/fullsize_cases.py for the bar
 import pytest
 import torch
 from tests import fullsize_cases as FC
+from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library; the noise-floor run needs TF32 off)
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 
 
 @pytest.fixture(scope='module', autouse=True)
-def cuda_lib():
-    from cc_b200 import _lib, pyramid, nn as cnn
-    _lib._lib = None
-    assert not _lib.is_simulator(), 'GPU tests must run on the sm_90a library'
+def production_dispatch(device_lib):
+    from cc_b200 import _lib, nn as cnn
     assert cnn.CONV_IMPL == _lib.IMPL_AUTO, 'full-size parity is defined on the production dispatch'
-    pyramid.clear()
-    torch.backends.cudnn.allow_tf32 = False       # the noise-floor run (oracle on the GPU) must be fp32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
 
 
 @pytest.mark.parametrize('cfg', ['cfg1', 'cfg2', 'cfg3'])

@@ -3,19 +3,9 @@ oracle and the golden fixtures, on the H100."""
 import pytest
 import torch
 from tests import kernel_cases as KC
+from tests.util import conv_impl, device_lib      # noqa: F401  (device_lib: module fixture, the sm_90a library)
 
-pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope='module', autouse=True)
-def cuda_lib():
-    from cc_b200 import _lib, pyramid
-    _lib._lib = None                      # make sure the real library (not a simulator) is bound
-    assert not _lib.is_simulator(), 'GPU tests must run on the sm_90a library'
-    pyramid.clear()
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 
 
 @pytest.mark.parametrize('case', KC.ALL_CASES, ids=lambda f: f.__name__)
@@ -132,15 +122,11 @@ def test_conv_weight_cache():
 
 
 def test_train_step_cfg1_vs_oracle():
-    from cc_b200 import nn as cnn, _lib
-    saved = cnn.CONV_IMPL
-    try:
-        cnn.CONV_IMPL = _lib.IMPL_FFMA
+    from cc_b200 import _lib
+    with conv_impl(_lib.IMPL_FFMA):
         SC.case_step_cfg1(torch.device('cuda:0'), gtol=4e-3)
-        cnn.CONV_IMPL = _lib.IMPL_AUTO
+    with conv_impl(_lib.IMPL_AUTO):
         SC.case_step_cfg1(torch.device('cuda:0'), gtol=5e-2)
-    finally:
-        cnn.CONV_IMPL = saved
 
 
 def test_conv_tensor_core_3xtf32():

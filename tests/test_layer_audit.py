@@ -9,9 +9,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 from tests import layer_audit as LA
-from tests.test_sim_kernels import sim_lib       # noqa: F401  (module fixture: the simulator library)
+from tests.util import conv_impl, sim_lib      # noqa: F401  (sim_lib: module fixture, the simulator library)
 from cc_b200 import nn as cnn, _lib, synth, models as CM
 from oracle import nets as ON
+
+pytestmark = pytest.mark.usefixtures('sim_lib')
 
 
 def _gen(seed):
@@ -235,16 +237,12 @@ def _net_outputs(which):
 def test_audit_simulator_nets(which):
     """One forward and one backward (of a seeded weighted sum of the outputs) of each net on the simulator build, every
     layer call audited; every Conv2d / ConvTranspose2d / BatchNorm2d module is audited forward and backward."""
-    saved = cnn.CONV_IMPL
-    try:
-        cnn.CONV_IMPL = _lib.IMPL_FFMA
+    with conv_impl(_lib.IMPL_FFMA):
         net, run = _net_outputs(which)
         net.train()
         with LA.LayerAudit(nets={which: net}, tag='sim_' + which) as audit:
             outs = run()
             sum((o * _wts(o.shape, 500 + i)).sum() for i, o in enumerate(outs)).backward()
-    finally:
-        cnn.CONV_IMPL = saved
     want = {which + ('.' + n if n else '') for n, m in net.named_modules()     # occlusion decoders: not run in training
             if isinstance(m, (cnn.Conv2d, cnn.ConvTranspose2d, cnn.BatchNorm2d)) and not n.startswith('decoder_occ')}
     for phase in ('fwd', 'bwd'):

@@ -8,10 +8,12 @@ loss layer at b2 64x128 with 4 levels, and a sweep over the template paths the s
 import pytest
 import torch
 from tests import loss_audit as LA
-from tests.test_sim_kernels import sim_lib       # noqa: F401  (module fixture: the simulator library)
+from tests.util import sim_lib      # noqa: F401  (module fixture: the simulator library)
 from cc_b200 import synth, _lib, loss_functions as CL, inverse_warp as CW, pyramid as CP
 import torch.nn.functional as F
 from oracle import losses as OL, geometry as OG, ssim as OSSIM
+
+pytestmark = pytest.mark.usefixtures('sim_lib')
 
 f32 = torch.float32
 

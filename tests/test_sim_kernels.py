@@ -2,25 +2,11 @@
 (tests/sim), checked against the oracle and the golden fixtures - so that indexing / reduction /
 derivation bugs are caught in the GPU-less container.  The same cases run on the real H100 in
 tests/test_gpu_parity.py."""
-import os
-import sys
 import pytest
 import torch
+from tests.util import sim_lib      # noqa: F401  (module fixture: the simulator library)
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'sim'))
-
-
-@pytest.fixture(scope='module', autouse=True)
-def sim_lib():
-    import build_sim
-    from cc_b200 import _lib, pyramid
-    prev = (_lib._lib, _lib._is_sim)
-    _lib.use_library(build_sim.build())
-    assert _lib.is_simulator()
-    pyramid.clear()
-    yield
-    _lib._lib, _lib._is_sim = prev
-    pyramid.clear()
+pytestmark = pytest.mark.usefixtures('sim_lib')
 
 
 from tests import kernel_cases as KC   # noqa: E402

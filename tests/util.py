@@ -1,10 +1,67 @@
-"""Shared helpers for the parity tests."""
+"""Shared helpers for the parity tests, and the fixtures that bind a build of the library for a test module."""
+import contextlib
 import os
+import sys
 import numpy as np
+import pytest
 import torch
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+HERE = os.path.dirname(os.path.abspath(__file__))
+GOLDEN = os.path.join(HERE, 'golden')
+SIM = os.path.join(HERE, 'sim')
 _cache = {}
+
+
+@contextlib.contextmanager
+def _bound(path):
+    """libccb200 at `path` (None: the in-tree sm_90a build) bound for the block, the pyramid memo cleared on both sides
+    (it holds tensors of the other build's calls); the previous binding is restored afterwards."""
+    from cc_b200 import _lib, pyramid
+    prev = (_lib._lib, _lib._is_sim)
+    if path is None:
+        _lib._lib = None
+        _lib.lib()
+    else:
+        _lib.use_library(path)
+    pyramid.clear()
+    try:
+        yield _lib
+    finally:
+        _lib._lib, _lib._is_sim = prev
+        pyramid.clear()
+
+
+@pytest.fixture(scope='module')
+def sim_lib():
+    """The product kernels compiled by g++ against the CPU simulator (tests/sim)."""
+    if SIM not in sys.path:
+        sys.path.insert(0, SIM)
+    import build_sim
+    with _bound(build_sim.build()) as lib:
+        assert lib.is_simulator()
+        yield
+
+
+@pytest.fixture(scope='module')
+def device_lib():
+    """The sm_90a library, with torch's TF32 off (torch computes some of the checks on the device in fp32)."""
+    with _bound(None) as lib:
+        assert not lib.is_simulator(), 'GPU tests must run on the sm_90a library'
+        torch.backends.cudnn.allow_tf32 = False
+        torch.backends.cuda.matmul.allow_tf32 = False
+        yield
+
+
+@contextlib.contextmanager
+def conv_impl(impl):
+    """cc_b200.nn's convolutions dispatched to `impl` (cc_b200._lib.IMPL_*) inside the block."""
+    from cc_b200 import nn as cnn
+    saved = cnn.CONV_IMPL
+    cnn.CONV_IMPL = impl
+    try:
+        yield
+    finally:
+        cnn.CONV_IMPL = saved
 
 
 def golden(name):
