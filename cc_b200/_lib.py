@@ -132,6 +132,8 @@ _SIGS = {
     'ccb_flow_metrics': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _F, _P, _P, _P, _P]),
     'ccb_depth_errors_workspace_bytes': (_LL, [_I, _I, _I]),
     'ccb_depth_errors': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
+    'ccb_mask_iou_workspace_bytes': (_LL, [_I, _I, _I, _I, _I]),
+    'ccb_mask_iou': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P, _LL, _P, _P]),
     'ccb_prep_frames': (_I, [_P, C.POINTER(_P), _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     'ccb_prep_frames_unit': (_I, [_P, C.POINTER(_P), _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     'ccb_rotate_frames_u8': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),

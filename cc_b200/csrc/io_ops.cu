@@ -11,7 +11,10 @@
 //       RandomRotate (:75-85) as Pillow's bilinear affine transform, Scale (:120-137) as Pillow's 8-bit resampler,
 //       NormalizeLocally (:33-44) as per-sample channel statistics.
 //
-// All reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize).
+//   N3  motion segmentation scores: the three rigidity masks and the IoU counts of test_mask.py:129-156,224-262
+//
+// All floating-point reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize); the
+// segmentation counts are integer sums (atomics, the same in any order).
 #include "ccb_common.cuh"
 
 #ifdef CCB_CPU_SIM
@@ -550,6 +553,129 @@ __global__ void __launch_bounds__(256) normlocal_apply_kernel(const NormLocalArg
     }
 }
 
+// ================================================================================================
+// Motion segmentation scores (test_mask.py:129-134 and mask_error :224-262).  Per sample, at the nets' resolution h x w:
+//   bare     = 1 - (1 - e1)(1 - e2) > 0.5                        e1, e2: channels 1 and 2 of the mask net's eval output
+//   soft     = 1 - d / max(d),  d = sqrt(sum_c (flow_cam - flow)^2)   the maximum over the sample's whole map
+//   census   = soft > thresh,   combined = bare or census
+// and, over the ground-truth grid Hg x Wg, the confusion matrix n[pred][gt] of each mask read at the source pixel that
+// scipy.ndimage.zoom(order=0) reads, against gt = (obj_map != 0), counted where semantic_map == car_label.  A mask value 1
+// (rigid) is class 0: argmax([mask, 1 - mask]).
+// The census comparison decides integer counts, so d, the division and the subtraction are single correctly rounded
+// fp32 operations (no contraction): the counts are those of an IEEE evaluation of the expressions, operation by operation.
+// max(d) == 0 gives 0/0 = NaN and an empty census, as in the reference.
+struct MaskIouArgs {
+    const float* emask;             // [B, C, h, w]
+    const float* flow_cam;          // [B, 2, h, w]
+    const float* flow;              // [B, 2, h, w]
+    const float* obj;               // [B, Hg, Wg]
+    const float* sem;               // [B, Hg, Wg]
+    float* masks;                   // [B, 4, h, w] or null
+    unsigned long long* dmax;       // [B]: bit pattern of max(d), zero-extended
+    unsigned long long* counts;     // [B, 3, 2, 2]
+    int B, C, h, w, Hg, Wg;
+    float thresh, car;
+};
+
+__device__ __forceinline__ float flow_gap(const MaskIouArgs& a, int b, long long p) {
+    const long long hw = (long long)a.h * a.w;
+    const float du = __fsub_rn(__ldg(a.flow_cam + 2ll * b * hw + p), __ldg(a.flow + 2ll * b * hw + p));
+    const float dv = __fsub_rn(__ldg(a.flow_cam + (2ll * b + 1) * hw + p), __ldg(a.flow + (2ll * b + 1) * hw + p));
+    return __fsqrt_rn(__fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)));
+}
+
+// bit 0 combined, bit 1 census, bit 2 bare of source pixel p
+__device__ __forceinline__ unsigned mask_bits(const MaskIouArgs& a, int b, long long p, float dmax, float* soft_out) {
+    const long long hw = (long long)a.h * a.w;
+    const float e1 = __ldg(a.emask + ((long long)b * a.C + 1) * hw + p), e2 = __ldg(a.emask + ((long long)b * a.C + 2) * hw + p);
+    const bool bare = __fsub_rn(1.f, __fmul_rn(__fsub_rn(1.f, e1), __fsub_rn(1.f, e2))) > 0.5f;
+    const float soft = __fsub_rn(1.f, __fdiv_rn(flow_gap(a, b, p), dmax));
+    const bool census = soft > a.thresh;
+    *soft_out = soft;
+    return ((bare || census) ? 1u : 0u) | (census ? 2u : 0u) | (bare ? 4u : 0u);
+}
+
+// max(d) per sample on the bit patterns: d is non-negative or NaN, so unsigned order is value order with NaN on top
+// (torch's max propagates NaN too), and a maximum is the same in any order.
+__global__ void __launch_bounds__(256) mask_iou_max_kernel(const MaskIouArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.y;
+    const long long hw = (long long)a.h * a.w;
+    unsigned m = 0;
+    for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < hw; p += (long long)gridDim.x * 256) {
+        const unsigned k = __float_as_uint(flow_gap(a, b, p));
+        m = (k > m) ? k : m;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned k = __shfl_xor_sync(0xffffffffu, m, o);
+        m = (k > m) ? k : m;
+    }
+    if ((threadIdx.x & 31) == 0) atomicMax(a.dmax + b, (unsigned long long)m);
+}
+
+__global__ void __launch_bounds__(256) mask_iou_masks_kernel(const MaskIouArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.y;
+    const long long hw = (long long)a.h * a.w;
+    const float dmax = __uint_as_float((unsigned)a.dmax[b]);
+    float* out = a.masks + 4ll * b * hw;
+    for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < hw; p += (long long)gridDim.x * 256) {
+        float soft;
+        const unsigned bits = mask_bits(a, b, p, dmax, &soft);
+        out[p] = (bits & 1u) ? 1.f : 0.f;
+        out[hw + p] = (bits & 2u) ? 1.f : 0.f;
+        out[2 * hw + p] = (bits & 4u) ? 1.f : 0.f;
+        out[3 * hw + p] = soft;
+    }
+}
+
+// scipy.ndimage.zoom(order=0) with its default grid_mode=False: output index o reads the input at coordinate
+// o * (n_in - 1) / (n_out - 1), evaluated in fp64 as (quotient first, then the product) and rounded half up.
+__device__ __forceinline__ int zoom_nearest(int o, double step, int n_in) {
+    return min((int)floor(__dadd_rn(__dmul_rn((double)o, step), 0.5)), n_in - 1);
+}
+
+// One thread per ground-truth pixel; per-thread counters, one warp + block reduction at the end, then 64-bit integer
+// atomics: integer sums do not depend on the order, so the counts are the same on every run.
+__global__ void __launch_bounds__(256) mask_iou_count_kernel(const MaskIouArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ unsigned scratch[12 * 8];
+    const int b = blockIdx.y;
+    const long long ng = (long long)a.Hg * a.Wg;
+    const float dmax = __uint_as_float((unsigned)a.dmax[b]);
+    const double step_y = (a.Hg > 1) ? __ddiv_rn((double)(a.h - 1), (double)(a.Hg - 1)) : 1.0;
+    const double step_x = (a.Wg > 1) ? __ddiv_rn((double)(a.w - 1), (double)(a.Wg - 1)) : 1.0;
+    unsigned n[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};      // [mask][pred][gt]
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < ng; i += (long long)gridDim.x * 256) {
+        if (__ldg(a.sem + b * ng + i) != a.car) continue;        // the ignore label of mask_error
+        const int y = (int)(i / a.Wg), x = (int)(i - (long long)y * a.Wg);
+        const long long p = (long long)zoom_nearest(y, step_y, a.h) * a.w + zoom_nearest(x, step_x, a.w);
+        float soft;
+        const unsigned bits = mask_bits(a, b, p, dmax, &soft);
+        const unsigned gt = (__ldg(a.obj + b * ng + i) != 0.f) ? 1u : 0u;
+#pragma unroll
+        for (int m = 0; m < 3; ++m) {
+            const unsigned cell = (((bits >> m) & 1u) ? 0u : 2u) + gt;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) n[m * 4 + k] += (cell == (unsigned)k) ? 1u : 0u;
+        }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < 12; ++k) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) n[k] += __shfl_xor_sync(0xffffffffu, n[k], o);
+        if (lane == 0) scratch[k * 8 + warp] = n[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < 12) {
+        unsigned long long s = 0;
+        for (int wi = 0; wi < 8; ++wi) s += scratch[threadIdx.x * 8 + wi];
+        if (s) atomicAdd(a.counts + b * 12 + threadIdx.x, s);
+    }
+}
+
 }  // namespace ccb
 
 using namespace ccb;
@@ -619,6 +745,36 @@ extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H
     CCB_LAUNCH(depth_errors_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     CCB_LAUNCH(depth_errors_finalize, dim3(1), dim3(32), 0, stream, a, nb);
     return check_launch("depth_errors");
+}
+
+static int mask_iou_blocks(int H, int W) {
+    const long long g = ((long long)H * W + 255) / 256;
+    return (int)(g < 1 ? 1 : (g > NUM_SMS * 4 ? NUM_SMS * 4 : g));
+}
+
+extern "C" long long ccb_mask_iou_workspace_bytes(int B, int h, int w, int Hg, int Wg) {
+    if (B <= 0 || h <= 0 || w <= 0 || Hg <= 0 || Wg <= 0) return -1;
+    return (long long)B * (long long)sizeof(unsigned long long);
+}
+
+extern "C" int ccb_mask_iou(const float* emask, const float* flow_cam, const float* flow, const float* obj_map,
+                            const float* semantic_map, int B, int C, int h, int w, int Hg, int Wg, float thresh, int car_label,
+                            float* masks, void* work, long long work_bytes, long long* counts, ccb_stream_t stream) {
+    CCB_REQUIRE(emask && flow_cam && flow && obj_map && semantic_map && counts, CCB_ERR_ARG, "mask_iou: null pointer");
+    CCB_REQUIRE(C >= 3, CCB_ERR_ARG, "mask_iou: the mask net output needs channels 1 and 2, got %d channels", C);
+    CCB_REQUIRE(B > 0 && h > 0 && w > 0 && Hg > 0 && Wg > 0, CCB_ERR_ARG, "mask_iou: bad sizes");
+    const long long need = ccb_mask_iou_workspace_bytes(B, h, w, Hg, Wg);
+    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "mask_iou: workspace of %lld bytes, %lld needed", work_bytes, need);
+    MaskIouArgs a;
+    a.emask = emask; a.flow_cam = flow_cam; a.flow = flow; a.obj = obj_map; a.sem = semantic_map; a.masks = masks;
+    a.dmax = (unsigned long long*)work; a.counts = (unsigned long long*)counts;
+    a.B = B; a.C = C; a.h = h; a.w = w; a.Hg = Hg; a.Wg = Wg; a.thresh = thresh; a.car = (float)car_label;
+    cudaMemsetAsync(a.dmax, 0, (size_t)need, (cudaStream_t)stream);
+    cudaMemsetAsync(a.counts, 0, (size_t)B * 12 * sizeof(unsigned long long), (cudaStream_t)stream);
+    CCB_LAUNCH(mask_iou_max_kernel, dim3(mask_iou_blocks(h, w), B), dim3(256), 0, stream, a);
+    if (masks) CCB_LAUNCH(mask_iou_masks_kernel, dim3(mask_iou_blocks(h, w), B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(mask_iou_count_kernel, dim3(mask_iou_blocks(Hg, Wg), B), dim3(256), 0, stream, a);
+    return check_launch("mask_iou");
 }
 
 template <bool UNIT>

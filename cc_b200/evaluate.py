@@ -3,6 +3,8 @@
   depth_sample_errors   test_disp.py:84-150 (+ compute_errors :171-187)   abs_rel sq_rel rms log_rms a1 a2 a3
   pose_snippet_errors   test_pose.py:50-90  (+ compute_pose_error :107-122) ATE, RE of one snippet
   flow_sample_errors    test_flow.py:112-140                               the 8 EPE / Fl numbers of one KITTI-2015 pair
+  mask_sample_errors    test_mask.py:119-156 (+ mask_error :224-262)       tp fp fn per class of the three rigidity masks
+                        (motion_mask_counts: the masks and counts alone; mask_iou: the script's final IoUs :199-201)
 
 The scripts' dataset crawlers, image IO and visualisation are out of scope (SURVEY.md section 2); these functions take what the
 reference's `test_framework` iterators yield (uint8 HxWx3 frames, ground truth arrays) and return what the scripts
@@ -12,7 +14,7 @@ reference - they are a few hundred flops per sample."""
 import numpy as np
 import torch
 from .inverse_warp import pose2flow, pose_vec2mat
-from . import loss_functions as LF, models
+from . import _lib, loss_functions as LF, models
 
 
 def _to_net_input(img_hwc, device):
@@ -116,3 +118,60 @@ def flow_sample_errors(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kin
     obj = obj_map_gt.unsqueeze(1).type_as(flow_fwd)
     errs = list(LF.compute_all_epes(flow_gt, flow_cam, flow_fwd, combined)) + list(LF.compute_all_epes(flow_gt, flow_cam, flow_fwd, 1 - obj))
     return errs, total
+
+
+@torch.no_grad()
+def motion_mask_counts(emask, flow_cam, flow_fwd, obj_map_gt, semantic_map_gt, THRESH=0.94, want_masks=False):
+    """The rigidity masks of test_mask.py:129-134 and mask_error (:224-262) of each against the ground truth, per sample,
+    in one fused call (ccb_mask_iou): emask [B,C,h,w] the mask net's eval output, flow_cam / flow_fwd [B,2,h,w], obj_map_gt /
+    semantic_map_gt [B,Hg,Wg] -> int64 [B,3,6] on the device: for combined, census and bare the script's
+    [tp_0, fp_0, fn_0, tp_1, fp_1, fn_1] (class 0 = rigid background, class 1 = moving car; pixels whose semantic label is
+    not 26 are ignored).  The maximum that normalises the census is taken per sample; the reference runs batch 1.
+    want_masks: also [B,4,h,w] = combined, census, bare (0/1) and the soft census.  No host synchronisation."""
+    emask, flow_cam, flow_fwd = (_lib.contig(t.float()) for t in (emask, flow_cam, flow_fwd))
+    obj, sem = _lib.contig(obj_map_gt.float()), _lib.contig(semantic_map_gt.float())
+    B, C, h, w = (int(v) for v in emask.shape)
+    Hg, Wg = int(obj.shape[1]), int(obj.shape[2])
+    assert flow_cam.shape == (B, 2, h, w) and flow_fwd.shape == (B, 2, h, w), (flow_cam.shape, flow_fwd.shape)
+    assert obj.shape == (B, Hg, Wg) and sem.shape == (B, Hg, Wg), (obj.shape, sem.shape)
+    lib = _lib.lib()
+    nbytes = int(lib.ccb_mask_iou_workspace_bytes(B, h, w, Hg, Wg))
+    work = torch.empty(max(nbytes, 0) // 8 + 1, device=emask.device, dtype=torch.int64)
+    n = torch.empty(B, 3, 4, device=emask.device, dtype=torch.int64)
+    masks = torch.empty(B, 4, h, w, device=emask.device) if want_masks else None
+    _lib.check(lib.ccb_mask_iou(_lib.ptr(emask, 'emask'), _lib.ptr(flow_cam, 'flow_cam'), _lib.ptr(flow_fwd, 'flow_fwd'),
+                                _lib.ptr(obj, 'obj_map_gt'), _lib.ptr(sem, 'semantic_map_gt'), B, C, h, w, Hg, Wg, float(THRESH), 26,
+                                _lib.ptr(masks), _lib.ptr(work, 'work', torch.int64), nbytes, _lib.ptr(n, 'counts', torch.int64),
+                                _lib.stream(emask)), 'mask_iou')
+    # n[pred][gt] = n00 n01 n10 n11 -> tp_0 fp_0 fn_0 tp_1 fp_1 fn_1: fp_1 = fn_0 = n10, fn_1 = fp_0 = n01
+    counts = torch.cat([n, n[..., 2:3], n[..., 1:2]], -1)
+    return (counts, masks) if want_masks else counts
+
+
+@torch.no_grad()
+def mask_sample_errors(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv, obj_map_gt, semantic_map_gt, THRESH=0.94):
+    """tgt/refs: normalised device tensors [1,3,H,W] (4 refs), obj_map_gt / semantic_map_gt [1,Hg,Wg] ->
+    (errors, errors_census, errors_bare, masks): the three lists of six counts test_mask.py:150-152 accumulates, and
+    masks [1,4,H,W] on the device (combined is what the script saves, the soft census what it draws)."""
+    for n in (disp_net, pose_net, mask_net, flow_net):
+        n.eval()
+    disp = disp_net(tgt)
+    depth = 1 / disp
+    pose = pose_net(tgt, refs)
+    emask = mask_net(tgt, refs)
+    # test_mask.py:123-126: Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
+    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
+    flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
+    counts, masks = motion_mask_counts(emask, flow_cam, flow_fwd, obj_map_gt, semantic_map_gt, THRESH, want_masks=True)
+    errors, errors_census, errors_bare = counts[0].cpu().tolist()
+    return errors, errors_census, errors_bare, masks
+
+
+def mask_iou(summed_counts):
+    """[tp_0, fp_0, fn_0, tp_1, fp_1, fn_1] summed over a dataset -> (avg_iou, bg_iou, fg_iou), test_mask.py:199-201.
+    A class with no pixel at all gives nan."""
+    c = np.asarray(summed_counts, np.float64)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        bg_iou = c[0] / (c[0] + c[1] + c[2])
+        fg_iou = c[3] / (c[3] + c[4] + c[5])
+    return float((bg_iou + fg_iou) / 2), float(bg_iou), float(fg_iou)

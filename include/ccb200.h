@@ -327,6 +327,26 @@ int ccb_flow_metrics(const float* gt, const float* pred_rigid, const float* pred
 long long ccb_depth_errors_workspace_bytes(int B, int H, int W);
 int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, int crop, void* work, float* out6,
                      ccb_stream_t stream);
+/* Motion segmentation scores of one sample each (test_mask.py:129-156, mask_error :224-262), no host sync.  emask
+ * [B,C,h,w] is the mask net's eval output (C >= 3; channels 1 and 2 are read), flow_cam and flow [B,2,h,w], obj_map and
+ * semantic_map [B,Hg,Wg] hold label values as floats.  Three rigidity masks at h x w:
+ *   bare = 1 - (1-e1)(1-e2) > 0.5;  census = soft > thresh with soft = 1 - d/max(d), d = |flow_cam - flow|_2 and the
+ *   maximum taken per sample (the reference runs batch 1);  combined = bare or census.
+ * d, the division and the subtraction are single correctly rounded fp32 operations (no contraction, no approximate
+ * division or root), so the counts are those of an IEEE evaluation of the expressions operation by operation;
+ * max(d) = 0 gives NaN and an empty census as in the reference.
+ * counts [B,3,4]: per sample and mask {combined, census, bare} the confusion matrix n[pred][gt] = {n00, n01, n10, n11}
+ * over the ground-truth pixels with semantic_map == car_label, where gt = (obj_map != 0), pred = 0 where the mask is 1
+ * (argmax([mask, 1-mask])), and the mask is read at the pixel scipy.ndimage.zoom(order=0) reads: index
+ * floor(o (n_in-1)/(n_out-1) + 0.5) per axis, in fp64.  mask_error's six numbers are tp0 = n00, fp0 = fn1 = n01,
+ * fn0 = fp1 = n10, tp1 = n11.  The counts are summed with 64-bit integer atomics: integer addition is associative, so
+ * every run gives the same counts.
+ * masks (optional, [B,4,h,w]) receives combined, census, bare as 0/1 and soft.
+ * work: ccb_mask_iou_workspace_bytes(B, h, w, Hg, Wg) bytes (-1 for bad sizes), 8-byte aligned. */
+long long ccb_mask_iou_workspace_bytes(int B, int h, int w, int Hg, int Wg);
+int ccb_mask_iou(const float* emask, const float* flow_cam, const float* flow, const float* obj_map,
+                 const float* semantic_map, int B, int C, int h, int w, int Hg, int Wg, float thresh, int car_label,
+                 float* masks, void* work, long long work_bytes, long long* counts, ccb_stream_t stream);
 /* Input pipeline on the device (train.py:448-451 H2D + custom_transforms.py:21-30,47-118): uint8 HWC frames
  * src [B,F,Hs,Ws,3] -> F normalised fp32 NCHW tensors dst[f] [B,3,H,W] = (v/255 - .5)/.5, per sample horizontally
  * flipped (params[b][0] != 0) and scale-cropped: resized by (params[b][1], params[b][2]) = (scaled_w/Ws, scaled_h/Hs)
