@@ -12,7 +12,7 @@
 //           stride-parity class (py,px): only the taps that hit integer output coordinates are
 //           enumerated, so stride-2 layers waste no MACs.  ConvTranspose2d forward == DGRAD.
 //   WGRAD : C[m=(ci,ky,kx)][n=co]     = sum_k=(b,oy,ox) x[...] * dy[b,co,oy,ox], split-K.
-#include "ccb_common.cuh"
+#include "conv.cuh"
 
 namespace ccb {
 
@@ -30,19 +30,9 @@ struct ConvArgs {
     int act;             // CCB_ACT_*
     float slope;
     int splits;
-    // DGRAD parity class
-    int py, px, Hc, Wc, ky0, kx0, nky, nkx;
+    DgradClass dc;       // DGRAD: the parity class of this launch
     int M, N, K;
 };
-
-__device__ __forceinline__ float apply_act(float v, int act, float slope) {
-    switch (act) {
-        case CCB_ACT_RELU: return fmaxf(v, 0.f);
-        case CCB_ACT_LEAKY: return v > 0.f ? v : v * slope;
-        case CCB_ACT_SIGMOID: return 1.f / (1.f + expf(-v));
-        default: return v;
-    }
-}
 
 // Tile configuration: BM x BN outputs per CTA, TM x TN per thread, 256 threads, BK = 16.
 template <int BM_, int BN_, int TM_, int TN_>
@@ -65,10 +55,10 @@ __device__ __forceinline__ KInfo decode_k(const ConvArgs& a, int k) {
         int ky = rem / a.kw, kx = rem - ky * a.kw;
         r.off = ci * a.Hi * a.Wi; r.a = ky; r.b = kx; r.off2 = 0;
     } else if (MODE == MODE_DGRAD) {
-        int nt = a.nky * a.nkx;
+        int nt = a.dc.nky * a.dc.nkx;
         int co = k / nt, rem = k - co * nt;
-        int tky = rem / a.nkx, tkx = rem - tky * a.nkx;
-        int ky = a.ky0 + tky * a.stride, kx = a.kx0 + tkx * a.stride;
+        int tky = rem / a.dc.nkx, tkx = rem - tky * a.dc.nkx;
+        int ky = a.dc.ky0 + tky * a.stride, kx = a.dc.kx0 + tkx * a.stride;
         if (ky >= a.kh || kx >= a.kw) return r;          // parity class without a valid tap
         r.off = co * a.Ho * a.Wo; r.a = ky; r.b = kx;
         r.off2 = co * a.Ci * a.kh * a.kw + ky * a.kw + kx;
@@ -95,11 +85,11 @@ __device__ __forceinline__ MInfo decode_m(const ConvArgs& a, int m) {
         int rem = m - r.b * hw;
         r.y = rem / a.Wo; r.x = rem - r.y * a.Wo;
     } else if (MODE == MODE_DGRAD) {
-        int hw = a.Hc * a.Wc;
+        int hw = a.dc.Hc * a.dc.Wc;
         r.b = m / hw;
         int rem = m - r.b * hw;
-        int jy = rem / a.Wc, jx = rem - jy * a.Wc;
-        r.y = a.py + jy * a.stride; r.x = a.px + jx * a.stride;
+        int jy = rem / a.dc.Wc, jx = rem - jy * a.dc.Wc;
+        r.y = a.dc.py + jy * a.stride; r.x = a.dc.px + jx * a.stride;
     } else {
         int kk = a.kh * a.kw;
         r.c = m / kk;
@@ -338,9 +328,8 @@ static int launch_gemm(const ConvArgs& a, long long out_numel, cudaStream_t st, 
     if (a.splits > 1) {
         int plane = (MODE == MODE_FPROP) ? a.Ho * a.Wo : (MODE == MODE_DGRAD) ? a.Hi * a.Wi : 1;
         int C = (MODE == MODE_FPROP) ? a.Co : (MODE == MODE_DGRAD) ? a.Ci : 1;
-        CCB_LAUNCH(splitk_reduce_kernel, dim3((unsigned)((out_numel + 255) / 256)), dim3(256), 0, st,
-                   a.work, a.out, (MODE == MODE_WGRAD) ? nullptr : a.bias, (MODE == MODE_WGRAD) ? nullptr : a.res,
-                   out_numel, a.splits, plane, C, (MODE == MODE_WGRAD) ? CCB_ACT_NONE : a.act, a.slope);
+        launch_splitk_reduce(a.work, a.out, (MODE == MODE_WGRAD) ? nullptr : a.bias, (MODE == MODE_WGRAD) ? nullptr : a.res,
+                             out_numel, a.splits, plane, C, (MODE == MODE_WGRAD) ? CCB_ACT_NONE : a.act, a.slope, st);
         rc = check_launch("splitk_reduce");
     }
     return rc;
@@ -387,16 +376,6 @@ static ConvArgs ffma_args(const ccb_conv_desc* d, int splits, float* work) {
     a.act = d->act; a.slope = d->slope; a.splits = splits; a.work = work;
     return a;
 }
-
-// tensor-core path (conv_tc.cu)
-bool tc_supported(const ccb_conv_desc* d, int op);
-bool tc_profitable(const ccb_conv_desc* d, int op);
-int tc_plan(const ccb_conv_desc* d, int op, long long& panel_floats);
-int tc_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias, const float* res, float* y,
-             float* wp, float* partial, int splits, cudaStream_t st);
-int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const float* bias, const float* res, float* dx,
-             float* wp, float* partial, int splits, cudaStream_t st);
-int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw, float* partial, int splits, cudaStream_t st);
 
 // the weight cache of the conv call in flight (wprep_get looks it up); sim builds have none
 struct WCacheScope {
@@ -521,13 +500,9 @@ extern "C" int ccb_conv2d_dgrad(const ccb_conv_desc* d, const float* dy, const f
     for (int py = 0; py < s && py < a.Hi; ++py)
         for (int px = 0; px < s && px < a.Wi; ++px) {
             ConvArgs c = a;
-            c.py = py; c.px = px;
-            c.Hc = (a.Hi - py + s - 1) / s; c.Wc = (a.Wi - px + s - 1) / s;
-            c.ky0 = (py + a.pad) % s; c.kx0 = (px + a.pad) % s;
-            c.nky = (a.kh > c.ky0) ? (a.kh - c.ky0 + s - 1) / s : 0;
-            c.nkx = (a.kw > c.kx0) ? (a.kw - c.kx0 + s - 1) / s : 0;
-            c.M = a.B * c.Hc * c.Wc; c.N = a.Ci; c.K = a.Co * c.nky * c.nkx;
-            if (c.K == 0) { c.K = 1; c.nky = c.nkx = 1; c.ky0 = a.kh; c.kx0 = a.kw; }   // no tap hits: output = epilogue(0)
+            c.dc = dgrad_class(d, py, px);
+            c.M = a.B * c.dc.Hc * c.dc.Wc; c.N = a.Ci; c.K = a.Co * c.dc.nky * c.dc.nkx;
+            if (c.K == 0) { c.K = 1; c.dc.nky = c.dc.nkx = 1; c.dc.ky0 = a.kh; c.dc.kx0 = a.kw; }   // no tap hits: output = epilogue(0)
             rc = launch_gemm<MODE_DGRAD>(c, (long long)a.B * a.Ci * a.Hi * a.Wi, (cudaStream_t)stream, p.kernel);
             if (rc) return rc;
         }

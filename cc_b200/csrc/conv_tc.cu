@@ -19,7 +19,7 @@
 //
 // The same kernel serves FPROP, stride-1 DGRAD and the stride-parity classes of strided DGRAD /
 // ConvTranspose2d forward through a per-tap offset table ("generalised fprop").
-#include "ccb_common.cuh"
+#include "conv.cuh"
 
 #ifndef CCB_CPU_SIM
 
@@ -50,10 +50,10 @@ struct TcArgs {
     int M;                 // B * Hc * Wc
     int act;
     float slope;
-    int splits, kt_per_split;          // split-K over k-tiles (grid.z); partials go to `partial`
+    int ktiles, kt_per_split, splits;  // k-tiles of 32 (Kp / 32), split-K over them (grid.z); partials go to `partial`
     float* partial;                    // [splits][numel(out)] raw accumulators (bias/res/act applied by the reduce kernel)
     long long out_numel;
-    int stages, b_tile_bytes;          // pipeline depth and bytes of one B operand copy (N-tile dependent)
+    int depth, b_tile_bytes;           // stage ring (tc_geometry)
     signed char off_y[TC_MAX_TAPS], off_x[TC_MAX_TAPS];
 };
 
@@ -175,51 +175,104 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[NT / 2], uint64_t da, uint
     else wgmma_tf32_n128(d, da, db);
 }
 
-// float4 index of (row, 16-byte chunk) inside one swizzled operand tile
-__device__ __forceinline__ int tile_idx(int row, int chunk) { return row * TC_KC + (chunk ^ (row & 7)); }
-
-__device__ __forceinline__ float tc_act(float v, int act, float slope) {
-    switch (act) {
-        case CCB_ACT_RELU: return fmaxf(v, 0.f);
-        case CCB_ACT_LEAKY: return v > 0.f ? v : v * slope;
-        case CCB_ACT_SIGMOID: return 1.f / (1.f + expf(-v));
-        default: return v;
-    }
-}
-
 constexpr int TC_TILE_BYTES = TC_KC * TC_M * 16;                   // one A operand copy of one stage: 16 KB
 constexpr int TC_SMEM_MAX = 227 * 1024;
 
-// Consumer side shared by both kernels: for each full stage, 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this
-// warpgroup's 64 rows into the scratch registers `part`, then acc += part in fp32 and the stage goes back to the producers.
+// float4 index of (row, 16-byte chunk) inside one swizzled operand tile
+__device__ __forceinline__ int tile_idx(int row, int chunk) { return row * TC_KC + (chunk ^ (row & 7)); }
+
+// x split into hi = tf32(x) and lo = tf32(x - hi), stored as float4 `idx` of the hi and the lo tile
+__device__ __forceinline__ void tc_split_store(unsigned char* hi, unsigned char* lo, int idx, float4 x) {
+    float4 h, l;
+    h.x = tf32_hi(x.x); h.y = tf32_hi(x.y); h.z = tf32_hi(x.z); h.w = tf32_hi(x.w);
+    ((float4*)hi)[idx] = h;
+    l.x = tf32_hi(x.x - h.x); l.y = tf32_hi(x.y - h.y); l.z = tf32_hi(x.z - h.z); l.w = tf32_hi(x.w - h.w);
+    ((float4*)lo)[idx] = l;
+}
+
+// The four operand tiles of one stage as byte addresses of type T: unsigned char* for the producers' stores, the
+// uint32_t shared-space address for the consumers' wgmma descriptors.
+template <typename T> struct TcTiles { T a_hi, a_lo, b_hi, b_lo; };
+
+// The stage ring of both kernels in dynamic shared memory: `depth` stages of [A hi | A lo | B hi | B lo] (A: the 128
+// rows of the tile, B: the wgmma N rows), then a full (producers -> consumers) and an empty (consumers -> producers)
+// mbarrier per stage.  The it-th k-tile of a CTA passes through stage it % depth in round it / depth.
+struct TcRing {
+    unsigned char* smem;        // stage 0, on a 1 KB boundary: SWIZZLE_128B atoms are 1 KB
+    int depth, stage_bytes, b_tile_bytes;
+    uint64_t *full, *empty;
+
+    template <typename T>
+    __device__ __forceinline__ TcTiles<T> tiles(T base, int s) const {
+        const T st = base + s * stage_bytes;
+        return {st, st + TC_TILE_BYTES, st + 2 * TC_TILE_BYTES, st + 2 * TC_TILE_BYTES + b_tile_bytes};
+    }
+    // producers: wait until the consumers have released stage s = it % depth (the first round finds every stage free),
+    // then write its tiles
+    __device__ __forceinline__ TcTiles<unsigned char*> acquire(int it, int s) const {
+        if (it >= depth) mbar_wait(&empty[s], ((it / depth) - 1) & 1);
+        return tiles(smem, s);
+    }
+    // producers: make this thread's stores into stage s visible to wgmma (the async proxy) and count them in
+    __device__ __forceinline__ void publish(int s) const { fence_proxy_async(); mbar_arrive(&full[s]); }
+};
+
+// Set-up at the top of both kernels: it touches no global data, so it overlaps the predecessor's tail (PDL), and
+// returns once the predecessor's results are visible.
+__device__ __forceinline__ TcRing tc_ring(int depth, int b_tile_bytes) {
+    CCB_PDL_TRIGGER();
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int stage_bytes = 2 * TC_TILE_BYTES + 2 * b_tile_bytes;
+    uint64_t* full = (uint64_t*)(smem + depth * stage_bytes);
+    const TcRing r = {smem, depth, stage_bytes, b_tile_bytes, full, full + TC_MAX_STAGES};
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < depth; ++s) { mbar_init(&r.full[s], TC_PRODUCERS); mbar_init(&r.empty[s], TC_CONSUMER_WARPS); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    CCB_PDL_SYNC();
+    return r;
+}
+
+// wgmma m64nN accumulator layout: register tc_acc_reg(i, half, e) of consumer warp wq of warpgroup wg holds row
+// tc_acc_row(wg, wq, lane, half) of the CTA's 128 rows and column tc_acc_col(lane, i, e), i < N / 8, half, e < 2.
+__device__ __forceinline__ int tc_acc_row(int wg, int wq, int lane, int half) { return wg * 64 + wq * 16 + (lane >> 2) + half * 8; }
+__device__ __forceinline__ int tc_acc_col(int lane, int i, int e) { return 8 * i + 2 * (lane & 3) + e; }
+__device__ __forceinline__ int tc_acc_reg(int i, int half, int e) { return 4 * i + 2 * half + e; }
+
+// Consumer side shared by both kernels: acc = 0 (an empty split contributes zeros), then for each of `nkt` full stages,
+// 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this warpgroup's 64 rows into the scratch registers `part`, then
+// acc += part in fp32 and the stage goes back to the producers.
 template <int NT>
-__device__ __forceinline__ void tc_consume(unsigned char* smem, int stage_bytes, int b_tile_bytes, int NST, int nst,
-                                           uint64_t* full_bar, uint64_t* empty_bar, int wg, int lane,
-                                           float (&acc)[NT / 2], float (&part)[NT / 2]) {
-    for (int it = 0; it < nst; ++it) {
-        const int s = it % NST;
-        mbar_wait(&full_bar[s], (it / NST) & 1);
-        const uint32_t base = smem_u32(smem + s * stage_bytes);
-        const uint32_t a_hi = base + wg * (TC_TILE_BYTES / 2), a_lo = a_hi + TC_TILE_BYTES;
-        const uint32_t b_hi = base + 2 * TC_TILE_BYTES, b_lo = b_hi + b_tile_bytes;
+__device__ __forceinline__ void tc_consume(const TcRing& ring, int nkt, int wg, int lane, float (&acc)[NT / 2]) {
+    float part[NT / 2];
+#pragma unroll
+    for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
+    const uint32_t base = smem_u32(ring.smem);
+    for (int it = 0; it < nkt; ++it) {
+        const int s = it % ring.depth;
+        mbar_wait(&ring.full[s], (it / ring.depth) & 1);
+        const TcTiles<uint32_t> t = ring.tiles(base, s);
+        const uint32_t a_hi = t.a_hi + wg * (TC_TILE_BYTES / 2), a_lo = t.a_lo + wg * (TC_TILE_BYTES / 2);
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
         wg_fence();
 #pragma unroll
         for (int ks = 0; ks < TC_KC / 2; ++ks) {
             const uint32_t koff = (uint32_t)ks * 32u;
-            wgmma_tf32<NT>(part, wg_desc(a_lo + koff), wg_desc(b_hi + koff));
-            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(b_lo + koff));
+            wgmma_tf32<NT>(part, wg_desc(a_lo + koff), wg_desc(t.b_hi + koff));
+            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(t.b_lo + koff));
         }
 #pragma unroll
         for (int ks = 0; ks < TC_KC / 2; ++ks) {
             const uint32_t koff = (uint32_t)ks * 32u;
-            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(b_hi + koff));
+            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(t.b_hi + koff));
         }
         wg_commit();
         wg_wait<0>();
         wg_fence_regs(part);
-        if (lane == 0) mbar_arrive(&empty_bar[s]);
+        if (lane == 0) mbar_arrive(&ring.empty[s]);
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) acc[j] += part[j];
     }
@@ -227,28 +280,13 @@ __device__ __forceinline__ void tc_consume(unsigned char* smem, int stage_bytes,
 
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) {
-    CCB_PDL_TRIGGER();
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B atoms are 1 KB
-    const int NST = a.stages;
-    const int stage_bytes = 2 * TC_TILE_BYTES + 2 * a.b_tile_bytes;     // A hi, A lo, B hi, B lo
-    uint64_t* full_bar = (uint64_t*)(smem + NST * stage_bytes);
-    uint64_t* empty_bar = full_bar + TC_MAX_STAGES;
-
+    const TcRing ring = tc_ring(a.depth, a.b_tile_bytes);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
     const int ntile = min(TC_NMAX, a.Ntot - n0);
-    const int ktiles_all = a.Kp / (TC_KC * 4);
     const int kt_beg = blockIdx.z * a.kt_per_split;
-    const int ktiles = max(0, min(ktiles_all, kt_beg + a.kt_per_split) - kt_beg);   // k-tiles of this split
+    const int nkt = max(0, min(a.ktiles, kt_beg + a.kt_per_split) - kt_beg);   // k-tiles of this split
     const long long HWin = (long long)a.Hin * a.Win;
-
-    if (tid == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], TC_PRODUCERS); mbar_init(&empty_bar[s], TC_CONSUMER_WARPS); }
-        fence_barrier_init();
-    }
-    __syncthreads();
-    CCB_PDL_SYNC();                                               // everything above touched no global data
 
     if (warp < TC_PRODUCERS / 32) {
         // ===================== producers: thread == tile row =====================
@@ -267,8 +305,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
         const int iy0 = oy * a.in_stride, ix0 = ox * a.in_stride;
         const int cpt = a.cpad >> 2;                 // chunks per tap
         const int nchunks = a.ntaps * cpt;           // real chunks; the rest of Kp is zero padding
-        for (int it = 0; it < ktiles; ++it) {
-            const int s = it % NST;
+        for (int it = 0; it < nkt; ++it) {
+            const int s = it % ring.depth;
             const int kt = kt_beg + it;                   // global k-tile
             // ---- A: the 8 chunks (32 floats) of this thread's pixel row
             float av[TC_KC][4];
@@ -309,12 +347,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
                     if (++c4 == cpt) { c4 = 0; ++tap; }
                 }
             }
-            if (it >= NST) mbar_wait(&empty_bar[s], ((it / NST) - 1) & 1);
-            unsigned char* st = smem + s * stage_bytes;
-            float4* a_hi = (float4*)st;
-            float4* a_lo = (float4*)(st + TC_TILE_BYTES);
-            float4* b_hi = (float4*)(st + 2 * TC_TILE_BYTES);
-            float4* b_lo = (float4*)(st + 2 * TC_TILE_BYTES + a.b_tile_bytes);
+            const TcTiles<unsigned char*> t = ring.acquire(it, s);
             // ---- B: the weights were split into tf32 hi / lo by the prep kernel: plain 16-byte async copies
             //      (pairs of threads cover one 32-byte sector of a weight row)
 #pragma unroll
@@ -326,35 +359,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
                     // rows in [ntile, NT) are clamped to row 0: the epilogue ignores those columns
                     const int nn = (n < ntile) ? n : 0;
                     const float* src = a.wp + (long long)(n0 + nn) * a.Kp + kt * (TC_KC * 4) + c * 4;
-                    cp_async16(&b_hi[tile_idx(n, c)], src);
-                    cp_async16(&b_lo[tile_idx(n, c)], src + (long long)a.Ntot * a.Kp);
+                    cp_async16((float4*)t.b_hi + tile_idx(n, c), src);
+                    cp_async16((float4*)t.b_lo + tile_idx(n, c), src + (long long)a.Ntot * a.Kp);
                 }
             }
             // ---- A: split + store
 #pragma unroll
-            for (int c = 0; c < TC_KC; ++c) {
-                float4 h, l;
-                h.x = tf32_hi(av[c][0]); h.y = tf32_hi(av[c][1]); h.z = tf32_hi(av[c][2]); h.w = tf32_hi(av[c][3]);
-                a_hi[tile_idx(r, c)] = h;
-                l.x = tf32_hi(av[c][0] - h.x); l.y = tf32_hi(av[c][1] - h.y); l.z = tf32_hi(av[c][2] - h.z); l.w = tf32_hi(av[c][3] - h.w);
-                a_lo[tile_idx(r, c)] = l;
-            }
+            for (int c = 0; c < TC_KC; ++c)
+                tc_split_store(t.a_hi, t.a_lo, tile_idx(r, c), make_float4(av[c][0], av[c][1], av[c][2], av[c][3]));
             cp_async_wait_all();
-            fence_proxy_async();
-            mbar_arrive(&full_bar[s]);
+            ring.publish(s);
         }
     } else {
         // ===================== consumers: MMA + epilogue =====================
         const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
-        float acc[NT / 2], part[NT / 2];
-#pragma unroll
-        for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;                  // an empty split contributes zeros
-        tc_consume<NT>(smem, stage_bytes, a.b_tile_bytes, NST, ktiles, full_bar, empty_bar, wg, lane, acc, part);
+        float acc[NT / 2];
+        tc_consume<NT>(ring, nkt, wg, lane, acc);
         const long long HWout = (long long)a.Hout * a.Wout;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
-            // accumulator layout of wgmma m64nN: row 16 * warp + lane / 4 (+ 8), columns 8 i + 2 (lane % 4) (+ 1)
-            const int em = m0 + wg * 64 + wq * 16 + (lane >> 2) + half * 8;
+            const int em = m0 + tc_acc_row(wg, wq, lane, half);
             if (em >= a.M) continue;
             int hw = a.Hc * a.Wc;
             int eb = em / hw;
@@ -366,10 +390,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
             for (int i = 0; i < NT / 8; ++i)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int nl = 8 * i + 2 * (lane & 3) + e;
+                    const int nl = tc_acc_col(lane, i, e);
                     if (nl < ntile) {
-                        const int j = 4 * i + 2 * half + e;
-                        float o = acc[j];
+                        float o = acc[tc_acc_reg(i, half, e)];
                         const int n = n0 + nl;
                         const long long off = obase + (long long)n * HWout;
                         if (a.splits > 1) {
@@ -377,7 +400,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
                         } else {
                             if (a.bias) o += __ldg(a.bias + n);
                             if (a.res) o += __ldg(a.res + off);
-                            a.out[off] = tc_act(o, a.act, a.slope);
+                            a.out[off] = apply_act(o, a.act, a.slope);
                         }
                     }
                 }
@@ -391,20 +414,17 @@ static int roundup(int v, int m) { return (v + m - 1) / m * m; }
 // Kp of `ntaps` taps of Cc channels: whole k-tiles; a parity class without taps still runs one all-zero k-tile
 static int tc_kp(int ntaps, int Cc) { return ntaps > 0 ? roundup(ntaps * roundup(Cc, 4), TC_KC * 4) : TC_KC * 4; }
 
-void launch_splitk_reduce(const float* work, float* out, const float* bias, const float* res, long long numel, int splits,
-                          int plane, int C, int act, float slope, cudaStream_t st);   // conv_ffma.cu
-
 // Operand tile geometry of one launch: the B tile holds the wgmma N (16/32/64/128) rows, and as many stages as fit
-// in shared memory (up to 4: 3 at N = 128 in 3xTF32 layout, 4 below).
-static void tc_geometry(int N, int& nt, int& b_tile_bytes, int& stages, int& smem) {
+// in shared memory as the ring's depth (up to 4: 3 at N = 128 in 3xTF32 layout, 4 below).
+static void tc_geometry(int N, int& nt, int& b_tile_bytes, int& depth, int& smem) {
     const int ntile_max = N < TC_NMAX ? N : TC_NMAX;
     nt = 16;
     while (nt < ntile_max) nt <<= 1;
     b_tile_bytes = nt * 128;
     const int stage = 2 * TC_TILE_BYTES + 2 * b_tile_bytes;
-    stages = (TC_SMEM_MAX - 2048) / stage;
-    if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
-    smem = stages * stage + 2048;                     // + barriers / alignment slack
+    depth = (TC_SMEM_MAX - 2048) / stage;
+    if (depth > TC_MAX_STAGES) depth = TC_MAX_STAGES;
+    smem = depth * stage + 2048;                      // + barriers / alignment slack
 }
 
 template <typename Args>
@@ -435,10 +455,11 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     a.wp = wpp;
     a.Ntot = N;
     a.splits = splits;
-    a.kt_per_split = cdiv(a.Kp / (TC_KC * 4), splits);
+    a.ktiles = a.Kp / (TC_KC * 4);
+    a.kt_per_split = cdiv(a.ktiles, splits);
     a.partial = partial;
     int nt, smem;
-    tc_geometry(N, nt, a.b_tile_bytes, a.stages, smem);
+    tc_geometry(N, nt, a.b_tile_bytes, a.depth, smem);
     dim3 grid(cdiv(a.M, TC_M), cdiv(N, TC_NMAX), splits);
     return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, grid, smem, st, "conv_tc");
 }
@@ -456,34 +477,20 @@ struct TcWgradArgs {
     int B, Ci, Hi, Wi, Co, Ho, Wo, kh, kw, stride, pad;
     int cpad, Mtot;      // channels padded to 4; Mtot = kh*kw*cpad rows
     int P;               // B*Ho*Wo pixels (Wo % 4 == 0)
-    int stages, per_split, splits;
-    int nstages, b_tile_bytes;   // pipeline depth / bytes of one dY operand copy (Co-tile dependent)
+    int ktiles, kt_per_split, splits;  // k-tiles of 32 pixels (P / 32 rounded up), split-K over them (grid.z)
+    int depth, b_tile_bytes;           // stage ring (tc_geometry)
 };
 
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWgradArgs a) {
-    CCB_PDL_TRIGGER();
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int NST = a.nstages;
-    const int stage_bytes = 2 * TC_TILE_BYTES + 2 * a.b_tile_bytes;
-    uint64_t* full_bar = (uint64_t*)(smem + NST * stage_bytes);
-    uint64_t* empty_bar = full_bar + TC_MAX_STAGES;
-
+    const TcRing ring = tc_ring(a.depth, a.b_tile_bytes);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
     const int ntile = min(TC_NMAX, a.Co - n0);
-    const int st_beg = blockIdx.z * a.per_split, st_end = min(a.stages, st_beg + a.per_split);
-    const int nst = st_end - st_beg;          // >= 1 by construction
+    const int kt_beg = blockIdx.z * a.kt_per_split;
+    const int nkt = min(a.ktiles, kt_beg + a.kt_per_split) - kt_beg;   // k-tiles of this split, >= 1 by construction
     const int KK = a.kh * a.kw;
     const int HWo = a.Ho * a.Wo, HWi = a.Hi * a.Wi;
-
-    if (tid == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], TC_PRODUCERS); mbar_init(&empty_bar[s], TC_CONSUMER_WARPS); }
-        fence_barrier_init();
-    }
-    __syncthreads();
-    CCB_PDL_SYNC();                                               // everything above touched no global data
 
     if (warp < TC_PRODUCERS / 32) {
         // 8 consecutive threads walk the 8 K-chunks (32 consecutive pixels) of one row, rows rbase + 16 j
@@ -505,9 +512,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
                 }
             }
         }
-        for (int it = 0; it < nst; ++it) {
-            const int s = it % NST;
-            const int p0 = ((st_beg + it) * TC_KC + c) * 4;       // first of this chunk's 4 pixels
+        for (int it = 0; it < nkt; ++it) {
+            const int s = it % ring.depth;
+            const int p0 = ((kt_beg + it) * TC_KC + c) * 4;       // first of this chunk's 4 pixels
             const bool pvalid = p0 < a.P;
             int b = 0, oy = 0, ox0 = 0;
             if (pvalid) {
@@ -542,41 +549,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
                 if (pvalid && n < ntile)
                     bv[j] = __ldg((const float4*)(a.dy + ((long long)b * a.Co + n0 + n) * HWo + oy * a.Wo + ox0));
             }
-            if (it >= NST) mbar_wait(&empty_bar[s], ((it / NST) - 1) & 1);
-            unsigned char* st = smem + s * stage_bytes;
-            float4* a_hi = (float4*)st;
-            float4* a_lo = (float4*)(st + TC_TILE_BYTES);
-            float4* b_hi = (float4*)(st + 2 * TC_TILE_BYTES);
-            float4* b_lo = (float4*)(st + 2 * TC_TILE_BYTES + a.b_tile_bytes);
+            const TcTiles<unsigned char*> t = ring.acquire(it, s);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const int r = rbase + 16 * j;
-                float4 h, l;
-                h.x = tf32_hi(av[j][0]); h.y = tf32_hi(av[j][1]); h.z = tf32_hi(av[j][2]); h.w = tf32_hi(av[j][3]);
-                a_hi[tile_idx(r, c)] = h;
-                l.x = tf32_hi(av[j][0] - h.x); l.y = tf32_hi(av[j][1] - h.y); l.z = tf32_hi(av[j][2] - h.z); l.w = tf32_hi(av[j][3] - h.w);
-                a_lo[tile_idx(r, c)] = l;
-                if (r < NT) {
-                    h.x = tf32_hi(bv[j].x); h.y = tf32_hi(bv[j].y); h.z = tf32_hi(bv[j].z); h.w = tf32_hi(bv[j].w);
-                    b_hi[tile_idx(r, c)] = h;
-                    l.x = tf32_hi(bv[j].x - h.x); l.y = tf32_hi(bv[j].y - h.y); l.z = tf32_hi(bv[j].z - h.z); l.w = tf32_hi(bv[j].w - h.w);
-                    b_lo[tile_idx(r, c)] = l;
-                }
+                const int r = rbase + 16 * j, idx = tile_idx(r, c);
+                tc_split_store(t.a_hi, t.a_lo, idx, make_float4(av[j][0], av[j][1], av[j][2], av[j][3]));
+                if (r < NT) tc_split_store(t.b_hi, t.b_lo, idx, bv[j]);
             }
-            fence_proxy_async();
-            mbar_arrive(&full_bar[s]);
+            ring.publish(s);
         }
     } else {
         // ---- consumers; epilogue: row m = (tap, ci); columns == co
         const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
-        float acc[NT / 2], part[NT / 2];
-#pragma unroll
-        for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
-        tc_consume<NT>(smem, stage_bytes, a.b_tile_bytes, NST, nst, full_bar, empty_bar, wg, lane, acc, part);
+        float acc[NT / 2];
+        tc_consume<NT>(ring, nkt, wg, lane, acc);
         float* outp = a.out + (long long)blockIdx.z * a.Co * a.Ci * KK;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
-            const int em = m0 + wg * 64 + wq * 16 + (lane >> 2) + half * 8;
+            const int em = m0 + tc_acc_row(wg, wq, lane, half);
             if (em >= a.Mtot) continue;
             const int etap = em / a.cpad;
             const int eci = em - etap * a.cpad;
@@ -585,9 +575,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
             for (int i = 0; i < NT / 8; ++i)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int nl = 8 * i + 2 * (lane & 3) + e;
-                    const int j = 4 * i + 2 * half + e;
-                    if (nl < ntile) outp[((long long)(n0 + nl) * a.Ci + eci) * KK + etap] = acc[j];
+                    const int nl = tc_acc_col(lane, i, e);
+                    if (nl < ntile) outp[((long long)(n0 + nl) * a.Ci + eci) * KK + etap] = acc[tc_acc_reg(i, half, e)];
                 }
         }
     }
@@ -595,17 +584,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWg
 
 static void (*const TC_WGRAD_KERNELS[4])(const TcWgradArgs) = {conv_tc_wgrad_kernel<16>, conv_tc_wgrad_kernel<32>,
                                                                 conv_tc_wgrad_kernel<64>, conv_tc_wgrad_kernel<128>};
-
-// out[i] = sum_s work[s][i]
-__global__ void __launch_bounds__(256) tc_splitk_sum_kernel(const float* __restrict__ work, float* __restrict__ out,
-                                                            long long numel, int splits) {
-    CCB_PDL_WAIT();
-    long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-    if (i >= numel) return;
-    float v = 0.f;
-    for (int s = 0; s < splits; ++s) v += __ldg(work + (long long)s * numel + i);
-    out[i] = v;
-}
 
 // Shapes the kernels can express, and those where they pay off (CCB_CONV_IMPL_AUTO)
 bool tc_supported(const ccb_conv_desc* d, int op) {
@@ -624,17 +602,17 @@ bool tc_profitable(const ccb_conv_desc* d, int op) {
 // Split-K count of a tensor-core call, and the prepared weights (tf32 hi + lo copies) a fprop / dgrad keeps at the start of
 // its workspace, in floats.  fprop / dgrad: enough CTAs for ~2 waves, >= 2 k-tiles per split, <= 32 splits; the data
 // gradient plans once for all its parity classes (they share the partials, each writes its own pixels), sized by the
-// class with the most taps.  wgrad: ~2 waves of (tap, channel) x Co tiles, >= 4 pixel stages per split.
+// class with the most taps.  wgrad: ~2 waves of (tap, channel) x Co tiles, >= 4 k-tiles of 32 pixels per split.
 int tc_plan(const ccb_conv_desc* d, int op, long long& panel_floats) {
     panel_floats = 0;
     if (op == CCB_CONV_WGRAD) {
-        const int stages = cdiv(d->B * d->Ho * d->Wo, 32);
+        const int ktiles = cdiv(d->B * d->Ho * d->Wo, 32);
         const int tiles = cdiv(d->kh * d->kw * roundup(d->Ci, 4), TC_M) * cdiv(d->Co, TC_NMAX);
         int splits = cdiv(2 * NUM_SMS, tiles);
-        if (splits > stages / 4) splits = stages / 4;
+        if (splits > ktiles / 4) splits = ktiles / 4;
         if (splits > 2 * NUM_SMS) splits = 2 * NUM_SMS;
         if (splits < 1) splits = 1;
-        return cdiv(stages, cdiv(stages, splits));          // no empty split
+        return cdiv(ktiles, cdiv(ktiles, splits));          // no empty split
     }
     const bool fp = op == CCB_CONV_FPROP;
     const int s = fp ? 1 : d->stride, N = fp ? d->Co : d->Ci;
@@ -685,30 +663,27 @@ int tc_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, const floa
     const long long out_numel = (long long)d->B * d->Ci * d->Hi * d->Wi;
     for (int py = 0; py < s && py < d->Hi; ++py)
         for (int px = 0; px < s && px < d->Wi; ++px) {
+            const DgradClass k = dgrad_class(d, py, px);
             TcArgs a;
             memset(&a, 0, sizeof(a));
             a.out_numel = out_numel;
             a.x = dy; a.bias = bias; a.res = res; a.out = dx;
             a.B = d->B; a.Cin = d->Co; a.Hin = d->Ho; a.Win = d->Wo;
             a.Hout = d->Hi; a.Wout = d->Wi;
-            a.Hc = (d->Hi - py + s - 1) / s; a.Wc = (d->Wi - px + s - 1) / s;
+            a.Hc = k.Hc; a.Wc = k.Wc;
             a.out_stride = s; a.out_oy = py; a.out_ox = px; a.in_stride = 1;
             a.M = d->B * a.Hc * a.Wc;
             a.act = d->act; a.slope = d->slope;
+            a.ntaps = k.nky * k.nkx;
             signed char tix[TC_MAX_TAPS];
-            int nt = 0;
-            for (int ky = 0; ky < d->kh; ++ky) {
-                if ((py + d->pad - ky) % s != 0) continue;
-                for (int kx = 0; kx < d->kw; ++kx) {
-                    if ((px + d->pad - kx) % s != 0) continue;
+            for (int ty = 0; ty < k.nky; ++ty)
+                for (int tx = 0; tx < k.nkx; ++tx) {
+                    const int ky = k.ky0 + ty * s, kx = k.kx0 + tx * s, t = ty * k.nkx + tx;
                     // oy = (iy + p - ky)/s = jy + (py + p - ky)/s   (exact division, may be negative)
-                    a.off_y[nt] = (signed char)((py + d->pad - ky) / s);
-                    a.off_x[nt] = (signed char)((px + d->pad - kx) / s);
-                    tix[nt] = (signed char)(ky * d->kw + kx);
-                    ++nt;
+                    a.off_y[t] = (signed char)((py + d->pad - ky) / s);
+                    a.off_x[t] = (signed char)((px + d->pad - kx) / s);
+                    tix[t] = (signed char)(ky * d->kw + kx);
                 }
-            }
-            a.ntaps = nt;
             int rc = launch_tc(a, w, 1, d->Ci, d->Co, d->kh * d->kw, d->Ci, tix, wp, partial, splits, st);
             if (rc) return rc;
         }
@@ -729,17 +704,17 @@ int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
     a.cpad = roundup(d->Ci, 4);
     a.Mtot = d->kh * d->kw * a.cpad;
     a.P = d->B * d->Ho * d->Wo;
-    a.stages = cdiv(a.P, 32);
-    a.per_split = cdiv(a.stages, splits);
+    a.ktiles = cdiv(a.P, 32);
+    a.kt_per_split = cdiv(a.ktiles, splits);
     a.splits = splits;
     a.out = splits > 1 ? partial : dw;
     const long long numel = (long long)d->Co * d->Ci * d->kh * d->kw;
     int nt, wsmem;
-    tc_geometry(d->Co, nt, a.b_tile_bytes, a.nstages, wsmem);
+    tc_geometry(d->Co, nt, a.b_tile_bytes, a.depth, wsmem);
     dim3 grid(cdiv(a.Mtot, TC_M), cdiv(d->Co, TC_NMAX), a.splits);
     int rc = tc_launch_kernel(TC_WGRAD_KERNELS, a, nt, grid, wsmem, st, "conv_tc_wgrad");
     if (rc || a.splits == 1) return rc;
-    CCB_LAUNCH(tc_splitk_sum_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), 0, st, (const float*)partial, dw, numel, a.splits);
+    launch_splitk_reduce(partial, dw, nullptr, nullptr, numel, splits, 1, 1, CCB_ACT_NONE, 0.f, st);
     return check_launch("conv_tc_wgrad_reduce");
 }
 
