@@ -1,4 +1,8 @@
-"""ctypes binding of libccb200.so (include/ccb200.h).
+"""ctypes binding of libccb200.so (include/ccb200.h, include/ccb200_debug.h).
+
+Every op reaches the library through ``call(name, *args)``, which converts each argument as the header declares that
+parameter (``_SIGS``) and raises on a non-zero status.  tests/test_cabi_symbols.py holds ``_SIGS`` and the descriptor
+Structures to the headers.
 
 The product path has NO CPU fallback: importing works without the library (so the package can be
 inspected), but the first op call raises if ``cc_b200/libccb200.so`` is missing, and every op
@@ -64,6 +68,8 @@ class ConvDesc(C.Structure):
                [('slope', C.c_float), ('impl', C.c_int), ('wcache', C.c_void_p)]
 
 
+STRUCTS = {'ccb_photo_desc': PhotoDesc, 'ccb_smooth_desc': SmoothDesc, 'ccb_bce_desc': BceDesc, 'ccb_conv_desc': ConvDesc}
+
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SIGMOID = 0, 1, 2, 3
 CONV_FPROP, CONV_DGRAD, CONV_WGRAD = 0, 1, 2
 IMPL_AUTO, IMPL_FFMA, IMPL_TC = 0, 1, 2
@@ -72,87 +78,187 @@ _lib = None
 _is_sim = False
 DEFAULT_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libccb200.so')
 
-_I, _F, _LL = C.c_int, C.c_float, C.c_longlong
+# Every prototype of the headers: (return, parameter types), each type written as the header writes it.  A pointer is a
+# device pointer unless marked 'host'; 'handle void*' is the weight-cache handle.  The return STATUS is an int
+# ccb_status that call() checks; any other return is handed back as it is.
+STATUS = 'status'
 _SIGS = {
-    'ccb_last_error_string': (C.c_char_p, []),
-    'ccb_version': (_I, []),
-    'ccb_is_simulator': (_I, []),
-    'ccb_image_pyramid': (_I, [_P, _I, _I, _I, _I, C.POINTER(_P), _P]),
-    'ccb_photo_partials_floats': (_LL, [C.POINTER(PhotoDesc)]),
-    'ccb_photo_pose_partials_floats': (_LL, [C.POINTER(PhotoDesc)]),
-    'ccb_photo_loss_fwd': (_I, [C.POINTER(PhotoDesc), _P]),
-    'ccb_photo_loss_bwd': (_I, [C.POINTER(PhotoDesc), _P]),
-    'ccb_consensus_targets': (_I, [C.POINTER(PhotoDesc), _P]),
-    'ccb_inverse_warp_fwd': (_I, [_P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
-    'ccb_inverse_warp_bwd': (_I, [_P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
-    'ccb_warp_pose_partials_floats': (_LL, [_I, _I, _I]),
-    'ccb_flow_warp_fwd': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),
-    'ccb_flow_warp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
-    'ccb_pose2flow_fwd': (_I, [_P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
-    'ccb_pose2flow_bwd': (_I, [_P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
-    'ccb_ssim_fwd': (_I, [_P, _P, _I, _I, _I, C.POINTER(_F), _P, _P]),
-    'ccb_ssim_bwd': (_I, [_P, _P, _I, _I, _I, C.POINTER(_F), _P, _P, _P, _P, _P]),
-    'ccb_smooth_partials_floats': (_LL, [C.POINTER(SmoothDesc)]),
-    'ccb_smooth_fwd': (_I, [C.POINTER(SmoothDesc), _P]),
-    'ccb_smooth_bwd': (_I, [C.POINTER(SmoothDesc), _P]),
-    'ccb_bce_partials_floats': (_LL, [C.POINTER(BceDesc)]),
-    'ccb_bce_fwd': (_I, [C.POINTER(BceDesc), _P]),
-    'ccb_bce_bwd': (_I, [C.POINTER(BceDesc), _P]),
-    'ccb_conv_workspace_floats': (_LL, [C.POINTER(ConvDesc), _I]),
-    'ccb_conv2d_fprop': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _LL, _P]),
-    'ccb_conv2d_dgrad': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _LL, _P]),
-    'ccb_conv2d_wgrad': (_I, [C.POINTER(ConvDesc), _P, _P, _P, _P, _LL, _P]),
-    'ccb_act_bwd_bias_workspace_floats': (_LL, [_I, _I, _I]),
-    'ccb_act_bwd_bias': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, _LL, _P]),
-    'ccb_debug_last_conv_kernel': (C.c_char_p, []),
-    'ccb_debug_tc_plan': (_I, [_I, C.POINTER(_I)]),
-    'ccb_wcache_create': (C.c_void_p, []),
-    'ccb_wcache_destroy': (None, [C.c_void_p]),
-    'ccb_wcache_plan_floats': (_LL, [C.c_void_p]),
-    'ccb_wcache_table_bytes': (_LL, [C.c_void_p]),
-    'ccb_wcache_commit': (_I, [C.c_void_p, _P, _LL, _P, _LL, _P]),
-    'ccb_wcache_refresh': (_I, [C.c_void_p, _P]),
-    'ccb_wcache_stats': (None, [C.c_void_p, C.POINTER(C.c_longlong * 4)]),
-    'ccb_corr81_fwd_workspace_floats': (_LL, [_I, _I, _I, _I]),
-    'ccb_corr81_fwd': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _LL, _P]),
-    'ccb_corr81_bwd': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
-    'ccb_corr441d_fwd': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
-    'ccb_corr441d_bwd': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
-    'ccb_featwarp_fwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
-    'ccb_featwarp_bwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
-    'ccb_bn_workspace_floats': (_LL, [_I, _I, _I]),
-    'ccb_bn_fwd': (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _I, _P, _P]),
-    'ccb_bn_bwd': (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
-    'ccb_upsample2x_fwd': (_I, [_P, _P, _I, _I, _I, _P]),
-    'ccb_upsample2x_bwd': (_I, [_P, _P, _I, _I, _I, _P]),
-    'ccb_adam_step': (_I, [_P, _P, _P, _P, _LL, _P, _F, _F, _F, _F, _F, _P]),
-    'ccb_adam_step_ranges': (_I, [_P, _P, _P, _P, _P, _I, _LL, _P, _I, _P, _F, _F, _F, _F, _F, _P]),
-    'ccb_launch_count': (_LL, []),
-    'ccb_flow_metrics_workspace_bytes': (_LL, [_I, _I, _I]),
-    'ccb_flow_metrics': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _F, _F, _P, _P, _P, _P]),
-    'ccb_depth_errors_workspace_bytes': (_LL, [_I, _I, _I]),
-    'ccb_depth_errors': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
-    'ccb_mask_iou_workspace_bytes': (_LL, [_I, _I, _I, _I, _I]),
-    'ccb_mask_iou': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P, _LL, _P, _P]),
-    'ccb_prep_frames': (_I, [_P, C.POINTER(_P), _P, _P, _I, _I, _I, _I, _I, _I, _P]),
-    'ccb_prep_frames_unit': (_I, [_P, C.POINTER(_P), _P, _P, _I, _I, _I, _I, _I, _I, _P]),
-    'ccb_rotate_frames_u8': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
-    'ccb_resize_u8_workspace_bytes': (_LL, [_I, _I, _I, _I, _I]),
-    'ccb_resize_u8': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _LL, _P]),
-    'ccb_normalize_local_workspace_bytes': (_LL, [_I, _I, _I]),
-    'ccb_normalize_local': (_I, [C.POINTER(_P), _I, _I, _I, _I, _P, _P, _LL, _P]),
+    'ccb_last_error_string': ('const char*', ''),
+    'ccb_version': ('int', ''),
+    'ccb_is_simulator': ('int', ''),
+    'ccb_image_pyramid': (STATUS, 'const float*, int, int, int, int, float* const*, ccb_stream_t'),
+    'ccb_photo_partials_floats': ('long long', 'const ccb_photo_desc*'),
+    'ccb_photo_pose_partials_floats': ('long long', 'const ccb_photo_desc*'),
+    'ccb_photo_loss_fwd': (STATUS, 'const ccb_photo_desc*, ccb_stream_t'),
+    'ccb_photo_loss_bwd': (STATUS, 'const ccb_photo_desc*, ccb_stream_t'),
+    'ccb_consensus_targets': (STATUS, 'const ccb_photo_desc*, ccb_stream_t'),
+    'ccb_inverse_warp_fwd': (STATUS, 'const float*, const float*, const float*, int, const float*, const float*, '
+                                     'int, int, int, int, int, float*, ccb_stream_t'),
+    'ccb_inverse_warp_bwd': (STATUS, 'const float*, const float*, const float*, int, const float*, const float*, '
+                                     'int, int, int, int, int, const float*, float*, float*, float*, ccb_stream_t'),
+    'ccb_warp_pose_partials_floats': ('long long', 'int, int, int'),
+    'ccb_flow_warp_fwd': (STATUS, 'const float*, const float*, int, int, int, int, int, float*, ccb_stream_t'),
+    'ccb_flow_warp_bwd': (STATUS, 'const float*, const float*, int, int, int, int, int, const float*, float*, '
+                                  'float*, unsigned long long*, ccb_stream_t'),
+    'ccb_pose2flow_fwd': (STATUS, 'const float*, const float*, int, const float*, const float*, int, int, int, int, '
+                                  'int, float*, ccb_stream_t'),
+    'ccb_pose2flow_bwd': (STATUS, 'const float*, const float*, int, const float*, const float*, int, int, int, int, '
+                                  'int, const float*, float*, float*, float*, ccb_stream_t'),
+    'ccb_ssim_fwd': (STATUS, 'const float*, const float*, int, int, int, host const float*, float*, ccb_stream_t'),
+    'ccb_ssim_bwd': (STATUS, 'const float*, const float*, int, int, int, host const float*, const float*, float*, '
+                             'float*, float*, ccb_stream_t'),
+    'ccb_smooth_partials_floats': ('long long', 'const ccb_smooth_desc*'),
+    'ccb_smooth_fwd': (STATUS, 'const ccb_smooth_desc*, ccb_stream_t'),
+    'ccb_smooth_bwd': (STATUS, 'const ccb_smooth_desc*, ccb_stream_t'),
+    'ccb_bce_partials_floats': ('long long', 'const ccb_bce_desc*'),
+    'ccb_bce_fwd': (STATUS, 'const ccb_bce_desc*, ccb_stream_t'),
+    'ccb_bce_bwd': (STATUS, 'const ccb_bce_desc*, ccb_stream_t'),
+    'ccb_wcache_create': ('void*', ''),
+    'ccb_wcache_destroy': ('void', 'handle void*'),
+    'ccb_wcache_plan_floats': ('long long', 'handle void*'),
+    'ccb_wcache_table_bytes': ('long long', 'handle void*'),
+    'ccb_wcache_commit': (STATUS, 'handle void*, float*, long long, void*, long long, ccb_stream_t'),
+    'ccb_wcache_refresh': (STATUS, 'handle void*, ccb_stream_t'),
+    'ccb_wcache_stats': ('void', 'handle void*, host long long*'),
+    'ccb_conv_workspace_floats': ('long long', 'const ccb_conv_desc*, int'),
+    'ccb_conv2d_fprop': (STATUS, 'const ccb_conv_desc*, const float*, const float*, const float*, const float*, '
+                                 'float*, float*, long long, ccb_stream_t'),
+    'ccb_conv2d_dgrad': (STATUS, 'const ccb_conv_desc*, const float*, const float*, const float*, const float*, '
+                                 'float*, float*, long long, ccb_stream_t'),
+    'ccb_conv2d_wgrad': (STATUS, 'const ccb_conv_desc*, const float*, const float*, float*, float*, long long, '
+                                 'ccb_stream_t'),
+    'ccb_act_bwd_bias_workspace_floats': ('long long', 'int, int, int'),
+    'ccb_act_bwd_bias': (STATUS, 'const float*, const float*, float*, float*, int, int, int, int, float, float*, '
+                                 'long long, ccb_stream_t'),
+    'ccb_corr81_fwd_workspace_floats': ('long long', 'int, int, int, int'),
+    'ccb_corr81_fwd': (STATUS, 'const float*, const float*, float*, int, int, int, int, int, float*, long long, '
+                               'ccb_stream_t'),
+    'ccb_corr81_bwd': (STATUS, 'const float*, const float*, const float*, float*, float*, int, int, int, int, int, '
+                               'float*, ccb_stream_t'),
+    'ccb_corr441d_fwd': (STATUS, 'const float*, const float*, float*, int, int, int, int, ccb_stream_t'),
+    'ccb_corr441d_bwd': (STATUS, 'const float*, const float*, const float*, const float*, float*, float*, int, int, '
+                                 'int, int, ccb_stream_t'),
+    'ccb_featwarp_fwd': (STATUS, 'const float*, const float*, int, int, int, int, float*, ccb_stream_t'),
+    'ccb_featwarp_bwd': (STATUS, 'const float*, const float*, int, int, int, int, const float*, float*, float*, '
+                                 'unsigned long long*, ccb_stream_t'),
+    'ccb_bn_workspace_floats': ('long long', 'int, int, int'),
+    'ccb_bn_fwd': (STATUS, 'const float*, const float*, const float*, float*, float*, float*, float*, int, int, int, '
+                           'float, float, int, float*, ccb_stream_t'),
+    'ccb_bn_bwd': (STATUS, 'const float*, const float*, const float*, const float*, float*, float*, float*, int, '
+                           'int, int, float*, ccb_stream_t'),
+    'ccb_upsample2x_fwd': (STATUS, 'const float*, float*, int, int, int, ccb_stream_t'),
+    'ccb_upsample2x_bwd': (STATUS, 'const float*, float*, int, int, int, ccb_stream_t'),
+    'ccb_adam_step_ranges': (STATUS, 'float*, const float*, float*, float*, const long long*, int, long long, '
+                                     'const int*, int, float*, float, float, float, float, float, ccb_stream_t'),
+    'ccb_flow_metrics_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_flow_metrics': (STATUS, 'const float*, const float*, const float*, const float*, int, int, int, int, int, '
+                                 'int, int, int, float, float, float, float*, void*, float*, ccb_stream_t'),
+    'ccb_depth_errors_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_depth_errors': (STATUS, 'const float*, const float*, int, int, int, int, void*, float*, ccb_stream_t'),
+    'ccb_mask_iou_workspace_bytes': ('long long', 'int, int, int, int, int'),
+    'ccb_mask_iou': (STATUS, 'const float*, const float*, const float*, const float*, const float*, int, int, int, '
+                             'int, int, int, float, int, float*, void*, long long, long long*, ccb_stream_t'),
+    'ccb_prep_frames': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, int, '
+                                'int, int, ccb_stream_t'),
+    'ccb_prep_frames_unit': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '
+                                     'int, int, int, ccb_stream_t'),
+    'ccb_rotate_frames_u8': (STATUS, 'const unsigned char*, const double*, unsigned char*, int, int, int, int, '
+                                     'ccb_stream_t'),
+    'ccb_resize_u8_workspace_bytes': ('long long', 'int, int, int, int, int'),
+    'ccb_resize_u8': (STATUS, 'const unsigned char*, unsigned char*, int, int, int, int, int, void*, long long, '
+                              'ccb_stream_t'),
+    'ccb_normalize_local_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_normalize_local': (STATUS, 'float* const*, int, int, int, int, float*, void*, long long, ccb_stream_t'),
+    'ccb_launch_count': ('long long', ''),
+    'ccb_debug_last_conv_kernel': ('const char*', ''),
+    'ccb_debug_tc_plan': (STATUS, 'int, host int*'),
 }
-# entry points added by later translation units register themselves here (conv, nets, optimiser ...)
-EXTRA_SIGS = {}
+
+_SCALARS = {'int': C.c_int, 'long long': C.c_longlong, 'float': C.c_float}
+_DTYPES = {'float': torch.float32, 'double': torch.float64, 'int': torch.int32, 'long long': torch.int64,
+           'unsigned long long': torch.int64, 'unsigned char': torch.uint8, 'void': None}
+_RESTYPES = {STATUS: C.c_int, 'int': C.c_int, 'long long': C.c_longlong, 'void*': C.c_void_p, 'const char*': C.c_char_p,
+             'void': None}
+
+
+def _where(name, pos):
+    return name if pos is None else '%s argument %d' % (name, pos)
+
+
+def ptr(t, name='tensor', dtype=torch.float32, pos=None):
+    """Device pointer of a contiguous tensor of `dtype` (fp32 unless stated; None: any dtype; t None -> NULL).
+    `pos`: the position of the argument of entry point `name` that `t` is for (error messages)."""
+    if t is None:
+        return None
+    if dtype is not None and t.dtype != dtype:
+        raise TypeError('cc_b200: %s must be %s, got %s' % (_where(name, pos), dtype, t.dtype))
+    if not t.is_contiguous():
+        raise ValueError('cc_b200: %s must be contiguous' % _where(name, pos))
+    if not t.is_cuda and not is_simulator():
+        raise RuntimeError('cc_b200: %s is on %s - the sm_90a kernels need CUDA tensors (no CPU fallback)'
+                           % (_where(name, pos), t.device))
+    return t.data_ptr()
+
+
+def stream(t=None):
+    """The current stream of tensor `t`'s device (NULL for a CPU tensor: the simulator)."""
+    if t is not None and t.is_cuda:
+        return torch.cuda.current_stream(t.device).cuda_stream
+    return None
+
+
+def _param(decl):
+    """(ctypes argtype, conversion (arg, entry point, position) -> ctypes value, None: as it is) of a declared parameter."""
+    if decl in _SCALARS:
+        return _SCALARS[decl], None
+    if decl == 'ccb_stream_t':
+        return C.c_void_p, lambda t, name, pos: stream(t)
+    if decl == 'handle void*':
+        return C.c_void_p, None
+    if decl == 'float* const*':             # host array of device pointers, given as a list of fp32 tensors
+        return C.POINTER(C.c_void_p), lambda ts, name, pos: (C.c_void_p * len(ts))(*[ptr(t, name, pos=pos) for t in ts])
+    base = decl.replace('const ', '').rstrip('*')
+    if base.startswith('host '):            # host array: an input given as a list of values, an output as a ctypes array
+        ct = _SCALARS[base[len('host '):]]
+        if 'const ' in decl:
+            return C.POINTER(ct), lambda a, name, pos: (ct * len(a))(*a)
+        return C.POINTER(ct), None
+    if base in STRUCTS:
+        return C.POINTER(STRUCTS[base]), lambda d, name, pos: C.byref(d)
+    dtype = _DTYPES[base]
+    return C.c_void_p, lambda t, name, pos: ptr(t, name, dtype, pos)
+
+
+_CALLS = {name: (ret, [_param(p) for p in params.split(', ') if p]) for name, (ret, params) in _SIGS.items()}
 
 
 def _bind(lib):
-    sigs = dict(_SIGS)
-    sigs.update(EXTRA_SIGS)
-    for name, (res, args) in sigs.items():
+    for name, (ret, params) in _CALLS.items():
         fn = getattr(lib, name)          # AttributeError => header/library mismatch: fail loudly
-        fn.restype = res
-        fn.argtypes = args
+        fn.restype = _RESTYPES[ret]
+        fn.argtypes = [argtype for argtype, _ in params]
+
+
+def call(name, *args):
+    """Entry point `name` on `args`, each converted as its parameter is declared: a tensor -> device pointer (checked like
+    ptr()), None -> NULL, a list of tensors -> host array of their pointers, a descriptor -> byref, and in the stream
+    slot a tensor -> its device's current stream.  A non-zero status raises RuntimeError.  The function is looked up
+    on every call and called with positional arguments (tools swap lib() for a proxy that times the calls)."""
+    ret, params = _CALLS[name]
+    if len(args) != len(params):
+        raise TypeError('cc_b200: %s takes %d arguments, got %d' % (name, len(params), len(args)))
+    fn = getattr(lib(), name)
+    rc = fn(*[a if conv is None else conv(a, name, i) for i, ((_, conv), a) in enumerate(zip(params, args))])
+    if ret == STATUS:
+        check(rc, name)
+    return rc
+
+
+def check(rc, what=''):
+    """Raise RuntimeError for a non-zero ccb_status `rc` of entry point `what`, with ccb_last_error_string()."""
+    if rc != 0:
+        msg = lib().ccb_last_error_string()
+        raise RuntimeError('libccb200 %s failed (status %d): %s' % (what, rc, msg.decode() if msg else ''))
 
 
 def use_library(path):
@@ -180,36 +286,11 @@ def is_simulator():
     return _is_sim
 
 
-def check(rc, what=''):
-    if rc != 0:
-        msg = lib().ccb_last_error_string()
-        raise RuntimeError('libccb200 %s failed (status %d): %s' % (what, rc, msg.decode() if msg else ''))
-
-
-def ptr(t, name='tensor', dtype=torch.float32):
-    """Device pointer of a contiguous tensor of `dtype` (fp32 unless stated; None -> NULL)."""
-    if t is None:
-        return None
-    if t.dtype != dtype:
-        raise TypeError('cc_b200: %s must be %s, got %s' % (name, dtype, t.dtype))
-    if not t.is_contiguous():
-        raise ValueError('cc_b200: %s must be contiguous' % name)
-    if not t.is_cuda and not is_simulator():
-        raise RuntimeError('cc_b200: %s is on %s - the sm_90a kernels need CUDA tensors (no CPU fallback)'
-                           % (name, t.device))
-    return t.data_ptr()
-
-
 def scatter_workspace(t):
     """Fixed-point accumulators (+1 word) for the image gradient of a warp of `t` (ccb_flow_warp_bwd / ccb_featwarp_bwd)."""
     return torch.empty(t.numel() + 1, dtype=torch.int64, device=t.device)
 
 
-def stream(t=None):
-    if t is not None and t.is_cuda:
-        return torch.cuda.current_stream(t.device).cuda_stream
-    return None
-
-
-def contig(t):
-    return t if t.is_contiguous() else t.contiguous()
+def f32(t):
+    """`t` detached, as contiguous fp32: how every op hands a tensor to the kernels."""
+    return t.detach().float().contiguous()

@@ -216,28 +216,23 @@ __global__ void adam_prep_kernel(float* __restrict__ state, const int* __restric
 }
 
 // grad_scale multiplies the gradient first (1/world_size after the NCCL sum).
-// Block -> range: the largest entry whose first_block <= blockIdx.x (binary search over the table; one range and no
-// table when ranges == nullptr).  The range decides only which elements and which group's bias corrections a thread
-// uses, never the per-element arithmetic.
+// Block -> range: the largest entry whose first_block <= blockIdx.x (binary search over the table).  The range decides
+// only which elements and which group's bias corrections a thread uses, never the per-element arithmetic.
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                                   float* __restrict__ v, long long n, const long long* __restrict__ ranges,
-                                                   int nranges, const float* __restrict__ state,
+                                                   float* __restrict__ v, const long long* __restrict__ ranges, int nranges,
+                                                   const float* __restrict__ state,
                                                    float lr, float b1, float b2, float eps, float grad_scale) {
     CCB_PDL_WAIT();
-    long long off = 0, cnt = n, blk = blockIdx.x;
-    int grp = 0;
-    if (ranges != nullptr) {
-        int lo = 0, hi = nranges - 1;
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (__ldg(ranges + 4 * mid + 3) <= blk) lo = mid;
-            else hi = mid - 1;
-        }
-        off = __ldg(ranges + 4 * lo);
-        cnt = __ldg(ranges + 4 * lo + 1);
-        grp = (int)__ldg(ranges + 4 * lo + 2);
-        blk -= __ldg(ranges + 4 * lo + 3);
+    long long blk = blockIdx.x;
+    int lo = 0, hi = nranges - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(ranges + 4 * mid + 3) <= blk) lo = mid;
+        else hi = mid - 1;
     }
+    const long long off = __ldg(ranges + 4 * lo), cnt = __ldg(ranges + 4 * lo + 1);
+    const int grp = (int)__ldg(ranges + 4 * lo + 2);
+    blk -= __ldg(ranges + 4 * lo + 3);
     const long long j = blk * 256 + threadIdx.x;
     if (j >= cnt) return;
     const long long i = off + j;
@@ -308,18 +303,6 @@ extern "C" int ccb_upsample2x_bwd(const float* dy, float* dx, int planes, int h,
     return check_launch("upsample2x_bwd");
 }
 
-extern "C" int ccb_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
-                             float* state, float lr, float beta1, float beta2, float eps, float grad_scale,
-                             ccb_stream_t stream) {
-    CCB_REQUIRE(params && grads && exp_avg && exp_avg_sq && state && n >= 0, CCB_ERR_ARG, "adam_step: bad argument");
-    CCB_LAUNCH(adam_prep_kernel, dim3(1), dim3(32), 0, stream, state, (const int*)nullptr, 1, beta1, beta2);
-    int rc = check_launch("adam_prep");
-    if (rc || n == 0) return rc;
-    CCB_LAUNCH(adam_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, params, grads, exp_avg, exp_avg_sq, n,
-               (const long long*)nullptr, 1, (const float*)state, lr, beta1, beta2, eps, grad_scale);
-    return check_launch("adam_step");
-}
-
 extern "C" int ccb_adam_step_ranges(float* params, const float* grads, float* exp_avg, float* exp_avg_sq,
                                     const long long* ranges, int nranges, long long nblocks, const int* group_active,
                                     int ngroups, float* group_state, float lr, float beta1, float beta2, float eps,
@@ -331,7 +314,7 @@ extern "C" int ccb_adam_step_ranges(float* params, const float* grads, float* ex
     CCB_LAUNCH(adam_prep_kernel, dim3(cdiv(ngroups, 32)), dim3(32), 0, stream, group_state, group_active, ngroups, beta1, beta2);
     int rc = check_launch("adam_prep");
     if (rc || nranges == 0) return rc;
-    CCB_LAUNCH(adam_kernel, dim3((unsigned)nblocks), dim3(256), 0, stream, params, grads, exp_avg, exp_avg_sq, 0LL, ranges,
-               nranges, (const float*)group_state, lr, beta1, beta2, eps, grad_scale);
+    CCB_LAUNCH(adam_kernel, dim3((unsigned)nblocks), dim3(256), 0, stream, params, grads, exp_avg, exp_avg_sq, ranges, nranges,
+               (const float*)group_state, lr, beta1, beta2, eps, grad_scale);
     return check_launch("adam_step_ranges");
 }

@@ -128,21 +128,18 @@ def motion_mask_counts(emask, flow_cam, flow_fwd, obj_map_gt, semantic_map_gt, T
     [tp_0, fp_0, fn_0, tp_1, fp_1, fn_1] (class 0 = rigid background, class 1 = moving car; pixels whose semantic label is
     not 26 are ignored).  The maximum that normalises the census is taken per sample; the reference runs batch 1.
     want_masks: also [B,4,h,w] = combined, census, bare (0/1) and the soft census.  No host synchronisation."""
-    emask, flow_cam, flow_fwd = (_lib.contig(t.float()) for t in (emask, flow_cam, flow_fwd))
-    obj, sem = _lib.contig(obj_map_gt.float()), _lib.contig(semantic_map_gt.float())
+    emask, flow_cam, flow_fwd = (_lib.f32(t) for t in (emask, flow_cam, flow_fwd))
+    obj, sem = _lib.f32(obj_map_gt), _lib.f32(semantic_map_gt)
     B, C, h, w = (int(v) for v in emask.shape)
     Hg, Wg = int(obj.shape[1]), int(obj.shape[2])
     assert flow_cam.shape == (B, 2, h, w) and flow_fwd.shape == (B, 2, h, w), (flow_cam.shape, flow_fwd.shape)
     assert obj.shape == (B, Hg, Wg) and sem.shape == (B, Hg, Wg), (obj.shape, sem.shape)
-    lib = _lib.lib()
-    nbytes = int(lib.ccb_mask_iou_workspace_bytes(B, h, w, Hg, Wg))
+    nbytes = int(_lib.call('ccb_mask_iou_workspace_bytes', B, h, w, Hg, Wg))
     work = torch.empty(max(nbytes, 0) // 8 + 1, device=emask.device, dtype=torch.int64)
     n = torch.empty(B, 3, 4, device=emask.device, dtype=torch.int64)
     masks = torch.empty(B, 4, h, w, device=emask.device) if want_masks else None
-    _lib.check(lib.ccb_mask_iou(_lib.ptr(emask, 'emask'), _lib.ptr(flow_cam, 'flow_cam'), _lib.ptr(flow_fwd, 'flow_fwd'),
-                                _lib.ptr(obj, 'obj_map_gt'), _lib.ptr(sem, 'semantic_map_gt'), B, C, h, w, Hg, Wg, float(THRESH), 26,
-                                _lib.ptr(masks), _lib.ptr(work, 'work', torch.int64), nbytes, _lib.ptr(n, 'counts', torch.int64),
-                                _lib.stream(emask)), 'mask_iou')
+    _lib.call('ccb_mask_iou', emask, flow_cam, flow_fwd, obj, sem, B, C, h, w, Hg, Wg, float(THRESH), 26, masks, work, nbytes, n,
+              emask)
     # n[pred][gt] = n00 n01 n10 n11 -> tp_0 fp_0 fn_0 tp_1 fp_1 fn_1: fp_1 = fn_0 = n10, fn_1 = fp_0 = n01
     counts = torch.cat([n, n[..., 2:3], n[..., 1:2]], -1)
     return (counts, masks) if want_masks else counts

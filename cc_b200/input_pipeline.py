@@ -24,7 +24,6 @@ The reference's other transforms run on the device as well, bit-exact with Pillo
 The reference's loaders hand scipy.misc float32 copies of the uint8 frames (load_as_float), and scipy.misc byte-scales a
 float image to its own [min, max] before resampling; this pipeline takes the uint8 frames as they are, which is the
 same whenever a frame spans 0..255."""
-import ctypes as C
 import math
 import random
 import numpy as np
@@ -95,8 +94,7 @@ def rotate_frames(src, affine):
     aff = torch.as_tensor(affine, dtype=torch.float64).to(src.device, non_blocking=True).contiguous()
     assert aff.shape == (B, 6)
     dst = torch.empty_like(src)
-    _lib.check(_lib.lib().ccb_rotate_frames_u8(_lib.ptr(src, 'frames', torch.uint8), _lib.ptr(aff, 'affine', torch.float64),
-                                               _lib.ptr(dst, 'dst', torch.uint8), B, F, H, W, _lib.stream(src)), 'rotate_frames_u8')
+    _lib.call('ccb_rotate_frames_u8', src, aff, dst, B, F, H, W, src)
     return dst
 
 
@@ -105,11 +103,10 @@ def resize_frames(src, h, w):
     Hs, Ws = src.shape[-3], src.shape[-2]
     N = src.numel() // (Hs * Ws * 3)
     dst = torch.empty(tuple(src.shape[:-3]) + (h, w, 3), dtype=torch.uint8, device=src.device)
-    nb = _lib.lib().ccb_resize_u8_workspace_bytes(N, Hs, Ws, h, w)
+    nb = _lib.call('ccb_resize_u8_workspace_bytes', N, Hs, Ws, h, w)
     assert nb >= 0, 'resize_frames: bad sizes'
     work = torch.empty(max(nb, 1), dtype=torch.uint8, device=src.device)
-    _lib.check(_lib.lib().ccb_resize_u8(_lib.ptr(src, 'frames', torch.uint8), _lib.ptr(dst, 'dst', torch.uint8), N, Hs, Ws, h, w,
-                                        _lib.ptr(work, 'work', torch.uint8), nb, _lib.stream(src)), 'resize_u8')
+    _lib.call('ccb_resize_u8', src, dst, N, Hs, Ws, h, w, work, nb, src)
     return dst
 
 
@@ -119,11 +116,9 @@ def normalize_local(frames):
     B, _, H, W = frames[0].shape
     F = len(frames)
     stats = torch.empty(B, 3, 2, device=frames[0].device)
-    nb = _lib.lib().ccb_normalize_local_workspace_bytes(B, H, W)
+    nb = _lib.call('ccb_normalize_local_workspace_bytes', B, H, W)
     work = torch.empty(nb, dtype=torch.uint8, device=frames[0].device)
-    arr = (C.c_void_p * F)(*[_lib.ptr(f) for f in frames])
-    _lib.check(_lib.lib().ccb_normalize_local(arr, B, F, H, W, _lib.ptr(stats), _lib.ptr(work, 'work', torch.uint8), nb,
-                                              _lib.stream(frames[0])), 'normalize_local')
+    _lib.call('ccb_normalize_local', frames, B, F, H, W, stats, work, nb, frames[0])
     return stats
 
 
@@ -131,10 +126,8 @@ def _prep(src, par, offs, B, F, Hs, Ws, H, W, normalization):
     """uint8 [B,F,Hs,Ws,3] on the device -> F tensors [B,3,H,W]: flip / scale-crop lookup, ArrayToTensor, then Normalize(.5,
     .5) (global) or NormalizeLocally (local; returns its statistics, else None)."""
     outs = [torch.empty(B, 3, H, W, device=src.device) for _ in range(F)]
-    arr = (C.c_void_p * F)(*[_lib.ptr(o) for o in outs])
-    fn, name = ('ccb_prep_frames', 'prep_frames') if normalization == 'global' else ('ccb_prep_frames_unit', 'prep_frames_unit')
-    _lib.check(getattr(_lib.lib(), fn)(_lib.ptr(src, 'frames', torch.uint8), arr, _lib.ptr(par), _lib.ptr(offs, 'offs', torch.int32),
-                                       B, F, Hs, Ws, H, W, _lib.stream(src)), name)
+    fn = 'ccb_prep_frames' if normalization == 'global' else 'ccb_prep_frames_unit'
+    _lib.call(fn, src, outs, par, offs, B, F, Hs, Ws, H, W, src)
     return outs, (normalize_local(outs) if normalization == 'local' else None)
 
 

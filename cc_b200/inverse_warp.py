@@ -20,19 +20,13 @@ def check_sizes(input, input_name, expected):
     assert(all(condition)), "wrong size for {}, expected {}, got  {}".format(input_name, 'x'.join(expected), list(input.size()))
 
 
-def _f(t):
-    return _lib.contig(t.detach().float())
-
-
 class _InverseWarp(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img, depth, pose, K, Kinv, rot, pad):
-        img, depth, pose, K, Kinv = _f(img), _f(depth), _f(pose), _f(K), _f(Kinv)
+        img, depth, pose, K, Kinv = _lib.f32(img), _lib.f32(depth), _lib.f32(pose), _lib.f32(K), _lib.f32(Kinv)
         B, _, h, w = img.shape
         out = torch.empty_like(img)
-        L = _lib.lib()
-        _lib.check(L.ccb_inverse_warp_fwd(_lib.ptr(img), _lib.ptr(depth), _lib.ptr(pose), 6, _lib.ptr(K), _lib.ptr(Kinv),
-                                          B, h, w, rot, pad, _lib.ptr(out), _lib.stream(img)), 'inverse_warp_fwd')
+        _lib.call('ccb_inverse_warp_fwd', img, depth, pose, 6, K, Kinv, B, h, w, rot, pad, out, img)
         ctx.save_for_backward(img, depth, pose, K, Kinv)
         ctx.cfg = (rot, pad)
         return out
@@ -42,26 +36,21 @@ class _InverseWarp(torch.autograd.Function):
         img, depth, pose, K, Kinv = ctx.saved_tensors
         rot, pad = ctx.cfg
         B, _, h, w = img.shape
-        g = _f(g)
-        L = _lib.lib()
+        g = _lib.f32(g)
         d_depth = torch.empty_like(depth)
         d_pose = torch.empty_like(pose)
-        part = torch.empty(L.ccb_warp_pose_partials_floats(B, h, w), device=img.device)
-        _lib.check(L.ccb_inverse_warp_bwd(_lib.ptr(img), _lib.ptr(depth), _lib.ptr(pose), 6, _lib.ptr(K), _lib.ptr(Kinv),
-                                          B, h, w, rot, pad, _lib.ptr(g), _lib.ptr(d_depth), _lib.ptr(d_pose),
-                                          _lib.ptr(part), _lib.stream(img)), 'inverse_warp_bwd')
+        part = torch.empty(_lib.call('ccb_warp_pose_partials_floats', B, h, w), device=img.device)
+        _lib.call('ccb_inverse_warp_bwd', img, depth, pose, 6, K, Kinv, B, h, w, rot, pad, g, d_depth, d_pose, part, img)
         return None, d_depth, d_pose, None, None, None, None
 
 
 class _Pose2Flow(torch.autograd.Function):
     @staticmethod
     def forward(ctx, depth, pose, K, Kinv, rot, pad):
-        depth, pose, K, Kinv = _f(depth), _f(pose), _f(K), _f(Kinv)
+        depth, pose, K, Kinv = _lib.f32(depth), _lib.f32(pose), _lib.f32(K), _lib.f32(Kinv)
         B, h, w = depth.shape
         out = torch.empty(B, 2, h, w, device=depth.device)
-        L = _lib.lib()
-        _lib.check(L.ccb_pose2flow_fwd(_lib.ptr(depth), _lib.ptr(pose), 6, _lib.ptr(K), _lib.ptr(Kinv), B, h, w, rot, pad,
-                                       _lib.ptr(out), _lib.stream(depth)), 'pose2flow_fwd')
+        _lib.call('ccb_pose2flow_fwd', depth, pose, 6, K, Kinv, B, h, w, rot, pad, out, depth)
         ctx.save_for_backward(depth, pose, K, Kinv)
         ctx.cfg = (rot, pad)
         return out
@@ -71,25 +60,21 @@ class _Pose2Flow(torch.autograd.Function):
         depth, pose, K, Kinv = ctx.saved_tensors
         rot, pad = ctx.cfg
         B, h, w = depth.shape
-        g = _f(g)
-        L = _lib.lib()
+        g = _lib.f32(g)
         d_depth = torch.empty_like(depth)
         d_pose = torch.empty_like(pose)
-        part = torch.empty(L.ccb_warp_pose_partials_floats(B, h, w), device=depth.device)
-        _lib.check(L.ccb_pose2flow_bwd(_lib.ptr(depth), _lib.ptr(pose), 6, _lib.ptr(K), _lib.ptr(Kinv), B, h, w, rot, pad,
-                                       _lib.ptr(g), _lib.ptr(d_depth), _lib.ptr(d_pose), _lib.ptr(part),
-                                       _lib.stream(depth)), 'pose2flow_bwd')
+        part = torch.empty(_lib.call('ccb_warp_pose_partials_floats', B, h, w), device=depth.device)
+        _lib.call('ccb_pose2flow_bwd', depth, pose, 6, K, Kinv, B, h, w, rot, pad, g, d_depth, d_pose, part, depth)
         return d_depth, d_pose, None, None, None, None
 
 
 class _FlowWarp(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img, flow, pad):
-        img, flow = _f(img), _f(flow)
+        img, flow = _lib.f32(img), _lib.f32(flow)
         B, Cc, h, w = img.shape
         out = torch.empty_like(img)
-        _lib.check(_lib.lib().ccb_flow_warp_fwd(_lib.ptr(img), _lib.ptr(flow), B, Cc, h, w, pad, _lib.ptr(out),
-                                                _lib.stream(img)), 'flow_warp_fwd')
+        _lib.call('ccb_flow_warp_fwd', img, flow, B, Cc, h, w, pad, out, img)
         ctx.save_for_backward(img, flow)
         ctx.pad = pad
         return out
@@ -98,13 +83,11 @@ class _FlowWarp(torch.autograd.Function):
     def backward(ctx, g):
         img, flow = ctx.saved_tensors
         B, Cc, h, w = img.shape
-        g = _f(g)
+        g = _lib.f32(g)
         d_flow = torch.empty_like(flow) if ctx.needs_input_grad[1] else None
         d_img = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
         work = _lib.scatter_workspace(img) if d_img is not None else None
-        _lib.check(_lib.lib().ccb_flow_warp_bwd(_lib.ptr(img), _lib.ptr(flow), B, Cc, h, w, ctx.pad, _lib.ptr(g),
-                                                _lib.ptr(d_flow), _lib.ptr(d_img), _lib.ptr(work, 'work', torch.int64),
-                                                _lib.stream(img)), 'flow_warp_bwd')
+        _lib.call('ccb_flow_warp_bwd', img, flow, B, Cc, h, w, ctx.pad, g, d_flow, d_img, work, img)
         return d_img, d_flow, None
 
 

@@ -10,7 +10,6 @@ Differences a maintainer should know:
     not replicated - nothing here synchronises the host;
   * pyramid levels must be exact 2^l reductions of the frame (true for every net in the reference).
 """
-import ctypes as C
 import torch
 from torch import nn
 from . import _lib, pyramid
@@ -20,10 +19,6 @@ from .ssim import ssim, taps13                                  # noqa: F401
 epsilon = 1e-8
 _ROT = {'euler': _lib.ROT_EULER, 'quat': _lib.ROT_QUAT}
 _PAD = {'zeros': _lib.PAD_ZEROS, 'border': _lib.PAD_BORDER}
-
-
-def _f(t):
-    return _lib.contig(t.detach().float())
 
 
 def _set_levels(arr, tensors, name):
@@ -57,12 +52,12 @@ class _PhotoLoss(torch.autograd.Function):
         for l in range(L):
             for i in range(R):
                 d.ref[l][i] = _lib.ptr(cfg['refs'][i][l], 'ref')
-        ts = [_f(t) for t in tensors]
+        ts = [_lib.f32(t) for t in tensors]
         keep += ts
         if mode == _lib.PHOTO_RIGID:
             pose, depth = ts[0], ts[1:1 + L]
             masks = ts[1 + L:1 + 2 * L] if cfg['has_mask'] else None
-            K, Kinv = _f(cfg['K']), _f(cfg['Kinv'])
+            K, Kinv = _lib.f32(cfg['K']), _lib.f32(cfg['Kinv'])
             keep += [K, Kinv]
             d.pose, d.K, d.Kinv = _lib.ptr(pose, 'pose'), _lib.ptr(K, 'K'), _lib.ptr(Kinv, 'Kinv')
             _set_levels(d.depth, depth, 'depth')
@@ -86,12 +81,11 @@ class _PhotoLoss(torch.autograd.Function):
         _set_levels(d.vo, vo, 'vo')
         if gm:
             _set_levels(d.gmask, gm, 'gmask')
-        lib = _lib.lib()
         scal = torch.empty(L * R * 4, device=dev)
-        part = torch.empty(max(1, lib.ccb_photo_partials_floats(C.byref(d))), device=dev)
+        part = torch.empty(max(1, _lib.call('ccb_photo_partials_floats', d)), device=dev)
         loss = torch.empty(1, device=dev)
         d.scal, d.partials, d.loss = _lib.ptr(scal), _lib.ptr(part), _lib.ptr(loss)
-        _lib.check(lib.ccb_photo_loss_fwd(C.byref(d), _lib.stream(loss)), 'photo_loss_fwd')
+        _lib.call('ccb_photo_loss_fwd', d, loss)
         ctx.desc, ctx.cfg = d, cfg
         ctx.keep = keep + dm + vo + gm + [scal, loss] + list(cfg['tgt']) + [t for r in cfg['refs'] for t in r]
         ctx.n_in = len(tensors)
@@ -103,14 +97,13 @@ class _PhotoLoss(torch.autograd.Function):
         mode, L, R, B = cfg['mode'], cfg['L'], cfg['R'], cfg['B']
         sizes = cfg['sizes']
         dev = cfg['tgt'][0].device
-        lib = _lib.lib()
-        g = _f(g).reshape(1)
+        g = _lib.f32(g).reshape(1)
         d.grad_out = _lib.ptr(g, 'grad_out')
         grads = []
         if mode == _lib.PHOTO_RIGID:
             d_pose = torch.empty(B, R, 6, device=dev)
             d_depth = [torch.empty(B, 1, h, w, device=dev) for (h, w) in sizes]
-            part = torch.empty(max(1, lib.ccb_photo_pose_partials_floats(C.byref(d))), device=dev)
+            part = torch.empty(max(1, _lib.call('ccb_photo_pose_partials_floats', d)), device=dev)
             d.d_pose, d.pose_partials = _lib.ptr(d_pose), _lib.ptr(part)
             _set_levels(d.d_depth, d_depth, 'd_depth')
             grads = [d_pose] + d_depth
@@ -126,7 +119,7 @@ class _PhotoLoss(torch.autograd.Function):
             grads = grads + d_mask
         elif cfg['has_mask']:
             grads = grads + [None] * L
-        _lib.check(lib.ccb_photo_loss_bwd(C.byref(d), _lib.stream(g)), 'photo_loss_bwd')
+        _lib.call('ccb_photo_loss_bwd', d, g)
         return (None,) + tuple(grads)
 
 
@@ -209,7 +202,7 @@ def consensus_exp_masks(cam_flows_fwd, cam_flows_bwd, flows_fwd, flows_bwd, tgt_
         d.taps[k] = v
     tgt = pyramid.levels_for(tgt_img, sizes)
     rf, rb = pyramid.levels_for(ref_img_fwd, sizes), pyramid.levels_for(ref_img_bwd, sizes)
-    fl = [[_f(cam_flows_fwd[l]), _f(cam_flows_bwd[l]), _f(flows_fwd[l])] for l in range(L)]
+    fl = [[_lib.f32(cam_flows_fwd[l]), _lib.f32(cam_flows_bwd[l]), _lib.f32(flows_fwd[l])] for l in range(L)]
     out = [torch.empty(B, 1, h, w, device=dev) for (h, w) in sizes]
     _set_levels(d.tgt, tgt, 'tgt')
     _set_levels(d.target, out, 'target')
@@ -217,7 +210,7 @@ def consensus_exp_masks(cam_flows_fwd, cam_flows_bwd, flows_fwd, flows_bwd, tgt_
         for i, r in enumerate((rf[l], rb[l], rf[l])):
             d.ref[l][i] = _lib.ptr(r, 'ref')
             d.flow[l][i] = _lib.ptr(fl[l][i], 'flow')
-    _lib.check(_lib.lib().ccb_consensus_targets(C.byref(d), _lib.stream(tgt_img)), 'consensus_targets')
+    _lib.call('ccb_consensus_targets', d, tgt_img)
     return out
 
 
@@ -227,7 +220,7 @@ def consensus_exp_masks(cam_flows_fwd, cam_flows_bwd, flows_fwd, flows_bwd, tgt_
 class _SmoothLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, cfg, *preds):
-        ps = [_f(p) for p in preds]
+        ps = [_lib.f32(p) for p in preds]
         L = len(ps)
         B, Cc = int(ps[0].size(0)), int(ps[0].size(1))
         dev = ps[0].device
@@ -239,23 +232,22 @@ class _SmoothLoss(torch.autograd.Function):
         _set_levels(d.pred, ps, 'pred')
         if cfg['kind'] == _lib.SMOOTH_EDGE:
             _set_levels(d.img, cfg['img'], 'img')
-        lib = _lib.lib()
-        part = torch.empty(max(1, lib.ccb_smooth_partials_floats(C.byref(d))), device=dev)
+        part = torch.empty(max(1, _lib.call('ccb_smooth_partials_floats', d)), device=dev)
         loss = torch.empty(1, device=dev)
         d.partials, d.loss = _lib.ptr(part), _lib.ptr(loss)
-        _lib.check(lib.ccb_smooth_fwd(C.byref(d), _lib.stream(loss)), 'smooth_fwd')
+        _lib.call('ccb_smooth_fwd', d, loss)
         ctx.desc, ctx.keep = d, ps + list(cfg.get('img', []))
         return loss[0]
 
     @staticmethod
     def backward(ctx, g):
         d = ctx.desc
-        g = _f(g).reshape(1)
+        g = _lib.f32(g).reshape(1)
         ps = ctx.keep[:d.nlevels]
         dp = [torch.empty_like(p) for p in ps]
         d.grad_out = _lib.ptr(g)
         _set_levels(d.d_pred, dp, 'd_pred')
-        _lib.check(_lib.lib().ccb_smooth_bwd(C.byref(d), _lib.stream(g)), 'smooth_bwd')
+        _lib.call('ccb_smooth_bwd', d, g)
         return (None,) + tuple(dp)
 
 
@@ -280,7 +272,7 @@ def smooth_loss(pred_disp):
 class _BceLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, cfg, *masks):
-        ms = [_f(m) for m in masks]
+        ms = [_lib.f32(m) for m in masks]
         L = len(ms)
         B, Cc = int(ms[0].size(0)), int(ms[0].size(1))
         dev = ms[0].device
@@ -293,26 +285,25 @@ class _BceLoss(torch.autograd.Function):
         keep = list(ms)
         if cfg['kind'] == _lib.BCE_CONSENSUS:
             for name in ('census_bwd', 'census_fwd', 'target_bwd', 'target_fwd'):
-                ts = [_f(t) for t in cfg[name]]
+                ts = [_lib.f32(t) for t in cfg[name]]
                 keep += ts
                 _set_levels(getattr(d, name), ts, name)
-        lib = _lib.lib()
-        part = torch.empty(max(1, lib.ccb_bce_partials_floats(C.byref(d))), device=dev)
+        part = torch.empty(max(1, _lib.call('ccb_bce_partials_floats', d)), device=dev)
         loss = torch.empty(1, device=dev)
         d.partials, d.loss = _lib.ptr(part), _lib.ptr(loss)
-        _lib.check(lib.ccb_bce_fwd(C.byref(d), _lib.stream(loss)), 'bce_fwd')
+        _lib.call('ccb_bce_fwd', d, loss)
         ctx.desc, ctx.keep = d, keep
         return loss[0]
 
     @staticmethod
     def backward(ctx, g):
         d = ctx.desc
-        g = _f(g).reshape(1)
+        g = _lib.f32(g).reshape(1)
         ms = ctx.keep[:d.nlevels]
         dm = [torch.empty_like(m) for m in ms]
         d.grad_out = _lib.ptr(g)
         _set_levels(d.d_mask, dm, 'd_mask')
-        _lib.check(_lib.lib().ccb_bce_bwd(C.byref(d), _lib.stream(g)), 'bce_bwd')
+        _lib.call('ccb_bce_bwd', d, g)
         return (None,) + tuple(dm)
 
 
@@ -413,21 +404,20 @@ def weighted_binary_cross_entropy(output, target, weights=None):
 # no intermediate up-sampled tensors.  Same names / arguments / python-float results as the reference, so
 # validate_flow_with_gt / validate_depth_with_gt (train.py:588-777) call them unchanged.
 def _flow_metrics(gt, pred_a, pred_b=None, mask=None, thresh=0.5, tau=(3, 0.05), want_map=False):
-    gt, pred_a = _f(gt), _f(pred_a)
+    gt, pred_a = _lib.f32(gt), _lib.f32(pred_a)
     B, nc, Hg, Wg = gt.shape
     hp, wp = int(pred_a.shape[2]), int(pred_a.shape[3])
     hm = wm = 0
     if mask is not None:
-        pred_b, mask = _f(pred_b), _f(mask)
+        pred_b, mask = _lib.f32(pred_b), _lib.f32(mask)
         assert pred_b.shape == pred_a.shape and mask.shape[1] == 1
         hm, wm = int(mask.shape[2]), int(mask.shape[3])
-    lib = _lib.lib()
-    work = torch.empty(int(lib.ccb_flow_metrics_workspace_bytes(B, Hg, Wg) // 8) + 1, device=gt.device, dtype=torch.float64)
+    work = torch.empty(int(_lib.call('ccb_flow_metrics_workspace_bytes', B, Hg, Wg) // 8) + 1, device=gt.device,
+                       dtype=torch.float64)
     out = torch.empty(4, device=gt.device)
     emap = torch.empty(B, Hg, Wg, device=gt.device) if want_map else None
-    _lib.check(lib.ccb_flow_metrics(_lib.ptr(gt, 'gt'), _lib.ptr(pred_a, 'pred'), _lib.ptr(pred_b), _lib.ptr(mask), B, int(nc),
-                                    int(Hg), int(Wg), hp, wp, hm, wm, float(thresh), float(tau[0]), float(tau[1]), _lib.ptr(emap),
-                                    _lib.ptr(work, 'work', torch.float64), _lib.ptr(out), _lib.stream(gt)), 'flow_metrics')
+    _lib.call('ccb_flow_metrics', gt, pred_a, pred_b, mask, B, int(nc), int(Hg), int(Wg), hp, wp, hm, wm, float(thresh),
+              float(tau[0]), float(tau[1]), emap, work, out, gt)
     return out, emap
 
 
@@ -457,11 +447,10 @@ def compute_errors(gt, pred, crop=True):
     """Depth metrics [abs_diff, abs_rel, sq_rel, a1, a2, a3] with median scaling and the Garg crop.
     Reference :430-467 (returns 0-dim tensors like the reference; the per-sample medians are found by a
     radix select on the device)."""
-    gt, pred = _f(gt), _f(pred)
+    gt, pred = _lib.f32(gt), _lib.f32(pred)
     B, H, W = gt.shape
-    lib = _lib.lib()
-    work = torch.empty(int(lib.ccb_depth_errors_workspace_bytes(B, H, W) // 8) + 1, device=gt.device, dtype=torch.float64)
+    work = torch.empty(int(_lib.call('ccb_depth_errors_workspace_bytes', B, H, W) // 8) + 1, device=gt.device,
+                       dtype=torch.float64)
     out = torch.empty(6, device=gt.device)
-    _lib.check(lib.ccb_depth_errors(_lib.ptr(gt, 'gt'), _lib.ptr(pred, 'pred'), B, H, W, int(bool(crop)), _lib.ptr(work, 'work', torch.float64), _lib.ptr(out),
-                                    _lib.stream(gt)), 'depth_errors')
+    _lib.call('ccb_depth_errors', gt, pred, B, H, W, int(bool(crop)), work, out, gt)
     return [out[i] for i in range(6)]

@@ -45,32 +45,30 @@ class WeightCache:
 
     def __init__(self, device):
         self.device = device
-        self.h = _lib.lib().ccb_wcache_create()
+        self.h = _lib.call('ccb_wcache_create')
         self.committed = False
         self.buf = self.table = None
 
     def commit(self):
-        lib = _lib.lib()
-        floats, tbytes = lib.ccb_wcache_plan_floats(self.h), lib.ccb_wcache_table_bytes(self.h)
+        floats, tbytes = _lib.call('ccb_wcache_plan_floats', self.h), _lib.call('ccb_wcache_table_bytes', self.h)
         self.buf = torch.empty(max(int(floats), 1), device=self.device, dtype=torch.float32)
         self.table = torch.empty(int(tbytes), device=self.device, dtype=torch.uint8)
-        _lib.check(lib.ccb_wcache_commit(self.h, self.buf.data_ptr(), floats, self.table.data_ptr(), tbytes,
-                                         torch.cuda.current_stream(self.device).cuda_stream), 'wcache_commit')
+        _lib.call('ccb_wcache_commit', self.h, self.buf, floats, self.table, tbytes, self.buf)
         self.committed = True
         self.refresh()
 
     def refresh(self):
         if self.committed:
-            _lib.check(_lib.lib().ccb_wcache_refresh(self.h, torch.cuda.current_stream(self.device).cuda_stream), 'wcache_refresh')
+            _lib.call('ccb_wcache_refresh', self.h, self.buf)
 
     def stats(self):
         out = (C.c_longlong * 4)()
-        _lib.lib().ccb_wcache_stats(self.h, C.byref(out))
+        _lib.call('ccb_wcache_stats', self.h, out)
         return dict(layouts=out[0], hits=out[1], misses=out[2], committed=bool(out[3]))
 
     def __del__(self):
         try:
-            _lib.lib().ccb_wcache_destroy(self.h)
+            _lib.call('ccb_wcache_destroy', self.h)
         except Exception:
             pass
 
@@ -84,17 +82,12 @@ def _desc(B, Ci, Hi, Wi, Co, Ho, Wo, k, stride, pad, act, slope):
     return d
 
 
-def _c(t):
-    return _lib.contig(t.detach())
+_CONV_OPS = ('ccb_conv2d_fprop', 'ccb_conv2d_dgrad', 'ccb_conv2d_wgrad')
 
 
 def _run(op, d, *args):
-    lib = _lib.lib()
-    dev = args[0].device
-    work, wf = _workspace(dev, lib.ccb_conv_workspace_floats(C.byref(d), op))
-    fn = (lib.ccb_conv2d_fprop, lib.ccb_conv2d_dgrad, lib.ccb_conv2d_wgrad)[op]
-    ptrs = [_lib.ptr(a) for a in args]
-    _lib.check(fn(C.byref(d), *ptrs, _lib.ptr(work), wf, _lib.stream(args[0])), 'conv op %d' % op)
+    work, wf = _workspace(args[0].device, _lib.call('ccb_conv_workspace_floats', d, op))
+    _lib.call(_CONV_OPS[op], d, *args, work, wf, args[0])
 
 
 def _grad_slot(param, like):
@@ -126,11 +119,9 @@ def _act_bwd_bias(g, y, act, slope, db):
     B, Cc = g.shape[0], g.shape[1]
     plane = g.numel() // (B * Cc)
     dz = torch.empty_like(g) if act != _lib.ACT_NONE else g
-    lib = _lib.lib()
-    wf = lib.ccb_act_bwd_bias_workspace_floats(B, Cc, plane) if db is not None else 0
+    wf = _lib.call('ccb_act_bwd_bias_workspace_floats', B, Cc, plane) if db is not None else 0
     work = torch.empty(wf, device=g.device, dtype=torch.float32) if wf else None
-    _lib.check(lib.ccb_act_bwd_bias(_lib.ptr(g), _lib.ptr(y), _lib.ptr(dz) if act != _lib.ACT_NONE else None, _lib.ptr(db),
-                                    B, Cc, plane, act, slope, _lib.ptr(work), wf, _lib.stream(g)), 'act_bwd_bias')
+    _lib.call('ccb_act_bwd_bias', g, y, dz if act != _lib.ACT_NONE else None, db, B, Cc, plane, act, slope, work, wf, g)
     return dz
 
 
@@ -140,9 +131,9 @@ class _Conv2dFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, bias, res, stride, pad, act, slope):
         w_in, b_in = w, bias
-        x, w = _c(x), _c(w)
-        bias = _c(bias) if bias is not None else None
-        res = _c(res) if res is not None else None
+        x, w = _lib.f32(x), _lib.f32(w)
+        bias = _lib.f32(bias) if bias is not None else None
+        res = _lib.f32(res) if res is not None else None
         B, Ci, Hi, Wi = x.shape
         Co, _, k, _ = w.shape
         Ho, Wo = (Hi + 2 * pad - k) // stride + 1, (Wi + 2 * pad - k) // stride + 1
@@ -162,7 +153,7 @@ class _Conv2dFn(torch.autograd.Function):
         Co, _, k, _ = w.shape
         want_w = ctx.needs_input_grad[1] or (has_bias and ctx.needs_input_grad[2])
         db, b_direct = _grad_slot(ctx.params[1], w.new_empty(Co)) if (has_bias and want_w) else (None, False)
-        dz = _act_bwd_bias(_c(g), y, act, slope, db)          # activation backward + bias gradient: one pass over g
+        dz = _act_bwd_bias(_lib.f32(g), y, act, slope, db)          # activation backward + bias gradient: one pass over g
         d = _desc(B, Ci, Hi, Wi, Co, dz.shape[2], dz.shape[3], k, stride, pad, _lib.ACT_NONE, 0.0)
         dx = dw = None
         if ctx.needs_input_grad[0]:
@@ -184,8 +175,8 @@ class _ConvT2dFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, bias, stride, pad, out_pad, act, slope):
         w_in, b_in = w, bias
-        x, w = _c(x), _c(w)
-        bias = _c(bias) if bias is not None else None
+        x, w = _lib.f32(x), _lib.f32(w)
+        bias = _lib.f32(bias) if bias is not None else None
         B, Cin, h, wd = x.shape
         _, Cout, k, _ = w.shape
         H = (h - 1) * stride - 2 * pad + k + out_pad
@@ -206,7 +197,7 @@ class _ConvT2dFn(torch.autograd.Function):
         _, Cout, k, _ = w.shape
         want_b = has_bias and ctx.needs_input_grad[2]
         db, b_direct = _grad_slot(ctx.params[1], w.new_empty(Cout)) if want_b else (None, False)
-        dz = _act_bwd_bias(_c(g), y, act, slope, db)
+        dz = _act_bwd_bias(_lib.f32(g), y, act, slope, db)
         if want_b:
             _grad_done(ctx.params[1] if b_direct else None)
             db = None if b_direct else db
@@ -227,14 +218,12 @@ class _BatchNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gamma, beta, rm, rv, training, eps, momentum):
         ctx.params = (gamma, beta)
-        x, gamma, beta = _c(x), _c(gamma), _c(beta)
+        x, gamma, beta = _lib.f32(x), _lib.f32(gamma), _lib.f32(beta)
         B, Cc, h, w = x.shape
         y = torch.empty_like(x)
         stats = torch.empty(Cc, 2, device=x.device) if training else None
-        work = torch.empty(_lib.lib().ccb_bn_workspace_floats(B, Cc, h * w), device=x.device) if training else None
-        _lib.check(_lib.lib().ccb_bn_fwd(_lib.ptr(x), _lib.ptr(gamma), _lib.ptr(beta), _lib.ptr(y), _lib.ptr(stats),
-                                         _lib.ptr(rm), _lib.ptr(rv), B, Cc, h * w, eps, momentum, int(training),
-                                         _lib.ptr(work), _lib.stream(x)), 'bn_fwd')
+        work = torch.empty(_lib.call('ccb_bn_workspace_floats', B, Cc, h * w), device=x.device) if training else None
+        _lib.call('ccb_bn_fwd', x, gamma, beta, y, stats, rm, rv, B, Cc, h * w, eps, momentum, int(training), work, x)
         ctx.save_for_backward(x, gamma, stats)
         ctx.training = training
         return y
@@ -245,13 +234,12 @@ class _BatchNormFn(torch.autograd.Function):
         if not ctx.training:
             raise NotImplementedError('cc_b200: BatchNorm backward is implemented for training mode only')
         B, Cc, h, w = x.shape
-        g = _c(g)
+        g = _lib.f32(g)
         dx = torch.empty_like(x)
         dg, g_direct = _grad_slot(ctx.params[0], gamma)
         db, b_direct = _grad_slot(ctx.params[1], gamma)
-        work = torch.empty(_lib.lib().ccb_bn_workspace_floats(B, Cc, h * w), device=x.device)
-        _lib.check(_lib.lib().ccb_bn_bwd(_lib.ptr(x), _lib.ptr(g), _lib.ptr(gamma), _lib.ptr(stats), _lib.ptr(dx),
-                                         _lib.ptr(dg), _lib.ptr(db), B, Cc, h * w, _lib.ptr(work), _lib.stream(x)), 'bn_bwd')
+        work = torch.empty(_lib.call('ccb_bn_workspace_floats', B, Cc, h * w), device=x.device)
+        _lib.call('ccb_bn_bwd', x, g, gamma, stats, dx, dg, db, B, Cc, h * w, work, x)
         _grad_done(ctx.params[0] if g_direct else None, ctx.params[1] if b_direct else None)
         return dx, (None if g_direct else dg), (None if b_direct else db), None, None, None, None, None
 
@@ -259,19 +247,19 @@ class _BatchNormFn(torch.autograd.Function):
 class _Upsample2xFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x):
-        x = _c(x)
+        x = _lib.f32(x)
         B, Cc, h, w = x.shape
         y = torch.empty(B, Cc, 2 * h, 2 * w, device=x.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ccb_upsample2x_fwd(_lib.ptr(x), _lib.ptr(y), B * Cc, h, w, _lib.stream(x)), 'upsample2x_fwd')
+        _lib.call('ccb_upsample2x_fwd', x, y, B * Cc, h, w, x)
         ctx.shape = (B, Cc, h, w)
         return y
 
     @staticmethod
     def backward(ctx, g):
         B, Cc, h, w = ctx.shape
-        g = _c(g)
+        g = _lib.f32(g)
         dx = torch.empty(B, Cc, h, w, device=g.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ccb_upsample2x_bwd(_lib.ptr(g), _lib.ptr(dx), B * Cc, h, w, _lib.stream(g)), 'upsample2x_bwd')
+        _lib.call('ccb_upsample2x_bwd', g, dx, B * Cc, h, w, g)
         return dx
 
 
@@ -378,13 +366,12 @@ def xavier_init_(module, bias_uniform=False):
 class _Corr81Fn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, f1, f2, reversed_):
-        f1, f2 = _c(f1), _c(f2)
+        f1, f2 = _lib.f32(f1), _lib.f32(f2)
         B, Cc, h, w = f1.shape
         out = torch.empty(B, 81, h, w, device=f1.device, dtype=torch.float32)
-        wf = _lib.lib().ccb_corr81_fwd_workspace_floats(B, Cc, h, w)
+        wf = _lib.call('ccb_corr81_fwd_workspace_floats', B, Cc, h, w)
         work = torch.empty(wf, device=f1.device, dtype=torch.float32) if wf else None
-        _lib.check(_lib.lib().ccb_corr81_fwd(_lib.ptr(f1), _lib.ptr(f2), _lib.ptr(out), B, Cc, h, w, int(reversed_),
-                                             _lib.ptr(work), wf, _lib.stream(f1)), 'corr81_fwd')
+        _lib.call('ccb_corr81_fwd', f1, f2, out, B, Cc, h, w, int(reversed_), work, wf, f1)
         ctx.save_for_backward(f1, f2)
         ctx.rev = int(reversed_)
         return out
@@ -393,27 +380,25 @@ class _Corr81Fn(torch.autograd.Function):
     def backward(ctx, g):
         f1, f2 = ctx.saved_tensors
         B, Cc, h, w = f1.shape
-        g = _c(g)
+        g = _lib.f32(g)
         d1 = torch.empty_like(f1) if ctx.needs_input_grad[0] else None
         d2 = torch.empty_like(f2) if ctx.needs_input_grad[1] else None
         if d1 is not None or d2 is not None:
             work = torch.empty(B * 81 * h * w, device=f1.device) if d2 is not None else None
-            _lib.check(_lib.lib().ccb_corr81_bwd(_lib.ptr(f1), _lib.ptr(f2), _lib.ptr(g), _lib.ptr(d1), _lib.ptr(d2), B, Cc,
-                                                 h, w, ctx.rev, _lib.ptr(work), _lib.stream(f1)), 'corr81_bwd')
+            _lib.call('ccb_corr81_bwd', f1, f2, g, d1, d2, B, Cc, h, w, ctx.rev, work, f1)
         return d1, d2, None
 
 
 class _Corr441dFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, f1, f2):
-        f1, f2 = _c(f1), _c(f2)
+        f1, f2 = _lib.f32(f1), _lib.f32(f2)
         if f1.shape != f2.shape or f1.dim() != 4:
             raise ValueError('cc_b200: corr441d needs two [B,C,h,w] maps of one shape, got %s and %s'
                              % (tuple(f1.shape), tuple(f2.shape)))
         B, Cc, h, w = f1.shape
         out = torch.empty(B, 441, h, w, device=f1.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ccb_corr441d_fwd(_lib.ptr(f1), _lib.ptr(f2), _lib.ptr(out), B, Cc, h, w, _lib.stream(f1)),
-                   'corr441d_fwd')
+        _lib.call('ccb_corr441d_fwd', f1, f2, out, B, Cc, h, w, f1)
         ctx.save_for_backward(f1, f2, out)
         return out
 
@@ -421,23 +406,21 @@ class _Corr441dFn(torch.autograd.Function):
     def backward(ctx, g):
         f1, f2, out = ctx.saved_tensors
         B, Cc, h, w = f1.shape
-        g = _c(g)
+        g = _lib.f32(g)
         d1 = torch.empty_like(f1) if ctx.needs_input_grad[0] else None
         d2 = torch.empty_like(f2) if ctx.needs_input_grad[1] else None
         if d1 is not None or d2 is not None:
-            _lib.check(_lib.lib().ccb_corr441d_bwd(_lib.ptr(f1), _lib.ptr(f2), _lib.ptr(out), _lib.ptr(g), _lib.ptr(d1),
-                                                   _lib.ptr(d2), B, Cc, h, w, _lib.stream(f1)), 'corr441d_bwd')
+            _lib.call('ccb_corr441d_bwd', f1, f2, out, g, d1, d2, B, Cc, h, w, f1)
         return d1, d2
 
 
 class _FeatWarpFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, flo):
-        x, flo = _c(x), _c(flo)
+        x, flo = _lib.f32(x), _lib.f32(flo)
         B, Cc, h, w = x.shape
         out = torch.empty_like(x)
-        _lib.check(_lib.lib().ccb_featwarp_fwd(_lib.ptr(x), _lib.ptr(flo), B, Cc, h, w, _lib.ptr(out), _lib.stream(x)),
-                   'featwarp_fwd')
+        _lib.call('ccb_featwarp_fwd', x, flo, B, Cc, h, w, out, x)
         ctx.save_for_backward(x, flo)
         return out
 
@@ -445,12 +428,11 @@ class _FeatWarpFn(torch.autograd.Function):
     def backward(ctx, g):
         x, flo = ctx.saved_tensors
         B, Cc, h, w = x.shape
-        g = _c(g)
+        g = _lib.f32(g)
         dx = torch.zeros_like(x) if ctx.needs_input_grad[0] else None
         df = torch.empty_like(flo) if ctx.needs_input_grad[1] else None
         work = _lib.scatter_workspace(x) if dx is not None else None
-        _lib.check(_lib.lib().ccb_featwarp_bwd(_lib.ptr(x), _lib.ptr(flo), B, Cc, h, w, _lib.ptr(g), _lib.ptr(df),
-                                               _lib.ptr(dx), _lib.ptr(work, 'work', torch.int64), _lib.stream(x)), 'featwarp_bwd')
+        _lib.call('ccb_featwarp_bwd', x, flo, B, Cc, h, w, g, df, dx, work, x)
         return dx, df
 
 

@@ -4,7 +4,7 @@ The reference builds a single torch.optim.Adam over chain(all nets' parameters)
 (train.py:307-310: lr, betas=(momentum, beta), weight_decay 0) and, under nn.DataParallel,
 broadcasts 297 MB of parameters and reduces 297 MB of gradients through GPU0 every step.  Here all
 trainable parameters are views into one flat buffer, all gradients views into another; a step is one
-`ccb_adam_step` launch, and data-parallel training all-reduces contiguous slices of the flat gradient
+`ccb_adam_step_ranges` call, and data-parallel training all-reduces contiguous slices of the flat gradient
 buffer (cc_b200/dist.py).
 
 The order of the parameters inside the flat buffers is an internal detail (`relayout()` re-packs them in
@@ -14,9 +14,9 @@ torch.optim.Adam's own per-parameter `state_dict()` format, indexed by the order
 
 Step groups (`groups=`, one per network) give each network its own step counter, as torch.optim.Adam's per-parameter
 counts do when a network is fixed for a phase of training (train.py --fix-*: requires_grad = False, so Adam skips it).
-`freeze()` names the groups the step skips: their parameters, moments and counters are not touched.  The step is then
-one `ccb_adam_step_ranges` launch over the maximal runs of active groups in the current flat layout; the device range
-table is rebuilt when the layout or the frozen set changes, never per step."""
+`freeze()` names the groups the step skips: their parameters, moments and counters are not touched.  The step runs over
+the maximal runs of active groups in the current flat layout; the device range table is rebuilt when the layout or the
+frozen set changes, never per step."""
 import torch
 from . import _lib
 
@@ -145,18 +145,9 @@ class FlatAdam:
             if g is not None and g.data_ptr() != p._ccb_grad.data_ptr():
                 p._ccb_grad.add_(g)
                 p.grad = p._ccb_grad
-        lib = _lib.lib()
-        if len(self.groups) == 1 and not self.frozen:
-            _lib.check(lib.ccb_adam_step(_lib.ptr(self.flat_p), _lib.ptr(self.flat_g), _lib.ptr(self.exp_avg),
-                                         _lib.ptr(self.exp_avg_sq), self.numel, _lib.ptr(self.state), self.lr,
-                                         self.betas[0], self.betas[1], self.eps, self.grad_scale,
-                                         _lib.stream(self.flat_p)), 'adam_step')
-            return
-        _lib.check(lib.ccb_adam_step_ranges(_lib.ptr(self.flat_p), _lib.ptr(self.flat_g), _lib.ptr(self.exp_avg),
-                                            _lib.ptr(self.exp_avg_sq), _lib.ptr(self._range_table, 'ranges', torch.int64),
-                                            self._nranges, self._nblocks, _lib.ptr(self._active, 'group_active', torch.int32),
-                                            len(self.groups), _lib.ptr(self.state), self.lr, self.betas[0], self.betas[1],
-                                            self.eps, self.grad_scale, _lib.stream(self.flat_p)), 'adam_step_ranges')
+        _lib.call('ccb_adam_step_ranges', self.flat_p, self.flat_g, self.exp_avg, self.exp_avg_sq, self._range_table,
+                  self._nranges, self._nblocks, self._active, len(self.groups), self.state, self.lr, self.betas[0],
+                  self.betas[1], self.eps, self.grad_scale, self.flat_p)
 
     def group_steps(self):
         """Step count of every group (host copy)."""

@@ -8,7 +8,6 @@ State: the C library keeps none; this Python-side memo holds at most 12 (frame t
 identity + version, and `Trainer.step` clears it on entry and exit, so no reference outlives a step.  Plain callers
 of the loss functions may call `clear()` themselves (stale entries are only ever evicted, never wrong: a changed
 tensor has a new version)."""
-import ctypes as C
 import torch
 from . import _lib
 
@@ -22,7 +21,7 @@ def level_sizes(H, W, nlevels):
 
 def build(img, nlevels):
     """img [B,C,H,W] -> [img, level1, ...]; level l is the exact 2^l box mean."""
-    img = _lib.contig(img.detach())
+    img = _lib.f32(img)
     B, Cc, H, W = img.shape
     if nlevels == 1:
         return [img]
@@ -31,9 +30,7 @@ def build(img, nlevels):
         raise NotImplementedError('cc_b200: frame size %dx%d is not divisible by %d (pyramid levels must '
                                   'be exact halvings)' % (H, W, div))
     outs = [torch.empty(B, Cc, H >> l, W >> l, device=img.device, dtype=torch.float32) for l in range(1, nlevels)]
-    arr = (C.c_void_p * (nlevels - 1))(*[_lib.ptr(o) for o in outs])
-    _lib.check(_lib.lib().ccb_image_pyramid(_lib.ptr(img, 'img'), B * Cc, H, W, nlevels, arr, _lib.stream(img)),
-               'image_pyramid')
+    _lib.call('ccb_image_pyramid', img, B * Cc, H, W, nlevels, outs, img)
     return [img] + outs
 
 

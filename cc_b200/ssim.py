@@ -1,6 +1,5 @@
 """Drop-in for the reference's ``ssim`` module (ssim.py): 13x13 Gaussian SSIM map, zero padded,
 depthwise - computed by the separable shared-memory kernels in csrc/warp_ops.cu + ssim_tile.cuh."""
-import ctypes as C
 from math import exp
 import torch
 from . import _lib
@@ -29,18 +28,13 @@ def taps13():
     return _TAPS
 
 
-def _taps_c():
-    return (C.c_float * 13)(*taps13())
-
-
 class _Ssim(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img1, img2):
-        a, b = _lib.contig(img1.detach().float()), _lib.contig(img2.detach().float())
+        a, b = _lib.f32(img1), _lib.f32(img2)
         Bn, Cc, h, w = a.shape
         out = torch.empty_like(a)
-        _lib.check(_lib.lib().ccb_ssim_fwd(_lib.ptr(a), _lib.ptr(b), Bn * Cc, h, w, _taps_c(), _lib.ptr(out),
-                                           _lib.stream(a)), 'ssim_fwd')
+        _lib.call('ccb_ssim_fwd', a, b, Bn * Cc, h, w, taps13(), out, a)
         ctx.save_for_backward(a, b)
         return out
 
@@ -48,12 +42,11 @@ class _Ssim(torch.autograd.Function):
     def backward(ctx, g):
         a, b = ctx.saved_tensors
         Bn, Cc, h, w = a.shape
-        g = _lib.contig(g.detach().float())
+        g = _lib.f32(g)
         d1 = torch.empty_like(a) if ctx.needs_input_grad[0] else None
         d2 = torch.empty_like(b) if ctx.needs_input_grad[1] else None
         work = torch.empty(5 * a.numel(), device=a.device)
-        _lib.check(_lib.lib().ccb_ssim_bwd(_lib.ptr(a), _lib.ptr(b), Bn * Cc, h, w, _taps_c(), _lib.ptr(g), _lib.ptr(d1),
-                                           _lib.ptr(d2), _lib.ptr(work), _lib.stream(a)), 'ssim_bwd')
+        _lib.call('ccb_ssim_bwd', a, b, Bn * Cc, h, w, taps13(), g, d1, d2, work, a)
         return d1, d2
 
 

@@ -290,21 +290,17 @@ int ccb_bn_bwd(const float* x, const float* dy, const float* gamma, const float*
 /* bilinear x2 upsample, align_corners=False (DispResNet6.py:174; back2future.py:60): [planes,h,w] -> [planes,2h,2w] */
 int ccb_upsample2x_fwd(const float* x, float* y, int planes, int h, int w, ccb_stream_t stream);
 int ccb_upsample2x_bwd(const float* dy, float* dx, int planes, int h, int w, ccb_stream_t stream);
-/* torch.optim.Adam step (train.py:307-310,568) on one flat fp32 buffer; grad_scale pre-multiplies the
- * gradient (1/world_size after the NCCL all-reduce sum).  state: 3 device floats {step count, 1-b1^t,
- * sqrt(1-b2^t)}, zero-initialised by the caller; the call increments the step on the device, so a
- * captured CUDA graph of the training step replays correctly. */
-int ccb_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
-                  float* state, float lr, float beta1, float beta2, float eps, float grad_scale,
-                  ccb_stream_t stream);
-/* The same Adam over listed ranges of the flat buffers, each range belonging to one parameter group with its own
- * step counter (torch.optim.Adam keeps one per parameter; a network that is fixed for a phase of training, train.py
- * --fix-*, keeps its count).  ranges: device table of nranges entries {offset, count, group, first_block}, where
- * first_block is the number of 256-element blocks of the entries before it; nblocks is that number over all entries.
- * Elements outside the listed ranges are neither read nor written.  group_state: 4*ngroups device floats, group g at
- * [4g, 4g+4) laid out as ccb_adam_step's state; group_active: ngroups device ints, the prep step advances the counter
- * and bias corrections of the groups that are non-zero there (NULL: all).  ccb_adam_step is the call with one range
- * {0, n, 0, 0} and one active group. */
+/* torch.optim.Adam step (train.py:307-310,568) over listed ranges of flat fp32 buffers (params, grads, exp_avg,
+ * exp_avg_sq), each range belonging to one parameter group with its own step counter (torch.optim.Adam keeps one per
+ * parameter; a network that is fixed for a phase of training, train.py --fix-*, keeps its count).  grad_scale
+ * pre-multiplies the gradient (1/world_size after the NCCL all-reduce sum).  ranges: device table of nranges entries
+ * {offset, count, group, first_block}, where first_block is the number of 256-element blocks of the entries before it;
+ * nblocks is that number over all entries.  Elements outside the listed ranges are neither read nor written.
+ * group_state: 4*ngroups device floats, group g at [4g, 4g+4) = {step count, 1-b1^t, sqrt(1-b2^t), unused},
+ * zero-initialised by the caller; group_active: ngroups device ints, the prep step advances the counter and bias
+ * corrections of the groups that are non-zero there (NULL: all).  The counters are incremented on the device, so a
+ * captured CUDA graph of the training step replays correctly.  One flat buffer of n elements trained as one group is
+ * the table {0, n, 0, 0}. */
 int ccb_adam_step_ranges(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const long long* ranges,
                          int nranges, long long nblocks, const int* group_active, int ngroups, float* group_state,
                          float lr, float beta1, float beta2, float eps, float grad_scale, ccb_stream_t stream);

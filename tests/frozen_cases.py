@@ -47,14 +47,9 @@ def _step_ranges(opt, table):
     for off, k, gi in table:
         rows += [off, k, gi, nb]
         nb += (k + ADAM_BLOCK - 1) // ADAM_BLOCK
-    dev = opt.flat_p.device
-    t = torch.tensor(rows, dtype=torch.int64).to(dev)
-    act = opt._active
-    _lib.check(_lib.lib().ccb_adam_step_ranges(_lib.ptr(opt.flat_p), _lib.ptr(opt.flat_g), _lib.ptr(opt.exp_avg),
-                                               _lib.ptr(opt.exp_avg_sq), _lib.ptr(t, 'ranges', torch.int64), len(table), nb,
-                                               _lib.ptr(act, 'active', torch.int32), len(opt.groups), _lib.ptr(opt.state),
-                                               opt.lr, opt.betas[0], opt.betas[1], opt.eps, opt.grad_scale,
-                                               _lib.stream(opt.flat_p)), 'adam_step_ranges')
+    t = torch.tensor(rows, dtype=torch.int64).to(opt.flat_p.device)
+    _lib.call('ccb_adam_step_ranges', opt.flat_p, opt.flat_g, opt.exp_avg, opt.exp_avg_sq, t, len(table), nb, opt._active,
+              len(opt.groups), opt.state, opt.lr, opt.betas[0], opt.betas[1], opt.eps, opt.grad_scale, opt.flat_p)
 
 
 def case_adam_ranges_fp64(device, steps=4):
@@ -95,22 +90,6 @@ def case_adam_ranges_fp64(device, steps=4):
             assert_adam_step(tuple(x[m] for x in before[:3]), tuple(x[m] for x in after[:3]) + (after[3][4 * gi:4 * gi + 4],),
                              g[m], t0 + s, opt.lr, opt.betas, opt.eps, 1.0, f'group {gi} step {t0 + s}')
     assert opt.group_steps() == [3 + steps, 0, 7 + steps]
-
-
-def case_adam_one_range_is_adam_step(device):
-    """ccb_adam_step and ccb_adam_step_ranges with one range and one group compute the same bits."""
-    opt, mag, gen = _adam_setup(device)
-    one = FlatAdam([torch.nn.Parameter(p.detach().clone()) for p in opt.params], lr=1e-3)
-    mirror = FlatAdam([torch.nn.Parameter(p.detach().clone()) for p in opt.params], lr=1e-3)
-    for s in range(3):
-        g = (mag * torch.where(torch.rand(opt.numel, generator=gen) < 0.5, -1.0, 1.0)).to(device)
-        one.flat_g.copy_(g)
-        one.step()                                                  # ccb_adam_step
-        ref = (one.flat_p.clone(), one.exp_avg.clone(), one.exp_avg_sq.clone(), one.state.clone())
-        mirror.flat_g.copy_(g)
-        _step_ranges(mirror, [(0, mirror.numel, 0)])
-        for a, b, nm in zip(ref, (mirror.flat_p, mirror.exp_avg, mirror.exp_avg_sq, mirror.state), ('p', 'm', 'v', 'state')):
-            assert torch.equal(a, b), f'step {s}: {nm}: one range differs from ccb_adam_step'
 
 
 # ---- FlatAdam against torch.optim.Adam over training phases -----------------------------------------------------------

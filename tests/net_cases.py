@@ -282,7 +282,8 @@ def case_conv_plan_from_shape(device):
             d.stride, d.pad, d.act, d.slope, d.impl, d.wcache = s, p, _lib.ACT_NONE, 0.0, impl, None
             for op, ins, out in ((_lib.CONV_FPROP, (x, w, None, None), dy), (_lib.CONV_DGRAD, (dy, w, None, None), x),
                                  (_lib.CONV_WGRAD, (x, dy), w)):
-                fn = (lib.ccb_conv2d_fprop, lib.ccb_conv2d_dgrad, lib.ccb_conv2d_wgrad)[op]
+                name = ('ccb_conv2d_fprop', 'ccb_conv2d_dgrad', 'ccb_conv2d_wgrad')[op]
+                fn = getattr(lib, name)
                 need = lib.ccb_conv_workspace_floats(C.byref(d), op)
                 tag = f'impl {impl} op {op} {Ci}->{Co} {H}x{W}'
                 assert need >= 0, tag
@@ -290,8 +291,7 @@ def case_conv_plan_from_shape(device):
                 for wf in (need, 8 * need + 4096):
                     work = torch.full((max(wf, 1),), float('nan'), device=device)
                     y = torch.empty_like(out)
-                    args = [_lib.ptr(t) for t in ins] + [y.data_ptr()]
-                    _lib.check(fn(C.byref(d), *args, work.data_ptr() if wf else None, wf, _lib.stream(x)), 'conv op %d' % op)
+                    _lib.call(name, d, *ins, y, work if wf else None, wf, x)
                     got = lib.ccb_debug_last_conv_kernel().decode()
                     assert got == kernels[op], f'{tag}: the call ran {kernels[op]}, labelled {got!r}'
                     res.append(y)

@@ -71,8 +71,8 @@ def assert_adam_step(before, after, g, t, lr, betas, eps, grad_scale, what):
 
 
 def case_adam_fp64(device, steps=5):
-    """FlatAdam (ccb_adam_step) over three parameters for 5 steps against the fp64 reference, element by element, on
-    synthetic gradients: exact zeros (every step, or every other step), values near eps (1e-9 .. 1e-7), large values
+    """FlatAdam (ccb_adam_step_ranges, one group) over three parameters for 5 steps against the fp64 reference, element by
+    element, on synthetic gradients: exact zeros (every step, or every other step), values near eps (1e-9 .. 1e-7), large values
     (1e4), ordinary ones, with random signs that change from step to step, and one step with grad_scale = 0.5.
     Parameters span 1 .. 1e-4 with exact zeros, so the updates are not hidden under the parameters' ulp.  Each step
     starts from the optimiser's own previous buffers; the bounds are adam_reference's."""

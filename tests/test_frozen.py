@@ -14,8 +14,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.usefixtures('sim_lib')
 
 
-@pytest.mark.parametrize('case', [FC.case_adam_ranges_fp64, FC.case_adam_one_range_is_adam_step, FC.case_flat_adam_phases,
-                                  FC.case_load_missing_group_state, FC.case_photo_value_only], ids=lambda f: f.__name__)
+@pytest.mark.parametrize('case', [FC.case_adam_ranges_fp64, FC.case_flat_adam_phases, FC.case_load_missing_group_state,
+                                  FC.case_photo_value_only], ids=lambda f: f.__name__)
 def test_frozen_case(case):
     case(torch.device('cpu'))
 

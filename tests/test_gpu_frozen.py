@@ -36,4 +36,3 @@ def test_photo_value_only_full_size():
 
 def test_adam_ranges_on_device():
     FC.case_adam_ranges_fp64(DEV)
-    FC.case_adam_one_range_is_adam_step(DEV)
