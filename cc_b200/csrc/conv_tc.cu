@@ -8,7 +8,8 @@
 //   consecutive input channels of one filter tap, so the 4 loads of a chunk share the tap's bounds
 //   check and are coalesced across the 128 pixels of the tile;
 // * operands are staged in shared memory K-major with the 128-byte swizzle ([row][128 B], 16 B chunk ^= row & 7,
-//   8-row atoms 1 KB apart): the layout wgmma reads for tf32, which it accepts only K-major;
+//   8-row atoms 1 KB apart): the layout wgmma reads for tf32, which it accepts only K-major.  In fprop / dgrad the
+//   weight tiles arrive by TMA, which writes that swizzle itself: no producer thread waits for them;
 // * fp32 parity: every fp32 operand is split hi = tf32(x), lo = x - hi and each k-step issues three
 //   tf32 MMAs (hi*hi + lo*hi + hi*lo) ("3xTF32", error ~2^-21).  The tensor core only sums one 32-deep stage (small
 //   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
@@ -23,6 +24,9 @@
 
 #ifndef CCB_CPU_SIM
 
+#include <cuda.h>            // CUtensorMap (the driver entry point is looked up at run time: no libcuda link)
+#include <cudaTypedefs.h>    // PFN_cuTensorMapEncodeTiled
+
 namespace ccb {
 
 constexpr int TC_M = 128;          // pixels per tile (two wgmma M = 64 halves)
@@ -35,8 +39,11 @@ constexpr int TC_THREADS = TC_PRODUCERS + 32 * TC_CONSUMER_WARPS;
 constexpr int TC_MAX_TAPS = 49;
 
 struct TcArgs {
+    // prepared weights wp: tf32 hi copy [N][Kp] followed by the lo copy [N][Kp] (k = tap*cpad + c), as a 3-D TMA map
+    // {Kp, N, 2} whose {32, NT, 1} box is one stage's B operand copy in the 128-byte-swizzled K-major layout; rows >= N
+    // read as zeros
+    CUtensorMap wmap;
     const float* x;        // input activations [B, Cin, Hin, Win]
-    const float* wp;       // prepared weights: tf32 hi copy [N][Kp] followed by the lo copy [N][Kp] (k = tap*cpad + c)
     const float* bias;
     const float* res;
     float* out;            // [B, N_total, Hout, Wout]
@@ -88,10 +95,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+// one arrival on `bar` that also makes its current phase wait for `bytes` more of asynchronous (TMA) transfer
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// TMA: the box of `map` at coordinates (c0, c1, c2) into shared memory at `dst`, counted in as transfer bytes on `bar`
+__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+__device__ __forceinline__ void tma_prefetch_map(const CUtensorMap* map) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
 __device__ __forceinline__ float tf32_hi(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -218,8 +235,9 @@ struct TcRing {
 };
 
 // Set-up at the top of both kernels: it touches no global data, so it overlaps the predecessor's tail (PDL), and
-// returns once the predecessor's results are visible.
-__device__ __forceinline__ TcRing tc_ring(int depth, int b_tile_bytes) {
+// returns once the predecessor's results are visible.  A full[s] phase completes after `full_arrivals` arrivals (and
+// the transfer bytes any of them announced).
+__device__ __forceinline__ TcRing tc_ring(int depth, int b_tile_bytes, int full_arrivals) {
     CCB_PDL_TRIGGER();
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -227,7 +245,7 @@ __device__ __forceinline__ TcRing tc_ring(int depth, int b_tile_bytes) {
     uint64_t* full = (uint64_t*)(smem + depth * stage_bytes);
     const TcRing r = {smem, depth, stage_bytes, b_tile_bytes, full, full + TC_MAX_STAGES};
     if (threadIdx.x == 0) {
-        for (int s = 0; s < depth; ++s) { mbar_init(&r.full[s], TC_PRODUCERS); mbar_init(&r.empty[s], TC_CONSUMER_WARPS); }
+        for (int s = 0; s < depth; ++s) { mbar_init(&r.full[s], full_arrivals); mbar_init(&r.empty[s], TC_CONSUMER_WARPS); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -279,8 +297,9 @@ __device__ __forceinline__ void tc_consume(const TcRing& ring, int nkt, int wg, 
 }
 
 template <int NT>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) {
-    const TcRing ring = tc_ring(a.depth, a.b_tile_bytes);
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
+    // full[s]: the 128 producers' A stores + producer 0's arrival that announces the B tiles' TMA bytes
+    const TcRing ring = tc_ring(a.depth, a.b_tile_bytes, TC_PRODUCERS + 1);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
     const int ntile = min(TC_NMAX, a.Ntot - n0);
@@ -305,6 +324,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
         const int iy0 = oy * a.in_stride, ix0 = ox * a.in_stride;
         const int cpt = a.cpad >> 2;                 // chunks per tap
         const int nchunks = a.ntaps * cpt;           // real chunks; the rest of Kp is zero padding
+        if (r == 0) tma_prefetch_map(&a.wmap);
         for (int it = 0; it < nkt; ++it) {
             const int s = it % ring.depth;
             const int kt = kt_beg + it;                   // global k-tile
@@ -348,26 +368,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcArgs a) 
                 }
             }
             const TcTiles<unsigned char*> t = ring.acquire(it, s);
-            // ---- B: the weights were split into tf32 hi / lo by the prep kernel: plain 16-byte async copies
-            //      (pairs of threads cover one 32-byte sector of a weight row)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int idx = r + j * 128;                      // 0 .. 1023
-                const int c = ((idx >> 8) << 1) | (idx & 1);
-                const int n = (idx >> 1) & 127;
-                if (n < NT) {
-                    // rows in [ntile, NT) are clamped to row 0: the epilogue ignores those columns
-                    const int nn = (n < ntile) ? n : 0;
-                    const float* src = a.wp + (long long)(n0 + nn) * a.Kp + kt * (TC_KC * 4) + c * 4;
-                    cp_async16((float4*)t.b_hi + tile_idx(n, c), src);
-                    cp_async16((float4*)t.b_lo + tile_idx(n, c), src + (long long)a.Ntot * a.Kp);
-                }
+            // ---- B: the weights were split into tf32 hi / lo by the prep kernel: one TMA box per copy; rows in
+            //      [ntile, NT) past the last channel are zero-filled, and the epilogue ignores those columns
+            if (r == 0) {
+                mbar_arrive_expect_tx(&ring.full[s], 2 * ring.b_tile_bytes);
+                tma_load_3d(t.b_hi, &a.wmap, &ring.full[s], kt * (TC_KC * 4), n0, 0);
+                tma_load_3d(t.b_lo, &a.wmap, &ring.full[s], kt * (TC_KC * 4), n0, 1);
             }
             // ---- A: split + store
 #pragma unroll
             for (int c = 0; c < TC_KC; ++c)
                 tc_split_store(t.a_hi, t.a_lo, tile_idx(r, c), make_float4(av[c][0], av[c][1], av[c][2], av[c][3]));
-            cp_async_wait_all();
             ring.publish(s);
         }
     } else {
@@ -439,6 +450,30 @@ static int tc_launch_kernel(void (*const (&kfns)[4])(const Args), const Args& a,
 static void (*const TC_FPROP_KERNELS[4])(const TcArgs) = {conv_tc_kernel<16>, conv_tc_kernel<32>, conv_tc_kernel<64>,
                                                           conv_tc_kernel<128>};
 
+// The TMA map of a prepared weight panel wp [2][N][Kp] (see TcArgs::wmap) with boxes of `nt` rows.  The encode is a host
+// call: under graph capture its result is baked into the launch, which holds because the panel (weight cache or
+// workspace) stays at the same address in replay.
+static int tc_weight_map(CUtensorMap* map, const float* wp, int N, int Kp, int nt) {
+    static PFN_cuTensorMapEncodeTiled_v12000 encode = [] {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            fn = nullptr;
+        return (PFN_cuTensorMapEncodeTiled_v12000)fn;
+    }();
+    CCB_REQUIRE(encode, CCB_ERR_LAUNCH, "conv_tc: the driver has no cuTensorMapEncodeTiled");
+    const cuuint64_t dims[3] = {(cuuint64_t)Kp, (cuuint64_t)N, 2};
+    const cuuint64_t strides[2] = {(cuuint64_t)Kp * sizeof(float), (cuuint64_t)N * Kp * sizeof(float)};
+    const cuuint32_t box[3] = {TC_KC * 4, (cuuint32_t)nt, 1};
+    const cuuint32_t estrides[3] = {1, 1, 1};
+    const CUresult rc = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)wp, dims, strides, box, estrides,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CCB_REQUIRE(rc == CUDA_SUCCESS, CCB_ERR_LAUNCH, "conv_tc: cuTensorMapEncodeTiled failed (%d) for N %d Kp %d", (int)rc, N, Kp);
+    return CCB_OK;
+}
+
 // One generalised-fprop launch (+ its weight preparation into `wp`, tf32 hi copy + lo copy).
 static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK, int Ci, const signed char* tap_index,
                      float* wp, float* partial, int splits, cudaStream_t st) {
@@ -452,7 +487,6 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     const float* wpp = nullptr;
     int rc = wprep_get(p, st, &wpp);
     if (rc) return rc;
-    a.wp = wpp;
     a.Ntot = N;
     a.splits = splits;
     a.ktiles = a.Kp / (TC_KC * 4);
@@ -460,6 +494,8 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     a.partial = partial;
     int nt, smem;
     tc_geometry(N, nt, a.b_tile_bytes, a.depth, smem);
+    rc = tc_weight_map(&a.wmap, wpp, N, a.Kp, nt);
+    if (rc) return rc;
     dim3 grid(cdiv(a.M, TC_M), cdiv(N, TC_NMAX), splits);
     return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, grid, smem, st, "conv_tc");
 }
@@ -483,7 +519,7 @@ struct TcWgradArgs {
 
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWgradArgs a) {
-    const TcRing ring = tc_ring(a.depth, a.b_tile_bytes);
+    const TcRing ring = tc_ring(a.depth, a.b_tile_bytes, TC_PRODUCERS);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
     const int ntile = min(TC_NMAX, a.Co - n0);
