@@ -158,6 +158,13 @@ _SIGS = {
     'ccb_mask_iou_workspace_bytes': ('long long', 'int, int, int, int, int'),
     'ccb_mask_iou': (STATUS, 'const float*, const float*, const float*, const float*, const float*, int, int, int, '
                              'int, int, int, float, int, float*, void*, long long, long long*, ccb_stream_t'),
+    'ccb_flow_submit': (STATUS, 'const float*, const float*, const float*, int, int, int, int, int, int, float, float*, '
+                                'float*, unsigned short*, float*, ccb_stream_t'),
+    'ccb_flow_color_workspace_bytes': ('long long', 'int, int, int, int'),
+    'ccb_flow_color': (STATUS, 'const float*, int, int, int, int, void*, long long, unsigned char*, ccb_stream_t'),
+    'ccb_kitti_flow_errors_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_kitti_flow_errors': (STATUS, 'const unsigned short*, const unsigned short*, int, int, int, void*, long long, '
+                                      'double*, long long*, ccb_stream_t'),
     'ccb_prep_frames': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, int, '
                                 'int, int, ccb_stream_t'),
     'ccb_prep_frames_unit': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '
@@ -176,7 +183,7 @@ _SIGS = {
 
 _SCALARS = {'int': C.c_int, 'long long': C.c_longlong, 'float': C.c_float}
 _DTYPES = {'float': torch.float32, 'double': torch.float64, 'int': torch.int32, 'long long': torch.int64,
-           'unsigned long long': torch.int64, 'unsigned char': torch.uint8, 'void': None}
+           'unsigned long long': torch.int64, 'unsigned char': torch.uint8, 'unsigned short': torch.uint16, 'void': None}
 _RESTYPES = {STATUS: C.c_int, 'int': C.c_int, 'long long': C.c_longlong, 'void*': C.c_void_p, 'const char*': C.c_char_p,
              'void': None}
 

@@ -24,6 +24,7 @@ static inline double __dadd_rn(double a, double b) { volatile double r = a + b; 
 static inline double __dsub_rn(double a, double b) { volatile double r = a - b; return r; }
 static inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
 static inline double __ddiv_rn(double a, double b) { volatile double r = a / b; return r; }
+static inline double __dsqrt_rn(double a) { volatile double r = sqrt(a); return r; }
 #endif
 
 namespace ccb {
@@ -676,6 +677,251 @@ __global__ void __launch_bounds__(256) mask_iou_count_kernel(const MaskIouArgs a
     }
 }
 
+// ================================================================================================
+// KITTI-2015 flow submission (submit_flow.py:119-156).  Per sample, at the nets' resolution h x w:
+//   bare     = 1 - (1 - e1)(1 - e2) > 0.5,   census = |cam_u - fwd_u| < T and |cam_v - fwd_v| < T
+//   combined = 1 - (1 - bare)(1 - census)                       (0 or 1; its bilinear resize to h x w is the identity)
+//   total    = (combined <= T) * fwd + (combined > T) * cam
+// then total, fwd and cam each resized bilinearly to Hg x Wg and u, v scaled by (float)(Wg / w), (float)(Hg / h).
+// The resize restates torch's CPU upsample_bilinear2d(align_corners=False) for float NCHW operation by operation: source
+// index fma(in/out, dst + 0.5, -0.5) clamped at 0, lambda1 = src - floor(src), lambda0 = 1 - lambda1, and per axis
+// fma(v0, lambda0, v1 * lambda1), the x axis inside the y axis.  Each output pixel composites its four taps.
+struct FlowSubmitArgs {
+    const float* emask;             // [B, C, h, w]
+    const float* cam;               // [B, 2, h, w]
+    const float* fwd;               // [B, 2, h, w]
+    float* mask;                    // [B, 1, h, w]
+    float* full;                    // [B, 3, 2, Hg, Wg] cam, fwd, total, or null
+    unsigned short* png;            // [B, Hg, Wg, 3]
+    float* flo;                     // [B, Hg, Wg, 2]
+    int B, C, h, w, Hg, Wg;
+    float thresh, fu, fv;
+};
+
+struct Tap { int i0, i1; float l0, l1; };
+__device__ __forceinline__ Tap aten_tap(int dst, int in_size, float scale) {
+    float s = __fmaf_rn(scale, __fadd_rn((float)dst, 0.5f), -0.5f);
+    if (s < 0.f) s = 0.f;
+    Tap t;
+    t.i0 = min((int)floorf(s), in_size - 1);
+    t.i1 = t.i0 + ((t.i0 < in_size - 1) ? 1 : 0);
+    t.l1 = fminf(fmaxf(__fsub_rn(s, (float)t.i0), 0.f), 1.f);
+    t.l0 = __fsub_rn(1.f, t.l1);
+    return t;
+}
+__device__ __forceinline__ float aten_lerp(float v0, float v1, float l0, float l1) {
+    return __fmaf_rn(v0, l0, __fmul_rn(v1, l1));
+}
+
+__device__ __forceinline__ float submit_combined(const FlowSubmitArgs& a, int b, long long p) {
+    const long long hw = (long long)a.h * a.w;
+    const float e1 = __ldg(a.emask + ((long long)b * a.C + 1) * hw + p), e2 = __ldg(a.emask + ((long long)b * a.C + 2) * hw + p);
+    const bool bare = __fsub_rn(1.f, __fmul_rn(__fsub_rn(1.f, e1), __fsub_rn(1.f, e2))) > 0.5f;
+    const float* c = a.cam + 2ll * b * hw + p;
+    const float* f = a.fwd + 2ll * b * hw + p;
+    const bool census = (fabsf(__fsub_rn(__ldg(c), __ldg(f))) < a.thresh) && (fabsf(__fsub_rn(__ldg(c + hw), __ldg(f + hw))) < a.thresh);
+    return (bare || census) ? 1.f : 0.f;
+}
+
+__global__ void __launch_bounds__(256) flow_submit_mask_kernel(const FlowSubmitArgs a) {
+    CCB_PDL_WAIT();
+    const long long hw = (long long)a.h * a.w, n = (long long)a.B * hw;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256)
+        a.mask[i] = submit_combined(a, (int)(i / hw), i % hw);
+}
+
+// numpy's float64 -> uint16 cast on x86-64: truncation to int32 (cvttsd2si; NaN and values outside the int32 range give
+// INT_MIN), then the low 16 bits.
+__device__ __forceinline__ unsigned short kitti_u16(float v) {
+    const double x = __dadd_rn(__dmul_rn((double)v, 64.0), 32768.0);
+    const int t = (x > -2147483649.0 && x < 2147483648.0) ? (int)x : (int)0x80000000u;
+    return (unsigned short)((unsigned)t & 0xffffu);
+}
+
+__global__ void __launch_bounds__(256) flow_submit_kernel(const FlowSubmitArgs a) {
+    CCB_PDL_WAIT();
+    const long long hw = (long long)a.h * a.w, ng = (long long)a.Hg * a.Wg, n = (long long)a.B * ng;
+    const float sy = (float)a.h / (float)a.Hg, sx = (float)a.w / (float)a.Wg;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const int b = (int)(i / ng);
+        const long long q = i - (long long)b * ng;
+        const int y = (int)(q / a.Wg), x = (int)(q - (long long)y * a.Wg);
+        const Tap ty = aten_tap(y, a.h, sy), tx = aten_tap(x, a.w, sx);
+        const long long taps[4] = {(long long)ty.i0 * a.w + tx.i0, (long long)ty.i0 * a.w + tx.i1,
+                                   (long long)ty.i1 * a.w + tx.i0, (long long)ty.i1 * a.w + tx.i1};
+        float v[3][2][4];       // [cam, fwd, total][u, v][tap]
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float m = submit_combined(a, b, taps[k]);
+            const float sr = (m > a.thresh) ? 1.f : 0.f, sn = (m <= a.thresh) ? 1.f : 0.f;
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const float cam = __ldg(a.cam + (2ll * b + c) * hw + taps[k]), fwd = __ldg(a.fwd + (2ll * b + c) * hw + taps[k]);
+                v[0][c][k] = cam;
+                v[1][c][k] = fwd;
+                v[2][c][k] = __fadd_rn(__fmul_rn(sn, fwd), __fmul_rn(sr, cam));
+            }
+        }
+        float o[3][2];
+#pragma unroll
+        for (int f = 0; f < 3; ++f)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const float r0 = aten_lerp(v[f][c][0], v[f][c][1], tx.l0, tx.l1);
+                const float r1 = aten_lerp(v[f][c][2], v[f][c][3], tx.l0, tx.l1);
+                o[f][c] = __fmul_rn(aten_lerp(r0, r1, ty.l0, ty.l1), c == 0 ? a.fu : a.fv);
+            }
+        if (a.full)
+#pragma unroll
+            for (int f = 0; f < 3; ++f) {
+                a.full[((3ll * b + f) * 2 + 0) * ng + q] = o[f][0];
+                a.full[((3ll * b + f) * 2 + 1) * ng + q] = o[f][1];
+            }
+        a.png[3 * i + 0] = kitti_u16(o[2][0]);
+        a.png[3 * i + 1] = kitti_u16(o[2][1]);
+        a.png[3 * i + 2] = 1;
+        a.flo[2 * i + 0] = o[2][0];
+        a.flo[2 * i + 1] = o[2][1];
+    }
+}
+
+// ================================================================================================
+// Middlebury flow colours (flowlib.py flow_to_image :189-226, compute_color :345-386, make_color_wheel :389-436).
+// Per image, P panels of [2, H, W] stacked along H (np.hstack of CHW arrays) share one maximum radius:
+//   pass 1  |u| or |v| > 1e7 (fp32) -> unknown, zeroed; rad = sqrt(u^2 + v^2) in fp32; maxrad = max(rad), and any NaN
+//           makes python's max(-1, nan) -1
+//   pass 2  u / (maxrad + DBL_EPSILON) in fp64, then the colour wheel in fp64; NaN and unknown pixels are black.
+// The levels are floor(255 * col) as uint8 (the reference returns them / 255).
+__constant__ double c_wheel[55][3] = {      // RY 15, YG 6, GC 4, CB 11, BM 13, MR 6 steps; ramps floor(255 k / n)
+    {255, 0, 0}, {255, 17, 0}, {255, 34, 0}, {255, 51, 0}, {255, 68, 0}, {255, 85, 0}, {255, 102, 0}, {255, 119, 0},
+    {255, 136, 0}, {255, 153, 0}, {255, 170, 0}, {255, 187, 0}, {255, 204, 0}, {255, 221, 0}, {255, 238, 0},
+    {255, 255, 0}, {213, 255, 0}, {170, 255, 0}, {128, 255, 0}, {85, 255, 0}, {43, 255, 0},
+    {0, 255, 0}, {0, 255, 63}, {0, 255, 127}, {0, 255, 191},
+    {0, 255, 255}, {0, 232, 255}, {0, 209, 255}, {0, 186, 255}, {0, 163, 255}, {0, 140, 255}, {0, 116, 255},
+    {0, 93, 255}, {0, 70, 255}, {0, 47, 255}, {0, 24, 255},
+    {0, 0, 255}, {19, 0, 255}, {39, 0, 255}, {58, 0, 255}, {78, 0, 255}, {98, 0, 255}, {117, 0, 255}, {137, 0, 255},
+    {156, 0, 255}, {176, 0, 255}, {196, 0, 255}, {215, 0, 255}, {235, 0, 255},
+    {255, 0, 255}, {255, 0, 213}, {255, 0, 170}, {255, 0, 128}, {255, 0, 85}, {255, 0, 43}};
+
+struct FlowColorArgs {
+    const float* flow;              // [B, P, 2, H, W]
+    unsigned long long* maxrad;     // [B]: bit pattern of max(rad), ~0 for NaN
+    unsigned char* out;             // [B, 3, P*H, W]
+    int B, P, H, W;
+};
+
+__device__ __forceinline__ bool flow_unknown(float u, float v) { return fabsf(u) > 1e7f || fabsf(v) > 1e7f; }
+
+__global__ void __launch_bounds__(256) flow_color_max_kernel(const FlowColorArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.y;
+    const long long hw = (long long)a.H * a.W, n = (long long)a.P * hw;
+    unsigned long long m = 0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const long long pnl = i / hw, p = i - pnl * hw;
+        const float* f = a.flow + ((long long)b * a.P + pnl) * 2 * hw + p;
+        float u = __ldg(f), v = __ldg(f + hw);
+        if (flow_unknown(u, v)) u = v = 0.f;
+        const float rad = __fsqrt_rn(__fadd_rn(__fmul_rn(u, u), __fmul_rn(v, v)));
+        const unsigned long long k = (rad != rad) ? ~0ull : (unsigned long long)__float_as_uint(rad);
+        m = (k > m) ? k : m;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long k = __shfl_xor_sync(0xffffffffu, m, o);
+        m = (k > m) ? k : m;
+    }
+    if ((threadIdx.x & 31) == 0) atomicMax(a.maxrad + b, m);
+}
+
+__global__ void __launch_bounds__(256) flow_color_kernel(const FlowColorArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.y;
+    const long long hw = (long long)a.H * a.W, n = (long long)a.P * hw;
+    const unsigned long long mk = a.maxrad[b];
+    const double den = __dadd_rn(mk == ~0ull ? -1.0 : (double)__uint_as_float((unsigned)mk), 2.220446049250313e-16);
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const long long pnl = i / hw, p = i - pnl * hw;
+        const float* f = a.flow + ((long long)b * a.P + pnl) * 2 * hw + p;
+        float uf = __ldg(f), vf = __ldg(f + hw);
+        const bool unknown = flow_unknown(uf, vf);
+        if (unknown) uf = vf = 0.f;
+        double u = __ddiv_rn((double)uf, den), v = __ddiv_rn((double)vf, den);
+        const bool nan = (u != u) || (v != v);
+        if (nan) u = v = 0.0;
+        const double rad = __dsqrt_rn(__dadd_rn(__dmul_rn(u, u), __dmul_rn(v, v)));
+        const double ang = __ddiv_rn(atan2(-v, -u), 3.141592653589793);
+        const double fk = __dadd_rn(__dmul_rn(__ddiv_rn(__dadd_rn(ang, 1.0), 2.0), 54.0), 1.0);
+        const int k0 = min(max((int)floor(fk), 1), 55);
+        const int k1 = (k0 + 1 == 56) ? 1 : k0 + 1;
+        const double fr = __dsub_rn(fk, (double)k0);
+        unsigned char* o = a.out + (long long)b * 3 * n + i;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const double col0 = __ddiv_rn(c_wheel[k0 - 1][c], 255.0), col1 = __ddiv_rn(c_wheel[k1 - 1][c], 255.0);
+            double col = __dadd_rn(__dmul_rn(__dsub_rn(1.0, fr), col0), __dmul_rn(fr, col1));
+            col = (rad <= 1.0) ? __dsub_rn(1.0, __dmul_rn(rad, __dsub_rn(1.0, col))) : __dmul_rn(col, 0.75);
+            const double level = floor(__dmul_rn(__dmul_rn(255.0, col), nan ? 0.0 : 1.0));
+            o[c * n] = unknown ? (unsigned char)0 : (unsigned char)(int)level;
+        }
+    }
+}
+
+// ================================================================================================
+// KITTI flow scores of decoded 16-bit PNGs (evaluate_flow.py compute_err :44-53, flow_io.flow_read_png :96-117), fp64:
+//   u = (U - 2^15) / 64,  epe = sqrt(du^2 + dv^2) * valid_gt,  aepe = sum(epe) / sum(valid_gt)
+//   Fl = sum([epe > 3] [epe / (|F_gt| + 1e-8) > 0.05] valid_gt) / sum(valid_gt)
+// Per-block fp64 partials (the two counts are integers, exact in fp64 below 2^53), one fixed-order finalize per image.
+struct KittiErrArgs {
+    const unsigned short* gt;       // [B, H, W, 3]
+    const unsigned short* pred;     // [B, H, W, 3]
+    double* partials;               // [B][blocks][3]: sum epe, sum valid, outliers
+    double* out;                    // [B, 2]
+    long long* counts;              // [B, 2] outliers, valid; or null
+    int B, H, W;
+};
+
+__global__ void __launch_bounds__(256) kitti_err_kernel(const KittiErrArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ double scratch[3 * 32];
+    const int b = blockIdx.y;
+    const long long n = (long long)a.H * a.W;
+    double acc[3] = {0, 0, 0};
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const unsigned short* g = a.gt + 3 * (b * n + i);
+        const unsigned short* p = a.pred + 3 * (b * n + i);
+        const double ug = __ddiv_rn((double)g[0] - 32768.0, 64.0), vg = __ddiv_rn((double)g[1] - 32768.0, 64.0);
+        const double up = __ddiv_rn((double)p[0] - 32768.0, 64.0), vp = __ddiv_rn((double)p[1] - 32768.0, 64.0);
+        const double valid = (double)g[2];
+        const double du = __dsub_rn(ug, up), dv = __dsub_rn(vg, vp);
+        const double epe = __dmul_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(du, du), __dmul_rn(dv, dv))), valid);
+        const double mag = __dsqrt_rn(__dadd_rn(__dmul_rn(ug, ug), __dmul_rn(vg, vg)));
+        acc[0] += epe;
+        acc[1] += valid;
+        if (epe > 3.0 && __ddiv_rn(epe, __dadd_rn(mag, 1e-8)) > 0.05) acc[2] += valid;
+    }
+    block_sum_d<3>(acc, scratch);
+    if (threadIdx.x == 0) {
+        double* o = a.partials + ((long long)b * gridDim.x + blockIdx.x) * 3;
+        o[0] = acc[0]; o[1] = acc[1]; o[2] = acc[2];
+    }
+}
+
+__global__ void kitti_err_finalize(const KittiErrArgs a, int nblk) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.B) return;
+    double s[3] = {0, 0, 0};
+    for (int k = 0; k < nblk; ++k)
+        for (int j = 0; j < 3; ++j) s[j] += a.partials[((long long)b * nblk + k) * 3 + j];
+    a.out[2 * b + 0] = __ddiv_rn(s[0], s[1]);
+    a.out[2 * b + 1] = __ddiv_rn(s[2], s[1]);
+    if (a.counts) {
+        a.counts[2 * b + 0] = (long long)s[2];
+        a.counts[2 * b + 1] = (long long)s[1];
+    }
+}
+
 }  // namespace ccb
 
 using namespace ccb;
@@ -775,6 +1021,66 @@ extern "C" int ccb_mask_iou(const float* emask, const float* flow_cam, const flo
     if (masks) CCB_LAUNCH(mask_iou_masks_kernel, dim3(mask_iou_blocks(h, w), B), dim3(256), 0, stream, a);
     CCB_LAUNCH(mask_iou_count_kernel, dim3(mask_iou_blocks(Hg, Wg), B), dim3(256), 0, stream, a);
     return check_launch("mask_iou");
+}
+
+extern "C" int ccb_flow_submit(const float* emask, const float* flow_cam, const float* flow_fwd, int B, int C, int h, int w,
+                               int Hg, int Wg, float thresh, float* mask, float* full, unsigned short* png, float* flo,
+                               ccb_stream_t stream) {
+    CCB_REQUIRE(emask && flow_cam && flow_fwd && mask && png && flo, CCB_ERR_ARG, "flow_submit: null pointer");
+    CCB_REQUIRE(C >= 3, CCB_ERR_ARG, "flow_submit: the mask net output needs channels 1 and 2, got %d channels", C);
+    CCB_REQUIRE(B > 0 && h > 0 && w > 0 && Hg > 0 && Wg > 0, CCB_ERR_ARG, "flow_submit: bad sizes");
+    FlowSubmitArgs a;
+    a.emask = emask; a.cam = flow_cam; a.fwd = flow_fwd; a.mask = mask; a.full = full; a.png = png; a.flo = flo;
+    a.B = B; a.C = C; a.h = h; a.w = w; a.Hg = Hg; a.Wg = Wg; a.thresh = thresh;
+    a.fu = (float)((double)Wg / (double)w);        // u * (w_gt / w_pred): the python float, cast to fp32 by torch's mul
+    a.fv = (float)((double)Hg / (double)h);
+    CCB_LAUNCH(flow_submit_mask_kernel, dim3(grid_for((long long)B * h * w)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(flow_submit_kernel, dim3(grid_for((long long)B * Hg * Wg)), dim3(256), 0, stream, a);
+    return check_launch("flow_submit");
+}
+
+extern "C" long long ccb_flow_color_workspace_bytes(int B, int P, int H, int W) {
+    if (B <= 0 || P <= 0 || H <= 0 || W <= 0) return -1;
+    return (long long)B * (long long)sizeof(unsigned long long);
+}
+
+extern "C" int ccb_flow_color(const float* flow, int B, int P, int H, int W, void* work, long long work_bytes, unsigned char* out,
+                              ccb_stream_t stream) {
+    CCB_REQUIRE(flow && out, CCB_ERR_ARG, "flow_color: null pointer");
+    CCB_REQUIRE(B > 0 && P > 0 && H > 0 && W > 0, CCB_ERR_ARG, "flow_color: bad sizes");
+    const long long need = ccb_flow_color_workspace_bytes(B, P, H, W);
+    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "flow_color: workspace of %lld bytes, %lld needed", work_bytes, need);
+    FlowColorArgs a;
+    a.flow = flow; a.maxrad = (unsigned long long*)work; a.out = out; a.B = B; a.P = P; a.H = H; a.W = W;
+    cudaMemsetAsync(a.maxrad, 0, (size_t)need, (cudaStream_t)stream);
+    const int nb = mask_iou_blocks(P * H, W);
+    CCB_LAUNCH(flow_color_max_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(flow_color_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    return check_launch("flow_color");
+}
+
+static int kitti_err_blocks(int H, int W) {
+    const long long g = ((long long)H * W + 2047) / 2048;
+    return (int)(g < 1 ? 1 : (g > 128 ? 128 : g));
+}
+
+extern "C" long long ccb_kitti_flow_errors_workspace_bytes(int B, int H, int W) {
+    if (B <= 0 || H <= 0 || W <= 0) return -1;
+    return (long long)B * kitti_err_blocks(H, W) * 3 * (long long)sizeof(double);
+}
+
+extern "C" int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned short* pred, int B, int H, int W, void* work,
+                                     long long work_bytes, double* out, long long* counts, ccb_stream_t stream) {
+    CCB_REQUIRE(gt && pred && out, CCB_ERR_ARG, "kitti_flow_errors: null pointer");
+    CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "kitti_flow_errors: bad sizes");
+    const long long need = ccb_kitti_flow_errors_workspace_bytes(B, H, W);
+    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "kitti_flow_errors: workspace of %lld bytes, %lld needed", work_bytes, need);
+    KittiErrArgs a;
+    a.gt = gt; a.pred = pred; a.partials = (double*)work; a.out = out; a.counts = counts; a.B = B; a.H = H; a.W = W;
+    const int nb = kitti_err_blocks(H, W);
+    CCB_LAUNCH(kitti_err_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(kitti_err_finalize, dim3((B + 63) / 64), dim3(64), 0, stream, a, nb);
+    return check_launch("kitti_flow_errors");
 }
 
 template <bool UNIT>

@@ -5,6 +5,9 @@
   flow_sample_errors    test_flow.py:112-140                               the 8 EPE / Fl numbers of one KITTI-2015 pair
   mask_sample_errors    test_mask.py:119-156 (+ mask_error :224-262)       tp fp fn per class of the three rigidity masks
                         (motion_mask_counts: the masks and counts alone; mask_iou: the script's final IoUs :199-201)
+  flow_submission_sample  submit_flow.py:109-175                           KITTI-2015 test-set files of one sample
+                        (flow_submission, flow_colors: the fused kernels; write_flow_submission: the script's files;
+                        kitti_flow_errors: evaluate_flow.py compute_err :44-53 of decoded 16-bit PNGs)
 
 The scripts' dataset crawlers, image IO and visualisation are out of scope (SURVEY.md section 2); these functions take what the
 reference's `test_framework` iterators yield (uint8 HxWx3 frames, ground truth arrays) and return what the scripts
@@ -172,3 +175,97 @@ def mask_iou(summed_counts):
         bg_iou = c[0] / (c[0] + c[1] + c[2])
         fg_iou = c[3] / (c[3] + c[4] + c[5])
     return float((bg_iou + fg_iou) / 2), float(bg_iou), float(fg_iou)
+
+
+@torch.no_grad()
+def flow_submission(emask, flow_cam, flow_fwd, Hg, Wg, THRESH=0.01, want_full=False):
+    """The per-sample files of submit_flow.py:119-156 in one fused call (ccb_flow_submit): emask [B,C,h,w], flow_cam /
+    flow_fwd [B,2,h,w] at the nets' resolution -> dict of device tensors:
+      mask [B,1,h,w]        the combined rigidity mask (what the script saves as mask/NNN.npy)
+      png  [B,Hg,Wg,3]      uint16 KITTI triplet of the full-resolution total flow (testing/NNNNNN_10.png)
+      flo  [B,Hg,Wg,2]      fp32 payload of testing_flo/NNNNNN_10.flo
+      full [B,3,2,Hg,Wg]    (want_full) the cam, fwd and total flows at full resolution, scaled as the script scales them
+    No host synchronisation."""
+    emask, flow_cam, flow_fwd = (_lib.f32(t) for t in (emask, flow_cam, flow_fwd))
+    B, C, h, w = (int(v) for v in emask.shape)
+    assert flow_cam.shape == (B, 2, h, w) and flow_fwd.shape == (B, 2, h, w), (flow_cam.shape, flow_fwd.shape)
+    dev = emask.device
+    out = dict(mask=torch.empty(B, 1, h, w, device=dev), png=torch.empty(B, Hg, Wg, 3, device=dev, dtype=torch.uint16),
+               flo=torch.empty(B, Hg, Wg, 2, device=dev))
+    if want_full:
+        out['full'] = torch.empty(B, 3, 2, Hg, Wg, device=dev)
+    _lib.call('ccb_flow_submit', emask, flow_cam, flow_fwd, B, C, h, w, int(Hg), int(Wg), float(THRESH), out['mask'],
+              out.get('full'), out['png'], out['flo'], emask)
+    return out
+
+
+@torch.no_grad()
+def flow_colors(flow):
+    """Middlebury colours (flowlib.flow_to_image) on the device (ccb_flow_color): flow [B,P,2,H,W] -> uint8 [B,3,P*H,W],
+    the P panels of each image stacked along H as np.hstack stacks [2,H,W] arrays and normalised by one maximum radius.
+    The levels are the reference's float image times 255.  No host synchronisation."""
+    flow = _lib.f32(flow)
+    B, P, two, H, W = (int(v) for v in flow.shape)
+    assert two == 2, flow.shape
+    nbytes = int(_lib.call('ccb_flow_color_workspace_bytes', B, P, H, W))
+    work = torch.empty(max(nbytes, 0) // 8 + 1, device=flow.device, dtype=torch.int64)
+    out = torch.empty(B, 3, P * H, W, device=flow.device, dtype=torch.uint8)
+    _lib.call('ccb_flow_color', flow, B, P, H, W, work, nbytes, out, flow)
+    return out
+
+
+@torch.no_grad()
+def flow_submission_sample(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv, Hg, Wg, THRESH=0.01, want_viz=False):
+    """submit_flow.py:109-175 for one batch: tgt/refs normalised device tensors [B,3,h,w] (4 refs), (Hg, Wg) the original
+    frame size -> flow_submission's dict of device tensors; want_viz adds 'full' and 'viz' = uint8 [B,3,3*Hg,Wg], row 2
+    of the script's visualisation (cam, fwd and total flow stacked, one radius).  Row 1 (matplotlib's magma map of the
+    target, disparity and mask) is not produced.  No host synchronisation."""
+    for n in (disp_net, pose_net, mask_net, flow_net):
+        n.eval()
+    disp = disp_net(tgt)
+    depth = 1 / disp
+    pose = pose_net(tgt, refs)
+    emask = mask_net(tgt, refs)
+    # submit_flow.py:113-116: Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
+    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
+    flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
+    out = flow_submission(emask, flow_cam, flow_fwd, Hg, Wg, THRESH, want_full=want_viz)
+    if want_viz:
+        out['viz'] = flow_colors(out['full'])
+    return out
+
+
+def write_flow_submission(out_dir, i, sample, tgt):
+    """Sample `i` (batch 1) of flow_submission_sample written as submit_flow.py:150-175 names it under `out_dir`:
+    images/iii.npy (the normalised target [3,h,w]), mask/iii.npy (the combined mask [1,h,w]), testing/iiiiii_10.png
+    (16-bit KITTI flow), testing_flo/iiiiii_10.flo and, when the sample has it, viz/iii02.png (8-bit RGB)."""
+    import os
+    from .flowutils import flow_io
+    for sub in ('images', 'mask', 'viz', 'testing', 'testing_flo'):
+        os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
+    np.save(os.path.join(out_dir, 'images', str(i).zfill(3)), tgt[0].detach().cpu().numpy())
+    np.save(os.path.join(out_dir, 'mask', str(i).zfill(3)), sample['mask'][0].cpu().numpy())
+    flow_io.write_png(os.path.join(out_dir, 'testing', str(i).zfill(6) + '_10.png'), sample['png'][0].cpu().numpy())
+    flow_io.write_flo_payload(os.path.join(out_dir, 'testing_flo', str(i).zfill(6) + '_10.flo'), sample['flo'][0].cpu().numpy())
+    if 'viz' in sample:
+        flow_io.write_png(os.path.join(out_dir, 'viz', str(i).zfill(3) + '02.png'),
+                          np.ascontiguousarray(sample['viz'][0].cpu().numpy().transpose(1, 2, 0)))
+
+
+@torch.no_grad()
+def kitti_flow_errors(gt_png, pred_png):
+    """evaluate_flow.py compute_err (:44-53) of decoded KITTI flow images on the device (ccb_kitti_flow_errors): gt_png and
+    pred_png uint16 [B,H,W,3] (or [H,W,3]; numpy arrays are copied to the current CUDA device) -> (errors fp64 [B,2] =
+    aepe, Fl; counts int64 [B,2] = outliers, valid pixels), both on the device.  The script averages the per-image rows."""
+    dev = pred_png.device if torch.is_tensor(pred_png) else (torch.device('cpu') if _lib.is_simulator() else torch.device('cuda'))
+    gt, pred = (torch.as_tensor(np.asarray(a) if not torch.is_tensor(a) else a).to(dev).contiguous() for a in (gt_png, pred_png))
+    if gt.dim() == 3:
+        gt, pred = gt[None], pred[None]
+    assert gt.shape == pred.shape and gt.shape[-1] == 3 and gt.dtype == torch.uint16, (gt.shape, pred.shape, gt.dtype)
+    B, H, W = (int(v) for v in gt.shape[:3])
+    nbytes = int(_lib.call('ccb_kitti_flow_errors_workspace_bytes', B, H, W))
+    work = torch.empty(max(nbytes, 0) // 8 + 1, device=dev, dtype=torch.int64)
+    out = torch.empty(B, 2, device=dev, dtype=torch.float64)
+    counts = torch.empty(B, 2, device=dev, dtype=torch.int64)
+    _lib.call('ccb_kitti_flow_errors', gt, pred, B, H, W, work, nbytes, out, counts, gt)
+    return out, counts

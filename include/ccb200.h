@@ -343,6 +343,33 @@ long long ccb_mask_iou_workspace_bytes(int B, int h, int w, int Hg, int Wg);
 int ccb_mask_iou(const float* emask, const float* flow_cam, const float* flow, const float* obj_map,
                  const float* semantic_map, int B, int C, int h, int w, int Hg, int Wg, float thresh, int car_label,
                  float* masks, void* work, long long work_bytes, long long* counts, ccb_stream_t stream);
+/* The KITTI-2015 flow submission of one sample each (submit_flow.py:119-156), no host sync.  emask [B,C,h,w] (C >= 3),
+ * flow_cam and flow_fwd [B,2,h,w] at the nets' resolution:
+ *   combined = bare or census, bare = 1 - (1-e1)(1-e2) > 0.5, census = |cam - fwd| < thresh in u and in v  -> mask [B,1,h,w]
+ *   total = (combined <= thresh) * fwd + (combined > thresh) * cam
+ * total, fwd and cam resized bilinearly to Hg x Wg as torch's CPU interpolate(align_corners=False) computes it when
+ * both axes change size and Wg >= 16 (fma source index, fma per axis, x inside y; see io_ops.cu), u times (float)(Wg/w) and v times (float)(Hg/h):
+ *   full  (optional) [B,3,2,Hg,Wg]  cam, fwd, total, fp32
+ *   png   [B,Hg,Wg,3] uint16        KITTI triplet of total: (uint16)(u*64.0 + 2^15) in fp64 with numpy's x86-64 cast
+ *                                   (truncate to int32, keep the low 16 bits: flows past +-512 px wrap), valid = 1
+ *   flo   [B,Hg,Wg,2] fp32          the .flo payload of total (u, v interleaved) */
+int ccb_flow_submit(const float* emask, const float* flow_cam, const float* flow_fwd, int B, int C, int h, int w, int Hg,
+                    int Wg, float thresh, float* mask, float* full, unsigned short* png, float* flo, ccb_stream_t stream);
+/* Middlebury flow colours (flowlib.py flow_to_image / compute_color), no host sync.  flow [B,P,2,H,W]: per image P
+ * panels stacked along H as np.hstack stacks CHW arrays, normalised by ONE maximum radius -> out [B,3,P*H,W] uint8
+ * levels (the reference's float image times 255).  |u| or |v| > 1e7 is unknown (black, left out of the maximum); NaN
+ * pixels are black and make the maximum -1, as python's max(-1, nan) does; the colour pass runs in fp64.
+ * work: ccb_flow_color_workspace_bytes(B, P, H, W) bytes (-1 for bad sizes), 8-byte aligned. */
+long long ccb_flow_color_workspace_bytes(int B, int P, int H, int W);
+int ccb_flow_color(const float* flow, int B, int P, int H, int W, void* work, long long work_bytes, unsigned char* out,
+                   ccb_stream_t stream);
+/* KITTI flow scores of two 16-bit triplets each (evaluate_flow.py compute_err :44-53 on flow_read_png's decoding), no host
+ * sync.  gt and pred [B,H,W,3] uint16 -> out [B,2] fp64 (aepe, Fl) and optionally counts [B,2] (outliers weighted by
+ * valid_gt, sum of valid_gt).  fp64 block partials with a fixed-order finalize: the same bits on every run.
+ * work: ccb_kitti_flow_errors_workspace_bytes(B, H, W) bytes (-1 for bad sizes), 8-byte aligned. */
+long long ccb_kitti_flow_errors_workspace_bytes(int B, int H, int W);
+int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned short* pred, int B, int H, int W, void* work,
+                          long long work_bytes, double* out, long long* counts, ccb_stream_t stream);
 /* Input pipeline on the device (train.py:448-451 H2D + custom_transforms.py:21-30,47-118): uint8 HWC frames
  * src [B,F,Hs,Ws,3] -> F normalised fp32 NCHW tensors dst[f] [B,3,H,W] = (v/255 - .5)/.5, per sample horizontally
  * flipped (params[b][0] != 0) and scale-cropped: resized by (params[b][1], params[b][2]) = (scaled_w/Ws, scaled_h/Hs)
