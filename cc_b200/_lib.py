@@ -41,16 +41,17 @@ class PhotoDesc(C.Structure):
         ('tgt', _LP), ('ref', _LRP), ('depth', _LP), ('flow', _LRP), ('mask', _LP),
         ('pose', _P), ('K', _P), ('Kinv', _P),
         ('dmaps', _LP), ('gmask', _LP), ('vo', _LP), ('scal', _P),
-        ('partials', _P), ('loss', _P), ('target', _LP),
+        ('partials', _P), ('partials_floats', C.c_longlong), ('loss', _P), ('target', _LP),
         ('grad_out', _P), ('d_depth', _LP), ('d_flow', _LRP), ('d_mask', _LP), ('d_pose', _P),
-        ('pose_partials', _P),
+        ('pose_partials', _P), ('pose_partials_floats', C.c_longlong),
     ]
 
 
 class SmoothDesc(C.Structure):
     _fields_ = [
         ('kind', C.c_int), ('B', C.c_int), ('C', C.c_int), ('nlevels', C.c_int), ('h', _LI), ('w', _LI),
-        ('img', _LP), ('pred', _LP), ('partials', _P), ('loss', _P), ('grad_out', _P), ('d_pred', _LP),
+        ('img', _LP), ('pred', _LP), ('partials', _P), ('partials_floats', C.c_longlong), ('loss', _P), ('grad_out', _P),
+        ('d_pred', _LP),
     ]
 
 
@@ -59,7 +60,7 @@ class BceDesc(C.Structure):
         ('kind', C.c_int), ('B', C.c_int), ('C', C.c_int), ('nlevels', C.c_int), ('h', _LI), ('w', _LI),
         ('thresh', C.c_float), ('wbce', C.c_float),
         ('mask', _LP), ('census_bwd', _LP), ('census_fwd', _LP), ('target_bwd', _LP), ('target_fwd', _LP),
-        ('partials', _P), ('loss', _P), ('grad_out', _P), ('d_mask', _LP),
+        ('partials', _P), ('partials_floats', C.c_longlong), ('loss', _P), ('grad_out', _P), ('d_mask', _LP),
     ]
 
 
@@ -95,18 +96,20 @@ _SIGS = {
     'ccb_inverse_warp_fwd': (STATUS, 'const float*, const float*, const float*, int, const float*, const float*, '
                                      'int, int, int, int, int, float*, ccb_stream_t'),
     'ccb_inverse_warp_bwd': (STATUS, 'const float*, const float*, const float*, int, const float*, const float*, '
-                                     'int, int, int, int, int, const float*, float*, float*, float*, ccb_stream_t'),
+                                     'int, int, int, int, int, const float*, float*, float*, float*, long long, '
+                                     'ccb_stream_t'),
     'ccb_warp_pose_partials_floats': ('long long', 'int, int, int'),
     'ccb_flow_warp_fwd': (STATUS, 'const float*, const float*, int, int, int, int, int, float*, ccb_stream_t'),
     'ccb_flow_warp_bwd': (STATUS, 'const float*, const float*, int, int, int, int, int, const float*, float*, '
-                                  'float*, unsigned long long*, ccb_stream_t'),
+                                  'float*, unsigned long long*, long long, ccb_stream_t'),
     'ccb_pose2flow_fwd': (STATUS, 'const float*, const float*, int, const float*, const float*, int, int, int, int, '
                                   'int, float*, ccb_stream_t'),
     'ccb_pose2flow_bwd': (STATUS, 'const float*, const float*, int, const float*, const float*, int, int, int, int, '
-                                  'int, const float*, float*, float*, float*, ccb_stream_t'),
+                                  'int, const float*, float*, float*, float*, long long, ccb_stream_t'),
     'ccb_ssim_fwd': (STATUS, 'const float*, const float*, int, int, int, host const float*, float*, ccb_stream_t'),
+    'ccb_ssim_bwd_workspace_floats': ('long long', 'int, int, int'),
     'ccb_ssim_bwd': (STATUS, 'const float*, const float*, int, int, int, host const float*, const float*, float*, '
-                             'float*, float*, ccb_stream_t'),
+                             'float*, float*, long long, ccb_stream_t'),
     'ccb_smooth_partials_floats': ('long long', 'const ccb_smooth_desc*'),
     'ccb_smooth_fwd': (STATUS, 'const ccb_smooth_desc*, ccb_stream_t'),
     'ccb_smooth_bwd': (STATUS, 'const ccb_smooth_desc*, ccb_stream_t'),
@@ -133,28 +136,30 @@ _SIGS = {
     'ccb_corr81_fwd_workspace_floats': ('long long', 'int, int, int, int'),
     'ccb_corr81_fwd': (STATUS, 'const float*, const float*, float*, int, int, int, int, int, float*, long long, '
                                'ccb_stream_t'),
+    'ccb_corr81_bwd_workspace_floats': ('long long', 'int, int, int, int'),
     'ccb_corr81_bwd': (STATUS, 'const float*, const float*, const float*, float*, float*, int, int, int, int, int, '
-                               'float*, ccb_stream_t'),
+                               'float*, long long, ccb_stream_t'),
     'ccb_corr441d_fwd': (STATUS, 'const float*, const float*, float*, int, int, int, int, ccb_stream_t'),
     'ccb_corr441d_bwd': (STATUS, 'const float*, const float*, const float*, const float*, float*, float*, int, int, '
                                  'int, int, ccb_stream_t'),
     'ccb_featwarp_fwd': (STATUS, 'const float*, const float*, int, int, int, int, float*, ccb_stream_t'),
     'ccb_featwarp_bwd': (STATUS, 'const float*, const float*, int, int, int, int, const float*, float*, float*, '
-                                 'unsigned long long*, ccb_stream_t'),
+                                 'unsigned long long*, long long, ccb_stream_t'),
     'ccb_bn_workspace_floats': ('long long', 'int, int, int'),
     'ccb_bn_fwd': (STATUS, 'const float*, const float*, const float*, float*, float*, float*, float*, int, int, int, '
-                           'float, float, int, float*, ccb_stream_t'),
+                           'float, float, int, float*, long long, ccb_stream_t'),
     'ccb_bn_bwd': (STATUS, 'const float*, const float*, const float*, const float*, float*, float*, float*, int, '
-                           'int, int, float*, ccb_stream_t'),
+                           'int, int, float*, long long, ccb_stream_t'),
     'ccb_upsample2x_fwd': (STATUS, 'const float*, float*, int, int, int, ccb_stream_t'),
     'ccb_upsample2x_bwd': (STATUS, 'const float*, float*, int, int, int, ccb_stream_t'),
     'ccb_adam_step_ranges': (STATUS, 'float*, const float*, float*, float*, const long long*, int, long long, '
                                      'const int*, int, float*, float, float, float, float, float, ccb_stream_t'),
     'ccb_flow_metrics_workspace_bytes': ('long long', 'int, int, int'),
     'ccb_flow_metrics': (STATUS, 'const float*, const float*, const float*, const float*, int, int, int, int, int, '
-                                 'int, int, int, float, float, float, float*, void*, float*, ccb_stream_t'),
+                                 'int, int, int, float, float, float, float*, void*, long long, float*, ccb_stream_t'),
     'ccb_depth_errors_workspace_bytes': ('long long', 'int, int, int'),
-    'ccb_depth_errors': (STATUS, 'const float*, const float*, int, int, int, int, void*, float*, ccb_stream_t'),
+    'ccb_depth_errors': (STATUS, 'const float*, const float*, int, int, int, int, void*, long long, float*, '
+                                 'ccb_stream_t'),
     'ccb_mask_iou_workspace_bytes': ('long long', 'int, int, int, int, int'),
     'ccb_mask_iou': (STATUS, 'const float*, const float*, const float*, const float*, const float*, int, int, int, '
                              'int, int, int, float, int, float*, void*, long long, long long*, ccb_stream_t'),
@@ -293,9 +298,22 @@ def is_simulator():
     return _is_sim
 
 
+def workspace(query, *args, like):
+    """(scratch buffer, its size) for the entry point whose size query `query` is, called on `args`: fp32 for a
+    `*_floats` query, uint8 for `*_bytes`, on `like`'s device; (None, 0) where nothing is needed.  A query's -1
+    (invalid sizes) raises."""
+    n = call(query, *args)
+    if n < 0:
+        raise RuntimeError('cc_b200: %s returned -1: invalid sizes' % query)
+    dtype = torch.float32 if query.endswith('_floats') else torch.uint8
+    return (torch.empty(n, dtype=dtype, device=like.device) if n else None), n
+
+
 def scatter_workspace(t):
-    """Fixed-point accumulators (+1 word) for the image gradient of a warp of `t` (ccb_flow_warp_bwd / ccb_featwarp_bwd)."""
-    return torch.empty(t.numel() + 1, dtype=torch.int64, device=t.device)
+    """(fixed-point accumulators, their size in words) for the image gradient of a warp of `t` (ccb_flow_warp_bwd /
+    ccb_featwarp_bwd): the gradient's element count + 1, as include/ccb200.h states."""
+    n = t.numel() + 1
+    return torch.empty(n, dtype=torch.int64, device=t.device), n
 
 
 def f32(t):

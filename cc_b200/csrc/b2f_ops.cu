@@ -171,6 +171,7 @@ __global__ void __launch_bounds__(CT * CT) corr81_dgrad_kernel(const float* __re
 using namespace ccb;
 
 extern "C" long long ccb_corr81_fwd_workspace_floats(int B, int C, int h, int w) {
+    if (B < 1 || C < 1 || h < 1 || w < 1) return -1;
     const int chunks = corr_chunks(B, C, h, w);
     return chunks > 1 ? (long long)chunks * B * 81 * h * w : 0;
 }
@@ -178,9 +179,8 @@ extern "C" long long ccb_corr81_fwd_workspace_floats(int B, int C, int h, int w)
 extern "C" int ccb_corr81_fwd(const float* f1, const float* f2, float* out, int B, int C, int h, int w, int reversed,
                               float* work, long long work_floats, ccb_stream_t stream) {
     CCB_REQUIRE(f1 && f2 && out && B >= 1 && C >= 1 && h >= 1 && w >= 1, CCB_ERR_ARG, "corr81_fwd: bad argument");
+    CCB_REQUIRE_WORK("corr81_fwd", "work", work, work_floats, ccb_corr81_fwd_workspace_floats(B, C, h, w));
     const int chunks = corr_chunks(B, C, h, w);
-    CCB_REQUIRE(chunks == 1 || (work && work_floats >= (long long)chunks * B * 81 * h * w), CCB_ERR_ARG,
-                "corr81_fwd: workspace of ccb_corr81_fwd_workspace_floats() floats required");
     CCB_LAUNCH(corr81_fwd_kernel, dim3(cdiv(w, CT), cdiv(h, CT), B * chunks), dim3(CT * CT), 0, stream, f1, f2, out, work, B, C, h, w,
                reversed, chunks);
     if (chunks > 1) {
@@ -191,10 +191,16 @@ extern "C" int ccb_corr81_fwd(const float* f1, const float* f2, float* out, int 
     return check_launch("corr81_fwd");
 }
 
+extern "C" long long ccb_corr81_bwd_workspace_floats(int B, int C, int h, int w) {
+    if (B < 1 || C < 1 || h < 1 || w < 1) return -1;
+    return (long long)B * 81 * h * w;
+}
+
 extern "C" int ccb_corr81_bwd(const float* f1, const float* f2, const float* grad_out, float* d_f1, float* d_f2, int B,
-                              int C, int h, int w, int reversed, float* work, ccb_stream_t stream) {
-    CCB_REQUIRE(f1 && f2 && grad_out && (d_f1 || d_f2), CCB_ERR_ARG, "corr81_bwd: bad argument");
-    CCB_REQUIRE(d_f2 == nullptr || work != nullptr, CCB_ERR_ARG, "corr81_bwd: d_f2 needs a workspace of B*81*h*w floats");
+                              int C, int h, int w, int reversed, float* work, long long work_floats, ccb_stream_t stream) {
+    CCB_REQUIRE(f1 && f2 && grad_out && (d_f1 || d_f2) && B >= 1 && C >= 1 && h >= 1 && w >= 1, CCB_ERR_ARG,
+                "corr81_bwd: bad argument");
+    CCB_REQUIRE_WORK("corr81_bwd", "work", work, work_floats, d_f2 ? ccb_corr81_bwd_workspace_floats(B, C, h, w) : 0);
     const int chunks = corr_chunks(B, C, h, w);
     const dim3 grid(cdiv(w, CT), cdiv(h, CT), B * chunks);
     if (d_f1) CCB_LAUNCH(corr81_dgrad_kernel, grid, dim3(CT * CT), 0, stream, grad_out, f2, d_f1, B, C, h, w, reversed, 0, chunks);

@@ -66,6 +66,15 @@ extern thread_local const char* g_last_conv;
         }                                       \
     } while (0)
 
+// The workspace contract of ccb200.h: the scratch buffer `buf`, given with its size `size` in the unit of its pointer
+// type, holds at least `need` (what the entry point's size query returns); it may be NULL only where `need` is 0.
+inline const char* work_unit(const float*) { return "floats"; }
+inline const char* work_unit(const unsigned long long*) { return "words"; }
+inline const char* work_unit(const void*) { return "bytes"; }
+#define CCB_REQUIRE_WORK(entry, name, buf, size, need)                                                              \
+    CCB_REQUIRE((size) >= (need) && ((buf) != nullptr || (need) == 0), CCB_ERR_ARG, "%s: %s of %lld %s, %lld needed", \
+                entry, name, (long long)(size), ccb::work_unit(buf), (long long)(need))
+
 // ---- weight preparation for the tensor-core conv kernels (wprep.cu) ----
 enum { WPREP_TC = 0 };
 struct WPrepDesc {

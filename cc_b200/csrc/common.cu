@@ -37,7 +37,7 @@ int check_launch(const char* what) {
 }  // namespace ccb
 
 extern "C" const char* ccb_last_error_string(void) { return ccb::g_err; }
-extern "C" int ccb_version(void) { return 100; }
+extern "C" int ccb_version(void) { return 101; }
 extern "C" const char* ccb_debug_last_conv_kernel(void) { return ccb::g_last_conv; }
 extern "C" long long ccb_launch_count(void) { return ccb::g_launches; }
 extern "C" int ccb_is_simulator(void) {

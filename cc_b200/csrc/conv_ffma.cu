@@ -537,6 +537,7 @@ extern "C" int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const fl
 }
 
 extern "C" long long ccb_act_bwd_bias_workspace_floats(int B, int C, int plane) {
+    if (B < 1 || C < 1 || plane < 1) return -1;
     if ((long long)B * plane <= ABB_SMALL) return 0;
     return (long long)C * B * cdiv(plane, ABB_CHUNK);
 }
@@ -551,7 +552,7 @@ extern "C" int ccb_act_bwd_bias(const float* dy, const float* y, float* dz, floa
         return check_launch("act_bwd_bias");
     }
     const int nchunk = cdiv(plane, ABB_CHUNK);
-    CCB_REQUIRE(db == nullptr || (work && work_floats >= (long long)C * B * nchunk), CCB_ERR_ARG, "act_bwd_bias: workspace too small");
+    CCB_REQUIRE_WORK("act_bwd_bias", "work", work, work_floats, db ? ccb_act_bwd_bias_workspace_floats(B, C, plane) : 0);
     CCB_REQUIRE(C <= 65535 && B <= 65535, CCB_ERR_ARG, "act_bwd_bias: grid too large");
     CCB_LAUNCH(abb_large_kernel, dim3(nchunk, B, C), dim3(256), 0, stream, dy, y, dz, db ? work : nullptr, C, plane, nchunk, act, slope);
     if (db) CCB_LAUNCH(abb_merge_kernel, dim3(cdiv(C, 128)), dim3(128), 0, stream, (const float*)work, db, C, B * nchunk);

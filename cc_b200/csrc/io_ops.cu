@@ -933,17 +933,19 @@ static int grid_for(long long n) {
 }
 
 extern "C" long long ccb_flow_metrics_workspace_bytes(int B, int Hg, int Wg) {
+    if (B <= 0 || Hg <= 0 || Wg <= 0) return -1;
     return (long long)grid_for((long long)B * Hg * Wg) * 8 * (long long)sizeof(double);
 }
 
 extern "C" int ccb_flow_metrics(const float* gt, const float* pred_rigid, const float* pred_nonrigid, const float* rigidity_mask,
                                 int B, int nc, int Hg, int Wg, int hp, int wp, int hm, int wm, float thresh, float tau0,
-                                float tau1, float* epe_map, void* work, float* out4, ccb_stream_t stream) {
-    CCB_REQUIRE(gt && pred_rigid && work && out4, CCB_ERR_ARG, "flow_metrics: null pointer");
+                                float tau1, float* epe_map, void* work, long long work_bytes, float* out4, ccb_stream_t stream) {
+    CCB_REQUIRE(gt && pred_rigid && out4, CCB_ERR_ARG, "flow_metrics: null pointer");
     CCB_REQUIRE(nc == 2 || nc == 3, CCB_ERR_ARG, "flow_metrics: ground truth must have 2 or 3 channels, got %d", nc);
     CCB_REQUIRE((rigidity_mask == nullptr) == (pred_nonrigid == nullptr), CCB_ERR_ARG,
                 "flow_metrics: rigidity mask and non-rigid prediction come together");
     CCB_REQUIRE(B > 0 && Hg > 0 && Wg > 0 && hp > 0 && wp > 0, CCB_ERR_ARG, "flow_metrics: bad sizes");
+    CCB_REQUIRE_WORK("flow_metrics", "work", work, work_bytes, ccb_flow_metrics_workspace_bytes(B, Hg, Wg));
     FlowMetArgs a;
     a.gt = gt; a.pa = pred_rigid; a.pb = pred_nonrigid; a.mask = rigidity_mask; a.partials = (double*)work; a.epe_map = epe_map;
     a.B = B; a.nc = nc; a.Hg = Hg; a.Wg = Wg; a.hp = hp; a.wp = wp; a.hm = hm; a.wm = wm;
@@ -960,13 +962,15 @@ static int depth_blocks(int H, int W) {
 }
 
 extern "C" long long ccb_depth_errors_workspace_bytes(int B, int H, int W) {
+    if (B <= 0 || H <= 0 || W <= 0) return -1;
     return (long long)B * 2 * 2048 * 4 + (long long)B * 2 * 4 * 4 + (long long)B * depth_blocks(H, W) * 6 * 8 + 64;
 }
 
-extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, int crop, void* work, float* out6,
-                                ccb_stream_t stream) {
-    CCB_REQUIRE(gt && pred && work && out6, CCB_ERR_ARG, "depth_errors: null pointer");
+extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, int crop, void* work, long long work_bytes,
+                                float* out6, ccb_stream_t stream) {
+    CCB_REQUIRE(gt && pred && out6, CCB_ERR_ARG, "depth_errors: null pointer");
     CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "depth_errors: bad sizes");
+    CCB_REQUIRE_WORK("depth_errors", "work", work, work_bytes, ccb_depth_errors_workspace_bytes(B, H, W));
     DepthArgs a;
     a.gt = gt; a.pred = pred; a.B = B; a.H = H; a.W = W; a.out = out6;
     a.y1 = 0; a.y2 = H; a.x1 = 0; a.x2 = W;
@@ -979,11 +983,7 @@ extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H
     a.hist = (unsigned*)p;     p += (long long)B * 2 * 2048 * 4;
     a.sel = (unsigned*)p;
     const int nb = depth_blocks(H, W);
-#ifdef CCB_CPU_SIM
-    memset(a.hist, 0, (size_t)B * 2 * 2048 * 4 + (size_t)B * 2 * 4 * 4);
-#else
     cudaMemsetAsync(a.hist, 0, (size_t)B * 2 * 2048 * 4 + (size_t)B * 2 * 4 * 4, (cudaStream_t)stream);
-#endif
     for (int pass = 0; pass < 3; ++pass) {
         CCB_LAUNCH(depth_hist_kernel, dim3(nb, B), dim3(256), 0, stream, a, pass);
         CCB_LAUNCH(depth_select_kernel, dim3((B * 2 + 63) / 64), dim3(64), 0, stream, a, pass);
@@ -1010,7 +1010,7 @@ extern "C" int ccb_mask_iou(const float* emask, const float* flow_cam, const flo
     CCB_REQUIRE(C >= 3, CCB_ERR_ARG, "mask_iou: the mask net output needs channels 1 and 2, got %d channels", C);
     CCB_REQUIRE(B > 0 && h > 0 && w > 0 && Hg > 0 && Wg > 0, CCB_ERR_ARG, "mask_iou: bad sizes");
     const long long need = ccb_mask_iou_workspace_bytes(B, h, w, Hg, Wg);
-    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "mask_iou: workspace of %lld bytes, %lld needed", work_bytes, need);
+    CCB_REQUIRE_WORK("mask_iou", "work", work, work_bytes, need);
     MaskIouArgs a;
     a.emask = emask; a.flow_cam = flow_cam; a.flow = flow; a.obj = obj_map; a.sem = semantic_map; a.masks = masks;
     a.dmax = (unsigned long long*)work; a.counts = (unsigned long long*)counts;
@@ -1049,7 +1049,7 @@ extern "C" int ccb_flow_color(const float* flow, int B, int P, int H, int W, voi
     CCB_REQUIRE(flow && out, CCB_ERR_ARG, "flow_color: null pointer");
     CCB_REQUIRE(B > 0 && P > 0 && H > 0 && W > 0, CCB_ERR_ARG, "flow_color: bad sizes");
     const long long need = ccb_flow_color_workspace_bytes(B, P, H, W);
-    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "flow_color: workspace of %lld bytes, %lld needed", work_bytes, need);
+    CCB_REQUIRE_WORK("flow_color", "work", work, work_bytes, need);
     FlowColorArgs a;
     a.flow = flow; a.maxrad = (unsigned long long*)work; a.out = out; a.B = B; a.P = P; a.H = H; a.W = W;
     cudaMemsetAsync(a.maxrad, 0, (size_t)need, (cudaStream_t)stream);
@@ -1074,7 +1074,7 @@ extern "C" int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned sh
     CCB_REQUIRE(gt && pred && out, CCB_ERR_ARG, "kitti_flow_errors: null pointer");
     CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "kitti_flow_errors: bad sizes");
     const long long need = ccb_kitti_flow_errors_workspace_bytes(B, H, W);
-    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "kitti_flow_errors: workspace of %lld bytes, %lld needed", work_bytes, need);
+    CCB_REQUIRE_WORK("kitti_flow_errors", "work", work, work_bytes, need);
     KittiErrArgs a;
     a.gt = gt; a.pred = pred; a.partials = (double*)work; a.out = out; a.counts = counts; a.B = B; a.H = H; a.W = W;
     const int nb = kitti_err_blocks(H, W);
@@ -1154,14 +1154,10 @@ extern "C" int ccb_resize_u8(const unsigned char* src, unsigned char* dst, int N
     CCB_REQUIRE(src != dst, CCB_ERR_ARG, "resize_u8: cannot resize in place");
     CCB_REQUIRE(N > 0 && Hs > 0 && Ws > 0 && H > 0 && W > 0, CCB_ERR_ARG, "resize_u8: bad sizes");
     const ResizePlan p = resize_plan(N, Hs, Ws, H, W);
-    CCB_REQUIRE(work && work_bytes >= p.bytes, CCB_ERR_ARG, "resize_u8: workspace of %lld bytes, %lld needed", work_bytes, p.bytes);
+    CCB_REQUIRE_WORK("resize_u8", "work", work, work_bytes, p.bytes);
     const bool hpass = W != Ws, vpass = H != Hs;
     if (!hpass && !vpass) {
-#ifdef CCB_CPU_SIM
-        memcpy(dst, src, (size_t)N * H * W * 3);
-#else
         cudaMemcpyAsync(dst, src, (size_t)N * H * W * 3, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
-#endif
         return check_launch("resize_u8");
     }
     char* w = (char*)work;
@@ -1201,7 +1197,7 @@ extern "C" int ccb_normalize_local(float* const* frames, int B, int F, int H, in
     CCB_REQUIRE(F >= 1 && F <= 8, CCB_ERR_ARG, "normalize_local: 1..8 frames per sample, got %d", F);
     CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "normalize_local: bad sizes");
     const long long need = ccb_normalize_local_workspace_bytes(B, H, W);
-    CCB_REQUIRE(work && work_bytes >= need, CCB_ERR_ARG, "normalize_local: workspace of %lld bytes, %lld needed", work_bytes, need);
+    CCB_REQUIRE_WORK("normalize_local", "work", work, work_bytes, need);
     NormLocalArgs a;
     for (int f = 0; f < 8; ++f) a.x[f] = (f < F) ? frames[f] : nullptr;
     for (int f = 0; f < F; ++f) CCB_REQUIRE(a.x[f] != nullptr, CCB_ERR_ARG, "normalize_local: frames[%d] is null", f);

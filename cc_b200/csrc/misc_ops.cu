@@ -251,16 +251,19 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
 using namespace ccb;
 
 extern "C" long long ccb_bn_workspace_floats(int B, int C, int plane) {
+    if (B < 1 || C < 1 || plane < 1) return -1;
     long long nsplit = ((long long)B * plane + BN_CHUNK - 1) / BN_CHUNK;
     return (long long)C * nsplit * 3 + 2 * C;
 }
 
 extern "C" int ccb_bn_fwd(const float* x, const float* gamma, const float* beta, float* y, float* stats,
                           float* running_mean, float* running_var, int B, int C, int plane, float eps, float momentum,
-                          int training, float* work, ccb_stream_t stream) {
+                          int training, float* work, long long work_floats, ccb_stream_t stream) {
     CCB_REQUIRE(x && gamma && beta && y, CCB_ERR_ARG, "bn_fwd: null pointer");
+    CCB_REQUIRE(B >= 1 && C >= 1 && plane >= 1, CCB_ERR_ARG, "bn_fwd: bad size");
+    CCB_REQUIRE_WORK("bn_fwd", "work", work, work_floats, training ? ccb_bn_workspace_floats(B, C, plane) : 0);
     if (training) {
-        CCB_REQUIRE(stats != nullptr && work != nullptr, CCB_ERR_ARG, "bn_fwd: stats/work null in training mode");
+        CCB_REQUIRE(stats != nullptr, CCB_ERR_ARG, "bn_fwd: stats null in training mode");
         const int nsplit = (int)(((long long)B * plane + BN_CHUNK - 1) / BN_CHUNK);
         const long long numel = (long long)B * C * plane;
         CCB_LAUNCH(bn_partial_kernel, dim3(C, nsplit), dim3(256), 0, stream, x, work, B, C, plane, nsplit);
@@ -277,8 +280,11 @@ extern "C" int ccb_bn_fwd(const float* x, const float* gamma, const float* beta,
 }
 
 extern "C" int ccb_bn_bwd(const float* x, const float* dy, const float* gamma, const float* stats, float* dx,
-                          float* dgamma, float* dbeta, int B, int C, int plane, float* work, ccb_stream_t stream) {
-    CCB_REQUIRE(x && dy && gamma && stats && dx && dgamma && dbeta && work, CCB_ERR_ARG, "bn_bwd: null pointer");
+                          float* dgamma, float* dbeta, int B, int C, int plane, float* work, long long work_floats,
+                          ccb_stream_t stream) {
+    CCB_REQUIRE(x && dy && gamma && stats && dx && dgamma && dbeta, CCB_ERR_ARG, "bn_bwd: null pointer");
+    CCB_REQUIRE(B >= 1 && C >= 1 && plane >= 1, CCB_ERR_ARG, "bn_bwd: bad size");
+    CCB_REQUIRE_WORK("bn_bwd", "work", work, work_floats, ccb_bn_workspace_floats(B, C, plane));
     const int nsplit = (int)(((long long)B * plane + BN_CHUNK - 1) / BN_CHUNK);
     const long long numel = (long long)B * C * plane;
     float* sums = work + (long long)C * nsplit * 3;

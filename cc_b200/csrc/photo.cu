@@ -575,7 +575,8 @@ extern "C" int ccb_photo_loss_fwd(const ccb_photo_desc* d, ccb_stream_t stream) 
     CCB_REQUIRE(d->mode == CCB_PHOTO_RIGID || d->mode == CCB_PHOTO_FLOW, CCB_ERR_ARG, "photo_loss_fwd: bad mode %d", d->mode);
     rc = check_common(d, false);
     if (rc) return rc;
-    CCB_REQUIRE(d->partials && d->scal && d->loss, CCB_ERR_ARG, "photo_loss_fwd: partials/scal/loss null");
+    CCB_REQUIRE(d->scal && d->loss, CCB_ERR_ARG, "photo_loss_fwd: scal/loss null");
+    CCB_REQUIRE_WORK("photo_loss_fwd", "partials", d->partials, d->partials_floats, ccb_photo_partials_floats(d));
     cudaStream_t st = (cudaStream_t)stream;
     const bool ss = d->wssim != 0.f;
     const SaveFlags sf = save_flags(d, false);
@@ -604,7 +605,9 @@ extern "C" int ccb_photo_loss_bwd(const ccb_photo_desc* d, ccb_stream_t stream) 
     cudaStream_t st = (cudaStream_t)stream;
     const bool ss = d->wssim != 0.f;
     if (d->mode == CCB_PHOTO_RIGID) {
-        CCB_REQUIRE(d->d_pose && d->pose_partials, CCB_ERR_ARG, "photo_loss_bwd: d_pose/pose_partials null");
+        CCB_REQUIRE(d->d_pose, CCB_ERR_ARG, "photo_loss_bwd: d_pose null");
+        CCB_REQUIRE_WORK("photo_loss_bwd", "pose_partials", d->pose_partials, d->pose_partials_floats,
+                         ccb_photo_pose_partials_floats(d));
         rc = launch_bwd_masking<CCB_PHOTO_RIGID>(a, ss, sf.gmask || !d->has_mask, st);
         if (rc) return rc;
         int nw = d->B * d->R;

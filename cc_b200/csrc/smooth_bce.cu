@@ -322,7 +322,8 @@ extern "C" int ccb_smooth_fwd(const ccb_smooth_desc* d, ccb_stream_t stream) {
     SmoothArgs a;
     int rc = smooth_args(d, a, false);
     if (rc) return rc;
-    CCB_REQUIRE(d->partials && d->loss, CCB_ERR_ARG, "smooth_fwd: partials/loss null");
+    CCB_REQUIRE(d->loss, CCB_ERR_ARG, "smooth_fwd: loss null");
+    CCB_REQUIRE_WORK("smooth_fwd", "partials", d->partials, d->partials_floats, ccb_smooth_partials_floats(d));
     dim3 grid(a.t.blk_off[d->nlevels]);
     if (d->kind == CCB_SMOOTH_EDGE) {
         CCB_LAUNCH(smooth_fwd_kernel<CCB_SMOOTH_EDGE>, grid, dim3(PNT), 0, stream, a);
@@ -372,7 +373,8 @@ extern "C" int ccb_bce_fwd(const ccb_bce_desc* d, ccb_stream_t stream) {
     BceArgs a;
     int rc = bce_args(d, a, false);
     if (rc) return rc;
-    CCB_REQUIRE(d->partials && d->loss, CCB_ERR_ARG, "bce_fwd: partials/loss null");
+    CCB_REQUIRE(d->loss, CCB_ERR_ARG, "bce_fwd: loss null");
+    CCB_REQUIRE_WORK("bce_fwd", "partials", d->partials, d->partials_floats, ccb_bce_partials_floats(d));
     dim3 grid(a.t.blk_off[d->nlevels]);
     if (d->kind == CCB_BCE_ONES) {
         CCB_LAUNCH(bce_fwd_kernel<CCB_BCE_ONES>, grid, dim3(PNT), 0, stream, a);

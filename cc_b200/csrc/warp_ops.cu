@@ -424,6 +424,7 @@ static int warp_common(WarpArgs& a, const float* depth, const float* pose, int p
 }
 
 extern "C" long long ccb_warp_pose_partials_floats(int B, int h, int w) {
+    if (B < 1 || h < 1 || w < 1) return -1;
     return (long long)B * cdiv(h * w, WNT) * 12;
 }
 
@@ -443,11 +444,12 @@ extern "C" int ccb_inverse_warp_fwd(const float* img, const float* depth, const 
 extern "C" int ccb_inverse_warp_bwd(const float* img, const float* depth, const float* pose, int pose_stride,
                                     const float* K, const float* Kinv, int B, int h, int w, int rotation_mode,
                                     int padding_mode, const float* grad_out, float* d_depth, float* d_pose,
-                                    float* pose_partials, ccb_stream_t stream) {
+                                    float* pose_partials, long long pose_partials_floats, ccb_stream_t stream) {
     WarpArgs a;
     int rc = warp_common(a, depth, pose, pose_stride, K, Kinv, B, h, w, rotation_mode, padding_mode);
     if (rc) return rc;
-    CCB_REQUIRE(img && grad_out && d_depth && d_pose && pose_partials, CCB_ERR_ARG, "inverse_warp_bwd: null pointer");
+    CCB_REQUIRE(img && grad_out && d_depth && d_pose, CCB_ERR_ARG, "inverse_warp_bwd: null pointer");
+    CCB_REQUIRE_WORK("inverse_warp_bwd", "pose_partials", pose_partials, pose_partials_floats, ccb_warp_pose_partials_floats(B, h, w));
     a.img = img; a.grad_out = grad_out; a.d_depth = d_depth; a.d_pose = d_pose; a.pose_partials = pose_partials;
     int nblk = cdiv(h * w, WNT);
     CCB_LAUNCH(rigid_bwd_kernel<false>, dim3(nblk, B), dim3(WNT), 0, stream, a);
@@ -472,11 +474,12 @@ extern "C" int ccb_pose2flow_fwd(const float* depth, const float* pose, int pose
 extern "C" int ccb_pose2flow_bwd(const float* depth, const float* pose, int pose_stride, const float* K,
                                  const float* Kinv, int B, int h, int w, int rotation_mode, int padding_mode,
                                  const float* grad_flow, float* d_depth, float* d_pose, float* pose_partials,
-                                 ccb_stream_t stream) {
+                                 long long pose_partials_floats, ccb_stream_t stream) {
     WarpArgs a;
     int rc = warp_common(a, depth, pose, pose_stride, K, Kinv, B, h, w, rotation_mode, padding_mode);
     if (rc) return rc;
-    CCB_REQUIRE(grad_flow && d_depth && d_pose && pose_partials, CCB_ERR_ARG, "pose2flow_bwd: null pointer");
+    CCB_REQUIRE(grad_flow && d_depth && d_pose, CCB_ERR_ARG, "pose2flow_bwd: null pointer");
+    CCB_REQUIRE_WORK("pose2flow_bwd", "pose_partials", pose_partials, pose_partials_floats, ccb_warp_pose_partials_floats(B, h, w));
     a.grad_out = grad_flow; a.d_depth = d_depth; a.d_pose = d_pose; a.pose_partials = pose_partials;
     int nblk = cdiv(h * w, WNT);
     CCB_LAUNCH(rigid_bwd_kernel<true>, dim3(nblk, B), dim3(WNT), 0, stream, a);
@@ -540,11 +543,13 @@ __global__ void __launch_bounds__(WNT) flow_warp_bwd_wpp_kernel(const WarpArgs a
     }
 }
 
+// The image gradient's fixed-point scatter buffer: one accumulator per element, then max |grad_out| (pass 1 above).
+static long long scatter_words(int B, int C, int h, int w) { return (long long)B * C * h * w + 1; }
 static bool warp_per_pixel(int B, int C, int h, int w) { return C >= 16 && (long long)B * h * w < 32768; }
 static void launch_flow_warp(const WarpArgs& a, bool bwd, cudaStream_t st) {
     const long long n = (long long)a.B * a.C * a.h * a.w;
     if (bwd && a.d_img) {
-        cudaMemsetAsync(a.d_img_fx, 0, (size_t)(n + 1) * sizeof(unsigned long long), st);
+        cudaMemsetAsync(a.d_img_fx, 0, (size_t)scatter_words(a.B, a.C, a.h, a.w) * sizeof(unsigned long long), st);
         const long long nb = (n + WNT - 1) / WNT;
         CCB_LAUNCH(fx_absmax_kernel, dim3((unsigned)(nb < 4 * NUM_SMS ? nb : 4 * NUM_SMS)), dim3(WNT), 0, st, a, n);
     }
@@ -572,9 +577,10 @@ extern "C" int ccb_flow_warp_fwd(const float* img, const float* flow, int B, int
 
 extern "C" int ccb_flow_warp_bwd(const float* img, const float* flow, int B, int C, int h, int w,
                                  int padding_mode, const float* grad_out, float* d_flow, float* d_img,
-                                 unsigned long long* work, ccb_stream_t stream) {
+                                 unsigned long long* work, long long work_words, ccb_stream_t stream) {
     CCB_REQUIRE(img && flow && grad_out, CCB_ERR_ARG, "flow_warp_bwd: null pointer");
-    CCB_REQUIRE(!d_img || work, CCB_ERR_ARG, "flow_warp_bwd: d_img needs the fixed-point workspace");
+    CCB_REQUIRE(B >= 1 && C >= 1 && h >= 1 && w >= 1, CCB_ERR_ARG, "flow_warp_bwd: bad size");
+    CCB_REQUIRE_WORK("flow_warp_bwd", "work", work, work_words, d_img ? scatter_words(B, C, h, w) : 0);
     WarpArgs a;
     memset(&a, 0, sizeof(a));
     a.img = img; a.flow = flow; a.grad_out = grad_out; a.d_flow = d_flow; a.d_img = d_img; a.d_img_fx = work;
@@ -595,9 +601,10 @@ extern "C" int ccb_featwarp_fwd(const float* x, const float* flow, int B, int C,
 }
 
 extern "C" int ccb_featwarp_bwd(const float* x, const float* flow, int B, int C, int h, int w, const float* grad_out,
-                                float* d_flow, float* d_x, unsigned long long* work, ccb_stream_t stream) {
+                                float* d_flow, float* d_x, unsigned long long* work, long long work_words, ccb_stream_t stream) {
     CCB_REQUIRE(x && flow && grad_out, CCB_ERR_ARG, "featwarp_bwd: null pointer");
-    CCB_REQUIRE(!d_x || work, CCB_ERR_ARG, "featwarp_bwd: d_x needs the fixed-point workspace");
+    CCB_REQUIRE(B >= 1 && C >= 1 && h >= 1 && w >= 1, CCB_ERR_ARG, "featwarp_bwd: bad size");
+    CCB_REQUIRE_WORK("featwarp_bwd", "work", work, work_words, d_x ? scatter_words(B, C, h, w) : 0);
     WarpArgs a;
     memset(&a, 0, sizeof(a));
     a.img = x; a.flow = flow; a.grad_out = grad_out; a.d_flow = d_flow; a.d_img = d_x; a.d_img_fx = work;
@@ -622,9 +629,17 @@ extern "C" int ccb_ssim_fwd(const float* img1, const float* img2, int planes, in
     return check_launch("ssim_fwd");
 }
 
+extern "C" long long ccb_ssim_bwd_workspace_floats(int planes, int h, int w) {
+    if (planes < 1 || h < 1 || w < 1) return -1;
+    return 5LL * planes * h * w;
+}
+
 extern "C" int ccb_ssim_bwd(const float* img1, const float* img2, int planes, int h, int w, const float* taps_host,
-                            const float* grad_out, float* d_img1, float* d_img2, float* work, ccb_stream_t stream) {
-    CCB_REQUIRE(img1 && img2 && grad_out && work && taps_host, CCB_ERR_ARG, "ssim_bwd: null pointer");
+                            const float* grad_out, float* d_img1, float* d_img2, float* work, long long work_floats,
+                            ccb_stream_t stream) {
+    CCB_REQUIRE(img1 && img2 && grad_out && taps_host, CCB_ERR_ARG, "ssim_bwd: null pointer");
+    CCB_REQUIRE(planes >= 1 && h >= 1 && w >= 1, CCB_ERR_ARG, "ssim_bwd: bad size");
+    CCB_REQUIRE_WORK("ssim_bwd", "work", work, work_floats, ccb_ssim_bwd_workspace_floats(planes, h, w));
     SsimArgs a;
     memset(&a, 0, sizeof(a));
     a.x = img1; a.y = img2; a.gout = grad_out; a.dx = d_img1; a.dy = d_img2; a.work = work;

@@ -137,8 +137,7 @@ def motion_mask_counts(emask, flow_cam, flow_fwd, obj_map_gt, semantic_map_gt, T
     Hg, Wg = int(obj.shape[1]), int(obj.shape[2])
     assert flow_cam.shape == (B, 2, h, w) and flow_fwd.shape == (B, 2, h, w), (flow_cam.shape, flow_fwd.shape)
     assert obj.shape == (B, Hg, Wg) and sem.shape == (B, Hg, Wg), (obj.shape, sem.shape)
-    nbytes = int(_lib.call('ccb_mask_iou_workspace_bytes', B, h, w, Hg, Wg))
-    work = torch.empty(max(nbytes, 0) // 8 + 1, device=emask.device, dtype=torch.int64)
+    work, nbytes = _lib.workspace('ccb_mask_iou_workspace_bytes', B, h, w, Hg, Wg, like=emask)
     n = torch.empty(B, 3, 4, device=emask.device, dtype=torch.int64)
     masks = torch.empty(B, 4, h, w, device=emask.device) if want_masks else None
     _lib.call('ccb_mask_iou', emask, flow_cam, flow_fwd, obj, sem, B, C, h, w, Hg, Wg, float(THRESH), 26, masks, work, nbytes, n,
@@ -207,8 +206,7 @@ def flow_colors(flow):
     flow = _lib.f32(flow)
     B, P, two, H, W = (int(v) for v in flow.shape)
     assert two == 2, flow.shape
-    nbytes = int(_lib.call('ccb_flow_color_workspace_bytes', B, P, H, W))
-    work = torch.empty(max(nbytes, 0) // 8 + 1, device=flow.device, dtype=torch.int64)
+    work, nbytes = _lib.workspace('ccb_flow_color_workspace_bytes', B, P, H, W, like=flow)
     out = torch.empty(B, 3, P * H, W, device=flow.device, dtype=torch.uint8)
     _lib.call('ccb_flow_color', flow, B, P, H, W, work, nbytes, out, flow)
     return out
@@ -263,8 +261,7 @@ def kitti_flow_errors(gt_png, pred_png):
         gt, pred = gt[None], pred[None]
     assert gt.shape == pred.shape and gt.shape[-1] == 3 and gt.dtype == torch.uint16, (gt.shape, pred.shape, gt.dtype)
     B, H, W = (int(v) for v in gt.shape[:3])
-    nbytes = int(_lib.call('ccb_kitti_flow_errors_workspace_bytes', B, H, W))
-    work = torch.empty(max(nbytes, 0) // 8 + 1, device=dev, dtype=torch.int64)
+    work, nbytes = _lib.workspace('ccb_kitti_flow_errors_workspace_bytes', B, H, W, like=gt)
     out = torch.empty(B, 2, device=dev, dtype=torch.float64)
     counts = torch.empty(B, 2, device=dev, dtype=torch.int64)
     _lib.call('ccb_kitti_flow_errors', gt, pred, B, H, W, work, nbytes, out, counts, gt)

@@ -103,9 +103,7 @@ def resize_frames(src, h, w):
     Hs, Ws = src.shape[-3], src.shape[-2]
     N = src.numel() // (Hs * Ws * 3)
     dst = torch.empty(tuple(src.shape[:-3]) + (h, w, 3), dtype=torch.uint8, device=src.device)
-    nb = _lib.call('ccb_resize_u8_workspace_bytes', N, Hs, Ws, h, w)
-    assert nb >= 0, 'resize_frames: bad sizes'
-    work = torch.empty(max(nb, 1), dtype=torch.uint8, device=src.device)
+    work, nb = _lib.workspace('ccb_resize_u8_workspace_bytes', N, Hs, Ws, h, w, like=src)
     _lib.call('ccb_resize_u8', src, dst, N, Hs, Ws, h, w, work, nb, src)
     return dst
 
@@ -116,8 +114,7 @@ def normalize_local(frames):
     B, _, H, W = frames[0].shape
     F = len(frames)
     stats = torch.empty(B, 3, 2, device=frames[0].device)
-    nb = _lib.call('ccb_normalize_local_workspace_bytes', B, H, W)
-    work = torch.empty(nb, dtype=torch.uint8, device=frames[0].device)
+    work, nb = _lib.workspace('ccb_normalize_local_workspace_bytes', B, H, W, like=frames[0])
     _lib.call('ccb_normalize_local', frames, B, F, H, W, stats, work, nb, frames[0])
     return stats
 

@@ -39,8 +39,8 @@ class _InverseWarp(torch.autograd.Function):
         g = _lib.f32(g)
         d_depth = torch.empty_like(depth)
         d_pose = torch.empty_like(pose)
-        part = torch.empty(_lib.call('ccb_warp_pose_partials_floats', B, h, w), device=img.device)
-        _lib.call('ccb_inverse_warp_bwd', img, depth, pose, 6, K, Kinv, B, h, w, rot, pad, g, d_depth, d_pose, part, img)
+        part, pf = _lib.workspace('ccb_warp_pose_partials_floats', B, h, w, like=img)
+        _lib.call('ccb_inverse_warp_bwd', img, depth, pose, 6, K, Kinv, B, h, w, rot, pad, g, d_depth, d_pose, part, pf, img)
         return None, d_depth, d_pose, None, None, None, None
 
 
@@ -63,8 +63,8 @@ class _Pose2Flow(torch.autograd.Function):
         g = _lib.f32(g)
         d_depth = torch.empty_like(depth)
         d_pose = torch.empty_like(pose)
-        part = torch.empty(_lib.call('ccb_warp_pose_partials_floats', B, h, w), device=depth.device)
-        _lib.call('ccb_pose2flow_bwd', depth, pose, 6, K, Kinv, B, h, w, rot, pad, g, d_depth, d_pose, part, depth)
+        part, pf = _lib.workspace('ccb_warp_pose_partials_floats', B, h, w, like=depth)
+        _lib.call('ccb_pose2flow_bwd', depth, pose, 6, K, Kinv, B, h, w, rot, pad, g, d_depth, d_pose, part, pf, depth)
         return d_depth, d_pose, None, None, None, None
 
 
@@ -86,8 +86,8 @@ class _FlowWarp(torch.autograd.Function):
         g = _lib.f32(g)
         d_flow = torch.empty_like(flow) if ctx.needs_input_grad[1] else None
         d_img = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
-        work = _lib.scatter_workspace(img) if d_img is not None else None
-        _lib.call('ccb_flow_warp_bwd', img, flow, B, Cc, h, w, ctx.pad, g, d_flow, d_img, work, img)
+        work, words = _lib.scatter_workspace(img) if d_img is not None else (None, 0)
+        _lib.call('ccb_flow_warp_bwd', img, flow, B, Cc, h, w, ctx.pad, g, d_flow, d_img, work, words, img)
         return d_img, d_flow, None
 
 

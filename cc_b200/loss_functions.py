@@ -82,7 +82,7 @@ class _PhotoLoss(torch.autograd.Function):
         if gm:
             _set_levels(d.gmask, gm, 'gmask')
         scal = torch.empty(L * R * 4, device=dev)
-        part = torch.empty(max(1, _lib.call('ccb_photo_partials_floats', d)), device=dev)
+        part, d.partials_floats = _lib.workspace('ccb_photo_partials_floats', d, like=scal)
         loss = torch.empty(1, device=dev)
         d.scal, d.partials, d.loss = _lib.ptr(scal), _lib.ptr(part), _lib.ptr(loss)
         _lib.call('ccb_photo_loss_fwd', d, loss)
@@ -103,7 +103,7 @@ class _PhotoLoss(torch.autograd.Function):
         if mode == _lib.PHOTO_RIGID:
             d_pose = torch.empty(B, R, 6, device=dev)
             d_depth = [torch.empty(B, 1, h, w, device=dev) for (h, w) in sizes]
-            part = torch.empty(max(1, _lib.call('ccb_photo_pose_partials_floats', d)), device=dev)
+            part, d.pose_partials_floats = _lib.workspace('ccb_photo_pose_partials_floats', d, like=d_pose)
             d.d_pose, d.pose_partials = _lib.ptr(d_pose), _lib.ptr(part)
             _set_levels(d.d_depth, d_depth, 'd_depth')
             grads = [d_pose] + d_depth
@@ -232,7 +232,7 @@ class _SmoothLoss(torch.autograd.Function):
         _set_levels(d.pred, ps, 'pred')
         if cfg['kind'] == _lib.SMOOTH_EDGE:
             _set_levels(d.img, cfg['img'], 'img')
-        part = torch.empty(max(1, _lib.call('ccb_smooth_partials_floats', d)), device=dev)
+        part, d.partials_floats = _lib.workspace('ccb_smooth_partials_floats', d, like=ps[0])
         loss = torch.empty(1, device=dev)
         d.partials, d.loss = _lib.ptr(part), _lib.ptr(loss)
         _lib.call('ccb_smooth_fwd', d, loss)
@@ -288,7 +288,7 @@ class _BceLoss(torch.autograd.Function):
                 ts = [_lib.f32(t) for t in cfg[name]]
                 keep += ts
                 _set_levels(getattr(d, name), ts, name)
-        part = torch.empty(max(1, _lib.call('ccb_bce_partials_floats', d)), device=dev)
+        part, d.partials_floats = _lib.workspace('ccb_bce_partials_floats', d, like=ms[0])
         loss = torch.empty(1, device=dev)
         d.partials, d.loss = _lib.ptr(part), _lib.ptr(loss)
         _lib.call('ccb_bce_fwd', d, loss)
@@ -412,12 +412,11 @@ def _flow_metrics(gt, pred_a, pred_b=None, mask=None, thresh=0.5, tau=(3, 0.05),
         pred_b, mask = _lib.f32(pred_b), _lib.f32(mask)
         assert pred_b.shape == pred_a.shape and mask.shape[1] == 1
         hm, wm = int(mask.shape[2]), int(mask.shape[3])
-    work = torch.empty(int(_lib.call('ccb_flow_metrics_workspace_bytes', B, Hg, Wg) // 8) + 1, device=gt.device,
-                       dtype=torch.float64)
+    work, nbytes = _lib.workspace('ccb_flow_metrics_workspace_bytes', B, Hg, Wg, like=gt)
     out = torch.empty(4, device=gt.device)
     emap = torch.empty(B, Hg, Wg, device=gt.device) if want_map else None
     _lib.call('ccb_flow_metrics', gt, pred_a, pred_b, mask, B, int(nc), int(Hg), int(Wg), hp, wp, hm, wm, float(thresh),
-              float(tau[0]), float(tau[1]), emap, work, out, gt)
+              float(tau[0]), float(tau[1]), emap, work, nbytes, out, gt)
     return out, emap
 
 
@@ -449,8 +448,7 @@ def compute_errors(gt, pred, crop=True):
     radix select on the device)."""
     gt, pred = _lib.f32(gt), _lib.f32(pred)
     B, H, W = gt.shape
-    work = torch.empty(int(_lib.call('ccb_depth_errors_workspace_bytes', B, H, W) // 8) + 1, device=gt.device,
-                       dtype=torch.float64)
+    work, nbytes = _lib.workspace('ccb_depth_errors_workspace_bytes', B, H, W, like=gt)
     out = torch.empty(6, device=gt.device)
-    _lib.call('ccb_depth_errors', gt, pred, B, H, W, int(bool(crop)), work, out, gt)
+    _lib.call('ccb_depth_errors', gt, pred, B, H, W, int(bool(crop)), work, nbytes, out, gt)
     return [out[i] for i in range(6)]

@@ -119,8 +119,7 @@ def _act_bwd_bias(g, y, act, slope, db):
     B, Cc = g.shape[0], g.shape[1]
     plane = g.numel() // (B * Cc)
     dz = torch.empty_like(g) if act != _lib.ACT_NONE else g
-    wf = _lib.call('ccb_act_bwd_bias_workspace_floats', B, Cc, plane) if db is not None else 0
-    work = torch.empty(wf, device=g.device, dtype=torch.float32) if wf else None
+    work, wf = _lib.workspace('ccb_act_bwd_bias_workspace_floats', B, Cc, plane, like=g) if db is not None else (None, 0)
     _lib.call('ccb_act_bwd_bias', g, y, dz if act != _lib.ACT_NONE else None, db, B, Cc, plane, act, slope, work, wf, g)
     return dz
 
@@ -222,8 +221,8 @@ class _BatchNormFn(torch.autograd.Function):
         B, Cc, h, w = x.shape
         y = torch.empty_like(x)
         stats = torch.empty(Cc, 2, device=x.device) if training else None
-        work = torch.empty(_lib.call('ccb_bn_workspace_floats', B, Cc, h * w), device=x.device) if training else None
-        _lib.call('ccb_bn_fwd', x, gamma, beta, y, stats, rm, rv, B, Cc, h * w, eps, momentum, int(training), work, x)
+        work, wf = _lib.workspace('ccb_bn_workspace_floats', B, Cc, h * w, like=x) if training else (None, 0)
+        _lib.call('ccb_bn_fwd', x, gamma, beta, y, stats, rm, rv, B, Cc, h * w, eps, momentum, int(training), work, wf, x)
         ctx.save_for_backward(x, gamma, stats)
         ctx.training = training
         return y
@@ -238,8 +237,8 @@ class _BatchNormFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dg, g_direct = _grad_slot(ctx.params[0], gamma)
         db, b_direct = _grad_slot(ctx.params[1], gamma)
-        work = torch.empty(_lib.call('ccb_bn_workspace_floats', B, Cc, h * w), device=x.device)
-        _lib.call('ccb_bn_bwd', x, g, gamma, stats, dx, dg, db, B, Cc, h * w, work, x)
+        work, wf = _lib.workspace('ccb_bn_workspace_floats', B, Cc, h * w, like=x)
+        _lib.call('ccb_bn_bwd', x, g, gamma, stats, dx, dg, db, B, Cc, h * w, work, wf, x)
         _grad_done(ctx.params[0] if g_direct else None, ctx.params[1] if b_direct else None)
         return dx, (None if g_direct else dg), (None if b_direct else db), None, None, None, None, None
 
@@ -369,8 +368,7 @@ class _Corr81Fn(torch.autograd.Function):
         f1, f2 = _lib.f32(f1), _lib.f32(f2)
         B, Cc, h, w = f1.shape
         out = torch.empty(B, 81, h, w, device=f1.device, dtype=torch.float32)
-        wf = _lib.call('ccb_corr81_fwd_workspace_floats', B, Cc, h, w)
-        work = torch.empty(wf, device=f1.device, dtype=torch.float32) if wf else None
+        work, wf = _lib.workspace('ccb_corr81_fwd_workspace_floats', B, Cc, h, w, like=f1)
         _lib.call('ccb_corr81_fwd', f1, f2, out, B, Cc, h, w, int(reversed_), work, wf, f1)
         ctx.save_for_backward(f1, f2)
         ctx.rev = int(reversed_)
@@ -384,8 +382,8 @@ class _Corr81Fn(torch.autograd.Function):
         d1 = torch.empty_like(f1) if ctx.needs_input_grad[0] else None
         d2 = torch.empty_like(f2) if ctx.needs_input_grad[1] else None
         if d1 is not None or d2 is not None:
-            work = torch.empty(B * 81 * h * w, device=f1.device) if d2 is not None else None
-            _lib.call('ccb_corr81_bwd', f1, f2, g, d1, d2, B, Cc, h, w, ctx.rev, work, f1)
+            work, wf = _lib.workspace('ccb_corr81_bwd_workspace_floats', B, Cc, h, w, like=f1) if d2 is not None else (None, 0)
+            _lib.call('ccb_corr81_bwd', f1, f2, g, d1, d2, B, Cc, h, w, ctx.rev, work, wf, f1)
         return d1, d2, None
 
 
@@ -431,8 +429,8 @@ class _FeatWarpFn(torch.autograd.Function):
         g = _lib.f32(g)
         dx = torch.zeros_like(x) if ctx.needs_input_grad[0] else None
         df = torch.empty_like(flo) if ctx.needs_input_grad[1] else None
-        work = _lib.scatter_workspace(x) if dx is not None else None
-        _lib.call('ccb_featwarp_bwd', x, flo, B, Cc, h, w, g, df, dx, work, x)
+        work, words = _lib.scatter_workspace(x) if dx is not None else (None, 0)
+        _lib.call('ccb_featwarp_bwd', x, flo, B, Cc, h, w, g, df, dx, work, words, x)
         return dx, df
 
 

@@ -45,8 +45,8 @@ class _Ssim(torch.autograd.Function):
         g = _lib.f32(g)
         d1 = torch.empty_like(a) if ctx.needs_input_grad[0] else None
         d2 = torch.empty_like(b) if ctx.needs_input_grad[1] else None
-        work = torch.empty(5 * a.numel(), device=a.device)
-        _lib.call('ccb_ssim_bwd', a, b, Bn * Cc, h, w, taps13(), g, d1, d2, work, a)
+        work, wf = _lib.workspace('ccb_ssim_bwd_workspace_floats', Bn * Cc, h, w, like=a)
+        _lib.call('ccb_ssim_bwd', a, b, Bn * Cc, h, w, taps13(), g, d1, d2, work, wf, a)
         return d1, d2
 
 

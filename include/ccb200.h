@@ -11,7 +11,13 @@
  *   - every entry point is asynchronous on `stream` (a cudaStream_t), never synchronises the host,
  *     never throws, and returns CCB_OK or a negative ccb_status; ccb_last_error_string() explains it;
  *   - shape errors that the reference reports as Python AssertionError (inverse_warp.py:23-28) are
- *     raised by the Python mirror (cc_b200/*.py) before the call; the ABI re-checks what it needs.
+ *     raised by the Python mirror (cc_b200/*.py) before the call; the ABI re-checks what it needs;
+ *   - every scratch buffer (a parameter or descriptor field named work, partials or *_partials) is followed by its size
+ *     in the unit of its pointer type: float* -> *_floats, unsigned long long* -> *_words, void* -> *_bytes.  The size
+ *     needed is what the entry point's size query returns for the same arguments (the warps' fixed-point scatter buffer
+ *     has no query: it needs the image gradient's element count + 1 words).  A smaller size returns CCB_ERR_ARG, naming
+ *     the entry point and the buffer, and launches nothing; a larger one changes nothing.  NULL with size 0 is allowed
+ *     exactly where the need is 0.  A size query returns -1 for invalid sizes.  void* workspaces must be 8-byte aligned.
  *
  * Each entry point names the reference interface it replaces (file:line relative to the reference).
  */
@@ -94,7 +100,8 @@ typedef struct ccb_photo_desc {
     float* vo[CCB_MAX_LEVELS];       /* [B,R,h,w]  valid * (1 - occ) */
     float* scal;                     /* [nlevels,R,4] : c_l, oob, sum_valid, level-ref loss */
     /* forward outputs / workspace */
-    float* partials;                 /* [ccb_photo_partials_floats()] */
+    float* partials;                 /* ccb_photo_partials_floats() */
+    long long partials_floats;
     float* loss;                     /* [1] */
     float* target[CCB_MAX_LEVELS];   /* consensus: [B,1,h,w] 0/1 */
     /* backward inputs / outputs / workspace */
@@ -103,7 +110,8 @@ typedef struct ccb_photo_desc {
     float* d_flow[CCB_MAX_LEVELS][CCB_MAX_REFS];    /* flow:  [B,2,h,w] */
     float* d_mask[CCB_MAX_LEVELS];                  /* [B,R,h,w] (has_mask) */
     float* d_pose;                                  /* rigid: [B,R,6] */
-    float* pose_partials;            /* [ccb_photo_pose_partials_floats()] */
+    float* pose_partials;            /* rigid: ccb_photo_pose_partials_floats() */
+    long long pose_partials_floats;
 } ccb_photo_desc;
 
 long long ccb_photo_partials_floats(const ccb_photo_desc* d);
@@ -120,20 +128,21 @@ int ccb_consensus_targets(const ccb_photo_desc* d, ccb_stream_t stream);
 int ccb_inverse_warp_fwd(const float* img, const float* depth, const float* pose, int pose_stride,
                          const float* K, const float* Kinv, int B, int h, int w, int rotation_mode,
                          int padding_mode, float* out, ccb_stream_t stream);
-/* grads wrt depth [B,h,w] and pose [B,6] (contiguous); pose_partials: B*ntiles*12 floats. */
+/* grads wrt depth [B,h,w] and pose [B,6] (contiguous); pose_partials: ccb_warp_pose_partials_floats(B, h, w). */
 int ccb_inverse_warp_bwd(const float* img, const float* depth, const float* pose, int pose_stride,
                          const float* K, const float* Kinv, int B, int h, int w, int rotation_mode,
                          int padding_mode, const float* grad_out, float* d_depth, float* d_pose,
-                         float* pose_partials, ccb_stream_t stream);
+                         float* pose_partials, long long pose_partials_floats, ccb_stream_t stream);
 long long ccb_warp_pose_partials_floats(int B, int h, int w);
 /* flow_warp (inverse_warp.py:164-192): img [B,C,h,w], flow [B,2,h,w]; padding zeros|border. */
 int ccb_flow_warp_fwd(const float* img, const float* flow, int B, int C, int h, int w,
                       int padding_mode, float* out, ccb_stream_t stream);
 /* d_flow [B,2,h,w] (may be NULL), d_img [B,C,h,w] (may be NULL; the gradient is ADDED to it).  With d_img, work holds
- * B*C*h*w + 1 64-bit words: the image gradient is a scatter, summed in fixed point so that it is the same on every run. */
+ * B*C*h*w + 1 words (0 without): the image gradient is a scatter, summed in fixed point so that it is the same on every
+ * run. */
 int ccb_flow_warp_bwd(const float* img, const float* flow, int B, int C, int h, int w,
                       int padding_mode, const float* grad_out, float* d_flow, float* d_img,
-                      unsigned long long* work, ccb_stream_t stream);
+                      unsigned long long* work, long long work_words, ccb_stream_t stream);
 /* pose2flow (inverse_warp.py:195-220): -> flow [B,2,h,w]; padding_mode CCB_PAD_NONE | CCB_PAD_ZEROS. */
 int ccb_pose2flow_fwd(const float* depth, const float* pose, int pose_stride, const float* K,
                       const float* Kinv, int B, int h, int w, int rotation_mode, int padding_mode,
@@ -141,14 +150,16 @@ int ccb_pose2flow_fwd(const float* depth, const float* pose, int pose_stride, co
 int ccb_pose2flow_bwd(const float* depth, const float* pose, int pose_stride, const float* K,
                       const float* Kinv, int B, int h, int w, int rotation_mode, int padding_mode,
                       const float* grad_flow, float* d_depth, float* d_pose, float* pose_partials,
-                      ccb_stream_t stream);
+                      long long pose_partials_floats, ccb_stream_t stream);
 
 /* ssim map (ssim.py:68-76, window 13, sigma 1.5, zero padding): img1,img2,out [planes,h,w]. */
 int ccb_ssim_fwd(const float* img1, const float* img2, int planes, int h, int w, const float* taps_host,
                  float* out, ccb_stream_t stream);
-/* d_img1/d_img2 may be NULL; work: 5*planes*h*w floats. */
+/* d_img1/d_img2 may be NULL. */
+long long ccb_ssim_bwd_workspace_floats(int planes, int h, int w);
 int ccb_ssim_bwd(const float* img1, const float* img2, int planes, int h, int w, const float* taps_host,
-                 const float* grad_out, float* d_img1, float* d_img2, float* work, ccb_stream_t stream);
+                 const float* grad_out, float* d_img1, float* d_img2, float* work, long long work_floats,
+                 ccb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Smoothness (loss_functions.py:287-341) for a list of predictions [B,C,h_l,w_l].
@@ -161,7 +172,8 @@ typedef struct ccb_smooth_desc {
     int h[CCB_MAX_LEVELS], w[CCB_MAX_LEVELS];
     const float* img[CCB_MAX_LEVELS];
     const float* pred[CCB_MAX_LEVELS];
-    float* partials;          /* [ccb_smooth_partials_floats()] */
+    float* partials;          /* ccb_smooth_partials_floats() */
+    long long partials_floats;
     float* loss;              /* [1] */
     const float* grad_out;    /* [1] */
     float* d_pred[CCB_MAX_LEVELS];
@@ -186,7 +198,8 @@ typedef struct ccb_bce_desc {
     const float* census_fwd[CCB_MAX_LEVELS];  /* [B,2,h,w] */
     const float* target_bwd[CCB_MAX_LEVELS];  /* [B,1,h,w] */
     const float* target_fwd[CCB_MAX_LEVELS];  /* [B,1,h,w] */
-    float* partials;
+    float* partials;          /* ccb_bce_partials_floats() */
+    long long partials_floats;
     float* loss;
     const float* grad_out;
     float* d_mask[CCB_MAX_LEVELS];
@@ -245,7 +258,8 @@ int ccb_conv2d_dgrad(const ccb_conv_desc* d, const float* dy, const float* w, co
 int ccb_conv2d_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
                      float* work, long long work_floats, ccb_stream_t stream);
 /* fused: dz = dy * act'(y) (not touched when act == CCB_ACT_NONE; in place allowed) and, when db != NULL,
- * db[c] = sum over (b, pixel) of dz - one pass over the gradient.  work: ccb_act_bwd_bias_workspace_floats() floats. */
+ * db[c] = sum over (b, pixel) of dz - one pass over the gradient.  work: ccb_act_bwd_bias_workspace_floats() with db,
+ * 0 without. */
 long long ccb_act_bwd_bias_workspace_floats(int B, int C, int plane);
 int ccb_act_bwd_bias(const float* dy, const float* y, float* dz, float* db, int B, int C, int plane, int act, float slope,
                      float* work, long long work_floats, ccb_stream_t stream);
@@ -256,14 +270,14 @@ int ccb_act_bwd_bias(const float* dy, const float* y, float* dz, float* db, int 
  * zero padded, divided by C) with the reference's channel permutation baked in (reversed=0: idx_fwd,
  * 1: idx_bwd, :56-59).  f1,f2 [B,C,h,w] -> out [B,81,h,w].   d_f1 / d_f2 may be NULL.
  * featwarp: Model.warp :287-321 = grid_sample(x, grid+flow, padding border, align_corners False). */
-/* work: ccb_corr81_fwd_workspace_floats() floats (per-channel-chunk partial sums; 0 when one CTA per tile sums all
- * channels) */
+/* work: per-channel-chunk partial sums (0 when one CTA per tile sums all channels) */
 long long ccb_corr81_fwd_workspace_floats(int B, int C, int h, int w);
 int ccb_corr81_fwd(const float* f1, const float* f2, float* out, int B, int C, int h, int w, int reversed,
                    float* work, long long work_floats, ccb_stream_t stream);
-/* work: B*81*h*w floats (the mirrored gradient planes), required when d_f2 != NULL */
+/* work: the mirrored gradient planes with d_f2, 0 without */
+long long ccb_corr81_bwd_workspace_floats(int B, int C, int h, int w);
 int ccb_corr81_bwd(const float* f1, const float* f2, const float* grad_out, float* d_f1, float* d_f2, int B,
-                   int C, int h, int w, int reversed, float* work, ccb_stream_t stream);
+                   int C, int h, int w, int reversed, float* work, long long work_floats, ccb_stream_t stream);
 /* FlowNetC6 operator (models/FlowNetC6.py).
  * corr441d: correlate() :18-30 (third-party spatial_correlation_sample, kernel 1, patch 21, stride 1, padding 0,
  * dilation_patch 2, divided by C) with corr_activation LeakyReLU(0.1) :54,112 fused:
@@ -275,18 +289,19 @@ int ccb_corr441d_bwd(const float* f1, const float* f2, const float* out, const f
                      int B, int C, int h, int w, ccb_stream_t stream);
 int ccb_featwarp_fwd(const float* x, const float* flow, int B, int C, int h, int w, float* out,
                      ccb_stream_t stream);
-/* d_flow / d_x may be NULL; the gradient is ADDED to d_x; with d_x, work holds B*C*h*w + 1 64-bit words (as flow_warp_bwd) */
+/* d_flow / d_x may be NULL; the gradient is ADDED to d_x; with d_x, work holds B*C*h*w + 1 words (as flow_warp_bwd) */
 int ccb_featwarp_bwd(const float* x, const float* flow, int B, int C, int h, int w, const float* grad_out,
-                     float* d_flow, float* d_x, unsigned long long* work, ccb_stream_t stream);
+                     float* d_flow, float* d_x, unsigned long long* work, long long work_words, ccb_stream_t stream);
 
 /* BatchNorm2d over [B,C,plane] (DispResNet6.py:45-52).  training: batch statistics, stats[C][2] =
  * {mean, invstd} saved for backward, running stats updated in place (momentum, unbiased var). */
-long long ccb_bn_workspace_floats(int B, int C, int plane);   /* `work` size for both calls */
+long long ccb_bn_workspace_floats(int B, int C, int plane);   /* `work` of both calls; bn_fwd needs 0 in eval mode */
 int ccb_bn_fwd(const float* x, const float* gamma, const float* beta, float* y, float* stats,
                float* running_mean, float* running_var, int B, int C, int plane, float eps, float momentum,
-               int training, float* work, ccb_stream_t stream);
+               int training, float* work, long long work_floats, ccb_stream_t stream);
 int ccb_bn_bwd(const float* x, const float* dy, const float* gamma, const float* stats, float* dx,
-               float* dgamma, float* dbeta, int B, int C, int plane, float* work, ccb_stream_t stream);
+               float* dgamma, float* dbeta, int B, int C, int plane, float* work, long long work_floats,
+               ccb_stream_t stream);
 /* bilinear x2 upsample, align_corners=False (DispResNet6.py:174; back2future.py:60): [planes,h,w] -> [planes,2h,2w] */
 int ccb_upsample2x_fwd(const float* x, float* y, int planes, int h, int w, ccb_stream_t stream);
 int ccb_upsample2x_bwd(const float* dy, float* dx, int planes, int h, int w, ccb_stream_t stream);
@@ -312,17 +327,16 @@ int ccb_adam_step_ranges(float* params, const float* grads, float* exp_avg, floa
  *   Otherwise compute_all_epes :409-427 (mask [B,1,hm,wm], composite by mask > thresh at prediction resolution,
  *   ground truth split at its own): out4 = {all, rigid, non-rigid EPE, outliers}.
  *   epe_map (optional, [B,Hg,Wg]) receives flow_diff :355-365 of the (composited) prediction.
- *   work: ccb_flow_metrics_workspace_bytes(B, Hg, Wg) bytes, 8-byte aligned.
  * ccb_depth_errors: compute_errors :430-467 on gt, pred [B,H,W]: valid = 0 < gt < 80 (inside the Garg crop when
  *   crop != 0), pred clamped to [1e-3, 80] and scaled by median(gt)/median(pred) per sample (lower medians, by radix
  *   select on the device), out6 = batch means of {abs_diff, abs_rel, sq_rel, a1, a2, a3}. */
 long long ccb_flow_metrics_workspace_bytes(int B, int Hg, int Wg);
 int ccb_flow_metrics(const float* gt, const float* pred_rigid, const float* pred_nonrigid, const float* rigidity_mask,
                      int B, int nc, int Hg, int Wg, int hp, int wp, int hm, int wm, float thresh, float tau0,
-                     float tau1, float* epe_map, void* work, float* out4, ccb_stream_t stream);
+                     float tau1, float* epe_map, void* work, long long work_bytes, float* out4, ccb_stream_t stream);
 long long ccb_depth_errors_workspace_bytes(int B, int H, int W);
-int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, int crop, void* work, float* out6,
-                     ccb_stream_t stream);
+int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, int crop, void* work, long long work_bytes,
+                     float* out6, ccb_stream_t stream);
 /* Motion segmentation scores of one sample each (test_mask.py:129-156, mask_error :224-262), no host sync.  emask
  * [B,C,h,w] is the mask net's eval output (C >= 3; channels 1 and 2 are read), flow_cam and flow [B,2,h,w], obj_map and
  * semantic_map [B,Hg,Wg] hold label values as floats.  Three rigidity masks at h x w:
@@ -337,8 +351,7 @@ int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, in
  * floor(o (n_in-1)/(n_out-1) + 0.5) per axis, in fp64.  mask_error's six numbers are tp0 = n00, fp0 = fn1 = n01,
  * fn0 = fp1 = n10, tp1 = n11.  The counts are summed with 64-bit integer atomics: integer addition is associative, so
  * every run gives the same counts.
- * masks (optional, [B,4,h,w]) receives combined, census, bare as 0/1 and soft.
- * work: ccb_mask_iou_workspace_bytes(B, h, w, Hg, Wg) bytes (-1 for bad sizes), 8-byte aligned. */
+ * masks (optional, [B,4,h,w]) receives combined, census, bare as 0/1 and soft. */
 long long ccb_mask_iou_workspace_bytes(int B, int h, int w, int Hg, int Wg);
 int ccb_mask_iou(const float* emask, const float* flow_cam, const float* flow, const float* obj_map,
                  const float* semantic_map, int B, int C, int h, int w, int Hg, int Wg, float thresh, int car_label,
@@ -358,15 +371,13 @@ int ccb_flow_submit(const float* emask, const float* flow_cam, const float* flow
 /* Middlebury flow colours (flowlib.py flow_to_image / compute_color), no host sync.  flow [B,P,2,H,W]: per image P
  * panels stacked along H as np.hstack stacks CHW arrays, normalised by ONE maximum radius -> out [B,3,P*H,W] uint8
  * levels (the reference's float image times 255).  |u| or |v| > 1e7 is unknown (black, left out of the maximum); NaN
- * pixels are black and make the maximum -1, as python's max(-1, nan) does; the colour pass runs in fp64.
- * work: ccb_flow_color_workspace_bytes(B, P, H, W) bytes (-1 for bad sizes), 8-byte aligned. */
+ * pixels are black and make the maximum -1, as python's max(-1, nan) does; the colour pass runs in fp64. */
 long long ccb_flow_color_workspace_bytes(int B, int P, int H, int W);
 int ccb_flow_color(const float* flow, int B, int P, int H, int W, void* work, long long work_bytes, unsigned char* out,
                    ccb_stream_t stream);
 /* KITTI flow scores of two 16-bit triplets each (evaluate_flow.py compute_err :44-53 on flow_read_png's decoding), no host
  * sync.  gt and pred [B,H,W,3] uint16 -> out [B,2] fp64 (aepe, Fl) and optionally counts [B,2] (outliers weighted by
- * valid_gt, sum of valid_gt).  fp64 block partials with a fixed-order finalize: the same bits on every run.
- * work: ccb_kitti_flow_errors_workspace_bytes(B, H, W) bytes (-1 for bad sizes), 8-byte aligned. */
+ * valid_gt, sum of valid_gt).  fp64 block partials with a fixed-order finalize: the same bits on every run. */
 long long ccb_kitti_flow_errors_workspace_bytes(int B, int H, int W);
 int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned short* pred, int B, int H, int W, void* work,
                           long long work_bytes, double* out, long long* counts, ccb_stream_t stream);
@@ -388,15 +399,14 @@ int ccb_rotate_frames_u8(const unsigned char* src, const double* affine, unsigne
                          ccb_stream_t stream);
 /* Scale (custom_transforms.py:120-137) = scipy.misc.imresize = Pillow resize((W, H), BILINEAR), bit-exact (8-bit
  * ImagingResample: antialiased on a downscale, 22-bit fixed-point weights, horizontal pass first, each pass rounded to
- * uint8): src [N,Hs,Ws,3] -> dst [N,H,W,3] uint8.  The weights are computed on the device into `work`
- * (ccb_resize_u8_workspace_bytes, -1 for bad sizes), so the call is asynchronous and can be captured in a graph. */
+ * uint8): src [N,Hs,Ws,3] -> dst [N,H,W,3] uint8.  The weights are computed on the device into `work`, so the call is
+ * asynchronous and can be captured in a graph. */
 long long ccb_resize_u8_workspace_bytes(int N, int Hs, int Ws, int H, int W);
 int ccb_resize_u8(const unsigned char* src, unsigned char* dst, int N, int Hs, int Ws, int H, int W, void* work,
                   long long work_bytes, ccb_stream_t stream);
 /* NormalizeLocally (custom_transforms.py:33-44) in place on F frames[f] [B,3,H,W]: per sample and channel, the mean and
  * unbiased std over all F*H*W values (fp64, deterministic), rounded to fp32, then x = (x - m) / s in fp32.  stats
- * ([B,3,2] = {mean, std}) may be NULL.  A zero std gives inf / nan, as in the reference.
- * work: ccb_normalize_local_workspace_bytes(B, H, W) bytes, 8-byte aligned. */
+ * ([B,3,2] = {mean, std}) may be NULL.  A zero std gives inf / nan, as in the reference. */
 long long ccb_normalize_local_workspace_bytes(int B, int H, int W);
 int ccb_normalize_local(float* const* frames, int B, int F, int H, int W, float* stats, void* work, long long work_bytes,
                         ccb_stream_t stream);

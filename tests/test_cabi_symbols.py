@@ -63,7 +63,7 @@ def header_structs():
 
 def _struct_fields(cls):
     """[(field, C type as far as ctypes tells it, array extents)]; a pointer field is c_void_p: any 'T*'."""
-    names = {ctypes.c_int: 'int', ctypes.c_float: 'float', ctypes.c_void_p: '*'}
+    names = {ctypes.c_int: 'int', ctypes.c_longlong: 'long long', ctypes.c_float: 'float', ctypes.c_void_p: '*'}
     out = []
     for field, t in cls._fields_:
         ext = []
