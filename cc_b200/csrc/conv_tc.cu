@@ -14,6 +14,12 @@
 //   tf32 MMAs (hi*hi + lo*hi + hi*lo) ("3xTF32", error ~2^-21).  The tensor core only sums one 32-deep stage (small
 //   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
 //   fp32 adds, so no long accumulation chain runs through the tensor core's own rounding;
+// * fprop / dgrad: the producers store the gathered A tile once, unsplit, in the order of the wgmma A register
+//   fragment (see tc_load_a); each consumer thread loads its 16 values with 4 conflict-free LDS.128, splits them and
+//   issues wgmma with A from registers (B by descriptor), so A crosses shared memory twice per stage instead of
+//   being stored twice and read three times.  The consumers load and split the next stage while the current
+//   stage's MMAs run, and take registers from the producers (setmaxnreg) to hold both.  The wgrad kernel splits both
+//   operands in its producers and reads both from shared memory;
 // * mbarrier pipeline of up to 4 stages: producers -> full[s] -> consumers (wgmma, commit group, wait, fp32 add)
 //   -> empty[s];
 //   the epilogue adds bias / residual, applies the activation and stores NCHW straight from the accumulators.
@@ -37,6 +43,11 @@ constexpr int TC_PRODUCERS = 128;
 constexpr int TC_CONSUMER_WARPS = 8;
 constexpr int TC_THREADS = TC_PRODUCERS + 32 * TC_CONSUMER_WARPS;
 constexpr int TC_MAX_TAPS = 49;
+// Registers per thread of the fprop kernel: 168 at launch (384 threads at 1 CTA/SM hold 64512); from there the producers
+// hand registers to the consumers, whose A fragments stay in registers: below wgmma N = 128 a consumer thread holds acc
+// + part + the split A of the stage in flight and of the next (2 x 32).  128 x 72 + 256 x 216 = 64512.
+// With nvcc 12.9, -Xptxas -v shows no spill and no stack for any N at these counts; 64 / 224 spills the producers.
+constexpr int TC_PRODUCER_REGS = 72, TC_CONSUMER_REGS = 216;
 
 struct TcArgs {
     // prepared weights wp: tf32 hi copy [N][Kp] followed by the lo copy [N][Kp] (k = tap*cpad + c), as a 3-D TMA map
@@ -131,6 +142,13 @@ __device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int K, int R>
+__device__ __forceinline__ void wg_fence_regs(uint32_t (&d)[K][R]) {
+#pragma unroll
+    for (int k = 0; k < K; ++k)
+#pragma unroll
+        for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[k][i])::"memory");
+}
 
 // D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 in, fp32 accumulators in registers (N / 2 per thread)
 __device__ __forceinline__ void wgmma_tf32_n16(float (&d)[8], uint64_t da, uint64_t db) {
@@ -191,6 +209,71 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[NT / 2], uint64_t da, uint
     else if constexpr (NT == 64) wgmma_tf32_n64(d, da, db);
     else wgmma_tf32_n128(d, da, db);
 }
+
+// The same with A from registers: the m64k8 tf32 fragment, a[i] = A[wq * 16 + lane / 4 + 8 * (i & 1)][lane % 4 + 4 * (i >> 1)]
+// for thread `lane` of warp wq of the warpgroup.  The registers must hold until the wgmma's group has been waited on.
+__device__ __forceinline__ void wgmma_tf32_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "{%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+__device__ __forceinline__ void wgmma_tf32_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+template <int NT>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[NT / 2], const uint32_t (&a)[4], uint64_t db) {
+    if constexpr (NT == 16) wgmma_tf32_rs_n16(d, a, db);
+    else if constexpr (NT == 32) wgmma_tf32_rs_n32(d, a, db);
+    else if constexpr (NT == 64) wgmma_tf32_rs_n64(d, a, db);
+    else wgmma_tf32_rs_n128(d, a, db);
+}
+
+// setmaxnreg: a warpgroup hands registers back to the CTA's pool or takes them from it (counts: multiples of 8)
+template <int R> __device__ __forceinline__ void wg_regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void wg_regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 constexpr int TC_TILE_BYTES = TC_KC * TC_M * 16;                   // one A operand copy of one stage: 16 KB
 constexpr int TC_SMEM_MAX = 227 * 1024;
@@ -259,9 +342,9 @@ __device__ __forceinline__ int tc_acc_row(int wg, int wq, int lane, int half) { 
 __device__ __forceinline__ int tc_acc_col(int lane, int i, int e) { return 8 * i + 2 * (lane & 3) + e; }
 __device__ __forceinline__ int tc_acc_reg(int i, int half, int e) { return 4 * i + 2 * half + e; }
 
-// Consumer side shared by both kernels: acc = 0 (an empty split contributes zeros), then for each of `nkt` full stages,
-// 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this warpgroup's 64 rows into the scratch registers `part`, then
-// acc += part in fp32 and the stage goes back to the producers.
+// Consumer side of the wgrad kernel, both operands split in shared memory: acc = 0 (an empty split contributes zeros),
+// then for each of `nkt` full stages, 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this warpgroup's 64 rows into the
+// scratch registers `part`, then acc += part in fp32 and the stage goes back to the producers.
 template <int NT>
 __device__ __forceinline__ void tc_consume(const TcRing& ring, int nkt, int wg, int lane, float (&acc)[NT / 2]) {
     float part[NT / 2];
@@ -296,6 +379,113 @@ __device__ __forceinline__ void tc_consume(const TcRing& ring, int nkt, int wg, 
     }
 }
 
+// The fprop kernel's A tile: one fp32 copy of the stage's 128 x 32 im2col values, unsplit, laid out for the consumers'
+// register fragments.  Row r is 8 16-byte chunks (the first A slot of the stage; the second goes unused):
+//
+//   A[r][k] is element k / 4 % 4 of float4 tile_idx(r, 2 * (k % 4) + k / 16),
+//
+// so chunks 2t and 2t + 1 hold k = t, t + 4, ..., t + 28: the k of fragment column t over all 4 k-steps of the stage.
+// A consumer thread (rows r0 = wg * 64 + wq * 16 + lane / 4 and r0 + 8, column t = lane % 4) reads its 16 values with
+// 4 LDS.128.  They are bank-conflict free: a 128-bit shared load is served 8 lanes at a time, and lanes 8p .. 8p + 7
+// read chunk 2t + h (t = 0..3, fixed h) of the rows with r0 & 7 = 2p and 2p + 1.  The swizzle puts that chunk at
+// 16-byte bank group (2t + h) ^ (r & 7), and a 128-byte row spans the 32 banks once, so row 2p's lanes hit groups
+// {(2t + h) ^ 2p} = {0, 2, 4, 6} + h and row 2p + 1's lanes {0, 2, 4, 6} + (1 - h): 8 distinct groups, 32 banks.
+// The producer of row r stores its 8 chunks with STS.128 as before; the 8 rows of a lane octet differ in r & 7, so
+// each chunk index lands on 8 distinct groups.
+struct TcAFrag { uint32_t hi[TC_KC / 2][4], lo[TC_KC / 2][4]; };   // [k-step][wgmma A register]
+
+// this thread's 16 raw values of the A tile at `tile`: v[h][j] = A[r0 + 8 h][t + 4 j].  `off` is the byte offset of
+// chunk 2t of row r0 (tc_a_off); chunk 2t + 1 sits at off ^ 16 (the swizzle flips the low chunk bit alike), row r0 + 8
+// 1 KB further on (same r & 7).
+__device__ __forceinline__ int tc_a_off(int r0, int t) { return tile_idx(r0, 2 * t) * 16; }
+__device__ __forceinline__ void tc_load_a(const unsigned char* tile, int off, float (&v)[2][8]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const float4 c0 = *(const float4*)(tile + (off + 1024 * h)), c1 = *(const float4*)(tile + ((off ^ 16) + 1024 * h));
+        v[h][0] = c0.x; v[h][1] = c0.y; v[h][2] = c0.z; v[h][3] = c0.w;
+        v[h][4] = c1.x; v[h][5] = c1.y; v[h][6] = c1.z; v[h][7] = c1.w;
+    }
+}
+// the split of tc_split_store, hi = tf32(x), lo = tf32(x - hi), into the fragment: k-step ks, register i holds
+// row r0 + 8 (i & 1), k = 8 ks + t + 4 (i >> 1)
+__device__ __forceinline__ void tc_split_a(const float (&v)[2][8], TcAFrag& f) {
+#pragma unroll
+    for (int ks = 0; ks < TC_KC / 2; ++ks)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float x = v[i & 1][2 * ks + (i >> 1)], h = tf32_hi(x);
+            f.hi[ks][i] = __float_as_uint(h);
+            f.lo[ks][i] = __float_as_uint(tf32_hi(x - h));
+        }
+}
+
+// Consumer side of the fprop kernel: tc_consume's products in its order, with A from registers.  Below N = 128, while a
+// stage's MMAs run the thread waits for the next stage and loads and splits its A fragment.  At N = 128 acc + part
+// already take 128 registers and a second fragment does not fit without spilling, so each stage's A is loaded and
+// split after its full barrier, as the producers used to.  B of the current stage is read by the MMAs until the wait,
+// so the stage is released after it.
+template <int NT>
+__device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int nkt, int wg, int wq, int lane, float (&acc)[NT / 2]) {
+    constexpr bool split_ahead = NT < 128;
+    float part[NT / 2];
+#pragma unroll
+    for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
+    const uint32_t base = smem_u32(ring.smem);
+    const int a_off = tc_a_off(wg * 64 + wq * 16 + (lane >> 2), lane & 3);
+    TcAFrag cur, nxt;
+    float v[2][8];
+    if constexpr (split_ahead) {
+        if (nkt > 0) {
+            mbar_wait(&ring.full[0], 0);
+            tc_load_a(ring.tiles(ring.smem, 0).a_hi, a_off, v);
+            tc_split_a(v, cur);
+        }
+    }
+    int s = 0;                // stage of k-tile it
+    uint32_t phase = 0;       // parity of k-tile it's round
+    for (int it = 0; it < nkt; ++it) {
+        if constexpr (!split_ahead) {
+            mbar_wait(&ring.full[s], phase);
+            tc_load_a(ring.tiles(ring.smem, s).a_hi, a_off, v);
+            tc_split_a(v, cur);
+        }
+        const TcTiles<uint32_t> tl = ring.tiles(base, s);
+#pragma unroll
+        for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < TC_KC / 2; ++ks) {
+            const uint32_t koff = (uint32_t)ks * 32u;
+            wgmma_tf32_rs<NT>(part, cur.lo[ks], wg_desc(tl.b_hi + koff));
+            wgmma_tf32_rs<NT>(part, cur.hi[ks], wg_desc(tl.b_lo + koff));
+        }
+#pragma unroll
+        for (int ks = 0; ks < TC_KC / 2; ++ks)
+            wgmma_tf32_rs<NT>(part, cur.hi[ks], wg_desc(tl.b_hi + (uint32_t)ks * 32u));
+        wg_commit();
+        const int s1 = s + 1 == ring.depth ? 0 : s + 1;
+        const uint32_t phase1 = phase ^ (s1 == 0);
+        if constexpr (split_ahead) {
+            if (it + 1 < nkt) {
+                mbar_wait(&ring.full[s1], phase1);
+                tc_load_a(ring.tiles(ring.smem, s1).a_hi, a_off, v);
+                tc_split_a(v, nxt);
+            }
+        }
+        wg_wait<0>();
+        wg_fence_regs(part);
+        // the MMAs read cur's registers until the wait: keep the compiler from giving them to nxt or v before it
+        wg_fence_regs(cur.hi);
+        wg_fence_regs(cur.lo);
+        if (lane == 0) mbar_arrive(&ring.empty[s]);
+#pragma unroll
+        for (int j = 0; j < NT / 2; ++j) acc[j] += part[j];
+        if constexpr (split_ahead) cur = nxt;
+        s = s1;
+        phase = phase1;
+    }
+}
+
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
     // full[s]: the 128 producers' A stores + producer 0's arrival that announces the B tiles' TMA bytes
@@ -309,6 +499,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 
     if (warp < TC_PRODUCERS / 32) {
         // ===================== producers: thread == tile row =====================
+        wg_regs_dec<TC_PRODUCER_REGS>();
         const int r = tid;
         const int m = m0 + r;
         const bool mvalid = m < a.M;
@@ -375,17 +566,22 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 tma_load_3d(t.b_hi, &a.wmap, &ring.full[s], kt * (TC_KC * 4), n0, 0);
                 tma_load_3d(t.b_lo, &a.wmap, &ring.full[s], kt * (TC_KC * 4), n0, 1);
             }
-            // ---- A: split + store
+            // ---- A: the row's 32 floats, unsplit, in the consumers' fragment order (k = 4c + e goes to chunk 2e + c / 4,
+            //      see tc_load_a); the consumers read them with ld.shared, so no proxy fence is needed
+            float4* at = (float4*)t.a_hi;
 #pragma unroll
-            for (int c = 0; c < TC_KC; ++c)
-                tc_split_store(t.a_hi, t.a_lo, tile_idx(r, c), make_float4(av[c][0], av[c][1], av[c][2], av[c][3]));
-            ring.publish(s);
+            for (int e = 0; e < 4; ++e)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    at[tile_idx(r, 2 * e + h)] = make_float4(av[4 * h][e], av[4 * h + 1][e], av[4 * h + 2][e], av[4 * h + 3][e]);
+            mbar_arrive(&ring.full[s]);
         }
     } else {
         // ===================== consumers: MMA + epilogue =====================
+        wg_regs_inc<TC_CONSUMER_REGS>();
         const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
         float acc[NT / 2];
-        tc_consume<NT>(ring, nkt, wg, lane, acc);
+        tc_consume_rs<NT>(ring, nkt, wg, wq, lane, acc);
         const long long HWout = (long long)a.Hout * a.Wout;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
