@@ -170,6 +170,14 @@ _SIGS = {
     'ccb_kitti_flow_errors_workspace_bytes': ('long long', 'int, int, int'),
     'ccb_kitti_flow_errors': (STATUS, 'const unsigned short*, const unsigned short*, int, int, int, void*, long long, '
                                       'double*, long long*, ccb_stream_t'),
+    'ccb_velo_depth_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_velo_depth': (STATUS, 'const float*, const long long*, const double*, long long, int, int, int, void*, long long, '
+                               'double*, ccb_stream_t'),
+    'ccb_spline_zoom_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_spline_zoom': (STATUS, 'const float*, int, int, int, int, int, float, float, void*, long long, float*, ccb_stream_t'),
+    'ccb_eigen_depth_errors_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_eigen_depth_errors': (STATUS, 'const double*, const float*, int, int, int, double, double, host const double*, '
+                                       'const float*, const double*, int, void*, long long, double*, ccb_stream_t'),
     'ccb_prep_frames': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, int, '
                                 'int, int, ccb_stream_t'),
     'ccb_prep_frames_unit': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '
@@ -186,7 +194,7 @@ _SIGS = {
     'ccb_debug_tc_plan': (STATUS, 'int, host int*'),
 }
 
-_SCALARS = {'int': C.c_int, 'long long': C.c_longlong, 'float': C.c_float}
+_SCALARS = {'int': C.c_int, 'long long': C.c_longlong, 'float': C.c_float, 'double': C.c_double}
 _DTYPES = {'float': torch.float32, 'double': torch.float64, 'int': torch.int32, 'long long': torch.int64,
            'unsigned long long': torch.int64, 'unsigned char': torch.uint8, 'unsigned short': torch.uint16, 'void': None}
 _RESTYPES = {STATUS: C.c_int, 'int': C.c_int, 'long long': C.c_longlong, 'void*': C.c_void_p, 'const char*': C.c_char_p,

@@ -12,6 +12,7 @@
 //       NormalizeLocally (:33-44) as per-sample channel statistics.
 //
 //   N3  motion segmentation scores: the three rigidity masks and the IoU counts of test_mask.py:129-156,224-262
+//       depth evaluation of test_disp.py:98-141: the velodyne ground truth, scipy's cubic zoom, both scalings' errors
 //
 // All floating-point reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize); the
 // segmentation counts are integer sums (atomics, the same in any order).
@@ -25,6 +26,9 @@ static inline double __dsub_rn(double a, double b) { volatile double r = a - b; 
 static inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
 static inline double __ddiv_rn(double a, double b) { volatile double r = a / b; return r; }
 static inline double __dsqrt_rn(double a) { volatile double r = sqrt(a); return r; }
+static inline double __fma_rn(double a, double b, double c) { return fma(a, b, c); }
+static inline long long __double_as_longlong(double d) { long long i; memcpy(&i, &d, 8); return i; }
+static inline double __longlong_as_double(long long i) { double d; memcpy(&d, &i, 8); return d; }
 #endif
 
 namespace ccb {
@@ -922,6 +926,394 @@ __global__ void kitti_err_finalize(const KittiErrArgs a, int nblk) {
     }
 }
 
+// ================================================================================================
+// KITTI depth ground truth from a velodyne sweep (kitti_eval/depth_evaluation_utils.py generate_depth_map :148-191), fp64:
+//   keep x >= 0;  (X, Y, Z) = P_velo2im (x, y, z, 1), each row summed as OpenBLAS's dgemm sums it (an fma chain over the
+//   columns);  u = rint(X / Z) - 1, v = rint(Y / Z) - 1 (numpy's round: half to even);  keep 0 <= u < W, 0 <= v < H
+//   depth[v, u] = Z of the LAST kept point on the pixel (numpy's fancy assignment)
+//   duplicates grouped by the reference's sub2ind key v * (W - 1) + u - 1 (which also joins (v, W-1) with (v+1, 0)): for a
+//   key with more than one point, the pixel of its FIRST point gets the least Z of the group;  finally depth < 0 -> 0.
+// Integer atomics only (largest index, count, smallest index, least Z as an order-preserving key): the same bits on every
+// run.  Pass 1 scatters the points, pass 2 writes every pixel.
+struct VeloArgs {
+    const float* pts;               // [total, 4]; column 3 is not read (the reference sets it to 1)
+    const long long* offs;          // [B + 1] first point of each sample
+    const double* P;                // [B, 3, 4]
+    unsigned long long* last;       // [B, H*W]   1 + index of the last kept point on the pixel, 0 for none
+    unsigned long long* cnt;        // [B, K]     kept points per key, indexed by key + 1 (K = H*(W-1) + 1 keys)
+    unsigned long long* first;      // [B, K]     ~index of the first point of the key
+    unsigned long long* zmin;       // [B, K]     ~ordered key of the least Z of the key
+    double* depth;                  // [B, H, W]
+    long long total;
+    int B, H, W;
+};
+
+struct VeloPt { double z; int u, v; bool keep; };
+
+__device__ __forceinline__ VeloPt velo_project(const VeloArgs& a, int b, long long i) {
+    VeloPt r;
+    r.keep = false; r.u = r.v = 0; r.z = 0.0;
+    const float* q = a.pts + 4 * i;
+    if (!(__ldg(q) >= 0.f)) return r;
+    const double x = (double)__ldg(q), y = (double)__ldg(q + 1), z = (double)__ldg(q + 2);
+    const double* P = a.P + 12ll * b;
+    double c[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+        c[k] = __dadd_rn(__fma_rn(__ldg(P + 4 * k + 2), z, __fma_rn(__ldg(P + 4 * k + 1), y, __dmul_rn(__ldg(P + 4 * k), x))),
+                         __ldg(P + 4 * k + 3));
+    const double u = __dsub_rn(rint(__ddiv_rn(c[0], c[2])), 1.0), v = __dsub_rn(rint(__ddiv_rn(c[1], c[2])), 1.0);
+    if (!(u >= 0.0 && v >= 0.0 && u < (double)a.W && v < (double)a.H)) return r;
+    r.keep = true; r.u = (int)u; r.v = (int)v; r.z = c[2];
+    return r;
+}
+
+// unsigned order of the key == value order of the double (NaN never reaches it: its u fails the bounds)
+__device__ __forceinline__ unsigned long long ordered_key(double d) {
+    const unsigned long long k = (unsigned long long)__double_as_longlong(d);
+    return (k >> 63) ? ~k : (k | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double ordered_value(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+__device__ __forceinline__ bool velo_range(const VeloArgs& a, int b, long long* i0, long long* i1) {
+    *i0 = a.offs[b];
+    *i1 = a.offs[b + 1];
+    return *i0 >= 0 && *i0 <= *i1 && *i1 <= a.total;       // malformed offsets: the sample gets no point
+}
+
+__global__ void __launch_bounds__(256) velo_scatter_kernel(const VeloArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.y;
+    long long i0, i1;
+    if (!velo_range(a, b, &i0, &i1)) return;
+    const long long hw = (long long)a.H * a.W, K = (long long)a.H * (a.W - 1) + 1;
+    for (long long i = i0 + (long long)blockIdx.x * 256 + threadIdx.x; i < i1; i += (long long)gridDim.x * 256) {
+        const VeloPt p = velo_project(a, b, i);
+        if (!p.keep) continue;
+        const long long key = (long long)p.v * (a.W - 1) + p.u;     // sub2ind + 1
+        atomicMax(a.last + b * hw + (long long)p.v * a.W + p.u, (unsigned long long)(i - i0 + 1));
+        atomicAdd(a.cnt + b * K + key, 1ull);
+        atomicMax(a.first + b * K + key, ~(unsigned long long)(i - i0));
+        atomicMax(a.zmin + b * K + key, ~ordered_key(p.z));
+    }
+}
+
+__global__ void __launch_bounds__(256) velo_depth_kernel(const VeloArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.y;
+    long long i0, i1;
+    const bool ok = velo_range(a, b, &i0, &i1);
+    const long long hw = (long long)a.H * a.W, K = (long long)a.H * (a.W - 1) + 1;
+    for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < hw; p += (long long)gridDim.x * 256) {
+        double d = 0.0;
+        const unsigned long long last = ok ? a.last[b * hw + p] : 0ull;
+        if (last) {
+            d = velo_project(a, b, i0 + (long long)last - 1).z;
+            const int v = (int)(p / a.W), u = (int)(p - (long long)v * a.W);
+            const long long key = (long long)v * (a.W - 1) + u;
+            if (a.cnt[b * K + key] > 1) {
+                const VeloPt f = velo_project(a, b, i0 + (long long)~a.first[b * K + key]);
+                if (f.v == v && f.u == u) d = ordered_value(~a.zmin[b * K + key]);
+            }
+        }
+        a.depth[b * hw + p] = (d < 0.0) ? 0.0 : d;
+    }
+}
+
+// ================================================================================================
+// scipy.ndimage.zoom(x, (H/h, W/w), order=3) (mode 'constant', grid_mode False, prefilter on) of fp32 images, in fp64:
+//   prefilter  per axis (0 then 1) the cubic B-spline recursion, pole z = sqrt(3) - 2, gain (1 - z)(1 - 1/z), causal and
+//              anti-causal initialisation with the mirror boundary (scipy's ni_splines.c for mode 'constant'); a line of
+//              length 1 is left as it is
+//   evaluate   at o * ((n - 1) / (m - 1)) per axis (1 when m == 1), 4 x 4 tensor-product B-spline weights, coefficient
+//              indices outside the line mirrored
+// then rounded to fp32 and clipped to [lo, hi] in fp32 (numpy's clip: NaN stays NaN).  One fp64 thread per line for the
+// recursions, one thread per output pixel for the evaluation.
+struct ZoomArgs {
+    const float* src;               // [N, h, w]
+    double* coef;                   // [N, h, w]
+    float* dst;                     // [N, H, W]
+    int N, h, w, H, W;
+    float lo, hi;
+};
+
+__device__ __forceinline__ void spline_line(double* c, int n, long long stride) {
+    if (n == 1) return;
+    const double z = -0.2679491924311227;       // sqrt(3) - 2
+    const double gain = (1.0 - z) * (1.0 - 1.0 / z);
+    for (int i = 0; i < n; ++i) c[i * stride] *= gain;
+    const double zn1 = pow(z, (double)(n - 1));
+    double c0 = c[0] + zn1 * c[(long long)(n - 1) * stride];
+    double zi = z;
+    for (int i = 1; i < n - 1; ++i) {
+        c0 += zi * (c[i * stride] + zn1 * c[(long long)(n - 1 - i) * stride]);
+        zi *= z;
+    }
+    c[0] = c0 / (1.0 - zn1 * zn1);
+    for (int i = 1; i < n; ++i) c[i * stride] += z * c[(i - 1) * stride];
+    c[(long long)(n - 1) * stride] = (z * c[(long long)(n - 2) * stride] + c[(long long)(n - 1) * stride]) * z / (z * z - 1.0);
+    for (int i = n - 2; i >= 0; --i) c[i * stride] = z * (c[(i + 1) * stride] - c[i * stride]);
+}
+
+// pass 0: one thread per column (copies the input and filters along axis 0); pass 1: one thread per row (axis 1)
+__global__ void __launch_bounds__(256) zoom_prefilter_kernel(const ZoomArgs a, int pass) {
+    CCB_PDL_WAIT();
+    const long long hw = (long long)a.h * a.w;
+    const long long nlines = (long long)a.N * (pass == 0 ? a.w : a.h);
+    for (long long t = (long long)blockIdx.x * 256 + threadIdx.x; t < nlines; t += (long long)gridDim.x * 256) {
+        if (pass == 0) {
+            const long long n = t / a.w, x = t - n * a.w;
+            double* c = a.coef + n * hw + x;
+            const float* s = a.src + n * hw + x;
+            for (int y = 0; y < a.h; ++y) c[(long long)y * a.w] = (double)__ldg(s + (long long)y * a.w);
+            spline_line(c, a.h, a.w);
+        } else {
+            spline_line(a.coef + t * a.w, a.w, 1);
+        }
+    }
+}
+
+// scipy's mirror of a coefficient index (period 2n - 2; a line of length 1 has one coefficient)
+__device__ __forceinline__ int mirror_index(int j, int n) {
+    if (n == 1) return 0;
+    const int period = 2 * n - 2;
+    j = j % period;
+    if (j < 0) j += period;
+    return (j >= n) ? period - j : j;
+}
+
+__device__ __forceinline__ void cubic_weights(double t, double (&wt)[4]) {
+    const double s = 1.0 - t;
+    wt[0] = s * s * s / 6.0;
+    wt[1] = (t * t * (t - 2.0) * 3.0 + 4.0) / 6.0;
+    wt[2] = (s * s * (s - 2.0) * 3.0 + 4.0) / 6.0;
+    wt[3] = t * t * t / 6.0;
+}
+
+__global__ void __launch_bounds__(256) zoom_eval_kernel(const ZoomArgs a) {
+    CCB_PDL_WAIT();
+    const long long HW = (long long)a.H * a.W, n_out = (long long)a.N * HW;
+    const double step_y = (a.H > 1) ? (double)(a.h - 1) / (double)(a.H - 1) : 1.0;
+    const double step_x = (a.W > 1) ? (double)(a.w - 1) / (double)(a.W - 1) : 1.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n_out; i += (long long)gridDim.x * 256) {
+        const long long n = i / HW, q = i - n * HW;
+        const int oy = (int)(q / a.W), ox = (int)(q - (long long)oy * a.W);
+        const double cy = __dmul_rn((double)oy, step_y), cx = __dmul_rn((double)ox, step_x);
+        const double fy = floor(cy), fx = floor(cx);
+        double wy[4], wx[4];
+        cubic_weights(cy - fy, wy);
+        cubic_weights(cx - fx, wx);
+        int xs[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) xs[k] = mirror_index((int)fx - 1 + k, a.w);
+        const double* c = a.coef + n * a.h * (long long)a.w;
+        double acc = 0.0;
+#pragma unroll
+        for (int ky = 0; ky < 4; ++ky) {
+            const double* row = c + (long long)mirror_index((int)fy - 1 + ky, a.h) * a.w;
+            double r = 0.0;
+#pragma unroll
+            for (int kx = 0; kx < 4; ++kx) r += wx[kx] * row[xs[kx]];
+            acc += wy[ky] * r;
+        }
+        const float v = (float)acc;
+        a.dst[i] = (v < a.lo) ? a.lo : ((v > a.hi) ? a.hi : v);
+    }
+}
+
+// ================================================================================================
+// One sample of test_disp.py:124-141 + compute_errors :171-187, in fp64.  mask = min_depth < gt < max_depth inside the
+// crop rows [y1, y2) and columns [x1, x2);  per row r of the output the prediction is (double)pred * scale_r:
+//   row 1  scale = median(gt[mask]) / median(pred[mask]), numpy medians (an even count averages the two middle values, in
+//          fp64 for gt and in fp32 for the fp32 prediction)
+//   row 0  scale = mean(s1 / |pose[:3]|) over the references with s1 > 0 (0 when there is none); zeros without poses
+//   errors abs_rel sq_rel rms log_rms a1 a2 a3;  a* are exact counts over n, the rest fp64 block partials summed in a
+//          fixed order.
+// Medians by radix select on order-preserving 64-bit keys (six passes of 11, 11, 11, 11, 11 and 9 bits), four selections
+// per sample: the lower and upper middle ranks of gt and of pred.
+struct EigenArgs {
+    const double* gt;               // [B, H, W]
+    const float* pred;              // [B, H, W]
+    const float* poses;             // [B, R, 6] or null
+    const double* disp;             // [B, R] or null
+    unsigned* hist;                 // [B][4][2048]
+    unsigned long long* sel;        // [B][4][3]: prefix, prefix mask, remaining rank
+    unsigned long long* count;      // [B] valid pixels
+    double* scale;                  // [B][2]
+    double* partials;               // [B][blocks][2][7]
+    double* out;                    // [B, 2, 7]
+    double min_depth, max_depth;
+    int B, H, W, R, y1, y2, x1, x2;
+};
+
+__device__ __forceinline__ bool eigen_valid(const EigenArgs& a, double g, int y, int x) {
+    return (g > a.min_depth) && (g < a.max_depth) && (y >= a.y1) && (y < a.y2) && (x >= a.x1) && (x < a.x2);
+}
+__device__ __forceinline__ unsigned long long ordered_key32(float f) {
+    const unsigned k = __float_as_uint(f);
+    return (unsigned long long)((k >> 31) ? ~k : (k | 0x80000000u));
+}
+__device__ __forceinline__ float ordered_value32(unsigned long long k) {
+    const unsigned u = (unsigned)k;
+    return __uint_as_float((u >> 31) ? (u & 0x7fffffffu) : ~u);
+}
+__device__ __forceinline__ int eigen_shift(int pass) { return pass < 5 ? 53 - 11 * pass : 0; }
+__device__ __forceinline__ unsigned eigen_bins(int pass) { return pass < 5 ? 2048u : 512u; }
+
+__global__ void __launch_bounds__(256) eigen_hist_kernel(const EigenArgs a, int pass) {
+    CCB_PDL_WAIT();
+    __shared__ unsigned h[4 * 2048];
+    const int b = blockIdx.y;
+    const int shift = eigen_shift(pass);
+    const unsigned nbins = eigen_bins(pass);
+    for (int i = threadIdx.x; i < 4 * 2048; i += 256) h[i] = 0;
+    __syncthreads();
+    const unsigned long long* s = a.sel + (long long)b * 12;
+    unsigned long long pre[4], msk[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { pre[k] = s[3 * k]; msk[k] = s[3 * k + 1]; }
+    const long long hw = (long long)a.H * a.W;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < hw; i += (long long)gridDim.x * 256) {
+        const int y = (int)(i / a.W), x = (int)(i - (long long)y * a.W);
+        const double g = __ldg(a.gt + b * hw + i);
+        if (!eigen_valid(a, g, y, x)) continue;
+        const unsigned long long kg = ordered_key(g), kp = ordered_key32(__ldg(a.pred + b * hw + i));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const unsigned long long key = (k < 2) ? kg : kp;
+            if ((key & msk[k]) == pre[k]) atomicAdd(h + k * 2048 + (unsigned)((key >> shift) & (nbins - 1)), 1u);
+        }
+    }
+    __syncthreads();
+    unsigned* g = a.hist + (long long)b * 4 * 2048;
+    for (int i = threadIdx.x; i < 4 * 2048; i += 256)
+        if (h[i]) atomicAdd(g + i, h[i]);
+}
+
+// one thread per (sample, selection): find the bin holding the rank, extend the prefix, clear the histogram
+__global__ void eigen_select_kernel(const EigenArgs a, int pass) {
+    CCB_PDL_WAIT();
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.B * 4) return;
+    const int b = t >> 2, k = t & 3;
+    unsigned* h = a.hist + (long long)t * 2048;
+    unsigned long long* s = a.sel + (long long)t * 3;
+    const int shift = eigen_shift(pass);
+    const unsigned nbins = eigen_bins(pass);
+    if (pass == 0) {
+        unsigned long long n = 0;
+        for (unsigned i = 0; i < nbins; ++i) n += h[i];
+        if (k == 0) a.count[b] = n;
+        // numpy's median: sorted[(n-1)//2] and sorted[n//2] (the same rank when n is odd)
+        s[2] = (n == 0) ? 0 : ((k & 1) ? n / 2 : (n - 1) / 2);
+    }
+    const unsigned long long rank = s[2];
+    unsigned long long cum = 0;
+    unsigned bin = 0;
+    for (unsigned i = 0; i < nbins; ++i) {
+        bin = i;
+        if (cum + h[i] > rank) break;
+        cum += h[i];
+    }
+    s[2] = rank - cum;
+    s[0] |= (unsigned long long)bin << shift;
+    s[1] |= (unsigned long long)(nbins - 1) << shift;
+    for (unsigned i = 0; i < 2048; ++i) h[i] = 0;
+}
+
+// one thread per sample: both scales
+__global__ void eigen_scale_kernel(const EigenArgs a) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.B) return;
+    const unsigned long long* s = a.sel + (long long)b * 12;
+    const double g0 = ordered_value(s[0]), g1 = ordered_value(s[3]);
+    const float p0 = ordered_value32(s[6]), p1 = ordered_value32(s[9]);
+    const bool even = (a.count[b] & 1ull) == 0;
+    const double med_g = even ? __ddiv_rn(__dadd_rn(g0, g1), 2.0) : g0;
+    const float med_p = even ? __fdiv_rn(__fadd_rn(p0, p1), 2.f) : p0;
+    a.scale[2 * b + 1] = __ddiv_rn(med_g, (double)med_p);
+    double sum = 0.0;
+    int n = 0;
+    if (a.poses)
+        for (int r = 0; r < a.R; ++r) {
+            const double s1 = a.disp[(long long)b * a.R + r];
+            if (!(s1 > 0.0)) continue;
+            const float* p = a.poses + ((long long)b * a.R + r) * 6;
+            const double x = p[0], y = p[1], z = p[2];
+            const float norm = (float)__dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
+            sum = __dadd_rn(sum, __ddiv_rn(s1, (double)norm));
+            ++n;
+        }
+    a.scale[2 * b] = n ? __ddiv_rn(sum, (double)n) : 0.0;
+}
+
+__device__ __forceinline__ double nan_max(double p, double q) { return (p != p || p > q) ? p : q; }   // np.maximum
+
+__global__ void __launch_bounds__(256) eigen_errors_kernel(const EigenArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ double scratch[14 * 32];
+    const int b = blockIdx.y;
+    const long long hw = (long long)a.H * a.W;
+    const int r0 = a.poses ? 0 : 1;
+    const double sc[2] = {a.scale[2 * b], a.scale[2 * b + 1]};
+    double acc[14];
+#pragma unroll
+    for (int k = 0; k < 14; ++k) acc[k] = 0.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < hw; i += (long long)gridDim.x * 256) {
+        const int y = (int)(i / a.W), x = (int)(i - (long long)y * a.W);
+        const double g = __ldg(a.gt + b * hw + i);
+        if (!eigen_valid(a, g, y, x)) continue;
+        const double p32 = (double)__ldg(a.pred + b * hw + i);
+        const double lg = log(g);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (r < r0) continue;
+            const double p = __dmul_rn(p32, sc[r]);
+            const double th = nan_max(__ddiv_rn(g, p), __ddiv_rn(p, g));
+            const double d = __dsub_rn(g, p), d2 = __dmul_rn(d, d), dl = __dsub_rn(lg, log(p));
+            double* o = acc + 7 * r;
+            o[0] += __ddiv_rn(fabs(d), g);
+            o[1] += __ddiv_rn(d2, g);
+            o[2] += d2;
+            o[3] += __dmul_rn(dl, dl);
+            o[4] += (th < 1.25) ? 1.0 : 0.0;
+            o[5] += (th < 1.5625) ? 1.0 : 0.0;
+            o[6] += (th < 1.953125) ? 1.0 : 0.0;
+        }
+    }
+    block_sum_d<14>(acc, scratch);
+    if (threadIdx.x == 0) {
+        double* o = a.partials + ((long long)b * gridDim.x + blockIdx.x) * 14;
+#pragma unroll
+        for (int k = 0; k < 14; ++k) o[k] = acc[k];
+    }
+}
+
+// one thread per (sample, row), the block partials in block order
+__global__ void eigen_finalize_kernel(const EigenArgs a, int nblk) {
+    CCB_PDL_WAIT();
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.B * 2) return;
+    const int b = t >> 1, r = t & 1;
+    double* o = a.out + (long long)t * 7;
+    if (r == 0 && !a.poses) {
+        for (int k = 0; k < 7; ++k) o[k] = 0.0;
+        return;
+    }
+    double s[7] = {0, 0, 0, 0, 0, 0, 0};
+    for (int k = 0; k < nblk; ++k)
+        for (int j = 0; j < 7; ++j) s[j] += a.partials[((long long)b * nblk + k) * 14 + 7 * r + j];
+    const double n = (double)a.count[b];
+    o[0] = __ddiv_rn(s[0], n);
+    o[1] = __ddiv_rn(s[1], n);
+    o[2] = __dsqrt_rn(__ddiv_rn(s[2], n));
+    o[3] = __dsqrt_rn(__ddiv_rn(s[3], n));
+    for (int j = 4; j < 7; ++j) o[j] = __ddiv_rn(s[j], n);
+}
+
 }  // namespace ccb
 
 using namespace ccb;
@@ -1081,6 +1473,109 @@ extern "C" int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned sh
     CCB_LAUNCH(kitti_err_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     CCB_LAUNCH(kitti_err_finalize, dim3((B + 63) / 64), dim3(64), 0, stream, a, nb);
     return check_launch("kitti_flow_errors");
+}
+
+// keys -1 .. H*(W-1) - 1 of the reference's sub2ind, stored at key + 1
+static long long velo_keys(int H, int W) { return (long long)H * (W - 1) + 1; }
+
+extern "C" long long ccb_velo_depth_workspace_bytes(int B, int H, int W) {
+    if (B <= 0 || H <= 0 || W <= 0) return -1;
+    return (long long)B * ((long long)H * W + 3 * velo_keys(H, W)) * (long long)sizeof(unsigned long long);
+}
+
+extern "C" int ccb_velo_depth(const float* points, const long long* offsets, const double* P_velo2im, long long total, int B, int H,
+                              int W, void* work, long long work_bytes, double* depth, ccb_stream_t stream) {
+    CCB_REQUIRE(offsets && P_velo2im && depth && (points || total == 0), CCB_ERR_ARG, "velo_depth: null pointer");
+    CCB_REQUIRE(B > 0 && H > 0 && W > 0 && total >= 0, CCB_ERR_ARG, "velo_depth: bad sizes");
+    const long long need = ccb_velo_depth_workspace_bytes(B, H, W);
+    CCB_REQUIRE_WORK("velo_depth", "work", work, work_bytes, need);
+    const long long hw = (long long)H * W, K = velo_keys(H, W);
+    VeloArgs a;
+    a.pts = points; a.offs = offsets; a.P = P_velo2im; a.depth = depth; a.total = total; a.B = B; a.H = H; a.W = W;
+    a.last = (unsigned long long*)work;
+    a.cnt = a.last + (long long)B * hw;
+    a.first = a.cnt + (long long)B * K;
+    a.zmin = a.first + (long long)B * K;
+    cudaMemsetAsync(work, 0, (size_t)need, (cudaStream_t)stream);
+    const long long per_sample = (total + B - 1) / B;
+    const long long g = (per_sample + 255) / 256;
+    const int nbp = (int)(g < 1 ? 1 : (g > NUM_SMS * 4 ? NUM_SMS * 4 : g));
+    if (total > 0) CCB_LAUNCH(velo_scatter_kernel, dim3(nbp, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(velo_depth_kernel, dim3(mask_iou_blocks(H, W), B), dim3(256), 0, stream, a);
+    return check_launch("velo_depth");
+}
+
+extern "C" long long ccb_spline_zoom_workspace_bytes(int N, int h, int w) {
+    if (N <= 0 || h <= 0 || w <= 0) return -1;
+    return (long long)N * h * w * (long long)sizeof(double);
+}
+
+extern "C" int ccb_spline_zoom(const float* src, int N, int h, int w, int H, int W, float lo, float hi, void* work,
+                               long long work_bytes, float* dst, ccb_stream_t stream) {
+    CCB_REQUIRE(src && dst, CCB_ERR_ARG, "spline_zoom: null pointer");
+    CCB_REQUIRE(N > 0 && h > 0 && w > 0 && H > 0 && W > 0, CCB_ERR_ARG, "spline_zoom: bad sizes");
+    CCB_REQUIRE_WORK("spline_zoom", "work", work, work_bytes, ccb_spline_zoom_workspace_bytes(N, h, w));
+    ZoomArgs a;
+    a.src = src; a.coef = (double*)work; a.dst = dst; a.N = N; a.h = h; a.w = w; a.H = H; a.W = W; a.lo = lo; a.hi = hi;
+    CCB_LAUNCH(zoom_prefilter_kernel, dim3(grid_for((long long)N * w)), dim3(256), 0, stream, a, 0);
+    CCB_LAUNCH(zoom_prefilter_kernel, dim3(grid_for((long long)N * h)), dim3(256), 0, stream, a, 1);
+    CCB_LAUNCH(zoom_eval_kernel, dim3(grid_for((long long)N * H * W)), dim3(256), 0, stream, a);
+    return check_launch("spline_zoom");
+}
+
+static int eigen_blocks(int H, int W) {
+    const long long g = ((long long)H * W + 2047) / 2048;
+    return (int)(g < 1 ? 1 : (g > 64 ? 64 : g));
+}
+
+// workspace: block partials, then the selections, counts and scales (cleared per call), then the histograms
+struct EigenPlan { long long partials, sel, count, scale, hist, bytes; };
+static EigenPlan eigen_plan(int B, int H, int W) {
+    EigenPlan p;
+    p.partials = 0;
+    p.sel = p.partials + (long long)B * eigen_blocks(H, W) * 14 * 8;
+    p.count = p.sel + (long long)B * 12 * 8;
+    p.scale = p.count + (long long)B * 8;
+    p.hist = p.scale + (long long)B * 2 * 8;
+    p.bytes = p.hist + (long long)B * 4 * 2048 * 4;
+    return p;
+}
+
+extern "C" long long ccb_eigen_depth_errors_workspace_bytes(int B, int H, int W) {
+    if (B <= 0 || H <= 0 || W <= 0) return -1;
+    return eigen_plan(B, H, W).bytes;
+}
+
+extern "C" int ccb_eigen_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
+                                      const double* crop, const float* poses, const double* displacements, int R, void* work,
+                                      long long work_bytes, double* out, ccb_stream_t stream) {
+    CCB_REQUIRE(gt && pred && crop && out, CCB_ERR_ARG, "eigen_depth_errors: null pointer");
+    CCB_REQUIRE((poses == nullptr) == (displacements == nullptr), CCB_ERR_ARG,
+                "eigen_depth_errors: poses and displacements come together");
+    CCB_REQUIRE(B > 0 && H > 0 && W > 0 && (poses == nullptr || R > 0), CCB_ERR_ARG, "eigen_depth_errors: bad sizes");
+    for (int k = 0; k < 4; ++k)
+        CCB_REQUIRE(crop[k] >= 0.0 && crop[k] <= 1.0, CCB_ERR_ARG, "eigen_depth_errors: crop fraction %d outside [0, 1]", k);
+    const EigenPlan p = eigen_plan(B, H, W);
+    CCB_REQUIRE_WORK("eigen_depth_errors", "work", work, work_bytes, p.bytes);
+    EigenArgs a;
+    char* w = (char*)work;
+    a.gt = gt; a.pred = pred; a.poses = poses; a.disp = displacements; a.out = out;
+    a.partials = (double*)(w + p.partials); a.sel = (unsigned long long*)(w + p.sel); a.count = (unsigned long long*)(w + p.count);
+    a.scale = (double*)(w + p.scale); a.hist = (unsigned*)(w + p.hist);
+    a.min_depth = min_depth; a.max_depth = max_depth;
+    a.B = B; a.H = H; a.W = W; a.R = poses ? R : 0;
+    // generate_mask: np.array([f0 * H, f1 * H, f2 * W, f3 * W]).astype(np.int32), fp64 products truncated
+    a.y1 = (int)(crop[0] * H); a.y2 = (int)(crop[1] * H); a.x1 = (int)(crop[2] * W); a.x2 = (int)(crop[3] * W);
+    cudaMemsetAsync(w + p.sel, 0, (size_t)(p.bytes - p.sel), (cudaStream_t)stream);
+    const int nb = eigen_blocks(H, W);
+    for (int pass = 0; pass < 6; ++pass) {
+        CCB_LAUNCH(eigen_hist_kernel, dim3(nb, B), dim3(256), 0, stream, a, pass);
+        CCB_LAUNCH(eigen_select_kernel, dim3((B * 4 + 63) / 64), dim3(64), 0, stream, a, pass);
+    }
+    CCB_LAUNCH(eigen_scale_kernel, dim3((B + 63) / 64), dim3(64), 0, stream, a);
+    CCB_LAUNCH(eigen_errors_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(eigen_finalize_kernel, dim3((B * 2 + 63) / 64), dim3(64), 0, stream, a, nb);
+    return check_launch("eigen_depth_errors");
 }
 
 template <bool UNIT>

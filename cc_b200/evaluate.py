@@ -8,12 +8,15 @@
   flow_submission_sample  submit_flow.py:109-175                           KITTI-2015 test-set files of one sample
                         (flow_submission, flow_colors: the fused kernels; write_flow_submission: the script's files;
                         kitti_flow_errors: evaluate_flow.py compute_err :44-53 of decoded 16-bit PNGs)
+  depth_eval_batch      test_disp.py:98-141 for a batch on the device, no host synchronisation
+                        (velodyne_depth: generate_depth_map's ground truth; spline_zoom: scipy's zoom(order=3);
+                        depth_errors: both scalings and compute_errors; depth_summary: the script's printed rows)
 
 The scripts' dataset crawlers, image IO and visualisation are out of scope (SURVEY.md section 2); these functions take what the
 reference's `test_framework` iterators yield (uint8 HxWx3 frames, ground truth arrays) and return what the scripts
 accumulate, so a maintainer swaps the loop body.  Nets run in eval mode through the CUDA kernels; the spline `zoom` of
 the predicted depth to the ground-truth size (scipy, order 3) and the 3x4 pose algebra stay on the host like in the
-reference - they are a few hundred flops per sample."""
+reference in the per-sample cores; depth_eval_batch does the depth sample on the device."""
 import numpy as np
 import torch
 from .inverse_warp import pose2flow, pose_vec2mat
@@ -266,3 +269,130 @@ def kitti_flow_errors(gt_png, pred_png):
     counts = torch.empty(B, 2, device=dev, dtype=torch.int64)
     _lib.call('ccb_kitti_flow_errors', gt, pred, B, H, W, work, nbytes, out, counts, gt)
     return out, counts
+
+
+# ------------------------------------------------------------------------------------------------
+# test_disp.py on the device: the velodyne ground truth, the spline zoom and the errors of each sample
+
+
+def read_calib_file(path):
+    """kitti_eval/depth_evaluation_utils.py read_calib_file (:104-121): {key: fp64 array, or the string when a value is
+    not a list of numbers}."""
+    float_chars = set('0123456789.e+- ')
+    data = {}
+    with open(path, 'r') as f:
+        for line in f.readlines():
+            key, value = line.split(':', 1)
+            value = value.strip()
+            data[key] = value
+            if float_chars.issuperset(value):
+                try:
+                    data[key] = np.array(list(map(float, value.split(' '))))
+                except ValueError:
+                    pass
+    return data
+
+
+def kitti_velo_to_image(calib_dir, cam=2):
+    """P_velo2im [3,4] fp64 of generate_depth_map (:150-160): P_rect_0<cam> @ R_cam2rect @ velo2cam, in the reference's
+    np.dot order, from calib_cam_to_cam.txt and calib_velo_to_cam.txt under `calib_dir`."""
+    import os
+    cam2cam = read_calib_file(os.path.join(calib_dir, 'calib_cam_to_cam.txt'))
+    velo2cam = read_calib_file(os.path.join(calib_dir, 'calib_velo_to_cam.txt'))
+    velo2cam = np.hstack((velo2cam['R'].reshape(3, 3), velo2cam['T'][..., np.newaxis]))
+    velo2cam = np.vstack((velo2cam, np.array([0, 0, 0, 1.0])))
+    R_cam2rect = np.eye(4)
+    R_cam2rect[:3, :3] = cam2cam['R_rect_00'].reshape(3, 3)
+    P_rect = cam2cam['P_rect_0' + str(cam)].reshape(3, 4)
+    return np.dot(np.dot(P_rect, R_cam2rect), velo2cam)
+
+
+def load_velodyne_points(file_name):
+    """A KITTI velodyne .bin as float32 [N,4] (forward, left, up, reflectance), the 4th column set to 1 (:97-101)."""
+    points = np.fromfile(file_name, dtype=np.float32).reshape(-1, 4)
+    points[:, 3] = 1
+    return points
+
+
+@torch.no_grad()
+def velodyne_depth(points, offsets, P_velo2im, H, W):
+    """generate_depth_map (:148-191) of B sweeps of one frame size on the device (ccb_velo_depth): points float32 [total,4]
+    (the sweeps one after the other), offsets int64 [B+1], P_velo2im fp64 [B,3,4] -> depth fp64 [B,H,W].  KITTI frames
+    come in a few sizes: group them by size, one call per size.  No host synchronisation."""
+    points, offsets, P = points.detach().contiguous(), offsets.detach().contiguous(), P_velo2im.detach().contiguous()
+    B = int(offsets.shape[0]) - 1
+    assert points.dim() == 2 and points.shape[1] == 4 and P.shape == (B, 3, 4), (points.shape, offsets.shape, P.shape)
+    work, nbytes = _lib.workspace('ccb_velo_depth_workspace_bytes', B, int(H), int(W), like=P)
+    depth = torch.empty(B, int(H), int(W), device=P.device, dtype=torch.float64)
+    _lib.call('ccb_velo_depth', points, offsets, P, int(points.shape[0]), B, int(H), int(W), work, nbytes, depth, P)
+    return depth
+
+
+@torch.no_grad()
+def spline_zoom(x, H, W, lo, hi):
+    """scipy.ndimage.zoom(x[n], (H/h, W/w), order=3).clip(lo, hi) of every image of x [N,h,w] on the device
+    (ccb_spline_zoom) -> fp32 [N,H,W].  No host synchronisation."""
+    x = _lib.f32(x)
+    N, h, w = (int(v) for v in x.shape)
+    work, nbytes = _lib.workspace('ccb_spline_zoom_workspace_bytes', N, h, w, like=x)
+    out = torch.empty(N, int(H), int(W), device=x.device)
+    _lib.call('ccb_spline_zoom', x, N, h, w, int(H), int(W), float(lo), float(hi), work, nbytes, out, x)
+    return out
+
+
+# generate_mask crops as fractions of (H, H, W, W): kitti_eval (Garg ECCV16, :194-206) and stillbox_eval (:68-80)
+CROPS = {'eigen': (0.40810811, 0.99189189, 0.03594771, 0.96405229), 'stillbox': (0.05, 0.95, 0.05, 0.95)}
+
+
+@torch.no_grad()
+def depth_errors(gt, pred, min_depth=1e-3, max_depth=80.0, crop='eigen', poses=None, displacements=None):
+    """The errors of test_disp.py:124-141 (compute_errors :171-187) per sample on the device (ccb_eigen_depth_errors):
+    gt fp64 [B,H,W], pred the zoomed and clipped prediction fp32 [B,H,W], crop a name of CROPS or four fractions, poses
+    [B,R,6] and displacements [B,R] (optional) -> fp64 [B,2,7] (abs_rel sq_rel rms log_rms a1 a2 a3); row 0 scaled by
+    PoseNet (zeros without poses), row 1 by the median ratio.  No host synchronisation."""
+    gt = gt.detach().to(torch.float64).contiguous()
+    pred = _lib.f32(pred)
+    B, H, W = (int(v) for v in gt.shape)
+    assert pred.shape == (B, H, W), (gt.shape, pred.shape)
+    fr = [float(f) for f in (CROPS[crop] if isinstance(crop, str) else crop)]
+    R = 0
+    if poses is not None:
+        poses = _lib.f32(poses)
+        R = int(poses.shape[1])
+        displacements = torch.as_tensor(displacements, dtype=torch.float64).to(gt.device).contiguous()
+        assert poses.shape == (B, R, 6) and displacements.shape == (B, R), (poses.shape, displacements.shape)
+    work, nbytes = _lib.workspace('ccb_eigen_depth_errors_workspace_bytes', B, H, W, like=gt)
+    out = torch.empty(B, 2, 7, device=gt.device, dtype=torch.float64)
+    _lib.call('ccb_eigen_depth_errors', gt, pred, B, H, W, float(min_depth), float(max_depth), fr, poses, displacements, R, work,
+              nbytes, out, gt)
+    return out
+
+
+@torch.no_grad()
+def depth_eval_batch(disp_net, tgt, gt_depth, min_depth=1e-3, max_depth=80.0, crop='eigen', pose_net=None, refs=None,
+                     displacements=None, spatial_normalize=False):
+    """test_disp.py:100-141 for a batch: tgt [B,3,h,w] and refs (list of [B,3,h,w]) normalised device tensors (DeviceScale
+    makes them from uint8 frames), gt_depth fp64 [B,H,W] (velodyne_depth), displacements [B,R] -> fp64 [B,2,7] on the
+    device, row 0 scaled by the pose net's displacements (zeros without a pose net), row 1 by the median ratio.  The pose
+    net may return PoseExpNet's (mask, pose).  No host synchronisation."""
+    disp_net.eval()
+    disp = disp_net(tgt)
+    if spatial_normalize:
+        disp = LF.spatial_normalize(disp)
+    H, W = int(gt_depth.shape[1]), int(gt_depth.shape[2])
+    pred = spline_zoom(1 / disp[:, 0], H, W, min_depth, max_depth)
+    poses = None
+    if pose_net is not None:
+        pose_net.eval()
+        res = pose_net(tgt, refs)
+        poses = res[1] if isinstance(res, tuple) else res
+    return depth_errors(gt_depth, pred, min_depth, max_depth, crop, poses, displacements if poses is not None else None)
+
+
+def depth_summary(per_sample):
+    """The rows test_disp.py prints (:143-158) from the [N,2,7] per-sample errors of a dataset: stored as float32 like the
+    script's `errors`, then averaged over the samples -> float32 [2,7]."""
+    per_sample = np.asarray(per_sample)
+    errors = np.zeros((2, 7, per_sample.shape[0]), np.float32)
+    errors[:] = per_sample.transpose(1, 2, 0)
+    return errors.mean(2)

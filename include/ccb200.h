@@ -381,6 +381,32 @@ int ccb_flow_color(const float* flow, int B, int P, int H, int W, void* work, lo
 long long ccb_kitti_flow_errors_workspace_bytes(int B, int H, int W);
 int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned short* pred, int B, int H, int W, void* work,
                           long long work_bytes, double* out, long long* counts, ccb_stream_t stream);
+/* Depth evaluation of test_disp.py on the device, no host sync.
+ * ccb_velo_depth: KITTI ground truth of B velodyne sweeps (kitti_eval/depth_evaluation_utils.py generate_depth_map
+ *   :148-191).  points [total,4] fp32 (column 3 is not read), offsets [B+1] int64 (sample b owns points
+ *   offsets[b] .. offsets[b+1]-1; malformed offsets give the sample no point), P_velo2im [B,3,4] fp64 -> depth [B,H,W] fp64.
+ *   Points with x >= 0 are projected in fp64, u = round(X/Z) - 1 and v = round(Y/Z) - 1 half to even, kept inside the
+ *   frame; each pixel takes the Z of its last point; for every sub2ind key v*(W-1) + u - 1 shared by several points the
+ *   pixel of the first of them takes their least Z; negative depths become 0.  Integer atomics: the same bits every run.
+ * ccb_spline_zoom: scipy.ndimage.zoom(order=3) of src [N,h,w] fp32 to dst [N,H,W] fp32 (mirror-initialised cubic
+ *   B-spline prefilter along rows then columns, evaluation at o*(n-1)/(m-1), all in fp64), then clip(lo, hi) in fp32.
+ * ccb_eigen_depth_errors: the errors of one sample each (test_disp.py:124-141, compute_errors :171-187) of gt [B,H,W] fp64
+ *   and the zoomed, clipped prediction pred [B,H,W] fp32 over mask = min_depth < gt < max_depth inside the crop
+ *   crop (host, 4 fractions in [0,1]: rows [int(crop[0]*H), int(crop[1]*H)), columns [int(crop[2]*W), int(crop[3]*W))).
+ *   out [B,2,7] fp64 = abs_rel sq_rel rms log_rms a1 a2 a3; row 1 scales pred by median(gt)/median(pred) (numpy medians),
+ *   row 0 by the mean of displacements/|poses[:3]| over the displacements > 0 (0 if none; poses [B,R,6] fp32,
+ *   displacements [B,R] fp64), zeros when poses is NULL.  a1..a3 are exact counts; the other sums are fp64 block partials
+ *   with a fixed-order finalize. */
+long long ccb_velo_depth_workspace_bytes(int B, int H, int W);
+int ccb_velo_depth(const float* points, const long long* offsets, const double* P_velo2im, long long total, int B, int H, int W,
+                   void* work, long long work_bytes, double* depth, ccb_stream_t stream);
+long long ccb_spline_zoom_workspace_bytes(int N, int h, int w);
+int ccb_spline_zoom(const float* src, int N, int h, int w, int H, int W, float lo, float hi, void* work, long long work_bytes,
+                    float* dst, ccb_stream_t stream);
+long long ccb_eigen_depth_errors_workspace_bytes(int B, int H, int W);
+int ccb_eigen_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
+                           const double* crop, const float* poses, const double* displacements, int R, void* work,
+                           long long work_bytes, double* out, ccb_stream_t stream);
 /* Input pipeline on the device (train.py:448-451 H2D + custom_transforms.py:21-30,47-118): uint8 HWC frames
  * src [B,F,Hs,Ws,3] -> F normalised fp32 NCHW tensors dst[f] [B,3,H,W] = (v/255 - .5)/.5, per sample horizontally
  * flipped (params[b][0] != 0) and scale-cropped: resized by (params[b][1], params[b][2]) = (scaled_w/Ws, scaled_h/Hs)
