@@ -178,6 +178,11 @@ _SIGS = {
     'ccb_eigen_depth_errors_workspace_bytes': ('long long', 'int, int, int'),
     'ccb_eigen_depth_errors': (STATUS, 'const double*, const float*, int, int, int, double, double, host const double*, '
                                        'const float*, const double*, int, void*, long long, double*, ccb_stream_t'),
+    'ccb_bytescale_u8_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_bytescale_u8': (STATUS, 'const unsigned char*, int, int, int, void*, long long, unsigned char*, ccb_stream_t'),
+    'ccb_make3d_depth_errors_workspace_bytes': ('long long', 'int, int, int'),
+    'ccb_make3d_depth_errors': (STATUS, 'const double*, const float*, int, int, int, double, double, void*, long long, '
+                                        'double*, ccb_stream_t'),
     'ccb_prep_frames': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, int, '
                                 'int, int, ccb_stream_t'),
     'ccb_prep_frames_unit': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '

@@ -13,6 +13,7 @@
 //
 //   N3  motion segmentation scores: the three rigidity masks and the IoU counts of test_mask.py:129-156,224-262
 //       depth evaluation of test_disp.py:98-141: the velodyne ground truth, scipy's cubic zoom, both scalings' errors
+//       Make3D depth evaluation of test_make3d.py:97-148: imresize's contrast stretch, the capped median scaling, log10
 //
 // All floating-point reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize); the
 // segmentation counts are integer sums (atomics, the same in any order).
@@ -1145,6 +1146,8 @@ struct EigenArgs {
     double* partials;               // [B][blocks][2][7]
     double* out;                    // [B, 2, 7]
     double min_depth, max_depth;
+    double cap;                     // scaled predictions above it become it (test_make3d.py:147; +inf: no cap)
+    int log10;                      // log_rms of log10 (test_make3d.py:183) instead of ln
     int B, H, W, R, y1, y2, x1, x2;
 };
 
@@ -1267,13 +1270,14 @@ __global__ void __launch_bounds__(256) eigen_errors_kernel(const EigenArgs a) {
         const double g = __ldg(a.gt + b * hw + i);
         if (!eigen_valid(a, g, y, x)) continue;
         const double p32 = (double)__ldg(a.pred + b * hw + i);
-        const double lg = log(g);
+        const double lg = a.log10 ? log10(g) : log(g);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             if (r < r0) continue;
-            const double p = __dmul_rn(p32, sc[r]);
+            double p = __dmul_rn(p32, sc[r]);
+            if (p > a.cap) p = a.cap;
             const double th = nan_max(__ddiv_rn(g, p), __ddiv_rn(p, g));
-            const double d = __dsub_rn(g, p), d2 = __dmul_rn(d, d), dl = __dsub_rn(lg, log(p));
+            const double d = __dsub_rn(g, p), d2 = __dmul_rn(d, d), dl = __dsub_rn(lg, a.log10 ? log10(p) : log(p));
             double* o = acc + 7 * r;
             o[0] += __ddiv_rn(fabs(d), g);
             o[1] += __ddiv_rn(d2, g);
@@ -1312,6 +1316,64 @@ __global__ void eigen_finalize_kernel(const EigenArgs a, int nblk) {
     o[2] = __dsqrt_rn(__ddiv_rn(s[2], n));
     o[3] = __dsqrt_rn(__ddiv_rn(s[3], n));
     for (int j = 4; j < 7; ++j) o[j] = __ddiv_rn(s[j], n);
+}
+
+// ================================================================================================
+// The contrast stretch scipy.misc.imresize gives a float32 image before Pillow resizes it (test_make3d.py:100-102; scipy
+// 1.1 imresize -> toimage -> bytescale): over the whole HxWx3 image, in float32 with each operation rounded on its own,
+//   cscale = cmax - cmin (1 when 0), scale = 255 / cscale, u8 = trunc(clip((x - cmin) * scale, 0, 255) + 0.5).
+// The frames hold the integers 0..255, so a table of the 256 values is the whole map.  The range is taken with integer
+// atomics (the largest value and the largest 255 - value), the same in any order.
+struct ByteScaleArgs {
+    const unsigned char* src;       // [N][len]
+    unsigned char* dst;             // [N][len]
+    unsigned long long* range;      // [N][2]: max, 255 - min
+    long long len;                  // H * W * 3
+};
+
+__global__ void __launch_bounds__(256) bytescale_range_kernel(const ByteScaleArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ unsigned red[2][256];
+    const int n = blockIdx.y, t = threadIdx.x;
+    const unsigned char* s = a.src + (long long)n * a.len;
+    unsigned hi = 0, lo = 0;
+    for (long long i = (long long)blockIdx.x * 256 + t; i < a.len; i += (long long)gridDim.x * 256) {
+        const unsigned v = s[i];
+        hi = v > hi ? v : hi;
+        lo = 255u - v > lo ? 255u - v : lo;
+    }
+    red[0][t] = hi;
+    red[1][t] = lo;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (t < o) {
+            red[0][t] = red[0][t + o] > red[0][t] ? red[0][t + o] : red[0][t];
+            red[1][t] = red[1][t + o] > red[1][t] ? red[1][t + o] : red[1][t];
+        }
+        __syncthreads();
+    }
+    if (t == 0) {
+        atomicMax(a.range + 2 * n, (unsigned long long)red[0][0]);
+        atomicMax(a.range + 2 * n + 1, (unsigned long long)red[1][0]);
+    }
+}
+
+// 256 threads: every block builds its image's table, then maps its share of the bytes
+__global__ void __launch_bounds__(256) bytescale_apply_kernel(const ByteScaleArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ unsigned char table[256];
+    const int n = blockIdx.y, t = threadIdx.x;
+    const float cmax = (float)a.range[2 * n], cmin = (float)(255ull - a.range[2 * n + 1]);
+    float cscale = __fsub_rn(cmax, cmin);
+    if (cscale == 0.f) cscale = 1.f;
+    const float scale = __fdiv_rn(255.f, cscale);
+    float v = __fmul_rn(__fsub_rn((float)t, cmin), scale);
+    v = v < 0.f ? 0.f : (v > 255.f ? 255.f : v);
+    table[t] = (unsigned char)__fadd_rn(v, 0.5f);
+    __syncthreads();
+    const unsigned char* s = a.src + (long long)n * a.len;
+    unsigned char* d = a.dst + (long long)n * a.len;
+    for (long long i = (long long)blockIdx.x * 256 + t; i < a.len; i += (long long)gridDim.x * 256) d[i] = table[s[i]];
 }
 
 }  // namespace ccb
@@ -1546,6 +1608,25 @@ extern "C" long long ccb_eigen_depth_errors_workspace_bytes(int B, int H, int W)
     return eigen_plan(B, H, W).bytes;
 }
 
+// a (validated) EigenArgs with the workspace laid out and the selections cleared, then the launches
+static int eigen_errors_launch(const char* what, EigenArgs a, void* work, ccb_stream_t stream) {
+    const EigenPlan p = eigen_plan(a.B, a.H, a.W);
+    char* w = (char*)work;
+    a.partials = (double*)(w + p.partials); a.sel = (unsigned long long*)(w + p.sel); a.count = (unsigned long long*)(w + p.count);
+    a.scale = (double*)(w + p.scale); a.hist = (unsigned*)(w + p.hist);
+    const int B = a.B;
+    cudaMemsetAsync(w + p.sel, 0, (size_t)(p.bytes - p.sel), (cudaStream_t)stream);
+    const int nb = eigen_blocks(a.H, a.W);
+    for (int pass = 0; pass < 6; ++pass) {
+        CCB_LAUNCH(eigen_hist_kernel, dim3(nb, B), dim3(256), 0, stream, a, pass);
+        CCB_LAUNCH(eigen_select_kernel, dim3((B * 4 + 63) / 64), dim3(64), 0, stream, a, pass);
+    }
+    CCB_LAUNCH(eigen_scale_kernel, dim3((B + 63) / 64), dim3(64), 0, stream, a);
+    CCB_LAUNCH(eigen_errors_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(eigen_finalize_kernel, dim3((B * 2 + 63) / 64), dim3(64), 0, stream, a, nb);
+    return check_launch(what);
+}
+
 extern "C" int ccb_eigen_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
                                       const double* crop, const float* poses, const double* displacements, int R, void* work,
                                       long long work_bytes, double* out, ccb_stream_t stream) {
@@ -1555,27 +1636,31 @@ extern "C" int ccb_eigen_depth_errors(const double* gt, const float* pred, int B
     CCB_REQUIRE(B > 0 && H > 0 && W > 0 && (poses == nullptr || R > 0), CCB_ERR_ARG, "eigen_depth_errors: bad sizes");
     for (int k = 0; k < 4; ++k)
         CCB_REQUIRE(crop[k] >= 0.0 && crop[k] <= 1.0, CCB_ERR_ARG, "eigen_depth_errors: crop fraction %d outside [0, 1]", k);
-    const EigenPlan p = eigen_plan(B, H, W);
-    CCB_REQUIRE_WORK("eigen_depth_errors", "work", work, work_bytes, p.bytes);
+    CCB_REQUIRE_WORK("eigen_depth_errors", "work", work, work_bytes, eigen_plan(B, H, W).bytes);
     EigenArgs a;
-    char* w = (char*)work;
     a.gt = gt; a.pred = pred; a.poses = poses; a.disp = displacements; a.out = out;
-    a.partials = (double*)(w + p.partials); a.sel = (unsigned long long*)(w + p.sel); a.count = (unsigned long long*)(w + p.count);
-    a.scale = (double*)(w + p.scale); a.hist = (unsigned*)(w + p.hist);
-    a.min_depth = min_depth; a.max_depth = max_depth;
+    a.min_depth = min_depth; a.max_depth = max_depth; a.cap = HUGE_VAL; a.log10 = 0;
     a.B = B; a.H = H; a.W = W; a.R = poses ? R : 0;
     // generate_mask: np.array([f0 * H, f1 * H, f2 * W, f3 * W]).astype(np.int32), fp64 products truncated
     a.y1 = (int)(crop[0] * H); a.y2 = (int)(crop[1] * H); a.x1 = (int)(crop[2] * W); a.x2 = (int)(crop[3] * W);
-    cudaMemsetAsync(w + p.sel, 0, (size_t)(p.bytes - p.sel), (cudaStream_t)stream);
-    const int nb = eigen_blocks(H, W);
-    for (int pass = 0; pass < 6; ++pass) {
-        CCB_LAUNCH(eigen_hist_kernel, dim3(nb, B), dim3(256), 0, stream, a, pass);
-        CCB_LAUNCH(eigen_select_kernel, dim3((B * 4 + 63) / 64), dim3(64), 0, stream, a, pass);
-    }
-    CCB_LAUNCH(eigen_scale_kernel, dim3((B + 63) / 64), dim3(64), 0, stream, a);
-    CCB_LAUNCH(eigen_errors_kernel, dim3(nb, B), dim3(256), 0, stream, a);
-    CCB_LAUNCH(eigen_finalize_kernel, dim3((B * 2 + 63) / 64), dim3(64), 0, stream, a, nb);
-    return check_launch("eigen_depth_errors");
+    return eigen_errors_launch("eigen_depth_errors", a, work, stream);
+}
+
+extern "C" long long ccb_make3d_depth_errors_workspace_bytes(int B, int H, int W) {
+    return ccb_eigen_depth_errors_workspace_bytes(B, H, W);
+}
+
+extern "C" int ccb_make3d_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
+                                       void* work, long long work_bytes, double* out, ccb_stream_t stream) {
+    CCB_REQUIRE(gt && pred && out, CCB_ERR_ARG, "make3d_depth_errors: null pointer");
+    CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "make3d_depth_errors: bad sizes");
+    CCB_REQUIRE_WORK("make3d_depth_errors", "work", work, work_bytes, eigen_plan(B, H, W).bytes);
+    EigenArgs a;
+    a.gt = gt; a.pred = pred; a.poses = nullptr; a.disp = nullptr; a.out = out;
+    a.min_depth = min_depth; a.max_depth = max_depth; a.cap = max_depth; a.log10 = 1;
+    a.B = B; a.H = H; a.W = W; a.R = 0;
+    a.y1 = 0; a.y2 = H; a.x1 = 0; a.x2 = W;        // no crop: the mask is the depth range alone
+    return eigen_errors_launch("make3d_depth_errors", a, work, stream);
 }
 
 template <bool UNIT>
@@ -1674,6 +1759,30 @@ extern "C" int ccb_resize_u8(const unsigned char* src, unsigned char* dst, int N
         CCB_LAUNCH(resample_pass_kernel, dim3(grid_for((long long)N * H * W)), dim3(256), 0, stream, r);
     }
     return check_launch("resize_u8");
+}
+
+static int bytescale_blocks(long long len) {
+    const long long g = (len + 8191) / 8192;
+    return (int)(g < 1 ? 1 : (g > 256 ? 256 : g));
+}
+
+extern "C" long long ccb_bytescale_u8_workspace_bytes(int N, int H, int W) {
+    if (N <= 0 || H <= 0 || W <= 0) return -1;
+    return (long long)N * 2 * (long long)sizeof(unsigned long long);
+}
+
+extern "C" int ccb_bytescale_u8(const unsigned char* src, int N, int H, int W, void* work, long long work_bytes, unsigned char* dst,
+                                ccb_stream_t stream) {
+    CCB_REQUIRE(src && dst, CCB_ERR_ARG, "bytescale_u8: null pointer");
+    CCB_REQUIRE(N > 0 && H > 0 && W > 0, CCB_ERR_ARG, "bytescale_u8: bad sizes");
+    CCB_REQUIRE_WORK("bytescale_u8", "work", work, work_bytes, ccb_bytescale_u8_workspace_bytes(N, H, W));
+    ByteScaleArgs a;
+    a.src = src; a.dst = dst; a.range = (unsigned long long*)work; a.len = (long long)H * W * 3;
+    cudaMemsetAsync(work, 0, (size_t)N * 2 * sizeof(unsigned long long), (cudaStream_t)stream);
+    const dim3 grid(bytescale_blocks(a.len), N);
+    CCB_LAUNCH(bytescale_range_kernel, grid, dim3(256), 0, stream, a);
+    CCB_LAUNCH(bytescale_apply_kernel, grid, dim3(256), 0, stream, a);
+    return check_launch("bytescale_u8");
 }
 
 static int normlocal_blocks(int H, int W) {

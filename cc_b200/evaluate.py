@@ -11,6 +11,10 @@
   depth_eval_batch      test_disp.py:98-141 for a batch on the device, no host synchronisation
                         (velodyne_depth: generate_depth_map's ground truth; spline_zoom: scipy's zoom(order=3);
                         depth_errors: both scalings and compute_errors; depth_summary: the script's printed rows)
+  make3d_eval_batch     test_make3d.py:97-148 for a batch on the device, no host synchronisation
+                        (make3d_files / load_make3d: test_framework's files and samples; make3d_frames: imresize's contrast
+                        stretch, Pillow's resize and the normalisation; make3d_depth_errors: the capped median scaling and
+                        compute_errors :174-190 with log10; depth_summary: the printed row, row 1)
 
 The scripts' dataset crawlers, image IO and visualisation are out of scope (SURVEY.md section 2); these functions take what the
 reference's `test_framework` iterators yield (uint8 HxWx3 frames, ground truth arrays) and return what the scripts
@@ -396,3 +400,92 @@ def depth_summary(per_sample):
     errors = np.zeros((2, 7, per_sample.shape[0]), np.float32)
     errors[:] = per_sample.transpose(1, 2, 0)
     return errors.mean(2)
+
+
+# ------------------------------------------------------------------------------------------------
+# test_make3d.py on the device: imresize's contrast stretch and resize, the zoom and the capped, log10 errors
+
+MAKE3D_ROWS = ((2272 - 852) // 2, (2272 + 852) // 2)       # test_make3d.py:50,62: the image rows kept, whatever its height
+MAKE3D_GT_ROWS = ((55 - 21) // 2, (55 + 21) // 2)           # :51,66: the ground-truth rows kept
+
+
+def make3d_files(root):
+    """test_framework's file lists (test_make3d.py:41-46): the sorted Test134/*.jpg and Gridlaserdata/*.mat under `root`,
+    element 61 popped from each (a corrupted file of the original dataset).  The lists are paired by index, not by name."""
+    import glob
+    import os
+    img_files = sorted(glob.glob(os.path.join(root, 'Test134', '*.jpg')))
+    depth_files = sorted(glob.glob(os.path.join(root, 'Gridlaserdata', '*.mat')))
+    img_files.pop(61)
+    depth_files.pop(61)
+    return img_files, depth_files
+
+
+def load_make3d(img_file, depth_file, min_depth=1e-3, max_depth=70.0):
+    """One sample of test_framework (test_make3d.py:53-71): {'tgt': uint8 [852,W,3] image rows 710:1562 (the reference's
+    float32 copy holds the same integers), 'gt_depth': fp64 [21,C] rows 17:38 of Position3DGrid[:, :, 3],
+    'mask': min_depth < gt_depth < max_depth}."""
+    from PIL import Image
+    from scipy import io
+    tgt = np.array(Image.open(img_file))[MAKE3D_ROWS[0]:MAKE3D_ROWS[1]]
+    gt = io.loadmat(depth_file)['Position3DGrid'][:, :, 3][MAKE3D_GT_ROWS[0]:MAKE3D_GT_ROWS[1]]
+    return {'tgt': tgt, 'gt_depth': gt, 'mask': np.logical_and(gt > min_depth, gt < max_depth)}
+
+
+def _on_library_device(a):
+    """A tensor as it is; a numpy array copied to the library's device (the current CUDA device, or the CPU simulator)."""
+    if torch.is_tensor(a):
+        return a.contiguous()
+    dev = torch.device('cpu') if _lib.is_simulator() else torch.device('cuda')
+    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+
+
+@torch.no_grad()
+def make3d_frames(crops_u8, h=256, w=256, resize=True):
+    """The net input of test_make3d.py:98-106 for a batch: crops_u8 uint8 [B,Hs,Ws,3] (load_make3d's 'tgt'; numpy arrays
+    go to the library's device) -> normalised fp32 [B,3,h,w] (or [B,3,Hs,Ws] without resizing).  Unless resize is False
+    or the crops already are h x w, each crop is contrast-stretched as scipy.misc.imresize stretches a float32 image
+    (input_pipeline.bytescale_frames) and resized as Pillow's BILINEAR (resize_frames); then (x/255 - 0.5)/0.5.
+    No host synchronisation."""
+    from .input_pipeline import bytescale_frames, resize_frames, _prep
+    src = _on_library_device(crops_u8)
+    assert src.dtype == torch.uint8 and src.dim() == 4 and src.size(3) == 3, (src.dtype, src.shape)
+    B, Hs, Ws = (int(v) for v in src.shape[:3])
+    if resize and (Hs, Ws) != (h, w):
+        src = resize_frames(bytescale_frames(src), h, w)
+    H, W = int(src.shape[1]), int(src.shape[2])
+    par = torch.zeros(B, 4, device=src.device)                 # no flip, scale 1 (filled on the device: capturable)
+    par[:, 1:3] = 1.0
+    offs = torch.zeros(B, 2, dtype=torch.int32, device=src.device)
+    return _prep(src, par, offs, B, 1, H, W, H, W, 'global')[0][0]
+
+
+@torch.no_grad()
+def make3d_depth_errors(gt, pred, min_depth=1e-3, max_depth=70.0):
+    """The errors of test_make3d.py:141-148 (compute_errors :174-190) per sample on the device (ccb_make3d_depth_errors):
+    gt fp64 [B,H,W], pred the zoomed and clipped prediction fp32 [B,H,W] -> fp64 [B,2,7] (abs_rel sq_rel rms log_rms a1 a2
+    a3).  Row 0 is zeros, as the script leaves it; row 1 scales by the median ratio over min_depth < gt < max_depth (no
+    crop), caps the scaled prediction at max_depth and takes log_rms in log10.  An empty mask gives a NaN row.  No host
+    synchronisation."""
+    gt = gt.detach().to(torch.float64).contiguous()
+    pred = _lib.f32(pred)
+    B, H, W = (int(v) for v in gt.shape)
+    assert pred.shape == (B, H, W), (gt.shape, pred.shape)
+    work, nbytes = _lib.workspace('ccb_make3d_depth_errors_workspace_bytes', B, H, W, like=gt)
+    out = torch.empty(B, 2, 7, device=gt.device, dtype=torch.float64)
+    _lib.call('ccb_make3d_depth_errors', gt, pred, B, H, W, float(min_depth), float(max_depth), work, nbytes, out, gt)
+    return out
+
+
+@torch.no_grad()
+def make3d_eval_batch(disp_net, crops_u8, gt_depth, h=256, w=256, min_depth=1e-3, max_depth=70.0, resize=True):
+    """test_make3d.py:97-148 for a batch: crops_u8 uint8 [B,852,W,3] and gt_depth fp64 [B,21,C] (load_make3d's 'tgt' and
+    'gt_depth', stacked; numpy arrays go to the library's device), disp_net any disparity net of cc_b200.models ->
+    fp64 [B,2,7] on the device, row 1 the script's errors and row 0 zeros (depth_summary gives the printed row).
+    No host synchronisation."""
+    disp_net.eval()
+    disp = disp_net(make3d_frames(crops_u8, h, w, resize))
+    gt = _on_library_device(gt_depth)
+    H, W = int(gt.shape[1]), int(gt.shape[2])
+    pred = spline_zoom(1 / disp[:, 0], H, W, min_depth, max_depth)
+    return make3d_depth_errors(gt, pred, min_depth, max_depth)

@@ -23,7 +23,8 @@ The reference's other transforms run on the device as well, bit-exact with Pillo
     the uint8 frames as Pillow's BILINEAR resize does (ccb_resize_u8, antialiased on a downscale), then normalises.
 The reference's loaders hand scipy.misc float32 copies of the uint8 frames (load_as_float), and scipy.misc byte-scales a
 float image to its own [min, max] before resampling; this pipeline takes the uint8 frames as they are, which is the
-same whenever a frame spans 0..255."""
+same whenever a frame spans 0..255.  bytescale_frames restates that stretch where an evaluation needs it (Make3D,
+cc_b200.evaluate.make3d_frames)."""
 import math
 import random
 import numpy as np
@@ -105,6 +106,18 @@ def resize_frames(src, h, w):
     dst = torch.empty(tuple(src.shape[:-3]) + (h, w, 3), dtype=torch.uint8, device=src.device)
     work, nb = _lib.workspace('ccb_resize_u8_workspace_bytes', N, Hs, Ws, h, w, like=src)
     _lib.call('ccb_resize_u8', src, dst, N, Hs, Ws, h, w, work, nb, src)
+    return dst
+
+
+def bytescale_frames(src):
+    """src [..., H, W, 3] uint8 on the device -> the contrast stretch scipy.misc.imresize gives a float32 copy of each image
+    before resizing it (scipy 1.1 bytescale: its [min, max] onto [0, 255] in float32), uint8 of the same shape
+    (ccb_bytescale_u8)."""
+    H, W = src.shape[-3], src.shape[-2]
+    N = src.numel() // (H * W * 3)
+    dst = torch.empty_like(src)
+    work, nb = _lib.workspace('ccb_bytescale_u8_workspace_bytes', N, H, W, like=src)
+    _lib.call('ccb_bytescale_u8', src, N, H, W, work, nb, dst, src)
     return dst
 
 

@@ -407,6 +407,23 @@ long long ccb_eigen_depth_errors_workspace_bytes(int B, int H, int W);
 int ccb_eigen_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
                            const double* crop, const float* poses, const double* displacements, int R, void* work,
                            long long work_bytes, double* out, ccb_stream_t stream);
+/* Make3D depth evaluation of test_make3d.py on the device, no host sync.
+ * ccb_bytescale_u8: the contrast stretch scipy.misc.imresize (scipy 1.1: toimage -> bytescale) applies to a float32 image
+ *   before Pillow resizes it (test_make3d.py:100-102), of src [N,H,W,3] uint8 (the float32 frame holds integers) into
+ *   dst [N,H,W,3] uint8: over each whole image cmin, cmax, cscale = cmax - cmin (1 when 0), scale = 255 / cscale and
+ *   dst = trunc(clip((src - cmin) * scale, 0, 255) + 0.5), every operation rounded in float32 on its own (no fused
+ *   multiply-add).  The range is taken with integer atomics: the same bytes every run.
+ * ccb_make3d_depth_errors: the errors of one sample each (test_make3d.py:139-148, compute_errors :174-190) of gt [B,H,W]
+ *   fp64 and the zoomed, clipped prediction pred [B,H,W] fp32 over mask = min_depth < gt < max_depth (no crop).
+ *   out [B,2,7] fp64: row 0 zeros (the script never writes it), row 1 = abs_rel sq_rel rms log_rms a1 a2 a3 of
+ *   min(pred * median(gt)/median(pred), max_depth) with numpy's medians, the product in fp64, and log_rms of log10.
+ *   An empty mask gives a NaN row.  The workspace and the reductions are those of ccb_eigen_depth_errors. */
+long long ccb_bytescale_u8_workspace_bytes(int N, int H, int W);
+int ccb_bytescale_u8(const unsigned char* src, int N, int H, int W, void* work, long long work_bytes, unsigned char* dst,
+                     ccb_stream_t stream);
+long long ccb_make3d_depth_errors_workspace_bytes(int B, int H, int W);
+int ccb_make3d_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
+                            void* work, long long work_bytes, double* out, ccb_stream_t stream);
 /* Input pipeline on the device (train.py:448-451 H2D + custom_transforms.py:21-30,47-118): uint8 HWC frames
  * src [B,F,Hs,Ws,3] -> F normalised fp32 NCHW tensors dst[f] [B,3,H,W] = (v/255 - .5)/.5, per sample horizontally
  * flipped (params[b][0] != 0) and scale-cropped: resized by (params[b][1], params[b][2]) = (scaled_w/Ws, scaled_h/Hs)
