@@ -93,15 +93,16 @@ extern thread_local WCache* g_cur_wcache;
 #endif
 
 // ---- small device helpers ----
-__device__ __forceinline__ float warp_sum(float v) {
+template <class T>
+__device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
 
-// Block-wide sum of NV values per thread; result valid in thread 0.  `scratch` holds >= NV*32 floats.
-template <int NV>
-__device__ __forceinline__ void block_sum(float (&v)[NV], float* scratch) {
+// Block-wide sum of NV values per thread (float or double); result valid in thread 0.  `scratch` holds >= NV*32 values.
+template <int NV, class T>
+__device__ __forceinline__ void block_sum(T (&v)[NV], T* scratch) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
 #pragma unroll
     for (int i = 0; i < NV; ++i) v[i] = warp_sum(v[i]);
@@ -114,7 +115,7 @@ __device__ __forceinline__ void block_sum(float (&v)[NV], float* scratch) {
     if (warp == 0) {
 #pragma unroll
         for (int i = 0; i < NV; ++i) {
-            float x = (lane < nwarps) ? scratch[i * 32 + lane] : 0.f;
+            T x = (lane < nwarps) ? scratch[i * 32 + lane] : T(0);
             v[i] = warp_sum(x);
         }
     }

@@ -55,27 +55,127 @@ __device__ __forceinline__ float bilerp(const float* __restrict__ p, int w, cons
            ly.w1 * (lx.w0 * __ldg(p + ly.i1 * w + lx.i0) + lx.w1 * __ldg(p + ly.i1 * w + lx.i1));
 }
 
+// s[j] = the sum over blocks k < nblk of p[k * stride + j], j < NV: the fp64 block partials of one reduction in block order,
+// a fixed order that gives the same bits on every run.
 template <int NV>
-__device__ __forceinline__ void block_sum_d(double (&v)[NV], double* scratch) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
+__device__ __forceinline__ void sum_partials(const double* p, int nblk, int stride, double (&s)[NV]) {
+    for (int j = 0; j < NV; ++j) s[j] = 0.0;
+    for (int k = 0; k < nblk; ++k)
+        for (int j = 0; j < NV; ++j) s[j] += p[(long long)k * stride + j];
+}
+
+// The maximum of m over the warp, then one atomicMax per warp into *dst.  The callers' keys are in the order they want,
+// and a maximum is the same in any order.
+template <class T>
+__device__ __forceinline__ void warp_max_into(unsigned long long* dst, T m) {
 #pragma unroll
-    for (int i = 0; i < NV; ++i)
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], o);
-    __syncthreads();
-    if (lane == 0)
-#pragma unroll
-        for (int i = 0; i < NV; ++i) scratch[i * 32 + warp] = v[i];
-    __syncthreads();
-    if (warp == 0) {
-#pragma unroll
-        for (int i = 0; i < NV; ++i) {
-            double x = (lane < nwarps) ? scratch[i * 32 + lane] : 0.0;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-            v[i] = x;
-        }
+    for (int o = 16; o > 0; o >>= 1) {
+        const T k = __shfl_xor_sync(0xffffffffu, m, o);
+        m = (k > m) ? k : m;
     }
+    if ((threadIdx.x & 31) == 0) atomicMax(dst, (unsigned long long)m);
+}
+
+// Order-preserving keys: the unsigned order of the key is the value order of the float / double (NaN is not ordered).
+__device__ __forceinline__ unsigned ordered_key32(float f) {
+    const unsigned k = __float_as_uint(f);
+    return (k >> 31) ? ~k : (k | 0x80000000u);
+}
+__device__ __forceinline__ float ordered_value32(unsigned k) {
+    return __uint_as_float((k >> 31) ? (k & 0x7fffffffu) : ~k);
+}
+__device__ __forceinline__ unsigned long long ordered_key(double d) {
+    const unsigned long long k = (unsigned long long)__double_as_longlong(d);
+    return (k >> 63) ? ~k : (k | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double ordered_value(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// ================================================================================================
+// Per-sample medians by radix select, for compute_errors (loss_functions.py:430-467), test_disp.py:124-141 and
+// test_make3d.py:141-148.  The argument struct A of a caller gives
+//   A::Key         the key type: 32 bits take 3 passes (11, 11, 10 bits), 64 bits 6 passes (11 x 5, then 9)
+//   A::SEL         the selections per sample
+//   A::UPPER       bit s set: selection s takes the upper middle rank n/2 (numpy's second middle value), else the lower
+//                  middle (n-1)/2 (torch.median, numpy's first); the two are the same rank when n is odd
+//   a.median_keys  the valid flag and the SEL order-preserving keys of element i of sample b
+//   a.med          the select's state
+// Each pass histograms, in block-shared memory, the keys that match the prefix found so far (median_hist_kernel); then one
+// thread per (sample, selection) finds the bin holding its rank, extends the prefix and clears the histogram
+// (median_select_kernel).  The first pass also counts the valid elements.  Integer counts: the same on every run.
+struct MedianState {
+    unsigned* hist;                 // [B][SEL][2048]
+    unsigned long long* sel;        // [B][SEL][3]: key prefix, prefix mask, remaining rank
+    unsigned long long* count;      // [B] valid elements
+};
+
+template <class Key> __host__ __device__ constexpr int radix_passes() { return (8 * (int)sizeof(Key) + 10) / 11; }
+template <class Key> __device__ __forceinline__ int radix_shift(int pass) {
+    return pass < radix_passes<Key>() - 1 ? 8 * (int)sizeof(Key) - 11 * (pass + 1) : 0;
+}
+template <class Key> __device__ __forceinline__ unsigned radix_bins(int pass) {
+    return pass < radix_passes<Key>() - 1 ? 2048u : 1u << (8 * (int)sizeof(Key) - 11 * pass);
+}
+
+template <class A>
+__global__ void __launch_bounds__(256) median_hist_kernel(const A a, int pass) {
+    CCB_PDL_WAIT();
+    using Key = typename A::Key;
+    constexpr int S = A::SEL;
+    __shared__ unsigned h[S * 2048];
+    const int b = blockIdx.y;
+    const int shift = radix_shift<Key>(pass);
+    const Key bin_mask = (Key)(radix_bins<Key>(pass) - 1);
+    for (int i = threadIdx.x; i < S * 2048; i += 256) h[i] = 0;
+    __syncthreads();
+    const unsigned long long* s = a.med.sel + (long long)b * S * 3;
+    Key pre[S], msk[S];
+#pragma unroll
+    for (int k = 0; k < S; ++k) { pre[k] = (Key)s[3 * k]; msk[k] = (Key)s[3 * k + 1]; }
+    const long long hw = (long long)a.H * a.W;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < hw; i += (long long)gridDim.x * 256) {
+        Key key[S];
+        if (!a.median_keys(b, i, key)) continue;
+#pragma unroll
+        for (int k = 0; k < S; ++k)
+            if ((key[k] & msk[k]) == pre[k]) atomicAdd(h + k * 2048 + (unsigned)((key[k] >> shift) & bin_mask), 1u);
+    }
+    __syncthreads();
+    unsigned* g = a.med.hist + (long long)b * S * 2048;
+    for (int i = threadIdx.x; i < S * 2048; i += 256)
+        if (h[i]) atomicAdd(g + i, h[i]);
+}
+
+template <class A>
+__global__ void median_select_kernel(const A a, int pass) {
+    CCB_PDL_WAIT();
+    using Key = typename A::Key;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.B * A::SEL) return;
+    const int b = t / A::SEL, k = t % A::SEL;
+    unsigned* h = a.med.hist + (long long)t * 2048;
+    unsigned long long* s = a.med.sel + (long long)t * 3;
+    const int shift = radix_shift<Key>(pass);
+    const unsigned nbins = radix_bins<Key>(pass);
+    if (pass == 0) {
+        unsigned long long n = 0;
+        for (unsigned i = 0; i < nbins; ++i) n += h[i];
+        if (k == 0) a.med.count[b] = n;
+        s[2] = (n == 0) ? 0 : (((A::UPPER >> k) & 1u) ? n / 2 : (n - 1) / 2);
+    }
+    const unsigned long long rank = s[2];
+    unsigned long long cum = 0;
+    unsigned bin = 0;
+    for (unsigned i = 0; i < nbins; ++i) {
+        bin = i;
+        if (cum + h[i] > rank) break;
+        cum += h[i];
+    }
+    s[2] = rank - cum;
+    s[0] |= (unsigned long long)bin << shift;
+    s[1] |= (unsigned long long)(nbins - 1) << shift;
+    for (unsigned i = 0; i < 2048; ++i) h[i] = 0;
 }
 
 // ================================================================================================
@@ -174,7 +274,7 @@ __global__ void __launch_bounds__(256) flow_metrics_kernel(const FlowMetArgs a) 
             }
         }
     }
-    block_sum_d<8>(acc, scratch);
+    block_sum<8>(acc, scratch);
     if (threadIdx.x == 0)
 #pragma unroll
         for (int k = 0; k < 8; ++k) a.partials[(long long)blockIdx.x * 8 + k] = acc[k];
@@ -184,9 +284,8 @@ __global__ void __launch_bounds__(256) flow_metrics_kernel(const FlowMetArgs a) 
 __global__ void flow_metrics_finalize(const double* __restrict__ partials, int nblocks, int nc, long long npx, float* __restrict__ out) {
     CCB_PDL_WAIT();
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    double s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int b = 0; b < nblocks; ++b)
-        for (int k = 0; k < 8; ++k) s[k] += partials[(long long)b * 8 + k];
+    double s[8];
+    sum_partials(partials, nblocks, 8, s);
     if (nc == 3) {
         out[0] = (float)s[0] / ((float)s[1] + 1e-8f);
         out[1] = (float)s[2] / ((float)s[3] + 1e-8f);
@@ -203,15 +302,17 @@ __global__ void flow_metrics_finalize(const double* __restrict__ partials, int n
 // Depth metrics (compute_errors :430-467).  Per sample: valid = 0 < gt < 80 (and inside the Garg crop);
 // pred clamped to [1e-3, 80]; pred *= median(gt) / median(pred) (torch.median = LOWER median); then
 // abs_diff, abs_rel, sq_rel, a1, a2, a3, each a mean over the valid pixels, averaged over the batch.
-// Medians by a 3-pass radix select over the float bit patterns (all keys are positive: bit order == value order).
 struct DepthArgs {
+    using Key = unsigned;            // the medians: the lower middle of gt and of the clamped pred
+    static constexpr int SEL = 2;
+    static constexpr unsigned UPPER = 0;
     const float* gt;
     const float* pred;
     int B, H, W, y1, y2, x1, x2;     // crop window (whole image when crop is off)
-    unsigned* hist;                  // [B][2][2048]
-    unsigned* sel;                   // [B][2][4]: prefix bits, prefix mask, remaining rank k, count
+    MedianState med;
     double* partials;                // [B][blocks][6]
     float* out;                      // [6]
+    __device__ __forceinline__ bool median_keys(int b, long long i, Key (&k)[SEL]) const;
 };
 
 __device__ __forceinline__ bool depth_valid(const DepthArgs& a, float g, int y, int x) {
@@ -219,55 +320,14 @@ __device__ __forceinline__ bool depth_valid(const DepthArgs& a, float g, int y, 
 }
 __device__ __forceinline__ float clamp_pred(float p) { return fminf(fmaxf(p, 1e-3f), 80.f); }
 
-// pass 0: count valid + histogram of the top 11 bits; pass 1/2: histogram of the next 11 / 10 bits among keys
-// matching the prefix found so far
-__global__ void __launch_bounds__(256) depth_hist_kernel(const DepthArgs a, int pass) {
-    CCB_PDL_WAIT();
-    const int b = blockIdx.y;
-    const int shift = (pass == 0) ? 21 : (pass == 1 ? 10 : 0);
-    const unsigned nb_mask = (pass == 2) ? 1023u : 2047u;
-    const long long hw = (long long)a.H * a.W;
-    unsigned* hg = a.hist + ((long long)b * 2 + 0) * 2048;
-    unsigned* hp = a.hist + ((long long)b * 2 + 1) * 2048;
-    const unsigned* sg = a.sel + ((long long)b * 2 + 0) * 4;
-    const unsigned* sp = a.sel + ((long long)b * 2 + 1) * 4;
-    const unsigned pg = sg[0], mg = sg[1], pp = sp[0], mp = sp[1];
-    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < hw; i += (long long)gridDim.x * 256) {
-        const int y = (int)(i / a.W), x = (int)(i - (long long)y * a.W);
-        const float g = __ldg(a.gt + b * hw + i);
-        if (!depth_valid(a, g, y, x)) continue;
-        const unsigned kg = __float_as_uint(g), kp = __float_as_uint(clamp_pred(__ldg(a.pred + b * hw + i)));
-        if ((kg & mg) == pg) atomicAdd(hg + ((kg >> shift) & nb_mask), 1u);
-        if ((kp & mp) == pp) atomicAdd(hp + ((kp >> shift) & nb_mask), 1u);
-    }
-}
-
-// one thread per (sample, which): find the bin holding rank k, extend the prefix, clear the histogram
-__global__ void depth_select_kernel(const DepthArgs a, int pass) {
-    CCB_PDL_WAIT();
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= a.B * 2) return;
-    unsigned* h = a.hist + (long long)t * 2048;
-    unsigned* s = a.sel + (long long)t * 4;
-    const int shift = (pass == 0) ? 21 : (pass == 1 ? 10 : 0);
-    const int nbins = (pass == 2) ? 1024 : 2048;
-    if (pass == 0) {
-        unsigned n = 0;
-        for (int i = 0; i < nbins; ++i) n += h[i];
-        s[3] = n;
-        s[2] = (n > 0) ? (n - 1) / 2 : 0;             // torch.median: lower median = sorted[(n-1)//2]
-    }
-    unsigned k = s[2], cum = 0;
-    int bin = 0;
-    for (int i = 0; i < nbins; ++i) {
-        if (cum + h[i] > k) { bin = i; break; }
-        cum += h[i];
-        bin = i;
-    }
-    s[2] = k - cum;
-    s[0] |= ((unsigned)bin) << shift;
-    s[1] |= ((pass == 2) ? 1023u : 2047u) << shift;
-    for (int i = 0; i < 2048; ++i) h[i] = 0;
+__device__ __forceinline__ bool DepthArgs::median_keys(int b, long long i, Key (&k)[SEL]) const {
+    const long long hw = (long long)H * W;
+    const int y = (int)(i / W), x = (int)(i - (long long)y * W);
+    const float g = __ldg(gt + b * hw + i);
+    if (!depth_valid(*this, g, y, x)) return false;
+    k[0] = ordered_key32(g);
+    k[1] = ordered_key32(clamp_pred(__ldg(pred + b * hw + i)));
+    return true;
 }
 
 __global__ void __launch_bounds__(256) depth_errors_kernel(const DepthArgs a) {
@@ -275,8 +335,8 @@ __global__ void __launch_bounds__(256) depth_errors_kernel(const DepthArgs a) {
     __shared__ double scratch[6 * 32];
     const int b = blockIdx.y;
     const long long hw = (long long)a.H * a.W;
-    const float med_g = __uint_as_float(a.sel[((long long)b * 2 + 0) * 4]);
-    const float med_p = __uint_as_float(a.sel[((long long)b * 2 + 1) * 4]);
+    const float med_g = ordered_value32((unsigned)a.med.sel[(long long)b * 6]);
+    const float med_p = ordered_value32((unsigned)a.med.sel[(long long)b * 6 + 3]);
     double acc[6] = {0, 0, 0, 0, 0, 0};
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < hw; i += (long long)gridDim.x * 256) {
         const int y = (int)(i / a.W), x = (int)(i - (long long)y * a.W);
@@ -292,7 +352,7 @@ __global__ void __launch_bounds__(256) depth_errors_kernel(const DepthArgs a) {
         acc[4] += (th < 1.5625f) ? 1.0 : 0.0;
         acc[5] += (th < 1.953125f) ? 1.0 : 0.0;
     }
-    block_sum_d<6>(acc, scratch);
+    block_sum<6>(acc, scratch);
     if (threadIdx.x == 0)
 #pragma unroll
         for (int k = 0; k < 6; ++k) a.partials[((long long)b * gridDim.x + blockIdx.x) * 6 + k] = acc[k];
@@ -303,10 +363,9 @@ __global__ void depth_errors_finalize(const DepthArgs a, int nblocks) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     double tot[6] = {0, 0, 0, 0, 0, 0};
     for (int b = 0; b < a.B; ++b) {
-        double s[6] = {0, 0, 0, 0, 0, 0};
-        for (int k = 0; k < nblocks; ++k)
-            for (int j = 0; j < 6; ++j) s[j] += a.partials[((long long)b * nblocks + k) * 6 + j];
-        const double n = (double)a.sel[((long long)b * 2) * 4 + 3];
+        double s[6];
+        sum_partials(a.partials + (long long)b * nblocks * 6, nblocks, 6, s);
+        const double n = (double)a.med.count[b];
         for (int j = 0; j < 6; ++j) tot[j] += (double)(float)(s[j] / n);      // per-sample fp32 means, summed (:453-463)
     }
     for (int j = 0; j < 6; ++j) a.out[j] = (float)(tot[j] / (double)a.B);
@@ -525,7 +584,7 @@ __global__ void __launch_bounds__(256) normlocal_partials_kernel(const NormLocal
             acc[1] += v * v;
         }
     }
-    block_sum_d<2>(acc, scratch);
+    block_sum<2>(acc, scratch);
     if (threadIdx.x == 0) {
         a.partials[((long long)bc * gridDim.x + blockIdx.x) * 2 + 0] = acc[0];
         a.partials[((long long)bc * gridDim.x + blockIdx.x) * 2 + 1] = acc[1];
@@ -536,14 +595,11 @@ __global__ void normlocal_finalize_kernel(const NormLocalArgs a, int nblk) {
     CCB_PDL_WAIT();
     const int bc = blockIdx.x * blockDim.x + threadIdx.x;
     if (bc >= a.B * 3) return;
-    double s1 = 0.0, s2 = 0.0;
-    for (int k = 0; k < nblk; ++k) {
-        s1 += a.partials[((long long)bc * nblk + k) * 2 + 0];
-        s2 += a.partials[((long long)bc * nblk + k) * 2 + 1];
-    }
+    double s[2];
+    sum_partials(a.partials + (long long)bc * nblk * 2, nblk, 2, s);
     const double n = (double)a.F * (double)a.hw;
-    const double mean = s1 / n;
-    const double var = (s2 - s1 * mean) / (n - 1.0);
+    const double mean = s[0] / n;
+    const double var = (s[1] - s[0] * mean) / (n - 1.0);
     a.stats[bc * 2 + 0] = (float)mean;
     a.stats[bc * 2 + 1] = (float)sqrt(var);
 }
@@ -612,12 +668,7 @@ __global__ void __launch_bounds__(256) mask_iou_max_kernel(const MaskIouArgs a) 
         const unsigned k = __float_as_uint(flow_gap(a, b, p));
         m = (k > m) ? k : m;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned k = __shfl_xor_sync(0xffffffffu, m, o);
-        m = (k > m) ? k : m;
-    }
-    if ((threadIdx.x & 31) == 0) atomicMax(a.dmax + b, (unsigned long long)m);
+    warp_max_into(a.dmax + b, m);
 }
 
 __global__ void __launch_bounds__(256) mask_iou_masks_kernel(const MaskIouArgs a) {
@@ -831,12 +882,7 @@ __global__ void __launch_bounds__(256) flow_color_max_kernel(const FlowColorArgs
         const unsigned long long k = (rad != rad) ? ~0ull : (unsigned long long)__float_as_uint(rad);
         m = (k > m) ? k : m;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long k = __shfl_xor_sync(0xffffffffu, m, o);
-        m = (k > m) ? k : m;
-    }
-    if ((threadIdx.x & 31) == 0) atomicMax(a.maxrad + b, m);
+    warp_max_into(a.maxrad + b, m);
 }
 
 __global__ void __launch_bounds__(256) flow_color_kernel(const FlowColorArgs a) {
@@ -905,7 +951,7 @@ __global__ void __launch_bounds__(256) kitti_err_kernel(const KittiErrArgs a) {
         acc[1] += valid;
         if (epe > 3.0 && __ddiv_rn(epe, __dadd_rn(mag, 1e-8)) > 0.05) acc[2] += valid;
     }
-    block_sum_d<3>(acc, scratch);
+    block_sum<3>(acc, scratch);
     if (threadIdx.x == 0) {
         double* o = a.partials + ((long long)b * gridDim.x + blockIdx.x) * 3;
         o[0] = acc[0]; o[1] = acc[1]; o[2] = acc[2];
@@ -916,9 +962,8 @@ __global__ void kitti_err_finalize(const KittiErrArgs a, int nblk) {
     CCB_PDL_WAIT();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.B) return;
-    double s[3] = {0, 0, 0};
-    for (int k = 0; k < nblk; ++k)
-        for (int j = 0; j < 3; ++j) s[j] += a.partials[((long long)b * nblk + k) * 3 + j];
+    double s[3];
+    sum_partials(a.partials + (long long)b * nblk * 3, nblk, 3, s);
     a.out[2 * b + 0] = __ddiv_rn(s[0], s[1]);
     a.out[2 * b + 1] = __ddiv_rn(s[2], s[1]);
     if (a.counts) {
@@ -969,15 +1014,6 @@ __device__ __forceinline__ VeloPt velo_project(const VeloArgs& a, int b, long lo
     return r;
 }
 
-// unsigned order of the key == value order of the double (NaN never reaches it: its u fails the bounds)
-__device__ __forceinline__ unsigned long long ordered_key(double d) {
-    const unsigned long long k = (unsigned long long)__double_as_longlong(d);
-    return (k >> 63) ? ~k : (k | 0x8000000000000000ull);
-}
-__device__ __forceinline__ double ordered_value(unsigned long long k) {
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
-
 __device__ __forceinline__ bool velo_range(const VeloArgs& a, int b, long long* i0, long long* i1) {
     *i0 = a.offs[b];
     *i1 = a.offs[b + 1];
@@ -997,7 +1033,7 @@ __global__ void __launch_bounds__(256) velo_scatter_kernel(const VeloArgs a) {
         atomicMax(a.last + b * hw + (long long)p.v * a.W + p.u, (unsigned long long)(i - i0 + 1));
         atomicAdd(a.cnt + b * K + key, 1ull);
         atomicMax(a.first + b * K + key, ~(unsigned long long)(i - i0));
-        atomicMax(a.zmin + b * K + key, ~ordered_key(p.z));
+        atomicMax(a.zmin + b * K + key, ~ordered_key(p.z));       // a NaN z never gets here: its u fails the bounds
     }
 }
 
@@ -1132,16 +1168,16 @@ __global__ void __launch_bounds__(256) zoom_eval_kernel(const ZoomArgs a) {
 //   row 0  scale = mean(s1 / |pose[:3]|) over the references with s1 > 0 (0 when there is none); zeros without poses
 //   errors abs_rel sq_rel rms log_rms a1 a2 a3;  a* are exact counts over n, the rest fp64 block partials summed in a
 //          fixed order.
-// Medians by radix select on order-preserving 64-bit keys (six passes of 11, 11, 11, 11, 11 and 9 bits), four selections
-// per sample: the lower and upper middle ranks of gt and of pred.
+// The medians: the lower and upper middle of gt and of pred.
 struct EigenArgs {
+    using Key = unsigned long long;
+    static constexpr int SEL = 4;                   // gt lower, gt upper, pred lower, pred upper
+    static constexpr unsigned UPPER = 0xa;
     const double* gt;               // [B, H, W]
     const float* pred;              // [B, H, W]
     const float* poses;             // [B, R, 6] or null
     const double* disp;             // [B, R] or null
-    unsigned* hist;                 // [B][4][2048]
-    unsigned long long* sel;        // [B][4][3]: prefix, prefix mask, remaining rank
-    unsigned long long* count;      // [B] valid pixels
+    MedianState med;
     double* scale;                  // [B][2]
     double* partials;               // [B][blocks][2][7]
     double* out;                    // [B, 2, 7]
@@ -1149,81 +1185,21 @@ struct EigenArgs {
     double cap;                     // scaled predictions above it become it (test_make3d.py:147; +inf: no cap)
     int log10;                      // log_rms of log10 (test_make3d.py:183) instead of ln
     int B, H, W, R, y1, y2, x1, x2;
+    __device__ __forceinline__ bool median_keys(int b, long long i, Key (&k)[SEL]) const;
 };
 
 __device__ __forceinline__ bool eigen_valid(const EigenArgs& a, double g, int y, int x) {
     return (g > a.min_depth) && (g < a.max_depth) && (y >= a.y1) && (y < a.y2) && (x >= a.x1) && (x < a.x2);
 }
-__device__ __forceinline__ unsigned long long ordered_key32(float f) {
-    const unsigned k = __float_as_uint(f);
-    return (unsigned long long)((k >> 31) ? ~k : (k | 0x80000000u));
-}
-__device__ __forceinline__ float ordered_value32(unsigned long long k) {
-    const unsigned u = (unsigned)k;
-    return __uint_as_float((u >> 31) ? (u & 0x7fffffffu) : ~u);
-}
-__device__ __forceinline__ int eigen_shift(int pass) { return pass < 5 ? 53 - 11 * pass : 0; }
-__device__ __forceinline__ unsigned eigen_bins(int pass) { return pass < 5 ? 2048u : 512u; }
 
-__global__ void __launch_bounds__(256) eigen_hist_kernel(const EigenArgs a, int pass) {
-    CCB_PDL_WAIT();
-    __shared__ unsigned h[4 * 2048];
-    const int b = blockIdx.y;
-    const int shift = eigen_shift(pass);
-    const unsigned nbins = eigen_bins(pass);
-    for (int i = threadIdx.x; i < 4 * 2048; i += 256) h[i] = 0;
-    __syncthreads();
-    const unsigned long long* s = a.sel + (long long)b * 12;
-    unsigned long long pre[4], msk[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { pre[k] = s[3 * k]; msk[k] = s[3 * k + 1]; }
-    const long long hw = (long long)a.H * a.W;
-    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < hw; i += (long long)gridDim.x * 256) {
-        const int y = (int)(i / a.W), x = (int)(i - (long long)y * a.W);
-        const double g = __ldg(a.gt + b * hw + i);
-        if (!eigen_valid(a, g, y, x)) continue;
-        const unsigned long long kg = ordered_key(g), kp = ordered_key32(__ldg(a.pred + b * hw + i));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const unsigned long long key = (k < 2) ? kg : kp;
-            if ((key & msk[k]) == pre[k]) atomicAdd(h + k * 2048 + (unsigned)((key >> shift) & (nbins - 1)), 1u);
-        }
-    }
-    __syncthreads();
-    unsigned* g = a.hist + (long long)b * 4 * 2048;
-    for (int i = threadIdx.x; i < 4 * 2048; i += 256)
-        if (h[i]) atomicAdd(g + i, h[i]);
-}
-
-// one thread per (sample, selection): find the bin holding the rank, extend the prefix, clear the histogram
-__global__ void eigen_select_kernel(const EigenArgs a, int pass) {
-    CCB_PDL_WAIT();
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= a.B * 4) return;
-    const int b = t >> 2, k = t & 3;
-    unsigned* h = a.hist + (long long)t * 2048;
-    unsigned long long* s = a.sel + (long long)t * 3;
-    const int shift = eigen_shift(pass);
-    const unsigned nbins = eigen_bins(pass);
-    if (pass == 0) {
-        unsigned long long n = 0;
-        for (unsigned i = 0; i < nbins; ++i) n += h[i];
-        if (k == 0) a.count[b] = n;
-        // numpy's median: sorted[(n-1)//2] and sorted[n//2] (the same rank when n is odd)
-        s[2] = (n == 0) ? 0 : ((k & 1) ? n / 2 : (n - 1) / 2);
-    }
-    const unsigned long long rank = s[2];
-    unsigned long long cum = 0;
-    unsigned bin = 0;
-    for (unsigned i = 0; i < nbins; ++i) {
-        bin = i;
-        if (cum + h[i] > rank) break;
-        cum += h[i];
-    }
-    s[2] = rank - cum;
-    s[0] |= (unsigned long long)bin << shift;
-    s[1] |= (unsigned long long)(nbins - 1) << shift;
-    for (unsigned i = 0; i < 2048; ++i) h[i] = 0;
+__device__ __forceinline__ bool EigenArgs::median_keys(int b, long long i, Key (&k)[SEL]) const {
+    const long long hw = (long long)H * W;
+    const int y = (int)(i / W), x = (int)(i - (long long)y * W);
+    const double g = __ldg(gt + b * hw + i);
+    if (!eigen_valid(*this, g, y, x)) return false;
+    k[0] = k[1] = ordered_key(g);
+    k[2] = k[3] = ordered_key32(__ldg(pred + b * hw + i));
+    return true;
 }
 
 // one thread per sample: both scales
@@ -1231,10 +1207,10 @@ __global__ void eigen_scale_kernel(const EigenArgs a) {
     CCB_PDL_WAIT();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.B) return;
-    const unsigned long long* s = a.sel + (long long)b * 12;
+    const unsigned long long* s = a.med.sel + (long long)b * 12;
     const double g0 = ordered_value(s[0]), g1 = ordered_value(s[3]);
-    const float p0 = ordered_value32(s[6]), p1 = ordered_value32(s[9]);
-    const bool even = (a.count[b] & 1ull) == 0;
+    const float p0 = ordered_value32((unsigned)s[6]), p1 = ordered_value32((unsigned)s[9]);
+    const bool even = (a.med.count[b] & 1ull) == 0;
     const double med_g = even ? __ddiv_rn(__dadd_rn(g0, g1), 2.0) : g0;
     const float med_p = even ? __fdiv_rn(__fadd_rn(p0, p1), 2.f) : p0;
     a.scale[2 * b + 1] = __ddiv_rn(med_g, (double)med_p);
@@ -1288,7 +1264,7 @@ __global__ void __launch_bounds__(256) eigen_errors_kernel(const EigenArgs a) {
             o[6] += (th < 1.953125) ? 1.0 : 0.0;
         }
     }
-    block_sum_d<14>(acc, scratch);
+    block_sum<14>(acc, scratch);
     if (threadIdx.x == 0) {
         double* o = a.partials + ((long long)b * gridDim.x + blockIdx.x) * 14;
 #pragma unroll
@@ -1307,10 +1283,9 @@ __global__ void eigen_finalize_kernel(const EigenArgs a, int nblk) {
         for (int k = 0; k < 7; ++k) o[k] = 0.0;
         return;
     }
-    double s[7] = {0, 0, 0, 0, 0, 0, 0};
-    for (int k = 0; k < nblk; ++k)
-        for (int j = 0; j < 7; ++j) s[j] += a.partials[((long long)b * nblk + k) * 14 + 7 * r + j];
-    const double n = (double)a.count[b];
+    double s[7];
+    sum_partials(a.partials + (long long)b * nblk * 14 + 7 * r, nblk, 14, s);
+    const double n = (double)a.med.count[b];
     o[0] = __ddiv_rn(s[0], n);
     o[1] = __ddiv_rn(s[1], n);
     o[2] = __dsqrt_rn(__ddiv_rn(s[2], n));
@@ -1380,15 +1355,32 @@ __global__ void __launch_bounds__(256) bytescale_apply_kernel(const ByteScaleArg
 
 using namespace ccb;
 
-static int grid_for(long long n) {
-    long long g = (n + 255) / 256;
-    const long long cap = NUM_SMS * 8;
+// blocks of a grid-stride loop over n elements: per_block elements each, at least 1 and at most cap.  A reduction's grid
+// fixes the order of its fp64 partial sums, so each entry point keeps its constants.
+static int blocks_for(long long n, int per_block, int cap) {
+    const long long g = (n + per_block - 1) / per_block;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+// A MedianState of B samples: the selections and the counts, then the histograms
+static long long median_state_bytes(int B, int sel) { return (long long)B * (3 * sel + 1) * 8 + (long long)B * sel * 2048 * 4; }
+
+// lays a.med out at `state` and clears it, then launches the passes of the select, nb histogram blocks per sample
+template <class A>
+static void median_select(A& a, char* state, int nb, ccb_stream_t stream) {
+    a.med.sel = (unsigned long long*)state;
+    a.med.count = a.med.sel + (long long)a.B * A::SEL * 3;
+    a.med.hist = (unsigned*)(a.med.count + a.B);
+    cudaMemsetAsync(state, 0, (size_t)median_state_bytes(a.B, A::SEL), (cudaStream_t)stream);
+    for (int pass = 0; pass < radix_passes<typename A::Key>(); ++pass) {
+        CCB_LAUNCH(median_hist_kernel<A>, dim3(nb, a.B), dim3(256), 0, stream, a, pass);
+        CCB_LAUNCH(median_select_kernel<A>, dim3((a.B * A::SEL + 63) / 64), dim3(64), 0, stream, a, pass);
+    }
 }
 
 extern "C" long long ccb_flow_metrics_workspace_bytes(int B, int Hg, int Wg) {
     if (B <= 0 || Hg <= 0 || Wg <= 0) return -1;
-    return (long long)grid_for((long long)B * Hg * Wg) * 8 * (long long)sizeof(double);
+    return (long long)blocks_for((long long)B * Hg * Wg, 256, NUM_SMS * 8) * 8 * (long long)sizeof(double);
 }
 
 extern "C" int ccb_flow_metrics(const float* gt, const float* pred_rigid, const float* pred_nonrigid, const float* rigidity_mask,
@@ -1404,20 +1396,15 @@ extern "C" int ccb_flow_metrics(const float* gt, const float* pred_rigid, const 
     a.gt = gt; a.pa = pred_rigid; a.pb = pred_nonrigid; a.mask = rigidity_mask; a.partials = (double*)work; a.epe_map = epe_map;
     a.B = B; a.nc = nc; a.Hg = Hg; a.Wg = Wg; a.hp = hp; a.wp = wp; a.hm = hm; a.wm = wm;
     a.thresh = thresh; a.tau0 = tau0; a.tau1 = tau1;
-    const int nb = grid_for((long long)B * Hg * Wg);
+    const int nb = blocks_for((long long)B * Hg * Wg, 256, NUM_SMS * 8);
     CCB_LAUNCH(flow_metrics_kernel, dim3(nb), dim3(256), 0, stream, a);
     CCB_LAUNCH(flow_metrics_finalize, dim3(1), dim3(32), 0, stream, (const double*)work, nb, nc, (long long)B * Hg * Wg, out4);
     return check_launch("flow_metrics");
 }
 
-static int depth_blocks(int H, int W) {
-    int g = (int)(((long long)H * W + 255) / 256);
-    return g < 1 ? 1 : (g > 64 ? 64 : g);
-}
-
 extern "C" long long ccb_depth_errors_workspace_bytes(int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0) return -1;
-    return (long long)B * 2 * 2048 * 4 + (long long)B * 2 * 4 * 4 + (long long)B * depth_blocks(H, W) * 6 * 8 + 64;
+    return (long long)B * blocks_for((long long)H * W, 256, 64) * 6 * 8 + median_state_bytes(B, DepthArgs::SEL);
 }
 
 extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H, int W, int crop, void* work, long long work_bytes,
@@ -1432,24 +1419,12 @@ extern "C" int ccb_depth_errors(const float* gt, const float* pred, int B, int H
         a.y1 = (int)(0.40810811 * H); a.y2 = (int)(0.99189189 * H);
         a.x1 = (int)(0.03594771 * W); a.x2 = (int)(0.96405229 * W);
     }
-    char* p = (char*)work;
-    a.partials = (double*)p;   p += (long long)B * depth_blocks(H, W) * 6 * 8;
-    a.hist = (unsigned*)p;     p += (long long)B * 2 * 2048 * 4;
-    a.sel = (unsigned*)p;
-    const int nb = depth_blocks(H, W);
-    cudaMemsetAsync(a.hist, 0, (size_t)B * 2 * 2048 * 4 + (size_t)B * 2 * 4 * 4, (cudaStream_t)stream);
-    for (int pass = 0; pass < 3; ++pass) {
-        CCB_LAUNCH(depth_hist_kernel, dim3(nb, B), dim3(256), 0, stream, a, pass);
-        CCB_LAUNCH(depth_select_kernel, dim3((B * 2 + 63) / 64), dim3(64), 0, stream, a, pass);
-    }
+    const int nb = blocks_for((long long)H * W, 256, 64);
+    a.partials = (double*)work;
+    median_select(a, (char*)work + (long long)B * nb * 6 * 8, nb, stream);
     CCB_LAUNCH(depth_errors_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     CCB_LAUNCH(depth_errors_finalize, dim3(1), dim3(32), 0, stream, a, nb);
     return check_launch("depth_errors");
-}
-
-static int mask_iou_blocks(int H, int W) {
-    const long long g = ((long long)H * W + 255) / 256;
-    return (int)(g < 1 ? 1 : (g > NUM_SMS * 4 ? NUM_SMS * 4 : g));
 }
 
 extern "C" long long ccb_mask_iou_workspace_bytes(int B, int h, int w, int Hg, int Wg) {
@@ -1471,9 +1446,10 @@ extern "C" int ccb_mask_iou(const float* emask, const float* flow_cam, const flo
     a.B = B; a.C = C; a.h = h; a.w = w; a.Hg = Hg; a.Wg = Wg; a.thresh = thresh; a.car = (float)car_label;
     cudaMemsetAsync(a.dmax, 0, (size_t)need, (cudaStream_t)stream);
     cudaMemsetAsync(a.counts, 0, (size_t)B * 12 * sizeof(unsigned long long), (cudaStream_t)stream);
-    CCB_LAUNCH(mask_iou_max_kernel, dim3(mask_iou_blocks(h, w), B), dim3(256), 0, stream, a);
-    if (masks) CCB_LAUNCH(mask_iou_masks_kernel, dim3(mask_iou_blocks(h, w), B), dim3(256), 0, stream, a);
-    CCB_LAUNCH(mask_iou_count_kernel, dim3(mask_iou_blocks(Hg, Wg), B), dim3(256), 0, stream, a);
+    const int nb = blocks_for((long long)h * w, 256, NUM_SMS * 4);
+    CCB_LAUNCH(mask_iou_max_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    if (masks) CCB_LAUNCH(mask_iou_masks_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(mask_iou_count_kernel, dim3(blocks_for((long long)Hg * Wg, 256, NUM_SMS * 4), B), dim3(256), 0, stream, a);
     return check_launch("mask_iou");
 }
 
@@ -1488,8 +1464,8 @@ extern "C" int ccb_flow_submit(const float* emask, const float* flow_cam, const 
     a.B = B; a.C = C; a.h = h; a.w = w; a.Hg = Hg; a.Wg = Wg; a.thresh = thresh;
     a.fu = (float)((double)Wg / (double)w);        // u * (w_gt / w_pred): the python float, cast to fp32 by torch's mul
     a.fv = (float)((double)Hg / (double)h);
-    CCB_LAUNCH(flow_submit_mask_kernel, dim3(grid_for((long long)B * h * w)), dim3(256), 0, stream, a);
-    CCB_LAUNCH(flow_submit_kernel, dim3(grid_for((long long)B * Hg * Wg)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(flow_submit_mask_kernel, dim3(blocks_for((long long)B * h * w, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(flow_submit_kernel, dim3(blocks_for((long long)B * Hg * Wg, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     return check_launch("flow_submit");
 }
 
@@ -1507,20 +1483,15 @@ extern "C" int ccb_flow_color(const float* flow, int B, int P, int H, int W, voi
     FlowColorArgs a;
     a.flow = flow; a.maxrad = (unsigned long long*)work; a.out = out; a.B = B; a.P = P; a.H = H; a.W = W;
     cudaMemsetAsync(a.maxrad, 0, (size_t)need, (cudaStream_t)stream);
-    const int nb = mask_iou_blocks(P * H, W);
+    const int nb = blocks_for((long long)P * H * W, 256, NUM_SMS * 4);
     CCB_LAUNCH(flow_color_max_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     CCB_LAUNCH(flow_color_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     return check_launch("flow_color");
 }
 
-static int kitti_err_blocks(int H, int W) {
-    const long long g = ((long long)H * W + 2047) / 2048;
-    return (int)(g < 1 ? 1 : (g > 128 ? 128 : g));
-}
-
 extern "C" long long ccb_kitti_flow_errors_workspace_bytes(int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0) return -1;
-    return (long long)B * kitti_err_blocks(H, W) * 3 * (long long)sizeof(double);
+    return (long long)B * blocks_for((long long)H * W, 2048, 128) * 3 * (long long)sizeof(double);
 }
 
 extern "C" int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned short* pred, int B, int H, int W, void* work,
@@ -1531,7 +1502,7 @@ extern "C" int ccb_kitti_flow_errors(const unsigned short* gt, const unsigned sh
     CCB_REQUIRE_WORK("kitti_flow_errors", "work", work, work_bytes, need);
     KittiErrArgs a;
     a.gt = gt; a.pred = pred; a.partials = (double*)work; a.out = out; a.counts = counts; a.B = B; a.H = H; a.W = W;
-    const int nb = kitti_err_blocks(H, W);
+    const int nb = blocks_for((long long)H * W, 2048, 128);
     CCB_LAUNCH(kitti_err_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     CCB_LAUNCH(kitti_err_finalize, dim3((B + 63) / 64), dim3(64), 0, stream, a, nb);
     return check_launch("kitti_flow_errors");
@@ -1559,11 +1530,9 @@ extern "C" int ccb_velo_depth(const float* points, const long long* offsets, con
     a.first = a.cnt + (long long)B * K;
     a.zmin = a.first + (long long)B * K;
     cudaMemsetAsync(work, 0, (size_t)need, (cudaStream_t)stream);
-    const long long per_sample = (total + B - 1) / B;
-    const long long g = (per_sample + 255) / 256;
-    const int nbp = (int)(g < 1 ? 1 : (g > NUM_SMS * 4 ? NUM_SMS * 4 : g));
+    const int nbp = blocks_for((total + B - 1) / B, 256, NUM_SMS * 4);
     if (total > 0) CCB_LAUNCH(velo_scatter_kernel, dim3(nbp, B), dim3(256), 0, stream, a);
-    CCB_LAUNCH(velo_depth_kernel, dim3(mask_iou_blocks(H, W), B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(velo_depth_kernel, dim3(blocks_for((long long)H * W, 256, NUM_SMS * 4), B), dim3(256), 0, stream, a);
     return check_launch("velo_depth");
 }
 
@@ -1579,27 +1548,21 @@ extern "C" int ccb_spline_zoom(const float* src, int N, int h, int w, int H, int
     CCB_REQUIRE_WORK("spline_zoom", "work", work, work_bytes, ccb_spline_zoom_workspace_bytes(N, h, w));
     ZoomArgs a;
     a.src = src; a.coef = (double*)work; a.dst = dst; a.N = N; a.h = h; a.w = w; a.H = H; a.W = W; a.lo = lo; a.hi = hi;
-    CCB_LAUNCH(zoom_prefilter_kernel, dim3(grid_for((long long)N * w)), dim3(256), 0, stream, a, 0);
-    CCB_LAUNCH(zoom_prefilter_kernel, dim3(grid_for((long long)N * h)), dim3(256), 0, stream, a, 1);
-    CCB_LAUNCH(zoom_eval_kernel, dim3(grid_for((long long)N * H * W)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(zoom_prefilter_kernel, dim3(blocks_for((long long)N * w, 256, NUM_SMS * 8)), dim3(256), 0, stream, a, 0);
+    CCB_LAUNCH(zoom_prefilter_kernel, dim3(blocks_for((long long)N * h, 256, NUM_SMS * 8)), dim3(256), 0, stream, a, 1);
+    CCB_LAUNCH(zoom_eval_kernel, dim3(blocks_for((long long)N * H * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     return check_launch("spline_zoom");
 }
 
-static int eigen_blocks(int H, int W) {
-    const long long g = ((long long)H * W + 2047) / 2048;
-    return (int)(g < 1 ? 1 : (g > 64 ? 64 : g));
-}
-
-// workspace: block partials, then the selections, counts and scales (cleared per call), then the histograms
-struct EigenPlan { long long partials, sel, count, scale, hist, bytes; };
+// nb blocks per sample; workspace: block partials, the scales, then the median select's state
+struct EigenPlan { int nb; long long partials, scale, med, bytes; };
 static EigenPlan eigen_plan(int B, int H, int W) {
     EigenPlan p;
+    p.nb = blocks_for((long long)H * W, 2048, 64);
     p.partials = 0;
-    p.sel = p.partials + (long long)B * eigen_blocks(H, W) * 14 * 8;
-    p.count = p.sel + (long long)B * 12 * 8;
-    p.scale = p.count + (long long)B * 8;
-    p.hist = p.scale + (long long)B * 2 * 8;
-    p.bytes = p.hist + (long long)B * 4 * 2048 * 4;
+    p.scale = p.partials + (long long)B * p.nb * 14 * 8;
+    p.med = p.scale + (long long)B * 2 * 8;
+    p.bytes = p.med + median_state_bytes(B, EigenArgs::SEL);
     return p;
 }
 
@@ -1612,15 +1575,9 @@ extern "C" long long ccb_eigen_depth_errors_workspace_bytes(int B, int H, int W)
 static int eigen_errors_launch(const char* what, EigenArgs a, void* work, ccb_stream_t stream) {
     const EigenPlan p = eigen_plan(a.B, a.H, a.W);
     char* w = (char*)work;
-    a.partials = (double*)(w + p.partials); a.sel = (unsigned long long*)(w + p.sel); a.count = (unsigned long long*)(w + p.count);
-    a.scale = (double*)(w + p.scale); a.hist = (unsigned*)(w + p.hist);
-    const int B = a.B;
-    cudaMemsetAsync(w + p.sel, 0, (size_t)(p.bytes - p.sel), (cudaStream_t)stream);
-    const int nb = eigen_blocks(a.H, a.W);
-    for (int pass = 0; pass < 6; ++pass) {
-        CCB_LAUNCH(eigen_hist_kernel, dim3(nb, B), dim3(256), 0, stream, a, pass);
-        CCB_LAUNCH(eigen_select_kernel, dim3((B * 4 + 63) / 64), dim3(64), 0, stream, a, pass);
-    }
+    a.partials = (double*)(w + p.partials); a.scale = (double*)(w + p.scale);
+    const int B = a.B, nb = p.nb;
+    median_select(a, w + p.med, nb, stream);
     CCB_LAUNCH(eigen_scale_kernel, dim3((B + 63) / 64), dim3(64), 0, stream, a);
     CCB_LAUNCH(eigen_errors_kernel, dim3(nb, B), dim3(256), 0, stream, a);
     CCB_LAUNCH(eigen_finalize_kernel, dim3((B * 2 + 63) / 64), dim3(64), 0, stream, a, nb);
@@ -1673,7 +1630,7 @@ static int prep_frames_launch(const char* what, const unsigned char* src_u8, flo
     a.src = src_u8; a.params = params; a.offs = offs; a.B = B; a.F = F; a.Hs = Hs; a.Ws = Ws; a.H = H; a.W = W;
     for (int f = 0; f < 8; ++f) a.dst[f] = (f < F) ? dst[f] : nullptr;
     for (int f = 0; f < F; ++f) CCB_REQUIRE(a.dst[f] != nullptr, CCB_ERR_ARG, "%s: dst[%d] is null", what, f);
-    CCB_LAUNCH(prep_frames_kernel<UNIT>, dim3(grid_for((long long)B * F * H * W)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(prep_frames_kernel<UNIT>, dim3(blocks_for((long long)B * F * H * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     return check_launch(what);
 }
 
@@ -1694,7 +1651,7 @@ extern "C" int ccb_rotate_frames_u8(const unsigned char* src, const double* affi
     CCB_REQUIRE(B > 0 && F > 0 && H > 0 && W > 0, CCB_ERR_ARG, "rotate_frames_u8: bad sizes");
     RotArgs a;
     a.src = src; a.affine = affine; a.dst = dst; a.B = B; a.F = F; a.H = H; a.W = W;
-    CCB_LAUNCH(rotate_frames_kernel, dim3(grid_for((long long)B * F * H * W)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(rotate_frames_kernel, dim3(blocks_for((long long)B * F * H * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     return check_launch("rotate_frames_u8");
 }
 
@@ -1750,20 +1707,15 @@ extern "C" int ccb_resize_u8(const unsigned char* src, unsigned char* dst, int N
         ResampleArgs r;
         r.src = src; r.dst = mid; r.kk = c.kk_x; r.bounds = c.bounds_x;
         r.outer = (long long)N * Hs; r.in_len = Ws; r.out_len = W; r.inner = 1; r.ksize = p.ks_x;
-        CCB_LAUNCH(resample_pass_kernel, dim3(grid_for((long long)N * Hs * W)), dim3(256), 0, stream, r);
+        CCB_LAUNCH(resample_pass_kernel, dim3(blocks_for((long long)N * Hs * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, r);
     }
     if (vpass) {
         ResampleArgs r;
         r.src = hpass ? mid : src; r.dst = dst; r.kk = c.kk_y; r.bounds = c.bounds_y;
         r.outer = N; r.in_len = Hs; r.out_len = H; r.inner = W; r.ksize = p.ks_y;
-        CCB_LAUNCH(resample_pass_kernel, dim3(grid_for((long long)N * H * W)), dim3(256), 0, stream, r);
+        CCB_LAUNCH(resample_pass_kernel, dim3(blocks_for((long long)N * H * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, r);
     }
     return check_launch("resize_u8");
-}
-
-static int bytescale_blocks(long long len) {
-    const long long g = (len + 8191) / 8192;
-    return (int)(g < 1 ? 1 : (g > 256 ? 256 : g));
 }
 
 extern "C" long long ccb_bytescale_u8_workspace_bytes(int N, int H, int W) {
@@ -1779,20 +1731,15 @@ extern "C" int ccb_bytescale_u8(const unsigned char* src, int N, int H, int W, v
     ByteScaleArgs a;
     a.src = src; a.dst = dst; a.range = (unsigned long long*)work; a.len = (long long)H * W * 3;
     cudaMemsetAsync(work, 0, (size_t)N * 2 * sizeof(unsigned long long), (cudaStream_t)stream);
-    const dim3 grid(bytescale_blocks(a.len), N);
+    const dim3 grid(blocks_for(a.len, 8192, 256), N);
     CCB_LAUNCH(bytescale_range_kernel, grid, dim3(256), 0, stream, a);
     CCB_LAUNCH(bytescale_apply_kernel, grid, dim3(256), 0, stream, a);
     return check_launch("bytescale_u8");
 }
 
-static int normlocal_blocks(int H, int W) {
-    const long long g = ((long long)H * W + 2047) / 2048;
-    return (int)(g < 1 ? 1 : (g > 64 ? 64 : g));
-}
-
 extern "C" long long ccb_normalize_local_workspace_bytes(int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0) return -1;
-    return (long long)B * 3 * normlocal_blocks(H, W) * 2 * (long long)sizeof(double) + (long long)B * 3 * 2 * (long long)sizeof(float);
+    return (long long)B * 3 * blocks_for((long long)H * W, 2048, 64) * 2 * (long long)sizeof(double) + (long long)B * 3 * 2 * (long long)sizeof(float);
 }
 
 extern "C" int ccb_normalize_local(float* const* frames, int B, int F, int H, int W, float* stats, void* work, long long work_bytes,
@@ -1805,7 +1752,7 @@ extern "C" int ccb_normalize_local(float* const* frames, int B, int F, int H, in
     NormLocalArgs a;
     for (int f = 0; f < 8; ++f) a.x[f] = (f < F) ? frames[f] : nullptr;
     for (int f = 0; f < F; ++f) CCB_REQUIRE(a.x[f] != nullptr, CCB_ERR_ARG, "normalize_local: frames[%d] is null", f);
-    const int nblk = normlocal_blocks(H, W);
+    const int nblk = blocks_for((long long)H * W, 2048, 64);
     a.partials = (double*)work;
     a.stats = stats ? stats : (float*)((char*)work + (long long)B * 3 * nblk * 2 * sizeof(double));
     a.B = B; a.F = F; a.hw = (long long)H * W;

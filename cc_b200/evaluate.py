@@ -33,6 +33,26 @@ def _to_net_input(img_hwc, device):
     return ((t / 255 - 0.5) / 0.5).to(device)
 
 
+def _pose(res):
+    """The pose of a pose net's output: PoseExpNet returns (mask, pose), PoseNet the pose alone."""
+    return res[1] if isinstance(res, tuple) else res
+
+
+def _flow_nets(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv):
+    """The four nets in eval mode on tgt and its 4 refs -> (emask, flow_cam, flow_fwd): the mask net's output, the camera
+    flow of the depth and the pose to ref 2, and the flow net's forward flow (test_flow.py:112-125, test_mask.py:119-126,
+    submit_flow.py:109-116)."""
+    for n in (disp_net, pose_net, mask_net, flow_net):
+        n.eval()
+    depth = 1 / disp_net(tgt)
+    pose = pose_net(tgt, refs)
+    emask = mask_net(tgt, refs)
+    # Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
+    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
+    flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
+    return emask, flow_cam, flow_fwd
+
+
 def compute_errors_np(gt, pred):
     """test_disp.py:171-187 (numpy, on the masked 1-D arrays)."""
     thresh = np.maximum(gt / pred, pred / gt)
@@ -61,8 +81,7 @@ def depth_sample_errors(disp_net, tgt_img, gt_depth, mask=None, min_depth=1e-3, 
     if pose_net is not None:
         pose_net.eval()
         refs = [_to_net_input(r, device) for r in ref_imgs]
-        res = pose_net(tgt, refs)
-        poses = res[1] if isinstance(res, tuple) else res           # PoseExpNet returns (mask, pose)
+        poses = _pose(pose_net(tgt, refs))
         disp_pred = poses[0, :, :3].norm(2, 1).cpu().numpy()
         sf = [s1 / s2 for s1, s2 in zip(displacements, disp_pred) if s1 > 0]
         out[0] = compute_errors_np(gt, z * (np.mean(sf) if len(sf) > 0 else 0))
@@ -90,8 +109,7 @@ def pose_snippet_errors(pose_net, imgs, gt_poses, rotation_mode='euler', device=
     pose_net.eval()
     ts = [_to_net_input(i, device) for i in imgs]
     mid = len(ts) // 2
-    res = pose_net(ts[mid], ts[:mid] + ts[mid + 1:])
-    poses = (res[1] if isinstance(res, tuple) else res)[0].float().cpu()
+    poses = _pose(pose_net(ts[mid], ts[:mid] + ts[mid + 1:]))[0].float().cpu()
     poses = torch.cat([poses[:mid], torch.zeros(1, 6), poses[mid:]])
     inv_t = pose_vec2mat(poses.to(device), rotation_mode=rotation_mode).cpu().numpy().astype(np.float64)
     rot = np.linalg.inv(inv_t[:, :, :3])
@@ -109,15 +127,7 @@ def flow_sample_errors(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kin
     """tgt/refs: normalised device tensors [1,3,H,W] (4 refs), flow_gt [1,3,Hg,Wg], obj_map_gt [1,Hg,Wg] ->
     [epe_total, epe_sp, epe_mv, Fl] with the learned rigidity mask and the same four with the ground-truth object map
     (test_flow.py:112-140), plus the composed flow."""
-    for n in (disp_net, pose_net, mask_net, flow_net):
-        n.eval()
-    disp = disp_net(tgt)
-    depth = 1 / disp
-    pose = pose_net(tgt, refs)
-    emask = mask_net(tgt, refs)
-    # test_flow.py:122-125: Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
-    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
-    flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
+    emask, flow_cam, flow_fwd = _flow_nets(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv)
     rigidity = (1 - (1 - emask[:, 1]) * (1 - emask[:, 2])).unsqueeze(1) > 0.5
     soft = (flow_cam - flow_fwd).abs()
     census = (soft[:, 0] < THRESH).type_as(flow_fwd) * (soft[:, 1] < THRESH).type_as(flow_fwd)
@@ -159,15 +169,7 @@ def mask_sample_errors(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kin
     """tgt/refs: normalised device tensors [1,3,H,W] (4 refs), obj_map_gt / semantic_map_gt [1,Hg,Wg] ->
     (errors, errors_census, errors_bare, masks): the three lists of six counts test_mask.py:150-152 accumulates, and
     masks [1,4,H,W] on the device (combined is what the script saves, the soft census what it draws)."""
-    for n in (disp_net, pose_net, mask_net, flow_net):
-        n.eval()
-    disp = disp_net(tgt)
-    depth = 1 / disp
-    pose = pose_net(tgt, refs)
-    emask = mask_net(tgt, refs)
-    # test_mask.py:123-126: Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
-    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
-    flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
+    emask, flow_cam, flow_fwd = _flow_nets(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv)
     counts, masks = motion_mask_counts(emask, flow_cam, flow_fwd, obj_map_gt, semantic_map_gt, THRESH, want_masks=True)
     errors, errors_census, errors_bare = counts[0].cpu().tolist()
     return errors, errors_census, errors_bare, masks
@@ -225,15 +227,7 @@ def flow_submission_sample(disp_net, pose_net, mask_net, flow_net, tgt, refs, K,
     frame size -> flow_submission's dict of device tensors; want_viz adds 'full' and 'viz' = uint8 [B,3,3*Hg,Wg], row 2
     of the script's visualisation (cam, fwd and total flow stacked, one radius).  Row 1 (matplotlib's magma map of the
     target, disparity and mask) is not produced.  No host synchronisation."""
-    for n in (disp_net, pose_net, mask_net, flow_net):
-        n.eval()
-    disp = disp_net(tgt)
-    depth = 1 / disp
-    pose = pose_net(tgt, refs)
-    emask = mask_net(tgt, refs)
-    # submit_flow.py:113-116: Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
-    flow_fwd = flow_net(tgt, refs[1:3])[0] if isinstance(flow_net, models.Back2Future) else flow_net(tgt, refs[2])
-    flow_cam = pose2flow(depth.squeeze(1), pose[:, 2], K, Kinv)
+    emask, flow_cam, flow_fwd = _flow_nets(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv)
     out = flow_submission(emask, flow_cam, flow_fwd, Hg, Wg, THRESH, want_full=want_viz)
     if want_viz:
         out['viz'] = flow_colors(out['full'])
@@ -388,8 +382,7 @@ def depth_eval_batch(disp_net, tgt, gt_depth, min_depth=1e-3, max_depth=80.0, cr
     poses = None
     if pose_net is not None:
         pose_net.eval()
-        res = pose_net(tgt, refs)
-        poses = res[1] if isinstance(res, tuple) else res
+        poses = _pose(pose_net(tgt, refs))
     return depth_errors(gt_depth, pred, min_depth, max_depth, crop, poses, displacements if poses is not None else None)
 
 

@@ -29,6 +29,19 @@ def case_depth_errors_golden(device):
         assert (got[3:] - T(g[key])[3:]).abs().max().item() <= 2e-7, 'a1..a3 are counts / n'
 
 
+def case_depth_errors_medians(device):
+    """compute_errors scales by torch.median, the LOWER middle value.  Even count: gt 1..8 against four 1s and four 2s
+    scales by 4 / 1 (the upper middle values would give 5 / 2); odd count: one pixel fewer.  Against the oracle, each
+    sample alone and both in one batch."""
+    gt = torch.arange(1, 9, dtype=torch.float32).reshape(1, 2, 4).repeat(2, 1, 1)
+    pred = torch.tensor([1., 2., 1., 2., 2., 1., 2., 1.]).reshape(1, 2, 4).repeat(2, 1, 1)
+    gt[1, 1, 3] = 0.                                                    # 7 valid pixels
+    for sl in (slice(0, 1), slice(1, 2), slice(0, 2)):
+        want = torch.stack([torch.as_tensor(v) for v in OM.compute_errors(gt[sl], pred[sl], crop=False)])
+        got = torch.stack([v.cpu() for v in CL.compute_errors(gt[sl].to(device), pred[sl].to(device), crop=False)])
+        assert_close(got, want, 1e-6, 'compute_errors medians, samples %s' % sl)
+
+
 def case_metrics_oracle_sizes(device, B=2, Hg=375, Wg=1242, hp=256, wp=832, seed=3):
     """KITTI-2015 ground-truth size against full-resolution predictions (validate_flow_with_gt, train.py:588-668), and a
     depth map pair with ties around the median."""
@@ -98,4 +111,4 @@ def case_input_pipeline_fullsize(device, B=4, Hs=256, Ws=832):
     assert tgt.shape == (B, 3, Hs, Ws) and len(refs) == 4 and out.min() >= -1 - 1e-6 and out.max() <= 1 + 1e-6
 
 
-IO_CASES = [case_flow_metrics_golden, case_depth_errors_golden, case_input_pipeline_golden]
+IO_CASES = [case_flow_metrics_golden, case_depth_errors_golden, case_depth_errors_medians, case_input_pipeline_golden]
