@@ -2,7 +2,8 @@
 //
 //   D[128 pixels x N<=128 channels] (fp32, registers) += A[128 x 32] (im2col tile) * B[N x 32]^T (weights)
 //
-// * one CTA = one 128-pixel x N-channel output tile; one producer warpgroup + two consumer warpgroups, each
+// * one CTA works on one 128-pixel x N-channel output tile at a time (fprop / dgrad: one persistent CTA per SM walks
+//   the tiles and splits through one stage ring); one producer warpgroup + two consumer warpgroups, each
 //   consumer owning 64 of the 128 rows (wgmma m64nNk8, N = the launch's channel tile rounded up to 16/32/64/128);
 // * A is gathered straight from the NCHW activations (no im2col buffer in HBM): a K-chunk is 4
 //   consecutive input channels of one filter tap, so the 4 loads of a chunk share the tap's bounds
@@ -14,9 +15,10 @@
 //   tf32 MMAs (hi*hi + lo*hi + hi*lo) ("3xTF32", error ~2^-21).  The tensor core only sums one 32-deep stage (small
 //   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
 //   fp32 adds, so no long accumulation chain runs through the tensor core's own rounding;
-// * fprop / dgrad: the producers store the gathered A tile once, unsplit, in the order of the wgmma A register
-//   fragment (see tc_load_a); each consumer thread loads its 16 values with 4 conflict-free LDS.128, splits them and
-//   issues wgmma with A from registers (B by descriptor), so A crosses shared memory twice per stage instead of
+// * fprop / dgrad: the producers gather the A tile once, unsplit, with zero-filling 4-byte cp.async straight from
+//   global into shared memory (k-major, see tc_a_idx); a producer never waits for its own copies, so up to `depth`
+//   stages of loads are in flight.  Each consumer thread loads its 16 values with 16 conflict-free LDS.32, splits them
+//   and issues wgmma with A from registers (B by descriptor), so A crosses shared memory twice per stage instead of
 //   being stored twice and read three times.  The consumers load and split the next stage while the current
 //   stage's MMAs run, and take registers from the producers (setmaxnreg) to hold both.  The wgrad kernel splits both
 //   operands in its producers and reads both from shared memory;
@@ -68,8 +70,9 @@ struct TcArgs {
     int M;                 // B * Hc * Wc
     int act;
     float slope;
-    int ktiles, kt_per_split, splits;  // k-tiles of 32 (Kp / 32), split-K over them (grid.z); partials go to `partial`
+    int ktiles, kt_per_split, splits;  // k-tiles of 32 (Kp / 32), split-K over them; partials go to `partial`
     float* partial;                    // [splits][numel(out)] raw accumulators (bias/res/act applied by the reduce kernel)
+    int tiles_m, tiles_n, units;       // work units: 128-pixel tile (fastest) x channel tile x split, units = product
     long long out_numel;
     int depth, b_tile_bytes;           // stage ring (tc_geometry)
     signed char off_y[TC_MAX_TAPS], off_x[TC_MAX_TAPS];
@@ -120,6 +123,17 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 __device__ __forceinline__ void tma_prefetch_map(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+// 4-byte asynchronous copy global -> shared (through L1, not through registers).  With `valid` false no byte is read
+// and the destination is zero-filled; `src` must still be a valid global address.
+__device__ __forceinline__ void cp_async_4(uint32_t dst, const float* src, bool valid) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(valid ? 4 : 0) : "memory");
+}
+// one arrival on `bar`, made once every cp.async this thread issued before it has landed; .noinc: the arrival counts
+// against the barrier's expected count
+__device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ float tf32_hi(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -379,32 +393,28 @@ __device__ __forceinline__ void tc_consume(const TcRing& ring, int nkt, int wg, 
     }
 }
 
-// The fprop kernel's A tile: one fp32 copy of the stage's 128 x 32 im2col values, unsplit, laid out for the consumers'
-// register fragments.  Row r is 8 16-byte chunks (the first A slot of the stage; the second goes unused):
+// The fprop kernel's A tile: one fp32 copy of the stage's 128 x 32 im2col values, unsplit (the first A slot of the
+// stage; the second goes unused), k-major with the row index swizzled by k:
 //
-//   A[r][k] is element k / 4 % 4 of float4 tile_idx(r, 2 * (k % 4) + k / 16),
+//   A[r][k] is float tc_a_idx(r, k) = 128 k + (r ^ 8 (k % 4)).
 //
-// so chunks 2t and 2t + 1 hold k = t, t + 4, ..., t + 28: the k of fragment column t over all 4 k-steps of the stage.
-// A consumer thread (rows r0 = wg * 64 + wq * 16 + lane / 4 and r0 + 8, column t = lane % 4) reads its 16 values with
-// 4 LDS.128.  They are bank-conflict free: a 128-bit shared load is served 8 lanes at a time, and lanes 8p .. 8p + 7
-// read chunk 2t + h (t = 0..3, fixed h) of the rows with r0 & 7 = 2p and 2p + 1.  The swizzle puts that chunk at
-// 16-byte bank group (2t + h) ^ (r & 7), and a 128-byte row spans the 32 banks once, so row 2p's lanes hit groups
-// {(2t + h) ^ 2p} = {0, 2, 4, 6} + h and row 2p + 1's lanes {0, 2, 4, 6} + (1 - h): 8 distinct groups, 32 banks.
-// The producer of row r stores its 8 chunks with STS.128 as before; the 8 rows of a lane octet differ in r & 7, so
-// each chunk index lands on 8 distinct groups.
+// Both sides are bank-conflict free.  The producers write it with 4-byte cp.async, a warp's 32 lanes being the 32
+// consecutive rows 32 w + lane at one k: r ^ 8 (k % 4) permutes those 32 rows among themselves (8 (k % 4) < 32), so
+// the 32 words land on the 32 banks.  A consumer thread (rows r0 = wg * 64 + wq * 16 + lane / 4 and r0 + 8, column
+// t = lane % 4) reads its 16 values with 16 LDS.32 at k = t + 4 j, all with k % 4 = t: lane l of a warp reads bank
+// (r0 + 8 h) ^ 8 t mod 32, whose low 3 bits are lane / 4 and whose bits 3-4 are those of wq * 16 + 8 h flipped by t,
+// so the 8 row offsets times the 4 columns of the warp cover the 32 banks once.
 struct TcAFrag { uint32_t hi[TC_KC / 2][4], lo[TC_KC / 2][4]; };   // [k-step][wgmma A register]
 
+__device__ __forceinline__ int tc_a_idx(int r, int k) { return k * TC_M + (r ^ (8 * (k & 3))); }
 // this thread's 16 raw values of the A tile at `tile`: v[h][j] = A[r0 + 8 h][t + 4 j].  `off` is the byte offset of
-// chunk 2t of row r0 (tc_a_off); chunk 2t + 1 sits at off ^ 16 (the swizzle flips the low chunk bit alike), row r0 + 8
-// 1 KB further on (same r & 7).
-__device__ __forceinline__ int tc_a_off(int r0, int t) { return tile_idx(r0, 2 * t) * 16; }
+// A[r0][t] (tc_a_off); r0 & 8 = 0, so row r0 + 8 flips bit 3 of the row, byte bit 5, and k + 4 j is 2 KB further on.
+__device__ __forceinline__ int tc_a_off(int r0, int t) { return tc_a_idx(r0, t) * 4; }
 __device__ __forceinline__ void tc_load_a(const unsigned char* tile, int off, float (&v)[2][8]) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const float4 c0 = *(const float4*)(tile + (off + 1024 * h)), c1 = *(const float4*)(tile + ((off ^ 16) + 1024 * h));
-        v[h][0] = c0.x; v[h][1] = c0.y; v[h][2] = c0.z; v[h][3] = c0.w;
-        v[h][4] = c1.x; v[h][5] = c1.y; v[h][6] = c1.z; v[h][7] = c1.w;
-    }
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[h][j] = *(const float*)(tile + ((off ^ (32 * h)) + 2048 * j));
 }
 // the split of tc_split_store, hi = tf32(x), lo = tf32(x - hi), into the fragment: k-step ks, register i holds
 // row r0 + 8 (i & 1), k = 8 ks + t + 4 (i >> 1)
@@ -423,9 +433,9 @@ __device__ __forceinline__ void tc_split_a(const float (&v)[2][8], TcAFrag& f) {
 // stage's MMAs run the thread waits for the next stage and loads and splits its A fragment.  At N = 128 acc + part
 // already take 128 registers and a second fragment does not fit without spilling, so each stage's A is loaded and
 // split after its full barrier, as the producers used to.  B of the current stage is read by the MMAs until the wait,
-// so the stage is released after it.
+// so the stage is released after it.  The unit's k-tiles are the CTA's g-th onwards: they start in stage g % depth.
 template <int NT>
-__device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int nkt, int wg, int wq, int lane, float (&acc)[NT / 2]) {
+__device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt, int wg, int wq, int lane, float (&acc)[NT / 2]) {
     constexpr bool split_ahead = NT < 128;
     float part[NT / 2];
 #pragma unroll
@@ -434,15 +444,15 @@ __device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int nkt, int w
     const int a_off = tc_a_off(wg * 64 + wq * 16 + (lane >> 2), lane & 3);
     TcAFrag cur, nxt;
     float v[2][8];
+    int s = g % ring.depth;                     // stage of k-tile it
+    uint32_t phase = (g / ring.depth) & 1;      // parity of k-tile it's round
     if constexpr (split_ahead) {
         if (nkt > 0) {
-            mbar_wait(&ring.full[0], 0);
-            tc_load_a(ring.tiles(ring.smem, 0).a_hi, a_off, v);
+            mbar_wait(&ring.full[s], phase);
+            tc_load_a(ring.tiles(ring.smem, s).a_hi, a_off, v);
             tc_split_a(v, cur);
         }
     }
-    int s = 0;                // stage of k-tile it
-    uint32_t phase = 0;       // parity of k-tile it's round
     for (int it = 0; it < nkt; ++it) {
         if constexpr (!split_ahead) {
             mbar_wait(&ring.full[s], phase);
@@ -486,131 +496,156 @@ __device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int nkt, int w
     }
 }
 
+// One work unit: the 128-pixel x 128-channel output tile and the k-tiles of one split.
+struct TcUnit { int m0, n0, z, kt_beg, nkt; };
+__device__ __forceinline__ TcUnit tc_unit(const TcArgs& a, int u) {
+    TcUnit w;
+    w.m0 = (u % a.tiles_m) * TC_M;
+    u /= a.tiles_m;
+    w.n0 = (u % a.tiles_n) * TC_NMAX;
+    w.z = u / a.tiles_n;
+    w.kt_beg = w.z * a.kt_per_split;
+    w.nkt = max(0, min(a.ktiles, w.kt_beg + a.kt_per_split) - w.kt_beg);   // k-tiles of this split
+    return w;
+}
+
+// Persistent: a CTA runs units blockIdx.x, blockIdx.x + gridDim.x, ... through one stage ring, its g-th k-tile in stage
+// g % depth, so the producers gather the next unit's first stages while the consumers finish the current one and
+// store it, and the set-up and the ring's first fill are paid once per CTA instead of once per tile.
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
-    // full[s]: the 128 producers' A stores + producer 0's arrival that announces the B tiles' TMA bytes
+    // full[s]: the 128 producers' arrivals, each made when that thread's A copies have landed, + producer 0's arrival
+    // that announces the B tiles' TMA bytes
     const TcRing ring = tc_ring(a.depth, a.b_tile_bytes, TC_PRODUCERS + 1);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
-    const int ntile = min(TC_NMAX, a.Ntot - n0);
-    const int kt_beg = blockIdx.z * a.kt_per_split;
-    const int nkt = max(0, min(a.ktiles, kt_beg + a.kt_per_split) - kt_beg);   // k-tiles of this split
     const long long HWin = (long long)a.Hin * a.Win;
 
     if (warp < TC_PRODUCERS / 32) {
         // ===================== producers: thread == tile row =====================
         wg_regs_dec<TC_PRODUCER_REGS>();
         const int r = tid;
-        const int m = m0 + r;
-        const bool mvalid = m < a.M;
-        int b = 0, oy = 0, ox = 0;
-        if (mvalid) {
-            int hw = a.Hc * a.Wc;
-            b = m / hw;
-            int rem = m - b * hw;
-            oy = rem / a.Wc;
-            ox = rem - oy * a.Wc;
-        }
-        const float* xb = a.x + (long long)b * a.Cin * HWin;
-        const int iy0 = oy * a.in_stride, ix0 = ox * a.in_stride;
         const int cpt = a.cpad >> 2;                 // chunks per tap
         const int nchunks = a.ntaps * cpt;           // real chunks; the rest of Kp is zero padding
         if (r == 0) tma_prefetch_map(&a.wmap);
-        for (int it = 0; it < nkt; ++it) {
-            const int s = it % ring.depth;
-            const int kt = kt_beg + it;                   // global k-tile
-            // ---- A: the 8 chunks (32 floats) of this thread's pixel row
-            float av[TC_KC][4];
-            const int q0 = kt * TC_KC;
-            const int tap0 = q0 / cpt, c40 = q0 - tap0 * cpt;
-            if (c40 + TC_KC <= cpt) {
-                // fast path (C_in % 32 == 0 layers): the whole stage reads one filter tap -> one bounds check,
-                // one base pointer, 32 loads that differ only by the channel-plane stride
-                bool ok = mvalid && tap0 < a.ntaps;
-                int pix = 0;
-                if (ok) {
-                    const int iy = iy0 + a.off_y[tap0], ix = ix0 + a.off_x[tap0];
-                    ok = (iy >= 0) && (iy < a.Hin) && (ix >= 0) && (ix < a.Win);
-                    pix = iy * a.Win + ix;
+        int g = 0;                                   // k-tiles this CTA has gathered
+        for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+            const TcUnit w = tc_unit(a, u);
+            const int m = w.m0 + r;
+            const bool mvalid = m < a.M;
+            int b = 0, oy = 0, ox = 0;
+            if (mvalid) {
+                int hw = a.Hc * a.Wc;
+                b = m / hw;
+                int rem = m - b * hw;
+                oy = rem / a.Wc;
+                ox = rem - oy * a.Wc;
+            }
+            const float* xb = a.x + (long long)b * a.Cin * HWin;
+            const int iy0 = oy * a.in_stride, ix0 = ox * a.in_stride;
+            for (int it = 0; it < w.nkt; ++it, ++g) {
+                const int s = g % ring.depth;
+                const int kt = w.kt_beg + it;                 // global k-tile
+                const TcTiles<unsigned char*> t = ring.acquire(g, s);
+                // ---- B: the weights were split into tf32 hi / lo by the prep kernel: one TMA box per copy; rows in
+                //      [ntile, NT) past the last channel are zero-filled, and the epilogue ignores those columns
+                if (r == 0) {
+                    mbar_arrive_expect_tx(&ring.full[s], 2 * ring.b_tile_bytes);
+                    tma_load_3d(t.b_hi, &a.wmap, &ring.full[s], kt * (TC_KC * 4), w.n0, 0);
+                    tma_load_3d(t.b_lo, &a.wmap, &ring.full[s], kt * (TC_KC * 4), w.n0, 1);
                 }
-                const float* p = xb + (long long)(c40 * 4) * HWin + pix;
-                const int nv = ok ? (a.Cin - c40 * 4) : 0;
-#pragma unroll
-                for (int c = 0; c < TC_KC; ++c)
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) av[c][j] = (c * 4 + j < nv) ? __ldg(p + (c * 4 + j) * HWin) : 0.f;
-            } else {
-                int q = q0, tap = tap0, c4 = c40;
-#pragma unroll
-                for (int c = 0; c < TC_KC; ++c) {
-                    av[c][0] = av[c][1] = av[c][2] = av[c][3] = 0.f;
-                    if (mvalid && q < nchunks) {
-                        const int iy = iy0 + a.off_y[tap], ix = ix0 + a.off_x[tap];
-                        if (iy >= 0 && iy < a.Hin && ix >= 0 && ix < a.Win) {
-                            const float* p = xb + (long long)(c4 * 4) * HWin + (iy * a.Win + ix);
-                            const int nv = a.Cin - c4 * 4;
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                if (j < nv) av[c][j] = __ldg(p + j * HWin);
-                        }
+                const uint32_t at = smem_u32(t.a_hi);
+                // ---- A: the 8 chunks (32 floats) of this thread's pixel row, k = 4c + j of the stage, copied by cp.async
+                //      straight into the tile (tc_a_idx) with zeros where the im2col matrix has none.  The thread never
+                //      waits for its copies: its arrival on full[s] is made when they land, so up to `depth` stages of
+                //      loads are in flight.  The consumers read A with ld.shared, so no proxy fence is needed.
+                const int q0 = kt * TC_KC;
+                const int tap0 = q0 / cpt, c40 = q0 - tap0 * cpt;
+                if (c40 + TC_KC <= cpt) {
+                    // fast path (C_in % 32 == 0 layers): the whole stage reads one filter tap -> one bounds check,
+                    // one base pointer, 32 loads that differ only by the channel-plane stride
+                    bool ok = mvalid && tap0 < a.ntaps;
+                    int pix = 0;
+                    if (ok) {
+                        const int iy = iy0 + a.off_y[tap0], ix = ix0 + a.off_x[tap0];
+                        ok = (iy >= 0) && (iy < a.Hin) && (ix >= 0) && (ix < a.Win);
+                        pix = iy * a.Win + ix;
                     }
-                    ++q;
-                    if (++c4 == cpt) { c4 = 0; ++tap; }
+                    const float* p = ok ? xb + (long long)(c40 * 4) * HWin + pix : a.x;
+                    const int nv = ok ? (a.Cin - c40 * 4) : 0;
+#pragma unroll
+                    for (int c = 0; c < TC_KC; ++c)
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            const bool v = c * 4 + j < nv;
+                            cp_async_4(at + 4 * tc_a_idx(r, 4 * c + j), v ? p + (c * 4 + j) * HWin : a.x, v);
+                        }
+                } else {
+                    int q = q0, tap = tap0, c4 = c40;
+#pragma unroll
+                    for (int c = 0; c < TC_KC; ++c) {
+                        const float* p = a.x;
+                        int nv = 0;
+                        if (mvalid && q < nchunks) {
+                            const int iy = iy0 + a.off_y[tap], ix = ix0 + a.off_x[tap];
+                            if (iy >= 0 && iy < a.Hin && ix >= 0 && ix < a.Win) {
+                                p = xb + (long long)(c4 * 4) * HWin + (iy * a.Win + ix);
+                                nv = a.Cin - c4 * 4;
+                            }
+                        }
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            const bool v = j < nv;
+                            cp_async_4(at + 4 * tc_a_idx(r, 4 * c + j), v ? p + j * HWin : a.x, v);
+                        }
+                        ++q;
+                        if (++c4 == cpt) { c4 = 0; ++tap; }
+                    }
                 }
+                cp_async_arrive(&ring.full[s]);
             }
-            const TcTiles<unsigned char*> t = ring.acquire(it, s);
-            // ---- B: the weights were split into tf32 hi / lo by the prep kernel: one TMA box per copy; rows in
-            //      [ntile, NT) past the last channel are zero-filled, and the epilogue ignores those columns
-            if (r == 0) {
-                mbar_arrive_expect_tx(&ring.full[s], 2 * ring.b_tile_bytes);
-                tma_load_3d(t.b_hi, &a.wmap, &ring.full[s], kt * (TC_KC * 4), n0, 0);
-                tma_load_3d(t.b_lo, &a.wmap, &ring.full[s], kt * (TC_KC * 4), n0, 1);
-            }
-            // ---- A: the row's 32 floats, unsplit, in the consumers' fragment order (k = 4c + e goes to chunk 2e + c / 4,
-            //      see tc_load_a); the consumers read them with ld.shared, so no proxy fence is needed
-            float4* at = (float4*)t.a_hi;
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    at[tile_idx(r, 2 * e + h)] = make_float4(av[4 * h][e], av[4 * h + 1][e], av[4 * h + 2][e], av[4 * h + 3][e]);
-            mbar_arrive(&ring.full[s]);
         }
+        cp_async_wait_all();      // no thread leaves copies in flight behind it
     } else {
         // ===================== consumers: MMA + epilogue =====================
         wg_regs_inc<TC_CONSUMER_REGS>();
         const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
-        float acc[NT / 2];
-        tc_consume_rs<NT>(ring, nkt, wg, wq, lane, acc);
         const long long HWout = (long long)a.Hout * a.Wout;
+        int g = 0;                                   // k-tiles this CTA has consumed
+        for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+            const TcUnit w = tc_unit(a, u);
+            const int ntile = min(TC_NMAX, a.Ntot - w.n0);
+            float acc[NT / 2];
+            tc_consume_rs<NT>(ring, g, w.nkt, wg, wq, lane, acc);
+            g += w.nkt;
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int em = m0 + tc_acc_row(wg, wq, lane, half);
-            if (em >= a.M) continue;
-            int hw = a.Hc * a.Wc;
-            int eb = em / hw;
-            int rem = em - eb * hw;
-            int eoy = rem / a.Wc, eox = rem - eoy * a.Wc;
-            const long long obase = (long long)eb * a.Ntot * HWout + (long long)(eoy * a.out_stride + a.out_oy) * a.Wout +
-                                    (eox * a.out_stride + a.out_ox);
+            for (int half = 0; half < 2; ++half) {
+                const int em = w.m0 + tc_acc_row(wg, wq, lane, half);
+                if (em >= a.M) continue;
+                int hw = a.Hc * a.Wc;
+                int eb = em / hw;
+                int rem = em - eb * hw;
+                int eoy = rem / a.Wc, eox = rem - eoy * a.Wc;
+                const long long obase = (long long)eb * a.Ntot * HWout + (long long)(eoy * a.out_stride + a.out_oy) * a.Wout +
+                                        (eox * a.out_stride + a.out_ox);
 #pragma unroll
-            for (int i = 0; i < NT / 8; ++i)
+                for (int i = 0; i < NT / 8; ++i)
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int nl = tc_acc_col(lane, i, e);
-                    if (nl < ntile) {
-                        float o = acc[tc_acc_reg(i, half, e)];
-                        const int n = n0 + nl;
-                        const long long off = obase + (long long)n * HWout;
-                        if (a.splits > 1) {
-                            a.partial[(long long)blockIdx.z * a.out_numel + off] = o;
-                        } else {
-                            if (a.bias) o += __ldg(a.bias + n);
-                            if (a.res) o += __ldg(a.res + off);
-                            a.out[off] = apply_act(o, a.act, a.slope);
+                    for (int e = 0; e < 2; ++e) {
+                        const int nl = tc_acc_col(lane, i, e);
+                        if (nl < ntile) {
+                            float o = acc[tc_acc_reg(i, half, e)];
+                            const int n = w.n0 + nl;
+                            const long long off = obase + (long long)n * HWout;
+                            if (a.splits > 1) {
+                                a.partial[(long long)w.z * a.out_numel + off] = o;
+                            } else {
+                                if (a.bias) o += __ldg(a.bias + n);
+                                if (a.res) o += __ldg(a.res + off);
+                                a.out[off] = apply_act(o, a.act, a.slope);
+                            }
                         }
                     }
-                }
+            }
         }
     }
 }
@@ -692,8 +727,17 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     tc_geometry(N, nt, a.b_tile_bytes, a.depth, smem);
     rc = tc_weight_map(&a.wmap, wpp, N, a.Kp, nt);
     if (rc) return rc;
-    dim3 grid(cdiv(a.M, TC_M), cdiv(N, TC_NMAX), splits);
-    return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, grid, smem, st, "conv_tc");
+    a.tiles_m = cdiv(a.M, TC_M);
+    a.tiles_n = cdiv(N, TC_NMAX);
+    a.units = a.tiles_m * a.tiles_n * splits;
+    // one CTA per SM (launch bounds, registers) runs units until none are left
+    static int sms = [] {
+        int dev = 0, n = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+        return n > 0 ? n : NUM_SMS;
+    }();
+    return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, dim3(a.units < sms ? a.units : sms), smem, st, "conv_tc");
 }
 
 // ================================================================================================
