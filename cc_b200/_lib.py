@@ -197,6 +197,7 @@ _SIGS = {
     'ccb_launch_count': ('long long', ''),
     'ccb_debug_last_conv_kernel': ('const char*', ''),
     'ccb_debug_tc_plan': (STATUS, 'int, host int*'),
+    'ccb_debug_conv_plan': (STATUS, 'const ccb_conv_desc*, int, host int*'),
 }
 
 _SCALARS = {'int': C.c_int, 'long long': C.c_longlong, 'float': C.c_float, 'double': C.c_double}

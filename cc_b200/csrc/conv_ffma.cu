@@ -471,6 +471,16 @@ extern "C" long long ccb_conv_workspace_floats(const ccb_conv_desc* d, int op) {
     return conv_plan(d, op).work_floats;
 }
 
+extern "C" int ccb_debug_conv_plan(const ccb_conv_desc* d, int op, int* out2) {
+    if (op < CCB_CONV_FPROP || op > CCB_CONV_WGRAD || !out2) return CCB_ERR_ARG;
+    const int rc = check_desc(d);
+    if (rc) return rc;
+    const ConvPlan p = conv_plan(d, op);
+    out2[0] = p.path;
+    out2[1] = p.splits;
+    return CCB_OK;
+}
+
 extern "C" int ccb_conv2d_fprop(const ccb_conv_desc* d, const float* x, const float* w, const float* bias,
                                 const float* res, float* y, float* work, long long work_floats, ccb_stream_t stream) {
     CCB_REQUIRE(x && w && y, CCB_ERR_ARG, "conv2d_fprop: null pointer");

@@ -13,6 +13,10 @@ const char* ccb_debug_last_conv_kernel(void);
 /* host-side geometry of the wgmma convolution kernels for N output channels (no launch; unit tests):
  * out4 = {wgmma N, bytes of one B operand copy, pipeline stages, dynamic shared memory bytes} */
 int ccb_debug_tc_plan(int N, int* out4);
+/* the plan a convolution call with this descriptor runs (no launch; the layer audit records it per call):
+ * out2 = {path: 0 CUDA-core GEMM, 1 tensor cores, 2 tensor-core weight gradient through rows padded to a multiple of 4;
+ *         split-K count} */
+int ccb_debug_conv_plan(const ccb_conv_desc* d, int op, int* out2);
 
 #ifdef __cplusplus
 }

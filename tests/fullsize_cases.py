@@ -192,24 +192,18 @@ def summarise(rep):
                                                                  '' if r['ok'] else 'FAIL'))
 
 
-def audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
-    """The layer audit (tests/layer_audit.py) of the step the benchmark times: Trainer(cfg) from the oracle's weights, one
-    eager step (it records the weight-cache layouts, which then commit), then the SECOND eager step - committed cache,
-    production IMPL_AUTO dispatch - with every layer call checked against fp64 element by element.
-      * completeness: every Conv2d / ConvTranspose2d / BatchNorm2d module of the nets is audited forward and backward
-        (the occlusion decoders do not run in training, see build_nets), and Back2Future's ten cost volumes and eight
-        feature warps;
-      * non-interference: the audited step's loss and flat gradient equal, bit for bit, an unaudited second step from
-        the same snapshot;
-      * coverage: the coarsest cost volume (C = 192 on a 4x13 map: one tile per sample) runs corr_chunks = 32 channel
-        chunks, and the BatchNorm of DispResNet6's iconv1 shortcut reduces its 851968 values per channel in 104 splits.
-    Returns the audit summary."""
-    from tests import layer_audit as LA
+def _second_step(device, cfg, B, H, W, seed, flownet):
+    """Trainer(cfg, flownet=flownet) from the oracle's weights (FlowNetC6: flownetc6_cases.step_flow_params, which keep
+    its flows finite), one eager step (it records the weight-cache layouts, which then commit), then an unaudited second
+    step from a snapshot that is restored.  -> (trainer, step arguments, loss and flat gradient of the second step)."""
+    from tests import flownetc6_cases as FC6
     tgt, refs = synth.frames(B, H, W, seed=seed)
     K, Kinv = synth.intrinsics(B, H, W)
     P = OS.make_params(cfg)
+    if flownet == 'FlowNetC6':
+        P['flow'] = FC6.step_flow_params()
     sd = {n: {k: v.detach().clone() for k, v in d.items()} for n, d in P.items()}
-    tr = Trainer(cfg, device, state_dicts=sd)
+    tr = Trainer(cfg, device, state_dicts=sd, flownet=flownet)
     args = (tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device))
     tr.step(*args)
     assert tr.wcache is not None and tr.wcache.committed
@@ -218,8 +212,12 @@ def audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
     grad_ref = tr.opt.flat_g.clone()
     tr._restore(snap)
     torch.cuda.synchronize(device)
+    return tr, args, loss_ref, grad_ref
+
+
+def _audited_step(device, tr, args, loss_ref, grad_ref, audit):
+    """The second step under `audit`, timed; its loss and flat gradient must equal the unaudited ones bit for bit."""
     t0 = time.perf_counter()
-    audit = LA.LayerAudit(nets=tr.nets, tag='%s_b%d_%dx%d' % (cfg, B, H, W))
     with audit:
         loss = tr.step(*args)[0]
     torch.cuda.synchronize(device)
@@ -229,54 +227,80 @@ def audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
     st = tr.wcache.stats()
     assert st['misses'] == 0 and st['hits'] > 0, st
 
+
+def _tc_only(row):
+    return bool(row.get('plans')) and all(p['path'] != 'ffma' for p in row['plans'])
+
+
+def audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50, flownet='Back2Future'):
+    """The layer audit (tests/layer_audit.py) of the step the benchmark times, with either flow net: Trainer(cfg) from the
+    oracle's weights, one eager step, then the SECOND eager step - committed cache, production IMPL_AUTO dispatch - with
+    every layer call checked against fp64 element by element.
+      * completeness: every Conv2d / ConvTranspose2d / BatchNorm2d module of the nets is audited forward and backward
+        (Back2Future's occlusion decoders do not run in training, see build_nets); Back2Future's ten cost volumes and
+        eight feature warps, or FlowNetC6's two dilated cost volumes (one per flow-net call) and nothing else;
+      * non-interference: the audited step's loss and flat gradient equal, bit for bit, an unaudited second step from
+        the same snapshot;
+      * coverage, Back2Future: the coarsest cost volume (C = 192 on a 4x13 map: one tile per sample) runs corr_chunks =
+        32 channel chunks, and the BatchNorm of DispResNet6's iconv1 shortcut reduces its 851968 values per channel in
+        104 splits.  FlowNetC6: conv3_1 (473 input channels, a ragged last 4-channel chunk) and deconv4 (its data
+        gradient an fprop with N = 1026 = 8 x 128 + 2) run the tensor-core kernels in both phases, a call with 1026
+        channels is audited, and the plans include split-K tensor-core fprop / dgrad calls and weight gradients through
+        padded rows.
+    Measured on an H100 80GB HBM3 (700 W power limit), cfg3 b4 256x832: worst r per family in layer_audit.R_MEASURED;
+    the audited step takes 2.0 s with Back2Future and 2.2-3.8 s with FlowNetC6 (wall time, fp64 references included).
+    Returns the audit summary."""
+    from tests import layer_audit as LA
+    tr, args, loss_ref, grad_ref = _second_step(device, cfg, B, H, W, seed, flownet)
+    audit = LA.LayerAudit(nets=tr.nets, tag='%s_b%d_%dx%d%s' % (cfg, B, H, W, '' if flownet == 'Back2Future' else '_' + flownet))
+    _audited_step(device, tr, args, loss_ref, grad_ref, audit)
+
     rows = audit.rows
     want = {'%s.%s' % (n, k) for n, net in tr.nets.items() for k, m in net.named_modules()
             if isinstance(m, (cnn.Conv2d, cnn.ConvTranspose2d, cnn.BatchNorm2d)) and not k.startswith('decoder_occ')}
     for phase in ('fwd', 'bwd'):
         got = {r['name'] for r in rows if r['phase'] == phase and r['op'] in ('conv', 'convT', 'bn')}
         assert got == want, (phase, sorted(want - got)[:10], sorted(got - want)[:10])
-    for op, n in (('corr81', 10), ('featwarp', 8)):
+    calls = dict(corr81=10, featwarp=8, corr441d=0) if flownet == 'Back2Future' else dict(corr81=0, featwarp=0, corr441d=2)
+    for op, n in calls.items():
         for phase in ('fwd', 'bwd'):
             k = sum(r['op'] == op and r['phase'] == phase and r['name'].startswith('flow') for r in rows)
             assert k == n, (op, phase, k)
-    h6, w6 = H // 64, W // 64
-    assert LA.corr_chunks(B, 192, h6, w6) == 32
-    assert {r['phase'] for r in rows if r['op'] == 'corr81' and r['shape'] == [B, 192, h6, w6] and r['chunks'] == 32} == {'fwd', 'bwd'}
+    assert not any(r['op'] == 'bn_eval' for r in rows)
+    if flownet == 'Back2Future':
+        h6, w6 = H // 64, W // 64
+        assert LA.corr_chunks(B, 192, h6, w6) == 32
+        assert {r['phase'] for r in rows if r['op'] == 'corr81' and r['shape'] == [B, 192, h6, w6] and r['chunks'] == 32} == {'fwd', 'bwd'}
+    else:
+        for name in ('flow.conv3_1.0', 'flow.deconv4.0'):            # the Conv2d / ConvTranspose2d of each block
+            assert {r['phase'] for r in rows if r['name'] == name and _tc_only(r)} == {'fwd', 'bwd'}, \
+                [(r['phase'], r['plans']) for r in rows if r['name'] == name]
+        assert any(r['op'] in ('conv', 'convT') and 1026 in r['shape'][:2] for r in rows)
+        plans = [p for r in rows for p in r.get('plans', ())]
+        assert any(p['path'] == 'tc' and p['call'] != 'wgrad' and p['splits'] > 1 for p in plans)
+        assert any(p['path'] == 'tc_padded' for p in plans)
     assert LA.bn_splits(B, H * W) == 104
     assert {r['phase'] for r in rows if r['op'] == 'bn' and r['name'] == 'disp.iconv1.0.downsample.1' and r['splits'] == 104} == {'fwd', 'bwd'}
     return audit.summary()
 
 
-def loss_audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
-    """The loss audit (tests/loss_audit.py) of the step the benchmark times, set up as audit_step: one eager step, then
-    the second step with the weight cache committed, every loss-layer call checked against fp64 element by element.
+def loss_audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50, flownet='Back2Future'):
+    """The loss audit (tests/loss_audit.py) of the step the benchmark times, with either flow net, set up as audit_step:
+    one eager step, then the second step with the weight cache committed, every loss-layer call checked against fp64
+    element by element.
       * completeness: one rigid and one flow photometric call (forward and backward), four smoothness and two BCE calls
-        (forward and backward), one consensus-target call, twelve pose2flow forwards; every level has partial tiles;
+        (forward and backward), one consensus-target call, twelve pose2flow forwards, whichever the flow net; every
+        level has partial tiles;
       * non-interference: the audited step's loss and flat gradient equal, bit for bit, an unaudited second step;
       * detectability: one dropped level-0 tile would put d_pose over its bound (the audit's tile_drop_r).
+    Measured on an H100 80GB HBM3 (700 W power limit), cfg3 b4 256x832: worst r per output in loss_audit.R_MEASURED
+    (the FlowNetC6 step's are no larger); the audited step takes 4.7-5.1 s with Back2Future and 7.1-7.3 s with FlowNetC6 (wall
+    time, fp64 references included).
     Returns the audit summary."""
     from tests import loss_audit as LSA
-    tgt, refs = synth.frames(B, H, W, seed=seed)
-    K, Kinv = synth.intrinsics(B, H, W)
-    P = OS.make_params(cfg)
-    sd = {n: {k: v.detach().clone() for k, v in d.items()} for n, d in P.items()}
-    tr = Trainer(cfg, device, state_dicts=sd)
-    args = (tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device))
-    tr.step(*args)
-    assert tr.wcache is not None and tr.wcache.committed
-    snap = tr._snapshot()
-    loss_ref = tr.step(*args)[0].clone()
-    grad_ref = tr.opt.flat_g.clone()
-    tr._restore(snap)
-    torch.cuda.synchronize(device)
-    t0 = time.perf_counter()
-    audit = LSA.LossAudit(tag='%s_b%d_%dx%d' % (cfg, B, H, W))
-    with audit:
-        loss = tr.step(*args)[0]
-    torch.cuda.synchronize(device)
-    print('   audited step: %.1f s (fp64 references included)' % (time.perf_counter() - t0))
-    assert torch.equal(loss, loss_ref), (loss.item(), loss_ref.item())
-    assert torch.equal(tr.opt.flat_g, grad_ref), 'the audit changed the flat gradient by %.3e' % (tr.opt.flat_g - grad_ref).abs().max().item()
+    tr, args, loss_ref, grad_ref = _second_step(device, cfg, B, H, W, seed, flownet)
+    audit = LSA.LossAudit(tag='%s_b%d_%dx%d%s' % (cfg, B, H, W, '' if flownet == 'Back2Future' else '_' + flownet))
+    _audited_step(device, tr, args, loss_ref, grad_ref, audit)
     n = {}
     for r in audit.rows:
         n[(r['op'], r['phase'])] = n.get((r['op'], r['phase']), 0) + 1
@@ -293,6 +317,84 @@ def loss_audit_step(device, cfg='cfg3', B=4, H=256, W=832, seed=50):
     assert summ['photo_rigid']['tile_drop_r'] > LSA.R_OUT[('photo_rigid', 'd_pose')], summ['photo_rigid']['tile_drop_r']
     print('   audited calls: %d' % len(audit.rows))
     return summ
+
+
+def seed_running_stats(nets, seed=31):
+    """Every BatchNorm's running statistics set far from their defaults (0, 1): mean ~ N(0, 0.5^2), var ~ U[0.25, 4]; a
+    kernel that ignored the mean, dropped eps or scaled by the variance would then miss the eval-mode bound."""
+    g = torch.Generator().manual_seed(seed)
+    n = 0
+    for net in nets.values():
+        for m in net.modules():
+            if isinstance(m, cnn.BatchNorm2d):
+                c = m.num_features
+                m.running_mean.copy_(0.5 * torch.randn(c, generator=g))
+                m.running_var.copy_(0.25 + 3.75 * torch.rand(c, generator=g))
+                n += 1
+    return n
+
+
+# Conv2d / ConvTranspose2d / BatchNorm2d modules evaluate._flow_nets does not run, with the reason.  None: every module of
+# the four nets runs in eval mode - DispResNet6 computes every disparity head (each feeds the next level), MaskNet6 is
+# built with output_exp=True, and Back2Future(nlevels=6) runs its occlusion decoders outside training.
+NOT_RUN_IN_EVAL = {}
+
+
+def eval_nets(device, flownet='Back2Future'):
+    """The four nets as the evaluation scripts load them: the oracle's weights, FlowNetC6 with step_flow_params."""
+    from cc_b200 import models as CM
+    from oracle import nets as ON
+    from tests import flownetc6_cases as FC6
+    nets = dict(disp=CM.DispResNet6(), pose=CM.PoseNetB6(nb_ref_imgs=4), mask=CM.MaskNet6(nb_ref_imgs=4, output_exp=True),
+                flow=CM.Back2Future(nlevels=6) if flownet == 'Back2Future' else CM.FlowNetC6())
+    sds = dict(disp=ON.disp_params(), pose=ON.pose_params(), mask=ON.mask_params(),
+               flow=ON.flow_params() if flownet == 'Back2Future' else FC6.step_flow_params())
+    for n, net in nets.items():
+        net.load_state_dict({k: v.detach().clone() for k, v in sds[n].items()})
+    return {n: net.to(device) for n, net in nets.items()}
+
+
+def audit_eval_forwards(device, flownet='Back2Future', H=256, W=832, seed=75, report=True):
+    """The layer audit of evaluate._flow_nets at B = 1 (test_flow.py / test_mask.py / submit_flow.py call the four nets
+    so, in eval mode): every BatchNorm's running statistics seeded far from the defaults (seed_running_stats), then
+      * non-interference: the audited outputs (mask, camera flow, flow-net flow) equal an unaudited run bit for bit;
+      * completeness: every Conv2d / ConvTranspose2d / BatchNorm2d has a forward row (NOT_RUN_IN_EVAL lists the
+        exceptions), every BatchNorm an eval-mode one (family bn_eval), and no call has a backward row;
+      * the flow net's cost volumes: Back2Future's ten corr81 calls and eight feature warps, FlowNetC6's one corr441d.
+    On an H100 80GB HBM3 (700 W power limit) at 256x832 the audited forwards take 0.4-0.6 s with Back2Future and 0.2 s with
+    FlowNetC6 (wall time, fp64 references included).
+    Returns the audit."""
+    from cc_b200 import evaluate as CE
+    from tests import layer_audit as LA
+    nets = eval_nets(device, flownet)
+    nbn = seed_running_stats(nets)
+    tgt, refs = synth.frames(1, H, W, seed=seed)
+    K, Kinv = synth.intrinsics(1, H, W)
+    args = (tgt.to(device), [r.to(device) for r in refs], K.to(device), Kinv.to(device))
+    order = ('disp', 'pose', 'mask', 'flow')
+    with torch.no_grad():
+        ref = [t.clone() for t in CE._flow_nets(*[nets[n] for n in order], *args)]
+        audit = LA.LayerAudit(nets=nets, tag='eval_%s_b1_%dx%d' % (flownet, H, W), report=report)
+        t0 = time.perf_counter()
+        with audit:
+            got = CE._flow_nets(*[nets[n] for n in order], *args)
+        if device.type == 'cuda':
+            torch.cuda.synchronize(device)
+    print('   audited eval forwards: %.1f s (fp64 references included)' % (time.perf_counter() - t0))
+    for what, a, b in zip(('emask', 'flow_cam', 'flow_fwd'), got, ref):
+        assert torch.equal(a, b), '%s: the audit changed the output' % what
+    rows = audit.rows
+    assert all(r['phase'] == 'fwd' for r in rows)
+    want = {'%s.%s' % (n, k) for n, net in nets.items() for k, m in net.named_modules()
+            if isinstance(m, (cnn.Conv2d, cnn.ConvTranspose2d, cnn.BatchNorm2d))} - set(NOT_RUN_IN_EVAL)
+    got_names = {r['name'] for r in rows if r['op'] in ('conv', 'convT', 'bn_eval')}
+    assert got_names == want, (sorted(want - got_names)[:10], sorted(got_names - want)[:10])
+    assert not any(r['op'] == 'bn' for r in rows)
+    assert nbn > 0 and len({r['name'] for r in rows if r['op'] == 'bn_eval'}) == nbn
+    calls = dict(corr81=10, featwarp=8, corr441d=0) if flownet == 'Back2Future' else dict(corr81=0, featwarp=0, corr441d=1)
+    for op, n in calls.items():
+        assert sum(r['op'] == op for r in rows) == n, (op, sum(r['op'] == op for r in rows))
+    return audit
 
 
 def _golden_rows(g, losses3, grads3, losses1, grads1):

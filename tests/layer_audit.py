@@ -1,8 +1,8 @@
 """Per-layer audit of the CUDA kernels against fp64, element by element, on the inputs a real run hands them.
 
-`LayerAudit` is a context manager.  While it is active, the forward and backward staticmethods of the six autograd
-Functions of cc_b200.nn (_Conv2dFn, _ConvT2dFn, _BatchNormFn, _Upsample2xFn, _Corr81Fn, _FeatWarpFn) are wrapped:
-after each real kernel call the wrapper takes the call's fp32 inputs (x, w, bias, res, upstream gradient, the saved
+`LayerAudit` is a context manager.  While it is active, the forward and backward staticmethods of the seven autograd
+Functions of cc_b200.nn (_Conv2dFn, _ConvT2dFn, _BatchNormFn, _Upsample2xFn, _Corr81Fn, _Corr441dFn, _FeatWarpFn) are
+wrapped: after each real kernel call the wrapper takes the call's fp32 inputs (x, w, bias, res, upstream gradient, the saved
 output / statistics), recomputes the operation in fp64 with torch, and checks every output element against the bound
 derived below.  Gradients a backward wrote straight into FlatAdam's flat buffer (cc_b200.nn._grad_slot) are read from
 `param._ccb_grad` right after the backward returns.  The audit is read-only: it works on fp64 copies, freed per call, and
@@ -10,8 +10,10 @@ changes no fp32 result (tests/test_gpu_fullsize.py holds the audited step bit-id
 
 Module names come from forward pre-hooks on the nets handed to the audit; the backward row of a call carries the name
 of its forward.  Convolution rows carry the kernels the call dispatched to (ccb_debug_last_conv_kernel after every
-fprop / dgrad / wgrad launch).  On exit the audit prints one table per op family - calls, worst and median normalised
-error, kernels seen - and raises an AssertionError listing every call over its bound.  With $CCB_PARITY_REPORT_DIR set,
+fprop / dgrad / wgrad launch) and the plan of each launch (ccb_debug_conv_plan: the path - CUDA-core GEMM, tensor cores,
+tensor-core weight gradient through padded rows - and the split-K count).  On exit the audit prints one table per op
+family - calls, worst and median normalised error, kernels seen - and raises an AssertionError listing every call over
+its bound.  With $CCB_PARITY_REPORT_DIR set,
 the rows are written there as layer_audit_<tag>.json.
 
 Error model (u = 2^-24, |.| elementwise, every bound gets TINY32 for products that underflow fp32)
@@ -27,7 +29,8 @@ So the scale of element i is
 where ||t_i||_2 is computed in fp64 by the same operation on squared operands (conv(x^2, w^2), convT(dz^2, w^2),
 wgrad(x^2, dz^2), sum dz^2, corr(f1^2, f2^2), ...), K is the largest number of products one element sums (Ci k^2 for
 fprop, Co ceil(k/s)^2 for a stride-s data gradient, B Ho Wo for the weight and bias gradients, C or 81 for the cost
-volume), and c_t is the error each product carries before it is summed, a per-term relative error of random sign:
+volume, C or 441 for FlowNetC6's dilated one), and c_t is the error each product carries before it is summed, a
+per-term relative error of random sign:
   C_TC   = 12u  tensor-core convolutions: the 3xTF32 split keeps hi*hi + hi*lo + lo*hi, so each product is off by
                 about 2^-21 = 8u of itself; plus ~4u for the fp32 rounding of the operand (dz = g * act'(y)) and product
   C_PROD =  4u  CUDA-core reductions: the product and its operand roundings
@@ -54,10 +57,24 @@ the backward's own inputs): y = xh gamma + beta within 4u (|xh gamma| + |beta|);
 sum g xh are long reductions (K = N, c_t = 0 and 4u); dx = gamma invstd (g - dbeta/N - xh dgamma/N) gets the
 reductions' bounds divided by N plus 6u of its three terms.
 
+Dilated cost volume (corr441d: FlowNetC6's 21x21 displacements at dilation 2, LeakyReLU(0.1) fused).
+  forward: the kernel sums the C products f1 f2 of an output in fp32, divides by C and applies the activation.  The
+           activation is inverted exactly in fp64 (out / 0.1f where out <= 0: the slope multiply adds u |z|), and the
+           pre-activation z is held to  s = (u sqrt(C) + C_PROD) ||t||_2 / C + 3u |z|  (K = C).
+  d f1 / d f2: sums of the 441 products dz f (dz = g * leaky'(out), from the sign of the forward's own output), divided
+           by C:  s = (u sqrt(441) + C_PROD) ||t||_2 / C + 2u |ref|  (K = 441).
+
 Elementwise and short ops: a worst-case count of roundings times u sum |terms|, so R = 1 is a proof, not a fit.
   upsample2x forward: hy (hx a + lx b) + ly (hx c + lx d) rounds each term at most 4 times (its x-weight product,
                       the inner add, the y-weight product, the outer add), weights non-negative: 4u upsample(|x|)
   upsample2x backward: a sequential sum of <= 16 weighted terms plus the weight product and the multiply: 17u sum |w g|
+  BatchNorm in eval mode (misc_ops.cu bn_eval_kernel), y = (x - rm) * inv * gamma + beta with inv = 1 / sqrtf(rv + eps)
+                      from the call's own fp32 running statistics (family bn_eval).  inv: the add is off by u of rv + eps,
+                      which the square root halves, then the square root and the divide round once each: 2.5u of inv.
+                      The subtract, the multiply by inv and the multiply by gamma add u each: x^ gamma is off by at most
+                      5.5u |x^ gamma| to first order; the final add rounds once more, u |y|.  The 0.5u left over covers the
+                      second-order terms:  s = 6u |x^ gamma| + u |y|.  (The build keeps IEEE sqrt and divide, no
+                      fast-math; a fused multiply-add only removes roundings.)
 
 Feature warp (bilinear sample of x at (i + flow), border padding, Back2Future's normalisation).  The kernel's fp32
 sample coordinate differs from the exact one by at most delta = 8u (|x + u| + W) pixels (about six roundings of
@@ -74,6 +91,7 @@ quantities of magnitude up to |x + u| + W).
 
 Every checked output must also meet rel_err <= 1e-4 (max |error| / max |fp64|, tests/util.rel_err), the bar of
 BASELINE.json."""
+import ctypes
 import json
 import math
 import os
@@ -90,14 +108,18 @@ C_PROD = 4 * U
 EPI = 3
 REL_BAR = 1e-4
 
-# Bound on r_i = |kernel - fp64| / s_i per op family, and the worst r measured over all calls of the second cfg3 step at
-# b4 256x832 on an H100 80GB HBM3 (700 W power limit; production dispatch, committed weight cache) and, for the CUDA-core
-# kernels, on the CPU simulator build over the four nets at 64x128 / 64x64.  The step is bit-reproducible, so these do
-# not vary from run to run.  Caps 1 / (u K_max) at 256x832: 19.7 for conv / convT / bn (K = 851968), 8.7e4 for corr81.
-R = dict(conv=10.0, convT=10.0, bn=6.0, upsample=1.0, corr81=6.0, featwarp=2.0)
-R_MEASURED = dict(conv=6.3, convT=5.41, bn=2.38, upsample=0.81, corr81=2.01, featwarp=0.37)      # H100
-R_MEASURED_SIM = dict(conv=1.78, convT=0.87, bn=0.92, upsample=0.73, corr81=1.19, featwarp=0.26)
-FAMILIES = ('conv', 'convT', 'bn', 'upsample', 'corr81', 'featwarp')
+# Bound on r_i = |kernel - fp64| / s_i per op family, and the worst r measured on an H100 80GB HBM3 (700 W power limit;
+# production dispatch) over all calls of the second cfg3 step at b4 256x832 (committed weight cache) with either flow net
+# and of the evaluation forwards at b1 256x832 (corr441d: 3.65 in the FlowNetC6 step, 3.47 in its eval forward; bn_eval:
+# 0.465), and, for the CUDA-core kernels, on the CPU simulator build over the five nets at 64x128 / 64x64 and the eval
+# forwards at b1 64x128.  The runs are bit-reproducible, so these do not vary from run to run.  Caps 1 / (u K_max) at
+# 256x832: 19.7 for conv / convT / bn (K = 851968), 8.7e4 for corr81, 3.8e4 for corr441d (K = 441).
+R = dict(conv=10.0, convT=10.0, bn=6.0, bn_eval=1.0, upsample=1.0, corr81=6.0, corr441d=6.0, featwarp=2.0)
+R_MEASURED = dict(conv=6.3, convT=5.41, bn=2.38, bn_eval=0.465, upsample=0.81, corr81=2.01, corr441d=3.65,
+                  featwarp=0.37)      # H100
+R_MEASURED_SIM = dict(conv=2.32, convT=2.35, bn=0.92, bn_eval=0.441, upsample=0.73, corr81=1.19, corr441d=2.42, featwarp=0.26)
+FAMILIES = ('conv', 'convT', 'bn', 'bn_eval', 'upsample', 'corr81', 'corr441d', 'featwarp')
+PLAN_PATHS = ('ffma', 'tc', 'tc_padded')      # ccb_debug_conv_plan's path codes
 
 NUM_SMS, BN_CHUNK, CORR_CT, CORR_CG = 132, 8192, 16, 4      # ccb_common.cuh, misc_ops.cu, b2f_ops.cu
 
@@ -261,6 +283,15 @@ def bn_fwd_checks(x, gamma, beta, rm_old, rv_old, rm_new, rv_new, stats, y, eps,
     return out, N
 
 
+def bn_eval_checks(x, gamma, beta, rm, rv, y, eps):
+    """Eval-mode BatchNorm: y against fp64 of (x - rm) / sqrt(rv + eps) gamma + beta from the call's fp32 running
+    statistics (module docstring: 6u |x^ gamma| + u |y|).  Elementwise: K = 1."""
+    v = lambda t: _d(t).view(1, -1, 1, 1)      # noqa: E731
+    xhg = (_d(x) - v(rm)) / (v(rv) + f32(eps)).sqrt() * v(gamma)
+    ref = xhg + v(beta)
+    return [('y', y, ref, 6 * U * xhg.abs() + U * ref.abs() + TINY32, None)], 1
+
+
 def bn_bwd_checks(x, gamma, stats, g, dx=None, dgamma=None, dbeta=None):
     xd, gd = _d(x), _d(g)
     B, C, h, w = x.shape
@@ -347,6 +378,59 @@ def corr81_bwd_checks(f1, f2, rev, g, d1=None, d2=None):
             ref = ref / C
             out.append((what, got, ref, (U * 9 + C_PROD) * tn.sqrt() / C + 2 * U * ref.abs() + TINY32, None))
     return out, 81
+
+
+# ---- FlowNetC6's dilated cost volume ---------------------------------------------------------------------------------
+CORR441D_N, CORR441D_R = 21, 20          # displacements per axis, reach in pixels (10 steps of 2)
+CORR441D_SLOPE32 = f32(0.1)              # the fused LeakyReLU's slope as the kernel holds it
+
+
+def corr441d_sample(a, b):
+    """The restated third-party correlation at FlowNetC6's call (patch 21, dilation 2) as [B,441,h,w], not divided by C."""
+    B, _, h, w = a.shape
+    return ON.spatial_correlation_sample(a, b, patch=CORR441D_N, dilation=2).reshape(B, CORR441D_N ** 2, h, w)
+
+
+def corr441d_adjoint(G, f1, f2):
+    """(sum_k G_k f2(. + d_k), sum_k G_k(. - d_k) f1(. - d_k)) over the 441 displacements d_k, no 1/C."""
+    B, C, h, w = f1.shape
+    N, R_ = CORR441D_N, CORR441D_R
+    f2p = F.pad(f2, (R_, R_, R_, R_))
+    d1 = torch.zeros_like(f1)
+    d2p = torch.zeros_like(f2p)
+    for i in range(N):
+        for j in range(N):
+            gk = G[:, N * i + j:N * i + j + 1]
+            sl = (slice(None), slice(None), slice(2 * i, 2 * i + h), slice(2 * j, 2 * j + w))
+            d1 += gk * f2p[sl]
+            d2p[sl] += gk * f1
+    return d1, d2p[:, :, R_:R_ + h, R_:R_ + w]
+
+
+def corr441d_fwd_checks(f1, f2, out):
+    """The pre-activation z recovered from the kernel's output against fp64 (module docstring); K = C."""
+    C = f1.shape[1]
+    a, b = _d(f1), _d(f2)
+    z = corr441d_sample(a, b) / C
+    tn = corr441d_sample(_sq(a), _sq(b)).sqrt() / C
+    o = _d(out)
+    zk = torch.where(o > 0, o, o / CORR441D_SLOPE32)
+    return [('z', zk, z, (U * math.sqrt(C) + C_PROD) * tn + 3 * U * z.abs() + TINY32, None)], C
+
+
+def corr441d_bwd_checks(f1, f2, out, g, d1=None, d2=None):
+    """d f1 and d f2 against fp64 (module docstring); K = 441."""
+    C = f1.shape[1]
+    a, b, gd = _d(f1), _d(f2), _d(g)
+    dz = torch.where(out > 0, gd, gd * CORR441D_SLOPE32)
+    r1, r2 = corr441d_adjoint(dz, a, b)
+    t1, t2 = corr441d_adjoint(_sq(dz), _sq(a), _sq(b))
+    checks = []
+    for what, got, ref, tn in (('d_f1', d1, r1, t1), ('d_f2', d2, r2, t2)):
+        if got is not None:
+            ref = ref / C
+            checks.append((what, got, ref, (U * CORR441D_N + C_PROD) * tn.sqrt() / C + 2 * U * ref.abs() + TINY32, None))
+    return checks, CORR441D_N ** 2
 
 
 # ---- feature warp ---------------------------------------------------------------------------------------------------
@@ -498,7 +582,7 @@ class LayerAudit:
     """with LayerAudit(nets={'disp': net, ...}) as audit: ... run forward / backward ...  (see the module docstring)"""
 
     FNS = {'conv': '_Conv2dFn', 'convT': '_ConvT2dFn', 'bn': '_BatchNormFn', 'upsample': '_Upsample2xFn',
-           'corr81': '_Corr81Fn', 'featwarp': '_FeatWarpFn'}
+           'corr81': '_Corr81Fn', 'corr441d': '_Corr441dFn', 'featwarp': '_FeatWarpFn'}
 
     def __init__(self, nets=None, tag='audit', report=True):
         self.nets = dict(nets or {})
@@ -547,7 +631,10 @@ class LayerAudit:
     def _run(self, op, d, *args):
         self._saved_run(op, d, *args)
         k = _lib.lib().ccb_debug_last_conv_kernel()
-        self._kern.append('%s:%s' % ((k or b'?').decode(), ('fprop', 'dgrad', 'wgrad')[op]))
+        plan = (ctypes.c_int * 2)()
+        _lib.call('ccb_debug_conv_plan', d, op, plan)
+        call = ('fprop', 'dgrad', 'wgrad')[op]
+        self._kern.append(('%s:%s' % ((k or b'?').decode(), call), dict(call=call, path=PLAN_PATHS[plan[0]], splits=plan[1])))
 
     def _name(self, fam):
         top = self._stack[-1] if self._stack else ''
@@ -609,12 +696,13 @@ class LayerAudit:
             shape = tuple(x.shape) + (w.shape[1], w.shape[2], stride)
         elif fam == 'bn':
             x, gamma, beta, rm, rv, training, eps, momentum = a
-            if not training:
-                return
-            stats = kept[2]
-            checks, K = bn_fwd_checks(x, gamma, beta, before[0], before[1], rm, rv, stats, out, eps, momentum)
             shape = tuple(x.shape)
-            extra['splits'] = bn_splits(x.shape[0], x.shape[2] * x.shape[3])
+            if training:
+                checks, K = bn_fwd_checks(x, gamma, beta, before[0], before[1], rm, rv, kept[2], out, eps, momentum)
+                extra['splits'] = bn_splits(x.shape[0], x.shape[2] * x.shape[3])
+            else:
+                fam = 'bn_eval'
+                checks, K = bn_eval_checks(x, gamma, beta, rm, rv, out, eps)
         elif fam == 'upsample':
             checks, K = upsample_fwd_checks(a[0], out)
             shape = tuple(a[0].shape)
@@ -623,6 +711,9 @@ class LayerAudit:
             checks, K = corr81_fwd_checks(f1, f2, bool(rev), out)
             shape = tuple(f1.shape)
             extra['chunks'] = corr_chunks(*f1.shape)
+        elif fam == 'corr441d':
+            checks, K = corr441d_fwd_checks(a[0], a[1], out)
+            shape = tuple(a[0].shape)
         else:
             checks, K = featwarp_fwd_checks(a[0], a[1], out)
             shape = tuple(a[0].shape)
@@ -658,6 +749,10 @@ class LayerAudit:
             checks, K = corr81_bwd_checks(f1, f2, bool(ctx.rev), g, d1=grads[0], d2=grads[1])
             shape = tuple(f1.shape)
             extra['chunks'] = corr_chunks(*f1.shape)
+        elif fam == 'corr441d':
+            f1, f2, out = saved
+            checks, K = corr441d_bwd_checks(f1, f2, out, g, d1=grads[0], d2=grads[1])
+            shape = tuple(f1.shape)
         else:
             x, flo = saved
             checks, K, extra = featwarp_bwd_checks(x, flo, g, dx=grads[0], dflow=grads[1])
@@ -666,8 +761,10 @@ class LayerAudit:
 
     def _record(self, fam, name, phase, shape, kern, checks, K, extra):
         res, r, bad = evaluate(fam, checks)
-        row = dict(op=fam, name=name, phase=phase, shape=list(shape), kernels=sorted(set(kern)), K=K, r=r,
+        row = dict(op=fam, name=name, phase=phase, shape=list(shape), kernels=sorted({k for k, _ in kern}), K=K, r=r,
                    checks={k: dict(r=v[0], rel=v[1], ties=v[2]) for k, v in res.items()}, bad=bad)
+        if kern:
+            row['plans'] = [p for _, p in kern]
         row.update(extra)
         self.rows.append(row)
 

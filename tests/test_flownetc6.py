@@ -10,7 +10,7 @@ import torch.nn.functional as F
 from cc_b200 import models as CM
 from cc_b200.train_step import build_nets
 from oracle import nets as ON
-from tests import flownetc6_cases as FC
+from tests import flownetc6_cases as FC, layer_audit as LA
 from tests.util import golden, sim_lib    # noqa: F401  (sim_lib: module fixture, the simulator library)
 
 NTOL = 2e-5        # tests/test_oracle_golden.py: module vs functional conv algorithms
@@ -68,35 +68,39 @@ def test_corr441d_sim_vs_fp64(sim_lib):
         s: {k: round(v, 3) for k, v in r.items()} for s, r in worst.items()}))
 
 
-def _flagged_fwd(f1, f2, bad):
-    return FC.corr441d_fwd_ratio(f1, f2, bad) > FC.R_CORR441D
+def _r(checks, what):
+    """Worst r of one check and whether the layer audit's bound (family corr441d) flags it."""
+    res, _, bad = LA.evaluate('corr441d', checks)
+    return res[what][0], any(b.startswith(what + ' ') for b in bad)
 
 
 def test_corr441d_planted_defects_fail_the_bound(sim_lib):
     B, C, h, w = 3, 13, 8, 16
+    N = LA.CORR441D_N
     f1, f2, go = FC._inputs(B, C, h, w, 'cpu', 5)
     out, d1, d2 = FC.run_corr441d(f1, f2, go)
-    assert FC.corr441d_fwd_ratio(f1, f2, out) <= FC.R_CORR441D
+    fwd = lambda o: _r(LA.corr441d_fwd_checks(f1, f2, o)[0], 'z')       # noqa: E731
+    assert not fwd(out)[1]
     j0 = 13
     # forward: one horizontal displacement skipped by the j loop (its 21 channels never accumulate)
     bad = out.clone()
-    bad[:, j0::FC.N] = 0
-    assert _flagged_fwd(f1, f2, bad)
+    bad[:, j0::N] = 0
+    assert fwd(bad)[1]
     # forward: the second staged channel group (channels 8..12) missing from every sum
-    part = FC.corr441d_sample(f1[:, :8], f2[:, :8]) / C
-    assert _flagged_fwd(f1, f2, F.leaky_relu(part, 0.1))
+    part = LA.corr441d_sample(f1[:, :8], f2[:, :8]) / C
+    assert fwd(F.leaky_relu(part, 0.1))[1]
     # d f1: the terms of displacement column j0 dropped for every i
-    dz = torch.where(out > 0, go, go * FC.SLOPE32)
+    dz = torch.where(out > 0, go, go * LA.CORR441D_SLOPE32)
     col = torch.zeros_like(dz)
-    col[:, j0::FC.N] = dz[:, j0::FC.N]
-    miss1, _ = FC.corr441d_adjoint(col, f1, f2)
-    r = FC.corr441d_bwd_ratios(f1, f2, out, go, d1=d1 - miss1 / C)['d_f1']
-    assert r > FC.R_CORR441D, r
+    col[:, j0::N] = dz[:, j0::N]
+    miss1, _ = LA.corr441d_adjoint(col, f1, f2)
+    r, flagged = _r(LA.corr441d_bwd_checks(f1, f2, out, go, d1=d1 - miss1 / C)[0], 'd_f1')
+    assert flagged and r > LA.R['corr441d'], r
     # d f2: one channel chunk never written (left at zero)
     bad2 = d2.clone()
     bad2[:, 8:] = 0
-    r = FC.corr441d_bwd_ratios(f1, f2, out, go, d2=bad2)['d_f2']
-    assert r > FC.R_CORR441D, r
+    r, flagged = _r(LA.corr441d_bwd_checks(f1, f2, out, go, d2=bad2)[0], 'd_f2')
+    assert flagged and r > LA.R['corr441d'], r
     # and the correct results pass
-    rs = FC.corr441d_bwd_ratios(f1, f2, out, go, d1=d1, d2=d2)
-    assert max(rs.values()) <= FC.R_CORR441D, rs
+    rs, bad = FC.corr441d_ratios(f1, f2, out, go, d1, d2)
+    assert not bad and max(rs.values()) <= LA.R['corr441d'], rs

@@ -1,12 +1,13 @@
 """FlowNetC6 on the H100: the cost-volume kernels at the benchmark shape, the network against the fixture frozen from
 the reference module, the training step with --flownet FlowNetC6 against the CPU oracle, CUDA-graph replay against eager
-steps, and the flow evaluation."""
+steps, every layer and loss-layer call of that step at b4 256x832 against fp64 (the layer and loss audits), and the flow
+evaluation."""
 import numpy as np
 import pytest
 import torch
 from cc_b200 import _lib, models as CM, synth, evaluate as CE
 from oracle import evaluate as OE, nets as ON
-from tests import flownetc6_cases as FC, step_cases as SC
+from tests import flownetc6_cases as FC, step_cases as SC, fullsize_cases as FS
 from tests.util import conv_impl, device_lib      # noqa: F401  (device_lib: module fixture, the sm_90a library)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
@@ -47,6 +48,21 @@ def test_flownetc6_step_graph_replay_vs_eager(cfg, B, H, W, loss_tol):
     """Trainer(cfg, flownet='FlowNetC6'): step_cases.case_step_graph_vs_eager, the eager losses against the CPU oracle
     step at the bar tests/test_gpu_parity.py GRAPH_CASES uses at that size."""
     SC.case_step_graph_vs_eager(DEV, cfg, B, H, W, loss_tol=loss_tol, seed=80, flownet='FlowNetC6')
+
+
+def test_layer_audit_flownetc6_step():
+    """Every layer call of the cfg3 b4 256x832 step with --flownet FlowNetC6 (second step, committed weight cache,
+    production dispatch) against fp64, element by element: the dilated cost volumes included
+    (fullsize_cases.audit_step)."""
+    with conv_impl(_lib.IMPL_AUTO):
+        FS.audit_step(DEV, flownet='FlowNetC6')
+
+
+def test_loss_audit_flownetc6_step():
+    """Every loss-layer call of the cfg3 b4 256x832 step with --flownet FlowNetC6 against fp64, element by element
+    (fullsize_cases.loss_audit_step)."""
+    with conv_impl(_lib.IMPL_AUTO):
+        FS.loss_audit_step(DEV, flownet='FlowNetC6')
 
 
 def test_flow_sample_errors_flownetc6():

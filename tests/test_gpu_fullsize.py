@@ -1,6 +1,7 @@
 """-m gpu: the production path (IMPL_AUTO: wgmma conv kernels + fused loss kernels) at the BASELINE.json
 configurations (b4, 256x832, 6 levels) against the CPU oracle, per tensor; and against the step fixture frozen
-from the reference's real train() body.  See tests/fullsize_cases.py for the bars."""
+from the reference's real train() body; the layer and loss audits of the timed step and the layer audit of the
+evaluation forwards at B = 1.  See tests/fullsize_cases.py for the bars."""
 import pytest
 import torch
 from tests import fullsize_cases as FC
@@ -28,6 +29,13 @@ def test_layer_audit_cfg3_second_step():
 def test_loss_audit_cfg3_second_step():
     """Every loss-layer call of the timed step (cfg3 b4 256x832, committed weight cache) against fp64, element by element."""
     FC.loss_audit_step(torch.device('cuda:0'))
+
+
+@pytest.mark.parametrize('flownet', ['Back2Future', 'FlowNetC6'])
+def test_layer_audit_eval_forwards(flownet):
+    """Every layer call of evaluate._flow_nets (the four nets in eval mode, B = 1, 256x832) against fp64, element by
+    element, with every BatchNorm's running statistics seeded far from the defaults (fullsize_cases.audit_eval_forwards)."""
+    FC.audit_eval_forwards(torch.device('cuda:0'), flownet)
 
 
 def test_step_vs_reference_fixture():

@@ -4,11 +4,13 @@ fp32 torch ops stand in for the kernels: correct fp32 results must pass every bo
 bugs applied to an otherwise correct result must be flagged.  The wrappers must restore the autograd Functions on exit,
 also when the audit raises.  Then the audit runs on the CPU simulator build of the product kernels over the four
 networks, one forward and one backward each (DispResNet6 and PoseNetB6 at b2 64x128, MaskNet6 and Back2Future at
-b1 64x64), which covers the CUDA-core convolutions and the BatchNorm, upsample, cost-volume and feature-warp kernels."""
+b1 64x64, FlowNetC6 at b1 64x128), which covers the CUDA-core convolutions and the BatchNorm, upsample, cost-volume and
+feature-warp kernels; and over the evaluation forwards in eval mode, which covers the eval-mode BatchNorm kernel.  Three
+mistakes in an eval-mode BatchNorm result (eps, the running mean, invstd) must each be flagged."""
 import pytest
 import torch
 import torch.nn.functional as F
-from tests import layer_audit as LA
+from tests import layer_audit as LA, flownetc6_cases as FC6, fullsize_cases as FS
 from tests.util import conv_impl, sim_lib      # noqa: F401  (sim_lib: module fixture, the simulator library)
 from cc_b200 import nn as cnn, _lib, synth, models as CM
 from oracle import nets as ON
@@ -104,6 +106,49 @@ def test_bn_dx_mean_term_removed():
     bad[:, 2] += gi[0, 2] * db[2] / N                 # channel 2 without its mean term
     flagged, (r, _, _) = _flagged('bn', LA.bn_bwd_checks(x, gamma, stats, gout, dx=bad)[0], 'dx')
     assert flagged and r > 1e3, r
+
+
+def _bn_eval_case(seed=8):
+    """An eval-mode BatchNorm call with running statistics far from their defaults, and its fp32 result."""
+    g = _gen(seed)
+    x = torch.randn(2, 6, 20, 30, generator=g) * 1.5 + 0.4
+    gamma, beta = torch.rand(6, generator=g) + 0.5, torch.randn(6, generator=g) * 0.1
+    rm, rv = 0.5 * torch.randn(6, generator=g), 0.25 + 3.75 * torch.rand(6, generator=g)
+    v = lambda t: t.view(1, -1, 1, 1)       # noqa: E731
+    y = (x - v(rm)) * v(1 / torch.sqrt(rv + 1e-5)) * v(gamma) + v(beta)
+    return x, gamma, beta, rm, rv, y, v
+
+
+def test_bn_eval_eps_mean_and_invstd_mistakes_flagged():
+    """The eval-mode bound is a rounding count (R = 1): a correct fp32 result passes; eps left out of the square root,
+    the running mean ignored, and the running variance used where invstd belongs are each flagged."""
+    x, gamma, beta, rm, rv, y, v = _bn_eval_case()
+    r = _passes('bn_eval', LA.bn_eval_checks(x, gamma, beta, rm, rv, y, 1e-5)[0])
+    assert r <= LA.R['bn_eval'], r
+    bad = {'eps omitted': (x - v(rm)) * v(1 / torch.sqrt(rv)) * v(gamma) + v(beta),
+           'running mean ignored': x * v(1 / torch.sqrt(rv + 1e-5)) * v(gamma) + v(beta),
+           'running_var for invstd': (x - v(rm)) * v(rv + 1e-5) * v(gamma) + v(beta)}
+    for what, yb in bad.items():
+        flagged, (r, _, _) = _flagged('bn_eval', LA.bn_eval_checks(x, gamma, beta, rm, rv, yb, 1e-5)[0], 'y')
+        assert flagged and r > LA.R['bn_eval'], (what, r)
+
+
+def test_bn_eval_kernel_vs_fp64():
+    """The eval-mode BatchNorm kernel of the simulator build through cc_b200.nn, audited as one call: a row of family
+    bn_eval within R = 1."""
+    x, gamma, beta, rm, rv, _, _ = _bn_eval_case(9)
+    bn = cnn.BatchNorm2d(6)
+    with torch.no_grad():
+        bn.weight.copy_(gamma)
+        bn.bias.copy_(beta)
+        bn.running_mean.copy_(rm)
+        bn.running_var.copy_(rv)
+    bn.eval()
+    with LA.LayerAudit(nets={'bn': bn}, report=False) as audit:
+        with torch.no_grad():
+            bn(x)
+    assert [(r['op'], r['name'], r['phase']) for r in audit.rows] == [('bn_eval', 'bn', 'fwd')], audit.rows
+    assert audit.rows[0]['r'] <= LA.R['bn_eval']
 
 
 def test_corr81_displacement_channels_swapped():
@@ -227,16 +272,22 @@ def _net_outputs(which):
         net.load_state_dict(ON.mask_params())
         tgt, refs = synth.frames(1, 64, 64, seed=42)
         return net, lambda: list(net(tgt, refs))
+    if which == 'flownetc6':
+        net = CM.FlowNetC6()
+        net.load_state_dict(FC6.step_flow_params())
+        tgt, refs = synth.frames(1, 64, 128, seed=42)
+        return net, lambda: list(net(tgt, refs[2]))
     net = CM.Back2Future(nlevels=6, compute_occ=False)
     net.load_state_dict(ON.flow_params())
     tgt, refs = synth.frames(1, 64, 64, seed=42)
     return net, lambda: (lambda ff, fb, _: list(ff) + list(fb))(*net(tgt, refs[1:3]))
 
 
-@pytest.mark.parametrize('which', ['disp', 'pose', 'mask', 'flow'])
+@pytest.mark.parametrize('which', ['disp', 'pose', 'mask', 'flow', 'flownetc6'])
 def test_audit_simulator_nets(which):
     """One forward and one backward (of a seeded weighted sum of the outputs) of each net on the simulator build, every
-    layer call audited; every Conv2d / ConvTranspose2d / BatchNorm2d module is audited forward and backward."""
+    layer call audited; every Conv2d / ConvTranspose2d / BatchNorm2d module is audited forward and backward, and the
+    flow nets' cost volumes and feature warps are all there."""
     with conv_impl(_lib.IMPL_FFMA):
         net, run = _net_outputs(which)
         net.train()
@@ -248,7 +299,15 @@ def test_audit_simulator_nets(which):
     for phase in ('fwd', 'bwd'):
         got = {r['name'] for r in audit.rows if r['phase'] == phase and r['op'] in ('conv', 'convT', 'bn')}
         assert got == want, (phase, sorted(want - got)[:10], sorted(got - want)[:10])
-    if which == 'flow':
-        for op, n in (('corr81', 10), ('featwarp', 8)):
-            assert sum(r['op'] == op and r['phase'] == 'fwd' for r in audit.rows) == n, op
-            assert sum(r['op'] == op and r['phase'] == 'bwd' for r in audit.rows) == n, op
+    calls = dict(flow=dict(corr81=10, featwarp=8), flownetc6=dict(corr441d=1)).get(which, {})
+    for op in ('corr81', 'corr441d', 'featwarp'):
+        for phase in ('fwd', 'bwd'):
+            assert sum(r['op'] == op and r['phase'] == phase for r in audit.rows) == calls.get(op, 0), (op, phase)
+
+
+def test_audit_simulator_eval_forwards():
+    """evaluate._flow_nets in eval mode over the four nets (Back2Future as the flow net) at b1 64x128 on the simulator
+    build, every BatchNorm's running statistics seeded far from the defaults: every layer call audited, the eval-mode
+    BatchNorms included (fullsize_cases.audit_eval_forwards).  FlowNetC6 in eval mode is audited on the H100."""
+    with conv_impl(_lib.IMPL_FFMA):
+        FS.audit_eval_forwards(torch.device('cpu'), 'Back2Future', H=64, W=128)
