@@ -183,6 +183,7 @@ _SIGS = {
     'ccb_make3d_depth_errors_workspace_bytes': ('long long', 'int, int, int'),
     'ccb_make3d_depth_errors': (STATUS, 'const double*, const float*, int, int, int, double, double, void*, long long, '
                                         'double*, ccb_stream_t'),
+    'ccb_pose_errors': (STATUS, 'const float*, int, int, int, const double*, double*, double*, ccb_stream_t'),
     'ccb_prep_frames': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, int, '
                                 'int, int, ccb_stream_t'),
     'ccb_prep_frames_unit': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '

@@ -14,10 +14,12 @@
 //   N3  motion segmentation scores: the three rigidity masks and the IoU counts of test_mask.py:129-156,224-262
 //       depth evaluation of test_disp.py:98-141: the velodyne ground truth, scipy's cubic zoom, both scalings' errors
 //       Make3D depth evaluation of test_make3d.py:97-148: imresize's contrast stretch, the capped median scaling, log10
+//       pose evaluation of test_pose.py / test_sintel_pose.py: the snippet's pose algebra, ATE and RE, one thread per snippet
 //
 // All floating-point reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize); the
 // segmentation counts are integer sums (atomics, the same in any order).
 #include "ccb_common.cuh"
+#include "geom.cuh"
 
 #ifdef CCB_CPU_SIM
 // The fp64 round-to-nearest intrinsics the Pillow restatements below use, for the host build of this file: one IEEE
@@ -1351,6 +1353,103 @@ __global__ void __launch_bounds__(256) bytescale_apply_kernel(const ByteScaleArg
     for (long long i = (long long)blockIdx.x * 256 + t; i < a.len; i += (long long)gridDim.x * 256) d[i] = table[s[i]];
 }
 
+// ================================================================================================
+// The pose algebra and errors of test_pose.py:74-92 and compute_pose_error (:107-122), one thread per snippet, all state in
+// registers.  A zero six-vector goes in at mid = L/2; each six-vector becomes [R|t] in fp32 with pose_vec2mat's arithmetic
+// (euler_rot / quat_rot), then everything is fp64: rot_i = inv(R_i) is a true inverse (the fp32-rounded R is orthonormal
+// to ~1e-7 only, and RE sees the difference), final_i = R_0 [rot_i | -rot_i t_i] + [0 | t_0].  ATE needs two passes over
+// the snippet (the scale, then the residual); final_i is rebuilt from the six-vectors in each instead of held in registers.
+constexpr int POSE_MAX_L = 15;
+
+struct PoseErrArgs {
+    const float* poses;             // [S][L-1][6]
+    const double* gt;               // [S][L][3][4], or null
+    double* final_poses;            // [S][L][3][4], or null
+    double* out;                    // [S][2] = ATE, RE (with gt)
+    int S, L, rot_mode;
+};
+
+// fp64 inverse of a row-major 3x3 matrix: its adjugate over its determinant
+__device__ __forceinline__ void inv3(const double* A, double* X) {
+    const double c00 = A[4] * A[8] - A[5] * A[7], c01 = A[5] * A[6] - A[3] * A[8], c02 = A[3] * A[7] - A[4] * A[6];
+    const double det = A[0] * c00 + A[1] * c01 + A[2] * c02;
+    X[0] = c00 / det; X[1] = (A[2] * A[7] - A[1] * A[8]) / det; X[2] = (A[1] * A[5] - A[2] * A[4]) / det;
+    X[3] = c01 / det; X[4] = (A[0] * A[8] - A[2] * A[6]) / det; X[5] = (A[2] * A[3] - A[0] * A[5]) / det;
+    X[6] = c02 / det; X[7] = (A[1] * A[6] - A[0] * A[7]) / det; X[8] = (A[0] * A[4] - A[1] * A[3]) / det;
+}
+
+// [R|t] of frame i of snippet s: pose_vec2mat of its six-vector in fp32 (the zero vector at mid), cast to fp64
+__device__ __forceinline__ void pose_mat(const PoseErrArgs& a, int s, int i, double* R, double* t) {
+    const int mid = a.L / 2;
+    float v[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (i != mid) {
+        const float* p = a.poses + ((long long)s * (a.L - 1) + (i < mid ? i : i - 1)) * 6;
+        for (int j = 0; j < 6; ++j) v[j] = p[j];
+    }
+    float Rf[9];
+    if (a.rot_mode == CCB_ROT_EULER) euler_rot(v[3], v[4], v[5], Rf);
+    else quat_rot(v[3], v[4], v[5], Rf);
+    for (int k = 0; k < 9; ++k) R[k] = (double)Rf[k];
+    for (int k = 0; k < 3; ++k) t[k] = (double)v[k];
+}
+
+// final_i [3][4] of snippet s, given frame 0's [R_0|t_0]
+__device__ __forceinline__ void pose_final(const PoseErrArgs& a, int s, int i, const double* R0, const double* t0, double* F) {
+    double R[9], t[3], X[9], tr[3];
+    pose_mat(a, s, i, R, t);
+    inv3(R, X);
+    for (int r = 0; r < 3; ++r) tr[r] = -(X[r * 3] * t[0] + X[r * 3 + 1] * t[1] + X[r * 3 + 2] * t[2]);
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) F[r * 4 + c] = R0[r * 3] * X[c] + R0[r * 3 + 1] * X[3 + c] + R0[r * 3 + 2] * X[6 + c];
+        F[r * 4 + 3] = (R0[r * 3] * tr[0] + R0[r * 3 + 1] * tr[1] + R0[r * 3 + 2] * tr[2]) + t0[r];
+    }
+}
+
+__global__ void __launch_bounds__(128) pose_errors_kernel(const PoseErrArgs a) {
+    CCB_PDL_WAIT();
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= a.S) return;
+    double R0[9], t0[3];
+    pose_mat(a, s, 0, R0, t0);
+    const double* g = a.gt ? a.gt + (long long)s * a.L * 12 : nullptr;
+    double gp = 0.0, pp = 0.0, re = 0.0;
+#pragma unroll 1
+    for (int i = 0; i < a.L; ++i) {
+        double F[12];
+        pose_final(a, s, i, R0, t0, F);
+        if (a.final_poses)
+            for (int k = 0; k < 12; ++k) a.final_poses[((long long)s * a.L + i) * 12 + k] = F[k];
+        if (!g) continue;
+        const double* G = g + i * 12;
+        for (int r = 0; r < 3; ++r) {
+            gp += G[r * 4 + 3] * F[r * 4 + 3];
+            pp += F[r * 4 + 3] * F[r * 4 + 3];
+        }
+        // the residual rotation gt_i[:, :3] inv(final_i[:, :3]) and its angle
+        const double Fr[9] = {F[0], F[1], F[2], F[4], F[5], F[6], F[8], F[9], F[10]};
+        double Fi[9], M[9];
+        inv3(Fr, Fi);
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) M[r * 3 + c] = G[r * 4] * Fi[c] + G[r * 4 + 1] * Fi[3 + c] + G[r * 4 + 2] * Fi[6 + c];
+        const double d0 = M[1] - M[3], d1 = M[5] - M[7], d2 = M[2] - M[6];
+        re += atan2(sqrt(d0 * d0 + d1 * d1 + d2 * d2), (M[0] + M[4] + M[8]) - 1.0);
+    }
+    if (!g) return;
+    const double k = gp / pp;       // numpy's 0/0: NaN when every predicted translation is zero
+    double e = 0.0;
+#pragma unroll 1
+    for (int i = 0; i < a.L; ++i) {
+        double F[12];
+        pose_final(a, s, i, R0, t0, F);
+        for (int r = 0; r < 3; ++r) {
+            const double d = g[i * 12 + r * 4 + 3] - k * F[r * 4 + 3];
+            e += d * d;
+        }
+    }
+    a.out[2 * s] = sqrt(e) / a.L;
+    a.out[2 * s + 1] = re / a.L;
+}
+
 }  // namespace ccb
 
 using namespace ccb;
@@ -1618,6 +1717,20 @@ extern "C" int ccb_make3d_depth_errors(const double* gt, const float* pred, int 
     a.B = B; a.H = H; a.W = W; a.R = 0;
     a.y1 = 0; a.y2 = H; a.x1 = 0; a.x2 = W;        // no crop: the mask is the depth range alone
     return eigen_errors_launch("make3d_depth_errors", a, work, stream);
+}
+
+extern "C" int ccb_pose_errors(const float* poses, int S, int L, int rot_mode, const double* gt, double* final_poses, double* out,
+                               ccb_stream_t stream) {
+    CCB_REQUIRE(poses, CCB_ERR_ARG, "pose_errors: null pointer");
+    CCB_REQUIRE((gt == nullptr) == (out == nullptr), CCB_ERR_ARG, "pose_errors: gt and out come together");
+    CCB_REQUIRE(gt || final_poses, CCB_ERR_ARG, "pose_errors: nothing to write (out and final_poses are null)");
+    CCB_REQUIRE(S > 0 && L >= 3 && L <= POSE_MAX_L && L % 2 == 1, CCB_ERR_ARG,
+                "pose_errors: bad sizes (S %d, L %d: an odd L in [3, %d])", S, L, POSE_MAX_L);
+    CCB_REQUIRE(rot_mode == CCB_ROT_EULER || rot_mode == CCB_ROT_QUAT, CCB_ERR_ARG, "pose_errors: bad rotation mode %d", rot_mode);
+    PoseErrArgs a;
+    a.poses = poses; a.gt = gt; a.final_poses = final_poses; a.out = out; a.S = S; a.L = L; a.rot_mode = rot_mode;
+    CCB_LAUNCH(pose_errors_kernel, dim3((S + 127) / 128), dim3(128), 0, stream, a);
+    return check_launch("pose_errors");
 }
 
 template <bool UNIT>

@@ -15,6 +15,10 @@
                         (make3d_files / load_make3d: test_framework's files and samples; make3d_frames: imresize's contrast
                         stretch, Pillow's resize and the normalisation; make3d_depth_errors: the capped median scaling and
                         compute_errors :174-190 with log10; depth_summary: the printed row, row 1)
+  pose_eval_batch       test_pose.py:50-92 / test_sintel_pose.py:55-97 for a batch of snippets on the device, no host
+                        synchronisation (kitti_pose_framework / sintel_pose_framework: the frameworks' files, snippets and
+                        compensated ground truth, load_pose_frames; pose_errors: the pose algebra, ATE and RE in one kernel;
+                        load_pose_net; pose_summary: the printed rows; write_pose_predictions: predictions.npy)
 
 The scripts' dataset crawlers, image IO and visualisation are out of scope (SURVEY.md section 2); these functions take what the
 reference's `test_framework` iterators yield (uint8 HxWx3 frames, ground truth arrays) and return what the scripts
@@ -482,3 +486,158 @@ def make3d_eval_batch(disp_net, crops_u8, gt_depth, h=256, w=256, min_depth=1e-3
     H, W = int(gt.shape[1]), int(gt.shape[2])
     pred = spline_zoom(1 / disp[:, 0], H, W, min_depth, max_depth)
     return make3d_depth_errors(gt, pred, min_depth, max_depth)
+
+
+# ------------------------------------------------------------------------------------------------
+# test_pose.py / test_sintel_pose.py on the device: every frame stretched and resized once, the snippets gathered on the
+# device, the pose net on all of them in one call, the pose algebra and the errors in one kernel
+
+POSE_NETS = ('PoseNetB6', 'PoseNet6', 'PoseExpNet')
+
+
+def load_pose_net(weights, name='PoseNetB6', device=None):
+    """The pose net of test_pose.py:35-38 -> (net, seq_length): weights a checkpoint path or the loaded dict holding
+    'state_dict'; seq_length = conv1.0.weight.size(1) / 3, the net built for seq_length - 1 references and loaded with
+    strict=False.  name is one of POSE_NETS (PoseNet6 and PoseExpNet from models/alternates.py)."""
+    assert name in POSE_NETS, name
+    if not isinstance(weights, dict):
+        weights = torch.load(weights, map_location='cpu')
+    seq_length = int(weights['state_dict']['conv1.0.weight'].size(1) / 3)
+    net = getattr(models, name)(nb_ref_imgs=seq_length - 1)
+    net.load_state_dict(weights['state_dict'], strict=False)
+    return net.to(device or torch.device('cuda')), seq_length
+
+
+def _snippet_indices(n, seq_length):
+    """read_scene_data's snippets of a sequence of n frames: the target frames demi..n-1-demi, each with its demi
+    neighbours either side (step 1) -> int64 [S, seq_length]."""
+    demi = (seq_length - 1) // 2
+    return np.arange(-demi, demi + 1).reshape(1, -1) + np.arange(demi, n - demi).reshape(-1, 1)
+
+
+def _compensate(poses):
+    """The framework's ground truth of the snippets' poses [S,L,3,4], in their dtype: every row loses the original first
+    translation (the reference subtracts through a view of row 0; numpy buffers the overlap, so row 0 ends at zero), then
+    is rotated by inv(R_0) (rotation unaffected)."""
+    poses = poses.copy()
+    poses[:, :, :, -1] -= poses[:, :1, :, -1].copy()
+    return np.linalg.inv(poses[:, 0, :, :3])[:, None] @ poses
+
+
+def _matching(parent, patterns, isdir):
+    """path.Path(parent).dirs(p) (isdir) or .files(p) for each pattern p, united and sorted: fnmatch on the entry names
+    (the reference iterates its sequences as a set, in hash order; here always in sorted order)."""
+    import fnmatch
+    import os
+    keep = os.path.isdir if isdir else os.path.isfile
+    names = [d for d in os.listdir(parent) if keep(os.path.join(parent, d))]
+    return sorted({os.path.join(parent, d) for p in patterns for d in names if fnmatch.fnmatch(d, p)})
+
+
+def kitti_pose_framework(root, sequences, seq_length):
+    """kitti_eval/pose_evaluation_utils.py test_framework_KITTI (step 1) -> (seqs, n_rows).  seqs: one dict per directory
+    under root/sequences matching a pattern of `sequences`, in sorted order: 'name', 'files' (sorted image_2/*.png),
+    'snippets' int64 [S,L] and 'gt' fp64 [S,L,3,4], the compensated poses of poses/<name>.txt.  n_rows = len(framework):
+    the image count, which the scripts size their arrays with (seq_length - 1 zero rows per sequence)."""
+    import os
+    seqs = []
+    for d in _matching(os.path.join(root, 'sequences'), sequences, True):
+        name = os.path.basename(d)
+        poses = np.genfromtxt(os.path.join(root, 'poses', '{}.txt'.format(name))).astype(np.float64).reshape(-1, 3, 4)
+        files = _matching(os.path.join(d, 'image_2'), ['*.png'], False)
+        snippets = _snippet_indices(len(files), seq_length)
+        seqs.append(dict(name=name, files=files, snippets=snippets, gt=_compensate(poses[snippets])))
+    return seqs, sum(len(s['files']) for s in seqs)
+
+
+def sintel_cam_read(path):
+    """sintel_io.cam_read(path, pose_only=True): the 202021.25 tag, then 9 + 12 fp64 values -> N, fp64 [3,4]."""
+    with open(path, 'rb') as f:
+        tag = np.fromfile(f, np.float32, 1)
+        assert tag.size == 1 and tag[0] == 202021.25, 'sintel_cam_read: %s: wrong tag %s' % (path, tag)
+        np.fromfile(f, np.float64, 9)
+        return np.fromfile(f, np.float64, 12).reshape(3, 4)
+
+
+def sintel_pose_framework(root, sequences, seq_length):
+    """sintel_eval/pose_evaluation_utils.py test_framework_Sintel (step 1) -> (seqs, n_rows), as kitti_pose_framework:
+    the directories under root/clean, their sorted *.png, and the .cam files of the same path with /clean/ replaced by
+    /camdata_left/.  The ground truth is float32 as the reference computes it (cam_read(...).astype(np.float32))."""
+    import os
+    seqs = []
+    for d in _matching(os.path.join(root, 'clean'), sequences, True):
+        cams = _matching(d.replace('/clean/', '/camdata_left/'), ['*.cam'], False)
+        files = _matching(d, ['*.png'], False)
+        snippets = _snippet_indices(len(files), seq_length)
+        poses = np.array([sintel_cam_read(c).astype(np.float32) for c in cams], np.float32).reshape(-1, 3, 4)
+        seqs.append(dict(name=os.path.basename(d), files=files, snippets=snippets, gt=_compensate(poses[snippets])))
+    return seqs, sum(len(s['files']) for s in seqs)
+
+
+def load_pose_frames(files):
+    """The frames of one sequence (or a chunk of one) decoded by Pillow on the host -> uint8 [N,H,W,3] (the reference's
+    imread(...).astype(np.float32) holds the same integers)."""
+    from PIL import Image
+    frames = np.stack([np.asarray(Image.open(f)) for f in files])
+    assert frames.dtype == np.uint8 and frames.ndim == 4 and frames.shape[3] == 3, (frames.dtype, frames.shape)
+    return frames
+
+
+@torch.no_grad()
+def pose_errors(poses, gt=None, rotation_mode='euler'):
+    """test_pose.py:74-92 per snippet on the device (ccb_pose_errors): poses [S,L-1,6] the pose net's output, gt the
+    framework's compensated ground truth [S,L,3,4] (numpy arrays go to the library's device, fp64; Sintel's float32
+    exactly upcast) -> (out fp64 [S,2] = ATE, RE or None without gt, final fp64 [S,L,3,4]).  Sintel's script keeps RE
+    alone.  No host synchronisation."""
+    poses = _lib.f32(poses)
+    S, R, six = (int(v) for v in poses.shape)
+    assert six == 6, poses.shape
+    L = R + 1
+    final = torch.empty(S, L, 3, 4, device=poses.device, dtype=torch.float64)
+    out = None
+    if gt is not None:
+        gt = _on_library_device(gt).to(poses.device, torch.float64).contiguous()
+        assert gt.shape == (S, L, 3, 4), (gt.shape, poses.shape)
+        out = torch.empty(S, 2, device=poses.device, dtype=torch.float64)
+    rot = {'euler': _lib.ROT_EULER, 'quat': _lib.ROT_QUAT}[rotation_mode]
+    _lib.call('ccb_pose_errors', poses, S, L, rot, gt, final, out, poses)
+    return out, final
+
+
+@torch.no_grad()
+def pose_eval_batch(pose_net, frames_u8, snippets, gt_poses=None, rotation_mode='euler', h=256, w=832, resize=True):
+    """test_pose.py:50-92 (test_sintel_pose.py:55-97 with h, w = 128, 416) for a batch of snippets: frames_u8 uint8
+    [N,H,W,3] the frames of one sequence or a chunk of one, snippets int64 [S,L] indices into them, gt_poses the
+    framework's [S,L,3,4] (numpy arrays go to the library's device) -> pose_errors' (out, final).  Each frame is
+    stretched, resized and normalised once (make3d_frames: imresize unless resize is False or the frames already are
+    h x w); the snippets are gathered on the device (target = column L/2, refs = the others in order) and the pose net runs
+    on all of them in one call.  No host synchronisation."""
+    x = make3d_frames(frames_u8, h, w, resize)
+    idx = _on_library_device(snippets).to(x.device, torch.int64)
+    L = int(idx.shape[1])
+    mid = L // 2
+    pose_net.eval()
+    tgt = x[idx[:, mid]]
+    refs = [x[idx[:, j]] for j in range(L) if j != mid]
+    return pose_errors(_pose(pose_net(tgt, refs)), gt_poses, rotation_mode)
+
+
+def pose_summary(per_snippet, n_rows, sintel=False):
+    """The rows the scripts print (test_pose.py:44,92-101; test_sintel_pose.py:49,96-102) from the [S,2] per-snippet
+    (ATE, RE) of a whole framework in its order: stored as float32 in an array of n_rows = len(framework) rows, the
+    rest zero, then its mean and std -> float32 [2,2] (rows mean, std; columns ATE, RE), or [2,1] (RE) for Sintel."""
+    per_snippet = np.asarray(per_snippet).reshape(-1, 2)
+    errors = np.zeros((n_rows, 1 if sintel else 2), np.float32)
+    errors[:len(per_snippet)] = per_snippet[:, 1:] if sintel else per_snippet
+    return np.stack([errors.mean(0), errors.std(0)])
+
+
+def write_pose_predictions(path, finals, n_rows):
+    """predictions.npy of --output-dir (test_pose.py:48,89,104) under the directory `path`: the [S,L,3,4] final poses of
+    the framework in its order, in an fp64 array of n_rows = len(framework) snippets, the rest zero."""
+    import os
+    finals = np.asarray(finals)
+    os.makedirs(path, exist_ok=True)
+    predictions = np.zeros((n_rows,) + finals.shape[1:])
+    predictions[:len(finals)] = finals
+    np.save(os.path.join(path, 'predictions.npy'), predictions)

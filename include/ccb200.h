@@ -424,6 +424,18 @@ int ccb_bytescale_u8(const unsigned char* src, int N, int H, int W, void* work, 
 long long ccb_make3d_depth_errors_workspace_bytes(int B, int H, int W);
 int ccb_make3d_depth_errors(const double* gt, const float* pred, int B, int H, int W, double min_depth, double max_depth,
                             void* work, long long work_bytes, double* out, ccb_stream_t stream);
+/* Pose evaluation of test_pose.py / test_sintel_pose.py on the device, no host sync, no workspace: one thread per snippet.
+ * ccb_pose_errors: poses [S,L-1,6] fp32 is the pose net's output for S snippets of L frames (L odd, 3 <= L <= 15).  Per
+ *   snippet (test_pose.py:74-92): a zero six-vector inserted at mid = L/2; each six-vector -> [R_i|t_i] in fp32 with
+ *   pose_vec2mat's arithmetic (rot_mode CCB_ROT_EULER / CCB_ROT_QUAT), cast to fp64; rot_i = inv(R_i) (a true inverse,
+ *   not a transpose); final_i = R_0 [rot_i | -rot_i t_i], final_i[:, 3] += t_0, written to final_poses [S,L,3,4] fp64
+ *   when it is not NULL.  gt [S,L,3,4] fp64 is the compensated ground truth the framework yields (Sintel's float32 gt
+ *   upcast exactly); with it out [S,2] fp64 = compute_pose_error (:107-122):
+ *     ATE = ||gt_t - k pred_t|| / L with k = sum(gt_t pred_t) / sum(pred_t^2) (NaN when every pred_t is zero, as numpy),
+ *     RE = sum_i atan2(||(R01-R10, R12-R21, R02-R20)||, tr R - 1) / L with R = gt_i[:, :3] inv(final_i[:, :3]).
+ *   gt and out come together; at least one of out and final_poses is written.  Every run gives the same bits. */
+int ccb_pose_errors(const float* poses, int S, int L, int rot_mode, const double* gt, double* final_poses, double* out,
+                    ccb_stream_t stream);
 /* Input pipeline on the device (train.py:448-451 H2D + custom_transforms.py:21-30,47-118): uint8 HWC frames
  * src [B,F,Hs,Ws,3] -> F normalised fp32 NCHW tensors dst[f] [B,3,H,W] = (v/255 - .5)/.5, per sample horizontally
  * flipped (params[b][0] != 0) and scale-cropped: resized by (params[b][1], params[b][2]) = (scaled_w/Ws, scaled_h/Hs)
