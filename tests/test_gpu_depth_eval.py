@@ -6,7 +6,7 @@ import pytest
 import torch
 from cc_b200 import evaluate as CE
 from tests import depth_eval_cases as DC
-from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library)
+from tests.util import assert_graph_replays, device_lib      # noqa: F401  (module fixture: the sm_90a library)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 DEV = torch.device('cuda:0')
@@ -61,20 +61,5 @@ def test_chain_in_cuda_graph():
         gt = CE.velodyne_depth(pts, offs, Pd, H, W)
         pred = CE.spline_zoom(1 / disp, H, W, 1e-3, 80.0)
         return CE.depth_errors(gt, pred, 1e-3, 80.0, 'eigen', poses, displacements)
-    first, second = inputs(1), inputs(2)
-    eager = [chain(*ins) for ins in (first, second)]
+    eager = assert_graph_replays(chain, inputs(1), inputs(2))
     assert not torch.equal(eager[0], eager[1])
-    static = [t.clone() for t in first]
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        chain(*static)
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out = chain(*static)
-    for ins, want in zip((first, second, first), eager + eager[:1]):
-        for dst, src in zip(static, ins):
-            dst.copy_(src)
-        graph.replay()
-        assert torch.equal(out, want)

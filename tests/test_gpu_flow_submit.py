@@ -5,7 +5,7 @@ import pytest
 import torch
 from cc_b200 import evaluate as CE
 from tests import flow_submit_cases as SC
-from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library)
+from tests.util import assert_graph_replays, device_lib      # noqa: F401  (module fixture: the sm_90a library)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 DEV = torch.device('cuda:0')
@@ -31,25 +31,10 @@ def test_submit_and_colors_in_cuda_graph():
     first = [t.to(DEV) for t in SC.random_submit_inputs(2, 64, 128, seed=51)]
     second = [t.to(DEV) for t in SC.random_submit_inputs(2, 64, 128, seed=52)]
 
-    def run(ins):
+    def run(*ins):
         out = CE.flow_submission(*ins, 96, 200, 0.01, want_full=True)
         out['viz'] = CE.flow_colors(out['full'])
         return out
 
-    eager = [run(ins) for ins in (first, second)]
+    eager = assert_graph_replays(run, first, second)
     assert not torch.equal(eager[0]['png'], eager[1]['png'])
-    static = [t.clone() for t in first]
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        run(static)
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out = run(static)
-    for ins, want in zip((first, second, first), eager + eager[:1]):
-        for dst, src in zip(static, ins):
-            dst.copy_(src)
-        graph.replay()
-        for k in want:
-            assert torch.equal(out[k], want[k]), k

@@ -5,7 +5,7 @@ import pytest
 import torch
 from cc_b200 import evaluate as CE
 from tests import mask_eval_cases as MC
-from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library)
+from tests.util import assert_graph_replays, device_lib      # noqa: F401  (module fixture: the sm_90a library)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 DEV = torch.device('cuda:0')
@@ -36,19 +36,5 @@ def test_motion_mask_counts_in_cuda_graph():
     """The call makes no host round-trip: captured once, replayed on new inputs in the same buffers."""
     first = [t.to(DEV) for t in MC.random_sample(2, 64, 128, 96, 200, seed=51, flow_scale=[1.0, 2.0])]
     second = [t.to(DEV) for t in MC.random_sample(2, 64, 128, 96, 200, seed=52, flow_scale=[2.0, 1.0])]
-    eager = [CE.motion_mask_counts(*ins, THRESH=0.6, want_masks=True) for ins in (first, second)]
+    eager = assert_graph_replays(lambda *ins: CE.motion_mask_counts(*ins, THRESH=0.6, want_masks=True), first, second)
     assert not torch.equal(eager[0][0], eager[1][0])
-    static = [t.clone() for t in first]
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        CE.motion_mask_counts(*static, THRESH=0.6, want_masks=True)          # warm-up outside the capture
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        counts, masks = CE.motion_mask_counts(*static, THRESH=0.6, want_masks=True)
-    for ins, (want_counts, want_masks) in zip((first, second, first), eager + eager[:1]):
-        for dst, src in zip(static, ins):
-            dst.copy_(src)
-        graph.replay()
-        assert torch.equal(counts, want_counts) and torch.equal(masks, want_masks)

@@ -8,7 +8,7 @@ import torch
 from cc_b200 import evaluate as CE, models as CM, synth
 from oracle import make3d_eval as OM, pose_eval as OP
 from tests import pose_eval_cases as PC
-from tests.util import device_lib      # noqa: F401  (module fixture: the sm_90a library)
+from tests.util import assert_graph_replays, device_lib      # noqa: F401  (module fixture: the sm_90a library)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('device_lib')]
 DEV = torch.device('cuda:0')
@@ -72,20 +72,5 @@ def test_chain_in_cuda_graph():
     def chain(frames, gt):
         return CE.pose_eval_batch(stand_in, frames, snippets, gt, 'euler', h, w)
     stand_in.eval = lambda: None
-    first, second = inputs(1), inputs(2)
-    eager = [chain(*ins) for ins in (first, second)]
+    eager = assert_graph_replays(chain, inputs(1), inputs(2))
     assert not torch.equal(eager[0][0], eager[1][0])
-    static = [t.clone() for t in first]
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        chain(*static)
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out, final = chain(*static)
-    for ins, want in zip((first, second, first), eager + eager[:1]):
-        for dst, src in zip(static, ins):
-            dst.copy_(src)
-        graph.replay()
-        assert torch.equal(out, want[0]) and torch.equal(final, want[1])

@@ -79,6 +79,43 @@ def golden(name):
     return _cache[name]
 
 
+def _assert_equal(got, want, where):
+    """torch.equal on every tensor of `want`, through tuples, lists and dicts."""
+    if isinstance(want, dict):
+        assert got.keys() == want.keys(), where
+        for k in want:
+            _assert_equal(got[k], want[k], '%s[%r]' % (where, k))
+    elif isinstance(want, (tuple, list)):
+        assert len(got) == len(want), where
+        for i, (g, w) in enumerate(zip(got, want)):
+            _assert_equal(g, w, '%s[%d]' % (where, i))
+    else:
+        assert torch.equal(got, want), where
+
+
+def assert_graph_replays(chain, first, second):
+    """`chain(*inputs)` makes no host round-trip: captured once in a CUDA graph on a clone of `first` (after a warm-up on a
+    side stream), then replayed with `first`, `second` and `first` again copied into the captured buffers, each replay
+    equal bit for bit to the eager run on the same inputs.  Returns the two eager results: the caller asserts that they
+    differ, on the output it cares about, so that the replays cannot pass vacuously."""
+    eager = [chain(*ins) for ins in (first, second)]
+    static = [t.clone() for t in first]
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        chain(*static)                          # warm-up outside the capture
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        out = chain(*static)
+    for i, (ins, want) in enumerate(zip((first, second, first), eager + eager[:1])):
+        for dst, src in zip(static, ins):
+            dst.copy_(src)
+        graph.replay()
+        _assert_equal(out, want, 'replay %d' % i)
+    return eager
+
+
 def T(a, device='cpu'):
     return torch.from_numpy(np.asarray(a)).to(device)
 

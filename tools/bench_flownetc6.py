@@ -8,22 +8,13 @@ Prints one JSON object with the card's name and power limit, read in the same ru
 import argparse
 import json
 import os
-import subprocess
 import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from cc_b200 import nn as cnn, synth, pyramid   # noqa: E402
 from cc_b200.train_step import Trainer           # noqa: E402
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
-                           stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, timeout=30).stdout.decode().strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return dict(name=torch.cuda.get_device_name(0), nvidia_smi=q or 'unavailable')
+from tools.card import card                      # noqa: E402
 
 
 def time_loop(fn, launches):

@@ -10,24 +10,15 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from cc_b200 import synth, pyramid, loss_functions as CL   # noqa: E402
 from cc_b200.train_step import Trainer                   # noqa: E402
+from tools.card import card                              # noqa: E402
 
 ARMS = (('cfg3', ()), ('canonical', ('mask', 'flow')))
-
-
-def card():
-    try:
-        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                             stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=60).stdout.decode().strip()
-    except Exception as e:                                   # the numbers stay valid; say where the card name is missing
-        out = 'nvidia-smi unavailable: %s' % e
-    return out.splitlines()[0] if out else ''
 
 
 def events_ms(fn, iters):

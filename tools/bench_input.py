@@ -12,7 +12,6 @@ import argparse
 import json
 import os
 import random
-import subprocess
 import sys
 import time
 import numpy as np
@@ -21,18 +20,9 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from cc_b200 import input_pipeline as CI   # noqa: E402
+from tools.card import card                # noqa: E402
 
 PEAK_BW = 3.35e12      # H100 SXM HBM3, data sheet
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader', '-i', '0'],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, timeout=30).stdout.decode().strip()
-    except (OSError, subprocess.SubprocessError):
-        pl = ''
-    return name, pl or 'not measured'
 
 
 def time_call(fn, iters, warmup):
@@ -100,9 +90,8 @@ def main():
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'bench_input.py measures on a GPU; there is no CPU fallback'
     dev = torch.device('cuda:0')
-    name, power = card()
     rotate_fn, resize_fn, host_label = host_path()
-    res = dict(card=name, power_limit=power, host_path=host_label, peak_bw_TBps=PEAK_BW / 1e12, rows={})
+    res = dict(card=card(), host_path=host_label, peak_bw_TBps=PEAK_BW / 1e12, rows={})
 
     B, F, H, W = 4, 5, 256, 832
     rs = np.random.RandomState(0)

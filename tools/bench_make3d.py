@@ -8,7 +8,6 @@ difference of the averaged rows.  Prints one JSON object with the card's name an
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 import numpy as np
@@ -17,15 +16,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from cc_b200 import evaluate as CE, models as CM, synth    # noqa: E402
 from tests import make3d_eval_cases as MC                 # noqa: E402
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
-                           stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, timeout=30).stdout.decode().strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return dict(name=torch.cuda.get_device_name(0), nvidia_smi=q or 'unavailable')
+from tools.card import card                               # noqa: E402
 
 
 def main():
