@@ -165,6 +165,9 @@ _SIGS = {
                              'int, int, int, float, int, float*, void*, long long, long long*, ccb_stream_t'),
     'ccb_flow_submit': (STATUS, 'const float*, const float*, const float*, int, int, int, int, int, int, float, float*, '
                                 'float*, unsigned short*, float*, ccb_stream_t'),
+    'ccb_flow_eval_workspace_bytes': ('long long', 'int, int, int, int, int'),
+    'ccb_flow_eval': (STATUS, 'const float*, const float*, const float*, const float*, const float*, int, int, int, int, '
+                              'int, int, float, float, float, float, float*, void*, long long, float*, ccb_stream_t'),
     'ccb_flow_color_workspace_bytes': ('long long', 'int, int, int, int'),
     'ccb_flow_color': (STATUS, 'const float*, int, int, int, int, void*, long long, unsigned char*, ccb_stream_t'),
     'ccb_kitti_flow_errors_workspace_bytes': ('long long', 'int, int, int'),

@@ -15,6 +15,8 @@
 //       depth evaluation of test_disp.py:98-141: the velodyne ground truth, scipy's cubic zoom, both scalings' errors
 //       Make3D depth evaluation of test_make3d.py:97-148: imresize's contrast stretch, the capped median scaling, log10
 //       pose evaluation of test_pose.py / test_sintel_pose.py: the snippet's pose algebra, ATE and RE, one thread per snippet
+//       KITTI-2015 flow evaluation of test_flow.py:112-140 / test_back2future.py: the combined mask and both
+//       compute_all_epes per sample, on the flow metrics' per-pixel body
 //
 // All floating-point reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize); the
 // segmentation counts are integer sums (atomics, the same in any order).
@@ -200,81 +202,100 @@ __device__ __forceinline__ float mask_at_pred(const FlowMetArgs& a, const float*
     return bilerp(m, a.wm, ly, lx);
 }
 
+// The resize factors of one FlowMetArgs, computed once per thread
+struct FlowMetScales {
+    float sy_p, sx_p, fu, fv, sy_mg, sx_mg, sy_mp, sx_mp;
+};
+__device__ __forceinline__ FlowMetScales flow_met_scales(const FlowMetArgs& a) {
+    FlowMetScales s;
+    s.sy_p = (float)a.hp / (float)a.Hg; s.sx_p = (float)a.wp / (float)a.Wg;                             // pred -> gt
+    s.fu = (float)((double)a.Wg / (double)a.wp); s.fv = (float)((double)a.Hg / (double)a.hp);             // python float ratio, cast on use
+    s.sy_mg = a.mask ? (float)a.hm / (float)a.Hg : 0.f; s.sx_mg = a.mask ? (float)a.wm / (float)a.Wg : 0.f;   // mask -> gt
+    s.sy_mp = a.mask ? (float)a.hm / (float)a.hp : 0.f; s.sx_mp = a.mask ? (float)a.wm / (float)a.wp : 0.f;   // mask -> pred
+    return s;
+}
+
+// Ground-truth pixel (b, y, x) of compute_all_epes / compute_epe / outlier_err, added to
+// acc = {epe_all, den_all, epe_rig, den_rig, epe_non, den_non, n_err, (unused)}; returns flow_diff of the (composited)
+// prediction there.
+__device__ __forceinline__ float flow_metrics_pixel(const FlowMetArgs& a, const FlowMetScales& s, int b, int y, int x,
+                                                    double (&acc)[8]) {
+    const float* g = a.gt + (long long)b * a.nc * a.Hg * a.Wg + (long long)y * a.Wg + x;
+    const float ug = __ldg(g), vg = __ldg(g + (long long)a.Hg * a.Wg);
+    const float valid = (a.nc == 3) ? __ldg(g + 2ll * a.Hg * a.Wg) : 1.f;
+    const Lin ly = lin_src(y, a.hp, s.sy_p), lx = lin_src(x, a.wp, s.sx_p);
+    const float* pa = a.pa + (long long)b * 2 * a.hp * a.wp;
+    float ua, va, ur = 0.f, vr = 0.f, un = 0.f, vn = 0.f;      // total, rigid-only, non-rigid-only (upsampled, unscaled)
+    if (!a.mask) {
+        ua = bilerp(pa, a.wp, ly, lx);
+        va = bilerp(pa + a.hp * a.wp, a.wp, ly, lx);
+    } else {
+        const float* pb = a.pb + (long long)b * 2 * a.hp * a.wp;
+        const float* m = a.mask + (long long)b * a.hm * a.wm;
+        // the composite is formed at prediction resolution, then upsampled: evaluate the four corner pixels
+        const int ys[2] = {ly.i0, ly.i1}, xs[2] = {lx.i0, lx.i1};
+        const float wy[2] = {ly.w0, ly.w1}, wx[2] = {lx.w0, lx.w1};
+        float rr[2][2][2], nn[2][2][2];
+#pragma unroll
+        for (int cy = 0; cy < 2; ++cy)
+#pragma unroll
+            for (int cx = 0; cx < 2; ++cx) {
+                const float mp = mask_at_pred(a, m, ys[cy], xs[cx], s.sy_mp, s.sx_mp);
+                const float sr = (mp > a.thresh) ? 1.f : 0.f, sn = (mp <= a.thresh) ? 1.f : 0.f;
+                const int o = ys[cy] * a.wp + xs[cx];
+                rr[cy][cx][0] = sr * __ldg(pa + o); rr[cy][cx][1] = sr * __ldg(pa + a.hp * a.wp + o);
+                nn[cy][cx][0] = sn * __ldg(pb + o); nn[cy][cx][1] = sn * __ldg(pb + a.hp * a.wp + o);
+            }
+        auto up = [&](float (&q)[2][2][2], int ch) {
+            return wy[0] * (wx[0] * q[0][0][ch] + wx[1] * q[0][1][ch]) + wy[1] * (wx[0] * q[1][0][ch] + wx[1] * q[1][1][ch]);
+        };
+        float tt[2][2][2];
+#pragma unroll
+        for (int cy = 0; cy < 2; ++cy)
+#pragma unroll
+            for (int cx = 0; cx < 2; ++cx) { tt[cy][cx][0] = nn[cy][cx][0] + rr[cy][cx][0]; tt[cy][cx][1] = nn[cy][cx][1] + rr[cy][cx][1]; }
+        ua = up(tt, 0); va = up(tt, 1);
+        ur = up(rr, 0); vr = up(rr, 1);
+        un = up(nn, 0); vn = up(nn, 1);
+    }
+    const float du = ug - ua * s.fu, dv = vg - va * s.fv;
+    const float epe = sqrtf(du * du + dv * dv);
+    const float ev = epe * valid;
+    acc[0] += ev;
+    acc[1] += valid;
+    const float mag = sqrtf(ug * ug + vg * vg);
+    const float e0 = (ev > a.tau0) ? 1.f : 0.f, e1 = ((ev / (mag + 1e-8f)) > a.tau1) ? 1.f : 0.f;
+    acc[6] += e0 * e1 * valid;
+    if (a.mask) {
+        const Lin my = lin_src(y, a.hm, s.sy_mg), mx = lin_src(x, a.wm, s.sx_mg);
+        const float mg = bilerp(a.mask + (long long)b * a.hm * a.wm, a.wm, my, mx);
+        const float sr = (mg > a.thresh) ? 1.f : 0.f, sn = (mg <= a.thresh) ? 1.f : 0.f;
+        {   // compute_epe(gt_rigid, rigid_pred): gt (all channels, valid included) times the gt-resolution mask
+            const float d0 = ug * sr - ur * s.fu, d1 = vg * sr - vr * s.fv, vv = valid * sr;
+            acc[2] += sqrtf(d0 * d0 + d1 * d1) * vv;
+            acc[3] += vv;
+        }
+        {
+            const float d0 = ug * sn - un * s.fu, d1 = vg * sn - vn * s.fv, vv = valid * sn;
+            acc[4] += sqrtf(d0 * d0 + d1 * d1) * vv;
+            acc[5] += vv;
+        }
+    }
+    return epe;
+}
+
 __global__ void __launch_bounds__(256) flow_metrics_kernel(const FlowMetArgs a) {
     CCB_PDL_WAIT();
     __shared__ double scratch[8 * 32];
     const long long npx = (long long)a.B * a.Hg * a.Wg;
-    const float sy_p = (float)a.hp / (float)a.Hg, sx_p = (float)a.wp / (float)a.Wg;          // pred -> gt
-    const float fu = (float)((double)a.Wg / (double)a.wp), fv = (float)((double)a.Hg / (double)a.hp);   // python float ratio, cast on use
-    const float sy_mg = a.mask ? (float)a.hm / (float)a.Hg : 0.f, sx_mg = a.mask ? (float)a.wm / (float)a.Wg : 0.f;   // mask -> gt
-    const float sy_mp = a.mask ? (float)a.hm / (float)a.hp : 0.f, sx_mp = a.mask ? (float)a.wm / (float)a.wp : 0.f;   // mask -> pred
-    double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // epe_all, den_all, epe_rig, den_rig, epe_non, den_non, n_err, (unused)
+    const FlowMetScales s = flow_met_scales(a);
+    double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < npx; i += (long long)gridDim.x * 256) {
         const int x = (int)(i % a.Wg);
         const int y = (int)((i / a.Wg) % a.Hg);
         const int b = (int)(i / ((long long)a.Wg * a.Hg));
-        const float* g = a.gt + (long long)b * a.nc * a.Hg * a.Wg + (long long)y * a.Wg + x;
-        const float ug = __ldg(g), vg = __ldg(g + (long long)a.Hg * a.Wg);
-        const float valid = (a.nc == 3) ? __ldg(g + 2ll * a.Hg * a.Wg) : 1.f;
-        const Lin ly = lin_src(y, a.hp, sy_p), lx = lin_src(x, a.wp, sx_p);
-        const float* pa = a.pa + (long long)b * 2 * a.hp * a.wp;
-        float ua, va, ur = 0.f, vr = 0.f, un = 0.f, vn = 0.f;      // total, rigid-only, non-rigid-only (upsampled, unscaled)
-        if (!a.mask) {
-            ua = bilerp(pa, a.wp, ly, lx);
-            va = bilerp(pa + a.hp * a.wp, a.wp, ly, lx);
-        } else {
-            const float* pb = a.pb + (long long)b * 2 * a.hp * a.wp;
-            const float* m = a.mask + (long long)b * a.hm * a.wm;
-            // the composite is formed at prediction resolution, then upsampled: evaluate the four corner pixels
-            const int ys[2] = {ly.i0, ly.i1}, xs[2] = {lx.i0, lx.i1};
-            const float wy[2] = {ly.w0, ly.w1}, wx[2] = {lx.w0, lx.w1};
-            float rr[2][2][2], nn[2][2][2];
-#pragma unroll
-            for (int cy = 0; cy < 2; ++cy)
-#pragma unroll
-                for (int cx = 0; cx < 2; ++cx) {
-                    const float mp = mask_at_pred(a, m, ys[cy], xs[cx], sy_mp, sx_mp);
-                    const float sr = (mp > a.thresh) ? 1.f : 0.f, sn = (mp <= a.thresh) ? 1.f : 0.f;
-                    const int o = ys[cy] * a.wp + xs[cx];
-                    rr[cy][cx][0] = sr * __ldg(pa + o); rr[cy][cx][1] = sr * __ldg(pa + a.hp * a.wp + o);
-                    nn[cy][cx][0] = sn * __ldg(pb + o); nn[cy][cx][1] = sn * __ldg(pb + a.hp * a.wp + o);
-                }
-            auto up = [&](float (&q)[2][2][2], int ch) {
-                return wy[0] * (wx[0] * q[0][0][ch] + wx[1] * q[0][1][ch]) + wy[1] * (wx[0] * q[1][0][ch] + wx[1] * q[1][1][ch]);
-            };
-            float tt[2][2][2];
-#pragma unroll
-            for (int cy = 0; cy < 2; ++cy)
-#pragma unroll
-                for (int cx = 0; cx < 2; ++cx) { tt[cy][cx][0] = nn[cy][cx][0] + rr[cy][cx][0]; tt[cy][cx][1] = nn[cy][cx][1] + rr[cy][cx][1]; }
-            ua = up(tt, 0); va = up(tt, 1);
-            ur = up(rr, 0); vr = up(rr, 1);
-            un = up(nn, 0); vn = up(nn, 1);
-        }
-        const float du = ug - ua * fu, dv = vg - va * fv;
-        const float epe = sqrtf(du * du + dv * dv);
+        const float epe = flow_metrics_pixel(a, s, b, y, x, acc);
         if (a.epe_map) a.epe_map[i] = epe;
-        const float ev = epe * valid;
-        acc[0] += ev;
-        acc[1] += valid;
-        const float mag = sqrtf(ug * ug + vg * vg);
-        const float e0 = (ev > a.tau0) ? 1.f : 0.f, e1 = ((ev / (mag + 1e-8f)) > a.tau1) ? 1.f : 0.f;
-        acc[6] += e0 * e1 * valid;
-        if (a.mask) {
-            const Lin my = lin_src(y, a.hm, sy_mg), mx = lin_src(x, a.wm, sx_mg);
-            const float mg = bilerp(a.mask + (long long)b * a.hm * a.wm, a.wm, my, mx);
-            const float sr = (mg > a.thresh) ? 1.f : 0.f, sn = (mg <= a.thresh) ? 1.f : 0.f;
-            {   // compute_epe(gt_rigid, rigid_pred): gt (all channels, valid included) times the gt-resolution mask
-                const float d0 = ug * sr - ur * fu, d1 = vg * sr - vr * fv, vv = valid * sr;
-                acc[2] += sqrtf(d0 * d0 + d1 * d1) * vv;
-                acc[3] += vv;
-            }
-            {
-                const float d0 = ug * sn - un * fu, d1 = vg * sn - vn * fv, vv = valid * sn;
-                acc[4] += sqrtf(d0 * d0 + d1 * d1) * vv;
-                acc[5] += vv;
-            }
-        }
     }
     block_sum<8>(acc, scratch);
     if (threadIdx.x == 0)
@@ -282,12 +303,8 @@ __global__ void __launch_bounds__(256) flow_metrics_kernel(const FlowMetArgs a) 
         for (int k = 0; k < 8; ++k) a.partials[(long long)blockIdx.x * 8 + k] = acc[k];
 }
 
-// out[0..3] = all_epe, rigid_epe, non_rigid_epe, outlier ratio   (nc == 2: plain mean over B*Hg*Wg, :384-385)
-__global__ void flow_metrics_finalize(const double* __restrict__ partials, int nblocks, int nc, long long npx, float* __restrict__ out) {
-    CCB_PDL_WAIT();
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    double s[8];
-    sum_partials(partials, nblocks, 8, s);
+// out[0..3] = all_epe, rigid_epe, non_rigid_epe, outlier ratio of the summed acc   (nc == 2: plain mean over npx, :384-385)
+__device__ __forceinline__ void flow_metrics_out(const double (&s)[8], int nc, long long npx, float* out) {
     if (nc == 3) {
         out[0] = (float)s[0] / ((float)s[1] + 1e-8f);
         out[1] = (float)s[2] / ((float)s[3] + 1e-8f);
@@ -298,6 +315,14 @@ __global__ void flow_metrics_finalize(const double* __restrict__ partials, int n
         out[2] = (float)s[4] / (float)npx;
     }
     out[3] = (float)s[6] / ((float)s[1] + 1e-8f);
+}
+
+__global__ void flow_metrics_finalize(const double* __restrict__ partials, int nblocks, int nc, long long npx, float* __restrict__ out) {
+    CCB_PDL_WAIT();
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    double s[8];
+    sum_partials(partials, nblocks, 8, s);
+    flow_metrics_out(s, nc, npx, out);
 }
 
 // ================================================================================================
@@ -771,14 +796,19 @@ __device__ __forceinline__ float aten_lerp(float v0, float v1, float l0, float l
     return __fmaf_rn(v0, l0, __fmul_rn(v1, l1));
 }
 
-__device__ __forceinline__ float submit_combined(const FlowSubmitArgs& a, int b, long long p) {
-    const long long hw = (long long)a.h * a.w;
-    const float e1 = __ldg(a.emask + ((long long)b * a.C + 1) * hw + p), e2 = __ldg(a.emask + ((long long)b * a.C + 2) * hw + p);
+// The combined rigidity mask (0 or 1) of pixel p of sample b: emask [B,C,h,w], cam and fwd [B,2,h,w], hw = h * w
+__device__ __forceinline__ float combined_rigidity(const float* emask, const float* cam, const float* fwd, int C, long long hw,
+                                                   int b, long long p, float thresh) {
+    const float e1 = __ldg(emask + ((long long)b * C + 1) * hw + p), e2 = __ldg(emask + ((long long)b * C + 2) * hw + p);
     const bool bare = __fsub_rn(1.f, __fmul_rn(__fsub_rn(1.f, e1), __fsub_rn(1.f, e2))) > 0.5f;
-    const float* c = a.cam + 2ll * b * hw + p;
-    const float* f = a.fwd + 2ll * b * hw + p;
-    const bool census = (fabsf(__fsub_rn(__ldg(c), __ldg(f))) < a.thresh) && (fabsf(__fsub_rn(__ldg(c + hw), __ldg(f + hw))) < a.thresh);
+    const float* c = cam + 2ll * b * hw + p;
+    const float* f = fwd + 2ll * b * hw + p;
+    const bool census = (fabsf(__fsub_rn(__ldg(c), __ldg(f))) < thresh) && (fabsf(__fsub_rn(__ldg(c + hw), __ldg(f + hw))) < thresh);
     return (bare || census) ? 1.f : 0.f;
+}
+
+__device__ __forceinline__ float submit_combined(const FlowSubmitArgs& a, int b, long long p) {
+    return combined_rigidity(a.emask, a.cam, a.fwd, a.C, (long long)a.h * a.w, b, p, a.thresh);
 }
 
 __global__ void __launch_bounds__(256) flow_submit_mask_kernel(const FlowSubmitArgs a) {
@@ -840,6 +870,69 @@ __global__ void __launch_bounds__(256) flow_submit_kernel(const FlowSubmitArgs a
         a.png[3 * i + 2] = 1;
         a.flo[2 * i + 0] = o[2][0];
         a.flo[2 * i + 1] = o[2][1];
+    }
+}
+
+// ================================================================================================
+// KITTI-2015 flow evaluation (test_flow.py:112-140, test_back2future.py), one sample each at batch-1 semantics:
+//   combined = bare or census at h x w (combined_rigidity), written to a.combined
+//   half 0   compute_all_epes(gt, cam, fwd, combined)                                  (mask h x w)
+//   half 1   compute_all_epes(gt, cam, fwd, 1 - obj), 1 - obj one fp32 subtraction    (mask Hg x Wg)
+// both with compute_all_epes' own THRESH, in one pass over the ground-truth grid: flow_metrics_pixel of each half's
+// FlowMetArgs.  Without the mask net (emask NULL) only half 1, with fwd as both predictions.  Per sample fp64 block
+// partials [B][blocks][16] and a fixed-order finalize: the same bits on every run and at any batch size.
+struct FlowEvalArgs {
+    FlowMetArgs half[2];            // gt, predictions and mask of each half; their B, partials and epe_map are not used
+    const float* emask;             // [B, C, h, w], or null
+    const float* cam;               // [B, 2, h, w], or null
+    const float* fwd;               // [B, 2, h, w]
+    const float* obj;               // [B, Hg, Wg]
+    float* combined;                // [B, h, w]
+    float* one_minus_obj;           // [B, Hg, Wg]
+    double* partials;               // [B][blocks][16]
+    float* out;                     // [B, 8]
+    int B, C, h, w, Hg, Wg;
+    float thresh;
+};
+
+__global__ void __launch_bounds__(256) flow_eval_masks_kernel(const FlowEvalArgs a) {
+    CCB_PDL_WAIT();
+    const long long hw = (long long)a.h * a.w, nm = a.emask ? (long long)a.B * hw : 0, n = nm + (long long)a.B * a.Hg * a.Wg;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        if (i < nm)
+            a.combined[i] = combined_rigidity(a.emask, a.cam, a.fwd, a.C, hw, (int)(i / hw), i % hw, a.thresh);
+        else
+            a.one_minus_obj[i - nm] = __fsub_rn(1.f, __ldg(a.obj + (i - nm)));
+    }
+}
+
+__global__ void __launch_bounds__(256) flow_eval_kernel(const FlowEvalArgs a) {
+    CCB_PDL_WAIT();
+    __shared__ double scratch[16 * 32];
+    const int b = blockIdx.y, first = a.emask ? 0 : 1;
+    const FlowMetScales s0 = flow_met_scales(a.half[0]), s1 = flow_met_scales(a.half[1]);
+    double acc[2][8] = {};
+    const long long ng = (long long)a.Hg * a.Wg;
+    for (long long q = (long long)blockIdx.x * 256 + threadIdx.x; q < ng; q += (long long)gridDim.x * 256) {
+        const int y = (int)(q / a.Wg), x = (int)(q - (long long)y * a.Wg);
+        if (first == 0) flow_metrics_pixel(a.half[0], s0, b, y, x, acc[0]);
+        flow_metrics_pixel(a.half[1], s1, b, y, x, acc[1]);
+    }
+    block_sum<16>(reinterpret_cast<double(&)[16]>(acc), scratch);
+    if (threadIdx.x == 0)
+#pragma unroll
+        for (int k = 0; k < 16; ++k) a.partials[((long long)b * gridDim.x + blockIdx.x) * 16 + k] = acc[k / 8][k % 8];
+}
+
+// out[b, 0:4] of half 0 (not written without the mask net), out[b, 4:8] of half 1
+__global__ void flow_eval_finalize(const FlowEvalArgs a, int nblocks) {
+    CCB_PDL_WAIT();
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.B) return;
+    for (int k = a.emask ? 0 : 1; k < 2; ++k) {
+        double s[8];
+        sum_partials(a.partials + (long long)b * nblocks * 16 + 8 * k, nblocks, 16, s);
+        flow_metrics_out(s, 3, (long long)a.Hg * a.Wg, a.out + 8ll * b + 4 * k);
     }
 }
 
@@ -1566,6 +1659,48 @@ extern "C" int ccb_flow_submit(const float* emask, const float* flow_cam, const 
     CCB_LAUNCH(flow_submit_mask_kernel, dim3(blocks_for((long long)B * h * w, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     CCB_LAUNCH(flow_submit_kernel, dim3(blocks_for((long long)B * Hg * Wg, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     return check_launch("flow_submit");
+}
+
+// blocks per sample of flow_eval_kernel: a function of the frame size alone, so that a sample's sums do not depend on
+// the batch it is evaluated in
+static int flow_eval_blocks(int Hg, int Wg) { return blocks_for((long long)Hg * Wg, 256, NUM_SMS); }
+
+extern "C" long long ccb_flow_eval_workspace_bytes(int B, int h, int w, int Hg, int Wg) {
+    if (B <= 0 || h <= 0 || w <= 0 || Hg <= 0 || Wg <= 0) return -1;
+    return (long long)B * flow_eval_blocks(Hg, Wg) * 16 * (long long)sizeof(double) +
+           ((long long)B * Hg * Wg + (long long)B * h * w) * (long long)sizeof(float);
+}
+
+extern "C" int ccb_flow_eval(const float* emask, const float* flow_cam, const float* flow_fwd, const float* flow_gt,
+                             const float* obj_map, int B, int C, int h, int w, int Hg, int Wg, float thresh,
+                             float epe_thresh, float tau0, float tau1, float* combined, void* work, long long work_bytes,
+                             float* out, ccb_stream_t stream) {
+    CCB_REQUIRE(flow_fwd && flow_gt && obj_map && out, CCB_ERR_ARG, "flow_eval: null pointer");
+    CCB_REQUIRE((emask == nullptr) == (flow_cam == nullptr), CCB_ERR_ARG, "flow_eval: emask and flow_cam come together");
+    CCB_REQUIRE(emask || !combined, CCB_ERR_ARG, "flow_eval: the combined mask needs the mask net output");
+    CCB_REQUIRE(!emask || C >= 3, CCB_ERR_ARG, "flow_eval: the mask net output needs channels 1 and 2, got %d channels", C);
+    CCB_REQUIRE(B > 0 && h > 0 && w > 0 && Hg > 0 && Wg > 0, CCB_ERR_ARG, "flow_eval: bad sizes");
+    CCB_REQUIRE_WORK("flow_eval", "work", work, work_bytes, ccb_flow_eval_workspace_bytes(B, h, w, Hg, Wg));
+    const int nb = flow_eval_blocks(Hg, Wg);
+    FlowEvalArgs a;
+    a.emask = emask; a.cam = flow_cam; a.fwd = flow_fwd; a.obj = obj_map; a.out = out;
+    a.B = B; a.C = C; a.h = h; a.w = w; a.Hg = Hg; a.Wg = Wg; a.thresh = thresh;
+    a.partials = (double*)work;
+    a.one_minus_obj = (float*)(a.partials + (long long)B * nb * 16);
+    a.combined = combined ? combined : a.one_minus_obj + (long long)B * Hg * Wg;
+    for (int k = 0; k < 2; ++k) {
+        FlowMetArgs& m = a.half[k];
+        m.gt = flow_gt; m.pa = emask ? flow_cam : flow_fwd; m.pb = flow_fwd; m.partials = nullptr; m.epe_map = nullptr;
+        m.mask = k == 0 ? a.combined : a.one_minus_obj;
+        m.B = B; m.nc = 3; m.Hg = Hg; m.Wg = Wg; m.hp = h; m.wp = w;
+        m.hm = k == 0 ? h : Hg; m.wm = k == 0 ? w : Wg;
+        m.thresh = epe_thresh; m.tau0 = tau0; m.tau1 = tau1;
+    }
+    const long long nmask = (emask ? (long long)B * h * w : 0) + (long long)B * Hg * Wg;
+    CCB_LAUNCH(flow_eval_masks_kernel, dim3(blocks_for(nmask, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(flow_eval_kernel, dim3(nb, B), dim3(256), 0, stream, a);
+    CCB_LAUNCH(flow_eval_finalize, dim3((B + 63) / 64), dim3(64), 0, stream, a, nb);
+    return check_launch("flow_eval");
 }
 
 extern "C" long long ccb_flow_color_workspace_bytes(int B, int P, int H, int W) {

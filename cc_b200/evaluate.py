@@ -19,6 +19,11 @@
                         synchronisation (kitti_pose_framework / sintel_pose_framework: the frameworks' files, snippets and
                         compensated ground truth, load_pose_frames; pose_errors: the pose algebra, ATE and RE in one kernel;
                         load_pose_net; pose_summary: the printed rows; write_pose_predictions: predictions.npy)
+  flow_eval_batch       test_flow.py:112-140 (and train.py's validate_flow_with_gt) for a batch of KITTI-2015 samples on the
+  back2future_eval_batch  device, no host synchronisation; test_back2future.py with the flow net alone
+                        (kitti_flow_framework / load_kitti_flow_samples: ValidationFlow's files and samples, grouped by
+                        frame size; flow_eval: the rigidity masks and both compute_all_epes in one kernel;
+                        load_flow_eval_nets; flow_summary: the printed row; write_flow_eval_outputs: --output-dir's files)
 
 The scripts' dataset crawlers, image IO and visualisation are out of scope (SURVEY.md section 2); these functions take what the
 reference's `test_framework` iterators yield (uint8 HxWx3 frames, ground truth arrays) and return what the scripts
@@ -42,13 +47,16 @@ def _pose(res):
     return res[1] if isinstance(res, tuple) else res
 
 
-def _flow_nets(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv):
+def _flow_nets(disp_net, pose_net, mask_net, flow_net, tgt, refs, K, Kinv, spatial_normalize=False):
     """The four nets in eval mode on tgt and its 4 refs -> (emask, flow_cam, flow_fwd): the mask net's output, the camera
     flow of the depth and the pose to ref 2, and the flow net's forward flow (test_flow.py:112-125, test_mask.py:119-126,
-    submit_flow.py:109-116)."""
+    submit_flow.py:109-116); spatial_normalize divides the disparity by its mean first (train.py:665-669)."""
     for n in (disp_net, pose_net, mask_net, flow_net):
         n.eval()
-    depth = 1 / disp_net(tgt)
+    disp = disp_net(tgt)
+    if spatial_normalize:
+        disp = LF.spatial_normalize(disp)
+    depth = 1 / disp
     pose = pose_net(tgt, refs)
     emask = mask_net(tgt, refs)
     # Back2Future takes both neighbours, another flow net (FlowNetC6) the forward one
@@ -641,3 +649,202 @@ def write_pose_predictions(path, finals, n_rows):
     predictions = np.zeros((n_rows,) + finals.shape[1:])
     predictions[:len(finals)] = finals
     np.save(os.path.join(path, 'predictions.npy'), predictions)
+
+
+# ------------------------------------------------------------------------------------------------
+# test_flow.py / test_back2future.py on the device: ValidationFlow's samples batched within a frame size, the nets at
+# batch B, the rigidity masks and both compute_all_epes of every sample in one kernel
+
+FLOW_ERROR_NAMES = ('epe_total', 'epe_sp', 'epe_mv', 'Fl', 'epe_total_gt_mask', 'epe_sp_gt_mask', 'epe_mv_gt_mask',
+                    'Fl_gt_mask')
+FLOW_EVAL_NETS = {'disp': ('DispResNet6', 'DispNetS6'), 'pose': ('PoseNetB6', 'PoseNet6'),
+                  'mask': ('MaskNet6', 'MaskResNet6'), 'flow': ('Back2Future', 'FlowNetC6')}
+
+
+def kitti_flow_framework(root, phase='training', occ='flow_occ', N=200, sequence_length=5):
+    """ValidationFlow's files (datasets/validation_flow.py:94-141) -> dict(samples, groups).  samples: N dicts, index i:
+    'frames' (image_2/iiiiii_10.png, then the references _08 _09 _11 _12 for sequence_length 5), 'flow'
+    (data_scene_flow/<phase>/<occ>/iiiiii_10.png; occ 'flow_occ' or 'flow_noc'), 'obj' (obj_map/iiiiii_10.png, or None
+    where it is missing: the reference then uses ones), 'calib' (calib_cam_to_cam/iiiiii.txt) and 'size' (H, W) of the
+    target frame, read from its PNG header.  groups: {(H, W): [indices in order]}; KITTI-2015 frames come in several sizes
+    and a batch takes one."""
+    import os
+    from PIL import Image
+    half = int(sequence_length / 2)
+    seq_ids = [k + 10 for k in range(-half, half + 1) if k != 0]
+    samples, groups = [], {}
+    for i in range(N):
+        name = str(i).zfill(6)
+        img = os.path.join(root, 'data_scene_flow_multiview', phase, 'image_2', name + '_%s.png')
+        obj = os.path.join(root, 'data_scene_flow', phase, 'obj_map', name + '_10.png')
+        with Image.open(img % '10') as im:
+            size = (im.size[1], im.size[0])
+        samples.append(dict(frames=[img % '10'] + [img % str(k).zfill(2) for k in seq_ids],
+                            flow=os.path.join(root, 'data_scene_flow', phase, occ, name + '_10.png'),
+                            obj=obj if os.path.isfile(obj) else None,
+                            calib=os.path.join(root, 'data_scene_flow_calib', phase, 'calib_cam_to_cam', name + '.txt'),
+                            size=size))
+        groups.setdefault(size, []).append(i)
+    return dict(samples=samples, groups=groups)
+
+
+def kitti_cam_intrinsics(path, cid='02'):
+    """get_intrinsics (validation_flow.py:33-37) as ValidationFlow uses it: P_rect_<cid>[:, :3] of a calib_cam_to_cam file,
+    parsed as read_raw_calib_file parses it (the last line of a key wins), in float32."""
+    data = {}
+    with open(path, 'r') as f:
+        for line in f.readlines():
+            key, value = line.split(':', 1)
+            try:
+                data[key] = np.array([float(x) for x in value.split()])
+            except ValueError:
+                pass
+    return np.reshape(data['P_rect_' + cid], (3, 4))[:, :3].astype('float32')
+
+
+def load_kitti_flow_samples(framework, indices):
+    """Samples `indices` of kitti_flow_framework, all of one frame size, decoded on the host -> dict of numpy arrays:
+    frames uint8 [B,F,Hs,Ws,3] (target first; the reference's imread(...).astype(np.float32) holds the same integers),
+    gt fp32 [B,3,Hg,Wg] (flow_read_png's u, v, valid), obj fp32 [B,Hg,Wg] (ones where the file is missing; the
+    reference's ones are float64, the same values), obj_found bool [B], K fp32 [B,3,3] (P_rect_02[:, :3])."""
+    from PIL import Image
+    from .flowutils import flow_io
+    ss = [framework['samples'][i] for i in indices]
+    assert len({s['size'] for s in ss}) == 1, 'a batch takes one frame size: %s' % sorted({s['size'] for s in ss})
+    frames = np.stack([np.stack([np.asarray(Image.open(f)) for f in s['frames']]) for s in ss])
+    assert frames.dtype == np.uint8 and frames.ndim == 5 and frames.shape[4] == 3, (frames.dtype, frames.shape)
+    gt = np.stack([np.stack(flow_io.flow_read_png(s['flow'])) for s in ss]).astype(np.float32)
+    obj = np.stack([np.asarray(Image.open(s['obj'])).astype(np.float32) if s['obj'] else np.ones(frames.shape[2:4], np.float32)
+                    for s in ss])
+    K = np.stack([kitti_cam_intrinsics(s['calib']) for s in ss])
+    return dict(frames=frames, gt=gt, obj=obj, obj_found=np.array([s['obj'] is not None for s in ss]), K=K)
+
+
+@torch.no_grad()
+def flow_eval(emask, flow_cam, flow_fwd, flow_gt, obj_map_gt, THRESH=0.01, epe_thresh=0.5, tau=(3, 0.05), want_mask=False):
+    """The numbers of test_flow.py:127-140 per sample in one fused call (ccb_flow_eval): emask [B,C,h,w] the mask net's eval
+    output, flow_cam / flow_fwd [B,2,h,w], flow_gt [B,3,Hg,Wg], obj_map_gt [B,Hg,Wg] -> fp32 [B,8] on the device =
+    compute_all_epes(gt, cam, fwd, combined) + compute_all_epes(gt, cam, fwd, 1 - obj), each {all, rigid, non-rigid EPE,
+    Fl}, at batch-1 semantics.  THRESH is the script's --THRESH (the census and the composite); epe_thresh is
+    compute_all_epes' own THRESH, which the script leaves at 0.5.  want_mask: also the combined mask [B,1,h,w] (0/1).
+    emask and flow_cam None: test_back2future.py's compute_all_epes(gt, fwd, fwd, 1 - obj) alone -> [B,4].
+    No host synchronisation."""
+    flow_fwd, flow_gt, obj = _lib.f32(flow_fwd), _lib.f32(flow_gt), _lib.f32(obj_map_gt)
+    B, two, h, w = (int(v) for v in flow_fwd.shape)
+    Hg, Wg = int(flow_gt.shape[2]), int(flow_gt.shape[3])
+    assert two == 2 and flow_gt.shape == (B, 3, Hg, Wg) and obj.shape == (B, Hg, Wg), (flow_fwd.shape, flow_gt.shape, obj.shape)
+    C = 0
+    if emask is not None:
+        emask, flow_cam = _lib.f32(emask), _lib.f32(flow_cam)
+        C = int(emask.shape[1])
+        assert emask.shape == (B, C, h, w) and flow_cam.shape == (B, 2, h, w), (emask.shape, flow_cam.shape)
+    else:
+        assert flow_cam is None and not want_mask
+    work, nbytes = _lib.workspace('ccb_flow_eval_workspace_bytes', B, h, w, Hg, Wg, like=flow_fwd)
+    out = torch.empty(B, 8, device=flow_fwd.device)
+    mask = torch.empty(B, 1, h, w, device=flow_fwd.device) if want_mask else None
+    _lib.call('ccb_flow_eval', emask, flow_cam, flow_fwd, flow_gt, obj, B, C, h, w, Hg, Wg, float(THRESH), float(epe_thresh),
+              float(tau[0]), float(tau[1]), mask, work, nbytes, out, flow_fwd)
+    if emask is None:
+        return out[:, 4:]
+    return (out, mask) if want_mask else out
+
+
+def flow_intrinsics(K, Hs, Ws, h=256, w=832, device=None):
+    """ValidationFlow's intrinsics after Scale (custom_transforms.py:133-134) and their float32 inverse
+    (validation_flow.py:141), from the raw K [B,3,3] of load_kitti_flow_samples, on the host -> (K, Kinv) fp32 on
+    `device` (the library's device by default)."""
+    from .input_pipeline import scale_intrinsics
+    K = scale_intrinsics(K.cpu().numpy() if torch.is_tensor(K) else K, Hs, Ws, h, w)
+    Kinv = np.linalg.inv(K).astype(np.float32)
+    dev = device or (torch.device('cpu') if _lib.is_simulator() else torch.device('cuda'))
+    return torch.from_numpy(K).to(dev), torch.from_numpy(Kinv).to(dev)
+
+
+def _flow_frames(frames_u8, h, w):
+    """uint8 [B,F,Hs,Ws,3] -> F normalised fp32 [B,3,h,w] tensors, each frame stretched and resized as make3d_frames does
+    it (Scale hands imresize a float32 frame)."""
+    src = _on_library_device(frames_u8)
+    assert src.dtype == torch.uint8 and src.dim() == 5 and src.size(4) == 3, (src.dtype, src.shape)
+    B, F, Hs, Ws = (int(v) for v in src.shape[:4])
+    x = make3d_frames(src.reshape(B * F, Hs, Ws, 3), h, w).view(B, F, 3, h, w)
+    return [x[:, f].contiguous() for f in range(F)]
+
+
+@torch.no_grad()
+def flow_eval_batch(disp_net, pose_net, mask_net, flow_net, frames_u8, K, flow_gt, obj_map, THRESH=0.01, h=256, w=832,
+                    spatial_normalize=False, want_mask=False):
+    """test_flow.py:112-140 for a batch of one frame size: frames_u8 uint8 [B,5,Hs,Ws,3] (target, then _08 _09 _11 _12),
+    K the raw intrinsics [B,3,3] (or the (K, Kinv) pair flow_intrinsics returns), flow_gt [B,3,Hg,Wg], obj_map [B,Hg,Wg]
+    (load_kitti_flow_samples' arrays; numpy arrays go to the library's device) -> flow_eval's fp32 [B,8] on the device
+    (and the combined mask with want_mask).  The frames are stretched, resized and normalised as Scale does it, the four
+    nets run at batch B (Back2Future on refs 1 and 2, another flow net on ref 2), flow_cam = pose2flow with pose[:, 2].
+    spatial_normalize: train.py's validate_flow_with_gt with --spatial-normalize.  No host synchronisation."""
+    x = _flow_frames(frames_u8, h, w)
+    Hs, Ws = int(frames_u8.shape[2]), int(frames_u8.shape[3])
+    K, Kinv = K if isinstance(K, tuple) else flow_intrinsics(K, Hs, Ws, h, w, x[0].device)
+    emask, flow_cam, flow_fwd = _flow_nets(disp_net, pose_net, mask_net, flow_net, x[0], x[1:], K, Kinv, spatial_normalize)
+    return flow_eval(emask, flow_cam, flow_fwd, _on_library_device(flow_gt), _on_library_device(obj_map), THRESH,
+                     want_mask=want_mask)
+
+
+@torch.no_grad()
+def back2future_eval_batch(flow_net, frames_u8, flow_gt, obj_map, h=256, w=832):
+    """test_back2future.py on KITTI-2015 for a batch of one frame size (frames, flow_gt and obj_map as flow_eval_batch takes
+    them; the script's nlevels 5 and 6 give the same eval output from the same checkpoint) -> fp32 [B,4] on the device =
+    compute_all_epes(gt, fwd, fwd, 1 - obj).  No host synchronisation."""
+    x = _flow_frames(frames_u8, h, w)
+    flow_net.eval()
+    flow_fwd = flow_net(x[0], x[2:4])[0]
+    return flow_eval(None, None, flow_fwd, _on_library_device(flow_gt), _on_library_device(obj_map))
+
+
+def load_flow_eval_nets(pretrained_disp, pretrained_pose, pretrained_mask, pretrained_flow, dispnet='DispResNet6',
+                        posenet='PoseNetB6', masknet='MaskNet6', flownet='Back2Future', nlevels=6, device=None):
+    """The four nets of test_flow.py:88-106 -> (disp, pose, mask, flow) in eval mode: each argument a checkpoint path or
+    the loaded dict holding 'state_dict', loaded strictly; the pose and mask nets built for 4 references, the flow net
+    with nlevels; the choices are FLOW_EVAL_NETS'."""
+    out = []
+    for kind, name, weights in (('disp', dispnet, pretrained_disp), ('pose', posenet, pretrained_pose),
+                                ('mask', masknet, pretrained_mask), ('flow', flownet, pretrained_flow)):
+        assert name in FLOW_EVAL_NETS[kind], (kind, name)
+        kw = {'nb_ref_imgs': 4} if kind in ('pose', 'mask') else {'nlevels': nlevels} if kind == 'flow' else {}
+        net = getattr(models, name)(**kw)
+        if not isinstance(weights, dict):
+            weights = torch.load(weights, map_location='cpu')
+        net.load_state_dict(weights['state_dict'])
+        out.append(net.to(device or torch.device('cuda')).eval())
+    return tuple(out)
+
+
+def flow_summary(per_sample):
+    """AverageMeter's averages of the per-sample rows in sample order -> (avg, row): each column summed as python floats
+    (fp64) in index order, then divided by the count, as test_flow.py / test_back2future.py accumulate .item() values.
+    row is the line the script prints: test_flow.py's 'Errors' row of 8 columns, or test_back2future.py's
+    'Averge EPE [...]' of 4.  test_back2future.py labels its 2nd and 3rd columns non-rigid and rigid, but its values are
+    compute_all_epes' rigid then non-rigid; avg keeps the values' order."""
+    per_sample = np.asarray(per_sample).reshape(len(per_sample), -1)
+    sums = [0] * per_sample.shape[1]
+    for r in per_sample.tolist():
+        for k, v in enumerate(r):
+            sums[k] += v
+    avg = [s / len(per_sample) for s in sums]
+    if len(avg) == 8:
+        row = 'Errors \t {:10.4f}, {:10.4f}, {:10.4f}, {:10.4f}, {:10.4f}, {:10.4f}, {:10.4f}, {:10.4f}'.format(*avg)
+    else:
+        row = 'Averge EPE ' + str(avg)
+    return avg, row
+
+
+def write_flow_eval_outputs(out_dir, i, tgt, mask, obj_map, obj_found=True):
+    """Sample `i` (batch 1) written as test_flow.py:142-153 names it under `out_dir`: images/iii.npy (the normalised target
+    [3,h,w] fp32), gt/iii.npy (the object map [Hg,Wg]: fp32, or the reference's fp64 ones where the file is missing) and
+    mask/iii.npy (the combined mask [1,h,w] fp32)."""
+    import os
+    for sub in ('images', 'gt', 'mask'):
+        os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
+    name = str(i).zfill(3)
+    obj = obj_map[0].cpu().numpy() if torch.is_tensor(obj_map) else np.asarray(obj_map)[0]
+    np.save(os.path.join(out_dir, 'images', name), tgt[0].detach().cpu().numpy())
+    np.save(os.path.join(out_dir, 'gt', name), obj.astype(np.float32 if obj_found else np.float64))
+    np.save(os.path.join(out_dir, 'mask', name), mask[0].detach().cpu().numpy())

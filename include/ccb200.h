@@ -368,6 +368,20 @@ int ccb_mask_iou(const float* emask, const float* flow_cam, const float* flow, c
  *   flo   [B,Hg,Wg,2] fp32          the .flo payload of total (u, v interleaved) */
 int ccb_flow_submit(const float* emask, const float* flow_cam, const float* flow_fwd, int B, int C, int h, int w, int Hg,
                     int Wg, float thresh, float* mask, float* full, unsigned short* png, float* flo, ccb_stream_t stream);
+/* The KITTI-2015 flow scores of one sample each (test_flow.py:112-140, test_back2future.py), no host sync.  emask
+ * [B,C,h,w] (C >= 3; channels 1 and 2 are read), flow_cam and flow_fwd [B,2,h,w] at the nets' resolution, flow_gt
+ * [B,3,Hg,Wg] (u, v, valid), obj_map [B,Hg,Wg] (labels as floats):
+ *   combined = bare or census, bare = 1 - (1-e1)(1-e2) > 0.5, census = |cam - fwd| < thresh in u and in v, each step
+ *   one rounded fp32 operation (0 or 1; written to combined [B,1,h,w] when it is not NULL)
+ *   out [B,8] = compute_all_epes(gt, cam, fwd, combined) and compute_all_epes(gt, cam, fwd, 1 - obj), each {all, rigid,
+ *   non-rigid EPE, Fl} with compute_all_epes' own THRESH epe_thresh (kept apart from thresh) and tau = (tau0, tau1),
+ *   with ccb_flow_metrics' semantics per sample (batch 1).
+ * emask and flow_cam NULL: test_back2future.py's compute_all_epes(gt, fwd, fwd, 1 - obj) alone, in out[:, 4:8]; out[:, 0:4]
+ * is not written.  fp64 block partials per sample with a fixed-order finalize: the same bits on every run and at any B. */
+long long ccb_flow_eval_workspace_bytes(int B, int h, int w, int Hg, int Wg);
+int ccb_flow_eval(const float* emask, const float* flow_cam, const float* flow_fwd, const float* flow_gt,
+                  const float* obj_map, int B, int C, int h, int w, int Hg, int Wg, float thresh, float epe_thresh,
+                  float tau0, float tau1, float* combined, void* work, long long work_bytes, float* out, ccb_stream_t stream);
 /* Middlebury flow colours (flowlib.py flow_to_image / compute_color), no host sync.  flow [B,P,2,H,W]: per image P
  * panels stacked along H as np.hstack stacks CHW arrays, normalised by ONE maximum radius -> out [B,3,P*H,W] uint8
  * levels (the reference's float image times 255).  |u| or |v| > 1e7 is unknown (black, left out of the maximum); NaN
