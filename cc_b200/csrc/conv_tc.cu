@@ -2,26 +2,26 @@
 //
 //   D[128 pixels x N<=128 channels] (fp32, registers) += A[128 x 32] (im2col tile) * B[N x 32]^T (weights)
 //
-// * one CTA works on one 128-pixel x N-channel output tile at a time (fprop / dgrad: one persistent CTA per SM walks
-//   the tiles and splits through one stage ring); one producer warpgroup + two consumer warpgroups, each
+// * one CTA works on one 128-row x N-channel output tile at a time (one persistent CTA per SM walks the tiles and
+//   splits through one stage ring); one producer warpgroup + two consumer warpgroups, each
 //   consumer owning 64 of the 128 rows (wgmma m64nNk8, N = the launch's channel tile rounded up to 16/32/64/128);
-// * A is gathered straight from the NCHW activations (no im2col buffer in HBM): a K-chunk is 4
-//   consecutive input channels of one filter tap, so the 4 loads of a chunk share the tap's bounds
-//   check and are coalesced across the 128 pixels of the tile;
+// * A is gathered straight from the NCHW activations (no im2col buffer in HBM): a K-chunk (wgrad: a group of 4 rows)
+//   is 4 consecutive input channels of one filter tap, so the 4 loads of a chunk share the tap's bounds check; they
+//   are coalesced across the 128 pixels of the tile (wgrad: the 32 pixels of the k-tile);
 // * operands are staged in shared memory K-major with the 128-byte swizzle ([row][128 B], 16 B chunk ^= row & 7,
 //   8-row atoms 1 KB apart): the layout wgmma reads for tf32, which it accepts only K-major.  In fprop / dgrad the
-//   weight tiles arrive by TMA, which writes that swizzle itself: no producer thread waits for them;
+//   weight tiles arrive by TMA, which writes that swizzle itself: no producer thread waits for them.  In wgrad, B is the
+//   output gradient: the producers copy it raw by 16-byte cp.async, the consumers split it into that layout;
 // * fp32 parity: every fp32 operand is split hi = tf32(x), lo = x - hi and each k-step issues three
 //   tf32 MMAs (hi*hi + lo*hi + hi*lo) ("3xTF32", error ~2^-21).  The tensor core only sums one 32-deep stage (small
 //   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
 //   fp32 adds, so no long accumulation chain runs through the tensor core's own rounding;
-// * fprop / dgrad: the producers gather the A tile once, unsplit, with zero-filling 4-byte cp.async straight from
-//   global into shared memory (k-major, see tc_a_idx); a producer never waits for its own copies, so up to `depth`
-//   stages of loads are in flight.  Each consumer thread loads its 16 values with 16 conflict-free LDS.32, splits them
-//   and issues wgmma with A from registers (B by descriptor), so A crosses shared memory twice per stage instead of
-//   being stored twice and read three times.  The consumers load and split the next stage while the current
-//   stage's MMAs run, and take registers from the producers (setmaxnreg) to hold both.  The wgrad kernel splits both
-//   operands in its producers and reads both from shared memory;
+// * the producers gather the A tile once, unsplit, with zero-filling 4-byte cp.async straight from global into shared
+//   memory (fprop / dgrad: k-major, see tc_a_idx; wgrad: row-major, see TcAWgrad), several stages of loads in flight.
+//   Each consumer thread loads its 16 values with 16 conflict-free LDS.32, splits them and issues wgmma with A from
+//   registers (B by descriptor), so A crosses shared memory twice per stage instead of being stored twice and read
+//   three times.  The consumers load and split the next stage while the current stage's MMAs run, and take registers
+//   from the producers (setmaxnreg) to hold both;
 // * mbarrier pipeline of up to 4 stages: producers -> full[s] -> consumers (wgmma, commit group, wait, fp32 add)
 //   -> empty[s];
 //   the epilogue adds bias / residual, applies the activation and stores NCHW straight from the accumulators.
@@ -134,6 +134,10 @@ __device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// 16-byte asynchronous copy global -> shared (L2 only); `src` 16-byte aligned, zero-fill as in cp_async_4
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, bool valid) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
 __device__ __forceinline__ float tf32_hi(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -164,67 +168,8 @@ __device__ __forceinline__ void wg_fence_regs(uint32_t (&d)[K][R]) {
         for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[k][i])::"memory");
 }
 
-// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 in, fp32 accumulators in registers (N / 2 per thread)
-__device__ __forceinline__ void wgmma_tf32_n16(float (&d)[8], uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
-        "%8, %9, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "l"(da), "l"(db));
-}
-__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-        "%16, %17, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(da), "l"(db));
-}
-__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "%32, %33, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db));
-}
-__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
-        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
-        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-        "%64, %65, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db));
-}
-template <int NT>
-__device__ __forceinline__ void wgmma_tf32(float (&d)[NT / 2], uint64_t da, uint64_t db) {
-    if constexpr (NT == 16) wgmma_tf32_n16(d, da, db);
-    else if constexpr (NT == 32) wgmma_tf32_n32(d, da, db);
-    else if constexpr (NT == 64) wgmma_tf32_n64(d, da, db);
-    else wgmma_tf32_n128(d, da, db);
-}
-
-// The same with A from registers: the m64k8 tf32 fragment, a[i] = A[wq * 16 + lane / 4 + 8 * (i & 1)][lane % 4 + 4 * (i >> 1)]
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 in, fp32 accumulators in registers (N / 2 per thread), A from registers:
+// the m64k8 tf32 fragment, a[i] = A[wq * 16 + lane / 4 + 8 * (i & 1)][lane % 4 + 4 * (i >> 1)]
 // for thread `lane` of warp wq of the warpgroup.  The registers must hold until the wgmma's group has been waited on.
 __device__ __forceinline__ void wgmma_tf32_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t db) {
     asm volatile(
@@ -356,65 +301,45 @@ __device__ __forceinline__ int tc_acc_row(int wg, int wq, int lane, int half) { 
 __device__ __forceinline__ int tc_acc_col(int lane, int i, int e) { return 8 * i + 2 * (lane & 3) + e; }
 __device__ __forceinline__ int tc_acc_reg(int i, int half, int e) { return 4 * i + 2 * half + e; }
 
-// Consumer side of the wgrad kernel, both operands split in shared memory: acc = 0 (an empty split contributes zeros),
-// then for each of `nkt` full stages, 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this warpgroup's 64 rows into the
-// scratch registers `part`, then acc += part in fp32 and the stage goes back to the producers.
-template <int NT>
-__device__ __forceinline__ void tc_consume(const TcRing& ring, int nkt, int wg, int lane, float (&acc)[NT / 2]) {
-    float part[NT / 2];
-#pragma unroll
-    for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
-    const uint32_t base = smem_u32(ring.smem);
-    for (int it = 0; it < nkt; ++it) {
-        const int s = it % ring.depth;
-        mbar_wait(&ring.full[s], (it / ring.depth) & 1);
-        const TcTiles<uint32_t> t = ring.tiles(base, s);
-        const uint32_t a_hi = t.a_hi + wg * (TC_TILE_BYTES / 2), a_lo = t.a_lo + wg * (TC_TILE_BYTES / 2);
-#pragma unroll
-        for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
-        wg_fence();
-#pragma unroll
-        for (int ks = 0; ks < TC_KC / 2; ++ks) {
-            const uint32_t koff = (uint32_t)ks * 32u;
-            wgmma_tf32<NT>(part, wg_desc(a_lo + koff), wg_desc(t.b_hi + koff));
-            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(t.b_lo + koff));
-        }
-#pragma unroll
-        for (int ks = 0; ks < TC_KC / 2; ++ks) {
-            const uint32_t koff = (uint32_t)ks * 32u;
-            wgmma_tf32<NT>(part, wg_desc(a_hi + koff), wg_desc(t.b_hi + koff));
-        }
-        wg_commit();
-        wg_wait<0>();
-        wg_fence_regs(part);
-        if (lane == 0) mbar_arrive(&ring.empty[s]);
-#pragma unroll
-        for (int j = 0; j < NT / 2; ++j) acc[j] += part[j];
-    }
-}
-
-// The fprop kernel's A tile: one fp32 copy of the stage's 128 x 32 im2col values, unsplit (the first A slot of the
-// stage; the second goes unused), k-major with the row index swizzled by k:
+// The A tile: one fp32 copy of the stage's 128 x 32 im2col values, unsplit, in the first A slot of the stage.  Each
+// consumer thread (rows r0 = wg * 64 + wq * 16 + lane / 4 and r0 + 8, column t = lane % 4) reads its 16 values with 16
+// LDS.32 at k = t + 4 j.  The two kernels gather along different axes, so each has its own swizzled layout, both
+// bank-conflict free on both sides.  A layout L gives the byte offset L::off(r0, t) of A[r0][t] and, from it, the byte
+// offset L::at(off, h, j) of A[r0 + 8 h][t + 4 j].
 //
-//   A[r][k] is float tc_a_idx(r, k) = 128 k + (r ^ 8 (k % 4)).
+// TcAFprop (fprop / dgrad), k-major with the row index swizzled by k:  A[r][k] is float tc_a_idx(r, k) = 128 k + (r ^ 8 (k % 4)).
+// The producers write it with 4-byte cp.async, a warp's 32 lanes being the 32 consecutive rows 32 w + lane at one k:
+// r ^ 8 (k % 4) permutes those 32 rows among themselves (8 (k % 4) < 32), so the 32 words land on the 32 banks.  The
+// consumers read all 16 values with k % 4 = t: lane l of a warp reads bank (r0 + 8 h) ^ 8 t mod 32, whose low 3 bits
+// are lane / 4 and whose bits 3-4 are those of wq * 16 + 8 h flipped by t, so the 8 row offsets times the 4 columns
+// of the warp cover the 32 banks once.  r0 & 8 = 0, so row r0 + 8 flips bit 3 of the row, byte bit 5, and k + 4 j is
+// 2 KB further on.
 //
-// Both sides are bank-conflict free.  The producers write it with 4-byte cp.async, a warp's 32 lanes being the 32
-// consecutive rows 32 w + lane at one k: r ^ 8 (k % 4) permutes those 32 rows among themselves (8 (k % 4) < 32), so
-// the 32 words land on the 32 banks.  A consumer thread (rows r0 = wg * 64 + wq * 16 + lane / 4 and r0 + 8, column
-// t = lane % 4) reads its 16 values with 16 LDS.32 at k = t + 4 j, all with k % 4 = t: lane l of a warp reads bank
-// (r0 + 8 h) ^ 8 t mod 32, whose low 3 bits are lane / 4 and whose bits 3-4 are those of wq * 16 + 8 h flipped by t,
-// so the 8 row offsets times the 4 columns of the warp cover the 32 banks once.
+// TcAWgrad (wgrad: rows (tap, ci), k = 32 pixels), row-major with k swizzled by the row:  A[r][k] is float
+// TcAWgrad::idx(r, k) = 32 r + (k ^ 4 (r % 8)).  The producers write one row per warp instruction, lane = k:
+// k ^ 4 (r % 8) permutes the 32 lanes, so the 32 words land on the 32 banks.  Consumer lane l reads word
+// 32 (r0 + 8 h) + (t + 4 j) ^ 4 (lane / 4) = ... + t + 4 (j ^ lane / 4) (r0 % 8 = lane / 4, t < 4): bank
+// t + 4 (j ^ lane / 4), which for one j covers the 32 banks once over the 4 t and 8 lane / 4.  In bytes that is
+// (off(r0, t) + 1024 h) ^ 16 j: bits 4-6 of off hold lane / 4, and no other term reaches them.
 struct TcAFrag { uint32_t hi[TC_KC / 2][4], lo[TC_KC / 2][4]; };   // [k-step][wgmma A register]
 
 __device__ __forceinline__ int tc_a_idx(int r, int k) { return k * TC_M + (r ^ (8 * (k & 3))); }
-// this thread's 16 raw values of the A tile at `tile`: v[h][j] = A[r0 + 8 h][t + 4 j].  `off` is the byte offset of
-// A[r0][t] (tc_a_off); r0 & 8 = 0, so row r0 + 8 flips bit 3 of the row, byte bit 5, and k + 4 j is 2 KB further on.
-__device__ __forceinline__ int tc_a_off(int r0, int t) { return tc_a_idx(r0, t) * 4; }
+struct TcAFprop {
+    __device__ __forceinline__ static int off(int r0, int t) { return tc_a_idx(r0, t) * 4; }
+    __device__ __forceinline__ static int at(int off, int h, int j) { return (off ^ (32 * h)) + 2048 * j; }
+};
+struct TcAWgrad {
+    __device__ __forceinline__ static int idx(int r, int k) { return 32 * r + (k ^ (4 * (r & 7))); }
+    __device__ __forceinline__ static int off(int r0, int t) { return idx(r0, t) * 4; }
+    __device__ __forceinline__ static int at(int off, int h, int j) { return (off + 1024 * h) ^ (16 * j); }
+};
+// this thread's 16 raw values of the A tile at `tile` in layout L: v[h][j] = A[r0 + 8 h][t + 4 j], off = L::off(r0, t)
+template <typename L>
 __device__ __forceinline__ void tc_load_a(const unsigned char* tile, int off, float (&v)[2][8]) {
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[h][j] = *(const float*)(tile + ((off ^ (32 * h)) + 2048 * j));
+        for (int j = 0; j < 8; ++j) v[h][j] = *(const float*)(tile + L::at(off, h, j));
 }
 // the split of tc_split_store, hi = tf32(x), lo = tf32(x - hi), into the fragment: k-step ks, register i holds
 // row r0 + 8 (i & 1), k = 8 ks + t + 4 (i >> 1)
@@ -429,36 +354,54 @@ __device__ __forceinline__ void tc_split_a(const float (&v)[2][8], TcAFrag& f) {
         }
 }
 
-// Consumer side of the fprop kernel: tc_consume's products in its order, with A from registers.  Below N = 128, while a
-// stage's MMAs run the thread waits for the next stage and loads and splits its A fragment.  At N = 128 acc + part
-// already take 128 registers and a second fragment does not fit without spilling, so each stage's A is loaded and
-// split after its full barrier, as the producers used to.  B of the current stage is read by the MMAs until the wait,
-// so the stage is released after it.  The unit's k-tiles are the CTA's g-th onwards: they start in stage g % depth.
-template <int NT>
-__device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt, int wg, int wq, int lane, float (&acc)[NT / 2]) {
+// The consumers' named barrier (barrier 0 is __syncthreads): the 256 threads of both consumer warpgroups
+__device__ __forceinline__ void tc_consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_CONSUMER_WARPS) : "memory"); }
+
+// What the consumers do to a full stage's B operand before its MMAs (tc_consume_rs): nothing in fprop / dgrad, whose B
+// tiles arrive by TMA already split.
+struct TcFpropFeed {
+    static constexpr bool split_b = false;
+    __device__ __forceinline__ void prep_b(const TcTiles<unsigned char*>&) const {}
+};
+
+// Consumer side of both kernels, A (in layout L) from registers: acc = 0 (an empty split contributes zeros), then for
+// each of the unit's `nkt` stages, 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this warpgroup's 64 rows into scratch
+// registers `part`, then acc += part in fp32 and the stage goes back to the producers.  Taking a full stage means
+// loading and splitting this thread's A fragment and, where Feed::split_b, its share of the B operand (prep_b, by all
+// 256 consumer threads, then made visible to wgmma: proxy fence, consumer barrier).  Below N = 128, while a stage's
+// MMAs run the thread waits for the next stage and takes it, so it releases a stage only once the next one is full.
+// At N = 128 acc + part already take 128 registers and a second fragment does not fit without spilling, so each stage
+// is taken after its full barrier.  B of the current stage is read by the MMAs until the wait, so the stage is
+// released after it.  The unit's k-tiles are the CTA's g-th onwards: they start in stage g % depth.
+template <int NT, typename L, typename Feed>
+__device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt, int wg, int wq, int lane, const Feed& feed,
+                                              float (&acc)[NT / 2]) {
     constexpr bool split_ahead = NT < 128;
-    float part[NT / 2];
 #pragma unroll
     for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
     const uint32_t base = smem_u32(ring.smem);
-    const int a_off = tc_a_off(wg * 64 + wq * 16 + (lane >> 2), lane & 3);
+    const int a_off = L::off(wg * 64 + wq * 16 + (lane >> 2), lane & 3);
     TcAFrag cur, nxt;
-    float v[2][8];
+    auto take = [&](int st, uint32_t ph, TcAFrag& f) {
+        mbar_wait(&ring.full[st], ph);
+        const TcTiles<unsigned char*> t = ring.tiles(ring.smem, st);
+        float v[2][8];
+        tc_load_a<L>(t.a_hi, a_off, v);
+        tc_split_a(v, f);
+        if constexpr (Feed::split_b) {
+            feed.prep_b(t);
+            fence_proxy_async();
+            tc_consumer_sync();
+        }
+    };
+    float part[NT / 2];
     int s = g % ring.depth;                     // stage of k-tile it
     uint32_t phase = (g / ring.depth) & 1;      // parity of k-tile it's round
     if constexpr (split_ahead) {
-        if (nkt > 0) {
-            mbar_wait(&ring.full[s], phase);
-            tc_load_a(ring.tiles(ring.smem, s).a_hi, a_off, v);
-            tc_split_a(v, cur);
-        }
+        if (nkt > 0) take(s, phase, cur);
     }
     for (int it = 0; it < nkt; ++it) {
-        if constexpr (!split_ahead) {
-            mbar_wait(&ring.full[s], phase);
-            tc_load_a(ring.tiles(ring.smem, s).a_hi, a_off, v);
-            tc_split_a(v, cur);
-        }
+        if constexpr (!split_ahead) take(s, phase, cur);
         const TcTiles<uint32_t> tl = ring.tiles(base, s);
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
@@ -476,11 +419,7 @@ __device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt
         const int s1 = s + 1 == ring.depth ? 0 : s + 1;
         const uint32_t phase1 = phase ^ (s1 == 0);
         if constexpr (split_ahead) {
-            if (it + 1 < nkt) {
-                mbar_wait(&ring.full[s1], phase1);
-                tc_load_a(ring.tiles(ring.smem, s1).a_hi, a_off, v);
-                tc_split_a(v, nxt);
-            }
+            if (it + 1 < nkt) take(s1, phase1, nxt);
         }
         wg_wait<0>();
         wg_fence_regs(part);
@@ -496,9 +435,10 @@ __device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt
     }
 }
 
-// One work unit: the 128-pixel x 128-channel output tile and the k-tiles of one split.
+// One work unit: the 128-row x 128-channel output tile and the k-tiles of one split (Args: TcArgs or TcWgradArgs).
 struct TcUnit { int m0, n0, z, kt_beg, nkt; };
-__device__ __forceinline__ TcUnit tc_unit(const TcArgs& a, int u) {
+template <typename Args>
+__device__ __forceinline__ TcUnit tc_unit(const Args& a, int u) {
     TcUnit w;
     w.m0 = (u % a.tiles_m) * TC_M;
     u /= a.tiles_m;
@@ -615,7 +555,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             const TcUnit w = tc_unit(a, u);
             const int ntile = min(TC_NMAX, a.Ntot - w.n0);
             float acc[NT / 2];
-            tc_consume_rs<NT>(ring, g, w.nkt, wg, wq, lane, acc);
+            tc_consume_rs<NT, TcAFprop>(ring, g, w.nkt, wg, wq, lane, TcFpropFeed(), acc);
             g += w.nkt;
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
@@ -705,6 +645,17 @@ static int tc_weight_map(CUtensorMap* map, const float* wp, int N, int Kp, int n
     return CCB_OK;
 }
 
+// The grid of a persistent launch: one CTA per SM (launch bounds, registers) runs units until none are left
+static dim3 tc_persistent_grid(int units) {
+    static int sms = [] {
+        int dev = 0, n = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+        return n > 0 ? n : NUM_SMS;
+    }();
+    return dim3(units < sms ? units : sms);
+}
+
 // One generalised-fprop launch (+ its weight preparation into `wp`, tf32 hi copy + lo copy).
 static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK, int Ci, const signed char* tap_index,
                      float* wp, float* partial, int splits, cudaStream_t st) {
@@ -730,22 +681,14 @@ static int launch_tc(TcArgs& a, const float* w, int mode, int N, int Cc, int KK,
     a.tiles_m = cdiv(a.M, TC_M);
     a.tiles_n = cdiv(N, TC_NMAX);
     a.units = a.tiles_m * a.tiles_n * splits;
-    // one CTA per SM (launch bounds, registers) runs units until none are left
-    static int sms = [] {
-        int dev = 0, n = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        return n > 0 ? n : NUM_SMS;
-    }();
-    return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, dim3(a.units < sms ? a.units : sms), smem, st, "conv_tc");
+    return tc_launch_kernel(TC_FPROP_KERNELS, a, nt, tc_persistent_grid(a.units), smem, st, "conv_tc");
 }
 
 // ================================================================================================
 // WGRAD on the tensor cores:  D[m=(tap,ci)][n=co] = sum_{k=pixel} X_im2col[m][k] * dY[n][k]
-// Both operands are K(=pixel)-contiguous in NCHW, so producers walk along K: 8 consecutive threads
-// load the 8 16-byte chunks (32 consecutive output pixels) of one row -> coalesced global loads, and
-// with the SWIZZLE_128B operand layout their shared-memory stores are conflict-free.
-// Split-K over pixel ranges (grid.z) with a deterministic two-stage reduce.
+// Rows m are (tap, ci) with ci padded to cpad (rows ci >= Ci are zero), k runs over the B*Ho*Wo output pixels in
+// k-tiles of 32.  Both operands are K(=pixel)-contiguous in NCHW, so the producers copy along K: 32 consecutive pixels
+// of one row per warp instruction.  Split-K over pixel ranges with a deterministic two-stage reduce.
 struct TcWgradArgs {
     const float* x;      // [B,Ci,Hi,Wi]
     const float* dy;     // [B,Co,Ho,Wo]
@@ -753,107 +696,160 @@ struct TcWgradArgs {
     int B, Ci, Hi, Wi, Co, Ho, Wo, kh, kw, stride, pad;
     int cpad, Mtot;      // channels padded to 4; Mtot = kh*kw*cpad rows
     int P;               // B*Ho*Wo pixels (Wo % 4 == 0)
-    int ktiles, kt_per_split, splits;  // k-tiles of 32 pixels (P / 32 rounded up), split-K over them (grid.z)
+    int ktiles, kt_per_split, splits;  // k-tiles of 32 pixels (P / 32 rounded up), split-K over them
+    int tiles_m, tiles_n, units;       // work units: 128-row tile (fastest) x channel tile x split, units = product
     int depth, b_tile_bytes;           // stage ring (tc_geometry)
 };
 
+// What the wgrad kernel's consumers do to a full stage's B operand (tc_consume_rs): dy, copied raw into the stage's
+// second A slot, is split into tf32 hi / lo in the B slots, float4 q at float4 q (the raw copy is already in the
+// swizzled K-major layout); consumer thread ct splits float4s ct, ct + 256, ...: a warp's 32 consecutive float4s are
+// conflict free.
+template <int NT>
+struct TcWgradFeed {
+    static constexpr bool split_b = true;
+    int ct;                                                  // consumer thread, 0 .. 255
+    __device__ __forceinline__ void prep_b(const TcTiles<unsigned char*>& t) const {
+        constexpr int n4 = NT * TC_KC, nthr = 32 * TC_CONSUMER_WARPS;      // float4s of one B copy: 128 .. 1024
+#pragma unroll
+        for (int i = 0; i < (n4 + nthr - 1) / nthr; ++i) {
+            const int q = ct + nthr * i;
+            if (n4 % nthr == 0 || q < n4) tc_split_store(t.b_hi, t.b_lo, q, ((const float4*)t.a_lo)[q]);
+        }
+    }
+};
+
+// Persistent, as conv_tc_kernel: a CTA runs units blockIdx.x, blockIdx.x + gridDim.x, ..., its g-th k-tile in stage
+// g % depth, and its producers gather the way that kernel's do: zero-filling cp.async straight into the stage, full[s]
+// counting each thread's arrival once its copies have landed, never a wait for its own copies, so up to `depth`
+// stages of loads are in flight.  A stage holds the raw im2col tile in its first A slot (layout TcAWgrad, read by
+// tc_consume_rs as in fprop), the raw dy tile [NT rows][32 pixels] in its second A slot (float4 tile_idx(n, chunk),
+// NT x 128 B <= 16 KB), and dy split into tf32 hi / lo in its B slots, in the swizzled K-major layout wgmma reads B
+// in.  The consumers split dy (TcWgradFeed) when they take a stage: below N = 128 while the previous stage's MMAs run.
+// A producer that had to split dy itself could publish a stage only between its waits for free stages, which would
+// put a consumer -> producer -> consumer round trip into the path of every stage.
 template <int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_wgrad_kernel(const TcWgradArgs a) {
     const TcRing ring = tc_ring(a.depth, a.b_tile_bytes, TC_PRODUCERS);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m0 = blockIdx.x * TC_M, n0 = blockIdx.y * TC_NMAX;
-    const int ntile = min(TC_NMAX, a.Co - n0);
-    const int kt_beg = blockIdx.z * a.kt_per_split;
-    const int nkt = min(a.ktiles, kt_beg + a.kt_per_split) - kt_beg;   // k-tiles of this split, >= 1 by construction
-    const int KK = a.kh * a.kw;
     const int HWo = a.Ho * a.Wo, HWi = a.Hi * a.Wi;
 
     if (warp < TC_PRODUCERS / 32) {
-        // 8 consecutive threads walk the 8 K-chunks (32 consecutive pixels) of one row, rows rbase + 16 j
-        const int c = tid & 7, rbase = tid >> 3;
-        // per-row constants: x offset of the row's (ci, ky, kx) relative to the pixel base, and its tap shift
-        int rowoff[8], dky[8], dkx[8];
-        unsigned rvalid = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            int m = m0 + rbase + 16 * j;
-            rowoff[j] = 0; dky[j] = dkx[j] = 0;
-            if (m < a.Mtot) {
-                int tap = m / a.cpad, ci = m - tap * a.cpad;
-                if (ci < a.Ci) {
-                    int ky = tap / a.kw, kx = tap - ky * a.kw;
-                    dky[j] = ky - a.pad; dkx[j] = kx - a.pad;
-                    rowoff[j] = ci * HWi + dky[j] * a.Wi + dkx[j];       // may be negative: only used where the tap is in bounds
-                    rvalid |= 1u << j;
-                }
+        // ===================== producers =====================
+        wg_regs_dec<TC_PRODUCER_REGS>();
+        // A: warp w copies rows 32 w + i (i < 32) of the tile, lane = pixel of the k-tile.  dy: the thread copies 16-byte
+        // chunk c = tid % 8 (pixels 4 c .. 4 c + 3 of the k-tile) of rows n = tid / 8 + 16 j, j < NT / 16; n % 8 does not
+        // depend on j, so chunk j is float4 tile_idx(tid / 8, c) + 128 j of the raw tile.
+        const int c = tid & 7, n_lo = tid >> 3, dy_idx = tile_idx(n_lo, c);
+        // the warp's row-group table for the current unit, in the shared memory past the stage barriers: tc_geometry
+        // keeps 2 KB there for the barriers and the 1 KB alignment, and the table fits beside both
+        static_assert(1023 + 2 * TC_MAX_STAGES * 8 + TC_PRODUCERS / 32 * 8 * 8 <= 2048, "row-group table past the ring");
+        int2* const gtab = (int2*)(ring.empty + TC_MAX_STAGES) + 8 * warp;
+        int g = 0;                                   // k-tiles this CTA has copied
+        for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+            const TcUnit w = tc_unit(a, u);
+            const int ntile = min(TC_NMAX, a.Co - w.n0);
+            // the warp's 8 row groups q, rows 32 w + 4 q .. + 3: one tap (ky, kx), channels ci .. ci + 3 (cpad % 4 == 0).
+            // gtab[q] = {ci * HWi + ky * Wi + kx: the x offset of the group's first row from its pixel's window corner,
+            // ky | kx << 8 | nv << 16: nv = the rows of the group that exist (ci + e < Ci and m < Mtot)}, by lane q
+            __syncwarp();                            // the previous unit's entries have been read
+            if (lane < 8) {
+                const int m = w.m0 + 32 * warp + 4 * lane;
+                const int tap = m / a.cpad, ci = m - tap * a.cpad, ky = tap / a.kw, kx = tap - ky * a.kw;
+                const int nv = m < a.Mtot ? max(0, min(4, a.Ci - ci)) : 0;
+                gtab[lane] = make_int2(ci * HWi + ky * a.Wi + kx, ky | kx << 8 | nv << 16);
             }
-        }
-        for (int it = 0; it < nkt; ++it) {
-            const int s = it % ring.depth;
-            const int p0 = ((kt_beg + it) * TC_KC + c) * 4;       // first of this chunk's 4 pixels
-            const bool pvalid = p0 < a.P;
-            int b = 0, oy = 0, ox0 = 0;
-            if (pvalid) {
-                b = p0 / HWo;
-                int rem = p0 - b * HWo;
-                oy = rem / a.Wo;
-                ox0 = rem - oy * a.Wo;
-            }
-            const float* xpix = a.x + (long long)b * a.Ci * HWi + (oy * a.stride) * a.Wi + ox0 * a.stride;
-            const int iyb = oy * a.stride, ixb = ox0 * a.stride;
-            float av[8][4];
-            float4 bv[8];
+            __syncwarp();
+            // this lane's pixel p = (b, oy, ox), the k-tile's first pixel + lane, advanced by 32 pixels per k-tile
+            int p = w.kt_beg * (TC_KC * 4) + lane;
+            int b = p / HWo, oy = (p - b * HWo) / a.Wo, ox = p - b * HWo - oy * a.Wo;
+            const float* dyn = a.dy + (long long)(w.n0 + n_lo) * HWo;     // row n0 + tid / 8 of image 0
+            for (int it = 0; it < w.nkt; ++it, ++g) {
+                const int s = g % ring.depth;
+                const TcTiles<unsigned char*> t = ring.acquire(g, s);
+                // ---- A: the group's rows share the pixel's bounds check; a copy without a value is zero-filled from xb
+                const bool pvalid = p < a.P;
+                const int iy0 = oy * a.stride - a.pad, ix0 = ox * a.stride - a.pad, pix = iy0 * a.Wi + ix0;
+                const float* xb = a.x + (pvalid ? (long long)b * a.Ci * HWi : 0ll);
+                asm("" : "+l"(xb));      // one 64-bit base: each copy's address is then one wide multiply-add
+                // row i of the warp is byte TcAWgrad::idx(32 w + i, lane) * 4 = ab[i % 8] + 128 i of the tile: the swizzle
+                // flips bits 4-6 of the row's lane offset, and 128 i reaches only bits 7 and up
+                uint32_t ab[8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                av[j][0] = av[j][1] = av[j][2] = av[j][3] = 0.f;
-                const int iy = iyb + dky[j], ix0 = ixb + dkx[j];
-                if (pvalid && ((rvalid >> j) & 1u) && iy >= 0 && iy < a.Hi) {
-                    const float* px = xpix + rowoff[j];
-                    if (ix0 >= 0 && ix0 + 3 * a.stride < a.Wi) {          // interior: no per-element checks
+                for (int k = 0; k < 8; ++k) ab[k] = (smem_u32(t.a_hi) + 4096 * warp + 4 * lane) ^ (16 * k);
+                int2 gh[4];                          // the table, 4 groups at a time: each copy is a compiler barrier
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) av[j][e] = __ldg(px + e * a.stride);
+                for (int q = 0; q < 8; ++q) {
+                    if (q % 4 == 0) {
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) gh[i] = gtab[q + i];
+                    }
+                    const int2 gq = gh[q % 4];
+                    const int ky = gq.y & 0xff, kx = (gq.y >> 8) & 0xff, nv = gq.y >> 16;
+                    const bool ok = pvalid && (unsigned)(iy0 + ky) < (unsigned)a.Hi && (unsigned)(ix0 + kx) < (unsigned)a.Wi;
+                    const int o = pix + gq.x;
+                    if (nv == 4) {                   // the warp's usual case (uniform): the 4 rows are channel planes apart
+                        const float* src = xb + (ok ? o : 0);
+                        const int step = ok ? HWi : 0;
+#pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                            cp_async_4(ab[(4 * q + e) % 8] + 128 * (4 * q + e), src + e * step, ok);
                     } else {
+                        const int n = ok ? nv : 0;
 #pragma unroll
                         for (int e = 0; e < 4; ++e) {
-                            const int ix = ix0 + e * a.stride;
-                            if (ix >= 0 && ix < a.Wi) av[j][e] = __ldg(px + e * a.stride);
+                            const bool v = e < n;
+                            cp_async_4(ab[(4 * q + e) % 8] + 128 * (4 * q + e), xb + (v ? o + e * HWi : 0), v);
                         }
                     }
                 }
-                bv[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                const int n = rbase + 16 * j;
-                if (pvalid && n < ntile)
-                    bv[j] = __ldg((const float4*)(a.dy + ((long long)b * a.Co + n0 + n) * HWo + oy * a.Wo + ox0));
-            }
-            const TcTiles<unsigned char*> t = ring.acquire(it, s);
+                // ---- dy: chunk c's 4 pixels lie in one output row (Wo % 4 == 0); lane 4 c holds the first of them
+                const int p0 = p - lane;                                   // the k-tile's first pixel
+                const int bc = __shfl_sync(0xffffffffu, b, 4 * c), remc = __shfl_sync(0xffffffffu, oy * a.Wo + ox, 4 * c);
+                const bool cvalid = p0 + 4 * c < a.P;
+                const float* dyc = dyn + (long long)bc * a.Co * HWo + remc;
+                const uint32_t bt = smem_u32(t.a_lo) + 16 * dy_idx;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int r = rbase + 16 * j, idx = tile_idx(r, c);
-                tc_split_store(t.a_hi, t.a_lo, idx, make_float4(av[j][0], av[j][1], av[j][2], av[j][3]));
-                if (r < NT) tc_split_store(t.b_hi, t.b_lo, idx, bv[j]);
-            }
-            ring.publish(s);
-        }
-    } else {
-        // ---- consumers; epilogue: row m = (tap, ci); columns == co
-        const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
-        float acc[NT / 2];
-        tc_consume<NT>(ring, nkt, wg, lane, acc);
-        float* outp = a.out + (long long)blockIdx.z * a.Co * a.Ci * KK;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int em = m0 + tc_acc_row(wg, wq, lane, half);
-            if (em >= a.Mtot) continue;
-            const int etap = em / a.cpad;
-            const int eci = em - etap * a.cpad;
-            if (eci >= a.Ci) continue;
-#pragma unroll
-            for (int i = 0; i < NT / 8; ++i)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int nl = tc_acc_col(lane, i, e);
-                    if (nl < ntile) outp[((long long)(n0 + nl) * a.Ci + eci) * KK + etap] = acc[tc_acc_reg(i, half, e)];
+                for (int j = 0; j < NT / 16; ++j) {
+                    const bool v = cvalid && n_lo + 16 * j < ntile;
+                    cp_async_16(bt + 2048 * j, v ? dyc + (long long)(16 * j) * HWo : a.dy, v);
                 }
+                p += TC_KC * 4;
+                for (ox += TC_KC * 4; ox >= a.Wo; ox -= a.Wo)
+                    if (++oy == a.Ho) { oy = 0; ++b; }
+                cp_async_arrive(&ring.full[s]);
+            }
+        }
+        cp_async_wait_all();      // no thread leaves copies in flight behind it
+    } else {
+        // ===================== consumers: MMA + epilogue; row m = (tap, ci), column = co =====================
+        wg_regs_inc<TC_CONSUMER_REGS>();
+        const int wg = (warp - TC_PRODUCERS / 32) >> 2, wq = warp & 3;
+        const int KK = a.kh * a.kw;
+        const TcWgradFeed<NT> feed = {tid - TC_PRODUCERS};
+        int g = 0;                                   // k-tiles this CTA has consumed
+        for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+            const TcUnit w = tc_unit(a, u);
+            const int ntile = min(TC_NMAX, a.Co - w.n0);
+            float acc[NT / 2];
+            tc_consume_rs<NT, TcAWgrad>(ring, g, w.nkt, wg, wq, lane, feed, acc);
+            g += w.nkt;
+            float* outp = a.out + (long long)w.z * a.Co * a.Ci * KK;
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                const int em = w.m0 + tc_acc_row(wg, wq, lane, half);
+                if (em >= a.Mtot) continue;
+                const int etap = em / a.cpad;
+                const int eci = em - etap * a.cpad;
+                if (eci >= a.Ci) continue;
+#pragma unroll
+                for (int i = 0; i < NT / 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int nl = tc_acc_col(lane, i, e);
+                        if (nl < ntile) outp[((long long)(w.n0 + nl) * a.Ci + eci) * KK + etap] = acc[tc_acc_reg(i, half, e)];
+                    }
+            }
         }
     }
 }
@@ -987,8 +983,10 @@ int tc_wgrad(const ccb_conv_desc* d, const float* x, const float* dy, float* dw,
     const long long numel = (long long)d->Co * d->Ci * d->kh * d->kw;
     int nt, wsmem;
     tc_geometry(d->Co, nt, a.b_tile_bytes, a.depth, wsmem);
-    dim3 grid(cdiv(a.Mtot, TC_M), cdiv(d->Co, TC_NMAX), a.splits);
-    int rc = tc_launch_kernel(TC_WGRAD_KERNELS, a, nt, grid, wsmem, st, "conv_tc_wgrad");
+    a.tiles_m = cdiv(a.Mtot, TC_M);
+    a.tiles_n = cdiv(d->Co, TC_NMAX);
+    a.units = a.tiles_m * a.tiles_n * splits;
+    int rc = tc_launch_kernel(TC_WGRAD_KERNELS, a, nt, tc_persistent_grid(a.units), wsmem, st, "conv_tc_wgrad");
     if (rc || a.splits == 1) return rc;
     launch_splitk_reduce(partial, dw, nullptr, nullptr, numel, splits, 1, 1, CCB_ACT_NONE, 0.f, st);
     return check_launch("conv_tc_wgrad_reduce");
