@@ -17,13 +17,18 @@
 //   cross terms first, then hi*hi) into a scratch register set; the stage's sum is added to the real accumulator with
 //   fp32 adds, so no long accumulation chain runs through the tensor core's own rounding;
 // * the producers gather the A tile once, unsplit, with zero-filling 4-byte cp.async straight from global into shared
-//   memory (fprop / dgrad: k-major, see tc_a_idx; wgrad: row-major, see TcAWgrad), several stages of loads in flight.
+//   memory (fprop / dgrad: k-major, see tc_a_idx; wgrad: row-major, see TcAWgrad), several stages of loads in flight;
+//   each copy is one wide multiply-add from a pointer and stride worked out once per tap, since below N = 128 the
+//   producers' instruction issue, not memory, is what paces the ring.
 //   Each consumer thread loads its 16 values with 16 conflict-free LDS.32, splits them and issues wgmma with A from
 //   registers (B by descriptor), so A crosses shared memory twice per stage instead of being stored twice and read
-//   three times.  The consumers load and split the next stage while the current stage's MMAs run, and take registers
-//   from the producers (setmaxnreg) to hold both;
+//   three times;
 // * mbarrier pipeline of up to 4 stages: producers -> full[s] -> consumers (wgmma, commit group, wait, fp32 add)
-//   -> empty[s];
+//   -> empty[s].  Below N = 128 the consumers double-buffer the stage sums: while one stage's MMAs run they add the
+//   previous stage's sum, release it and load and split the next stage, so the wgmma pipe is not drained between
+//   stages; they take registers from the producers (setmaxnreg) to hold two sums and two A fragments.  At N = 128,
+//   where one of each fills the registers, the two consumer warpgroups of fprop / dgrad issue their MMAs in turn
+//   (named-barrier token), so one warpgroup's wait, add and next load overlap the other's MMAs (tc_consume_rs);
 //   the epilogue adds bias / residual, applies the activation and stores NCHW straight from the accumulators.
 //
 // The same kernel serves FPROP, stride-1 DGRAD and the stride-parity classes of strided DGRAD /
@@ -34,6 +39,7 @@
 
 #include <cuda.h>            // CUtensorMap (the driver entry point is looked up at run time: no libcuda link)
 #include <cudaTypedefs.h>    // PFN_cuTensorMapEncodeTiled
+#include <type_traits>       // std::integral_constant: compile-time register-set index of tc_consume_rs
 
 namespace ccb {
 
@@ -47,8 +53,9 @@ constexpr int TC_THREADS = TC_PRODUCERS + 32 * TC_CONSUMER_WARPS;
 constexpr int TC_MAX_TAPS = 49;
 // Registers per thread of the fprop kernel: 168 at launch (384 threads at 1 CTA/SM hold 64512); from there the producers
 // hand registers to the consumers, whose A fragments stay in registers: below wgmma N = 128 a consumer thread holds acc
-// + part + the split A of the stage in flight and of the next (2 x 32).  128 x 72 + 256 x 216 = 64512.
-// With nvcc 12.9, -Xptxas -v shows no spill and no stack for any N at these counts; 64 / 224 spills the producers.
+// + two stage sums + the split A of the stage in flight and of the next (2 x 32): 160 at N = 64, as acc + part + one
+// fragment at N = 128.  128 x 72 + 256 x 216 = 64512.  With nvcc 12.9, -Xptxas -v shows no spill, no stack and no
+// serialized wgmma for any N at these counts (tests/test_conv_tc_resources.py); 64 / 224 spills the producers.
 constexpr int TC_PRODUCER_REGS = 72, TC_CONSUMER_REGS = 216;
 
 struct TcArgs {
@@ -364,24 +371,66 @@ struct TcFpropFeed {
     __device__ __forceinline__ void prep_b(const TcTiles<unsigned char*>&) const {}
 };
 
+// The token the two consumer warpgroups pass so that their MMAs reach the tensor cores in turn (tc_consume_rs, N = 128
+// fprop / dgrad): warpgroup 0 arrives on TC_BAR_WG0_ISSUED once it has issued a stage, warpgroup 1 on
+// TC_BAR_WG1_ISSUED.  Named barriers 2 and 3 (0 is __syncthreads, 1 tc_consumer_sync), each completed by the 128
+// arrivals of one warpgroup and the 128 waiting threads of the other.
+constexpr int TC_BAR_WG0_ISSUED = 2, TC_BAR_WG1_ISSUED = 3;
+template <int ID> __device__ __forceinline__ void tc_token_arrive() {
+    asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(32 * TC_CONSUMER_WARPS) : "memory");
+}
+template <int ID> __device__ __forceinline__ void tc_token_wait() {
+    asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(32 * TC_CONSUMER_WARPS) : "memory");
+}
+
+// One stage's MMAs on this warpgroup's 64 rows into `part`, zeroed first: 4 k-steps of (lo*hi) + (hi*lo), then the 4
+// (hi*hi), as one commit group.  The registers of `part` and `f` belong to the MMAs until that group is waited on.
+template <int NT>
+__device__ __forceinline__ void tc_issue_stage(const TcTiles<uint32_t>& tl, const TcAFrag& f, float (&part)[NT / 2]) {
+#pragma unroll
+    for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < TC_KC / 2; ++ks) {
+        const uint32_t koff = (uint32_t)ks * 32u;
+        wgmma_tf32_rs<NT>(part, f.lo[ks], wg_desc(tl.b_hi + koff));
+        wgmma_tf32_rs<NT>(part, f.hi[ks], wg_desc(tl.b_lo + koff));
+    }
+#pragma unroll
+    for (int ks = 0; ks < TC_KC / 2; ++ks)
+        wgmma_tf32_rs<NT>(part, f.hi[ks], wg_desc(tl.b_hi + (uint32_t)ks * 32u));
+    wg_commit();
+}
+
 // Consumer side of both kernels, A (in layout L) from registers: acc = 0 (an empty split contributes zeros), then for
-// each of the unit's `nkt` stages, 4 k-steps of (lo*hi) + (hi*lo) + (hi*hi) on this warpgroup's 64 rows into scratch
-// registers `part`, then acc += part in fp32 and the stage goes back to the producers.  Taking a full stage means
-// loading and splitting this thread's A fragment and, where Feed::split_b, its share of the B operand (prep_b, by all
-// 256 consumer threads, then made visible to wgmma: proxy fence, consumer barrier).  Below N = 128, while a stage's
-// MMAs run the thread waits for the next stage and takes it, so it releases a stage only once the next one is full.
+// each of the unit's `nkt` stages its MMAs into a scratch register set `part` (tc_issue_stage), then acc += part in
+// fp32, in stage order, and the stage goes back to the producers.  Taking a full stage means loading and splitting this
+// thread's A fragment and, where Feed::split_b, its share of the B operand (prep_b, by all 256 consumer threads, then
+// made visible to wgmma: proxy fence, consumer barrier).  B of a stage is read by its MMAs until their group is waited
+// on, so the stage is released after that wait.  The unit's k-tiles are the CTA's g-th onwards: they start in stage
+// g % depth.
+//
+// Below N = 128 the stage sums are double-buffered, part[2] with a fragment each, so the wgmma pipe is never drained
+// inside a unit: stage it goes into part[it & 1], then wg_wait<1> retires stage it - 1 alone, which is released and
+// added while stage it's MMAs run, and stage it + 1 is taken into the fragment stage it - 1 has freed.  The consumers
+// hold two stages, the one in flight and the one just taken.  The loop is unrolled by two so that it & 1 is a
+// compile-time index and both sets stay in registers, and each step is take, issue, wait, retire: the only branches
+// are the exits, so a set in flight never meets a retired one at a join, which ptxas answers by serializing every
+// wgmma (tests/test_conv_tc_resources.py).
+//
 // At N = 128 acc + part already take 128 registers and a second fragment does not fit without spilling, so each stage
-// is taken after its full barrier.  B of the current stage is read by the MMAs until the wait, so the stage is
-// released after it.  The unit's k-tiles are the CTA's g-th onwards: they start in stage g % depth.
+// is taken after the previous one's wait.  In fprop / dgrad the two warpgroups then issue in turn (`ordered`): warpgroup
+// 1 issues stage it once warpgroup 0 has, and warpgroup 0 issues stage it + 1 once warpgroup 1 has issued stage it, so
+// one warpgroup's wait, add and take overlap the other's MMAs instead of both draining the tensor cores together.  Each
+// unit ends with warpgroup 0 waiting for warpgroup 1's last token, so every arrival is matched within the unit.  In
+// wgrad prep_b's barrier keeps the two warpgroups in step at every stage, and they issue together.
 template <int NT, typename L, typename Feed>
 __device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt, int wg, int wq, int lane, const Feed& feed,
                                               float (&acc)[NT / 2]) {
-    constexpr bool split_ahead = NT < 128;
 #pragma unroll
     for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
     const uint32_t base = smem_u32(ring.smem);
     const int a_off = L::off(wg * 64 + wq * 16 + (lane >> 2), lane & 3);
-    TcAFrag cur, nxt;
     auto take = [&](int st, uint32_t ph, TcAFrag& f) {
         mbar_wait(&ring.full[st], ph);
         const TcTiles<unsigned char*> t = ring.tiles(ring.smem, st);
@@ -394,44 +443,75 @@ __device__ __forceinline__ void tc_consume_rs(const TcRing& ring, int g, int nkt
             tc_consumer_sync();
         }
     };
-    float part[NT / 2];
-    int s = g % ring.depth;                     // stage of k-tile it
-    uint32_t phase = (g / ring.depth) & 1;      // parity of k-tile it's round
-    if constexpr (split_ahead) {
-        if (nkt > 0) take(s, phase, cur);
-    }
-    for (int it = 0; it < nkt; ++it) {
-        if constexpr (!split_ahead) take(s, phase, cur);
-        const TcTiles<uint32_t> tl = ring.tiles(base, s);
-#pragma unroll
-        for (int j = 0; j < NT / 2; ++j) part[j] = 0.f;
-        wg_fence();
-#pragma unroll
-        for (int ks = 0; ks < TC_KC / 2; ++ks) {
-            const uint32_t koff = (uint32_t)ks * 32u;
-            wgmma_tf32_rs<NT>(part, cur.lo[ks], wg_desc(tl.b_hi + koff));
-            wgmma_tf32_rs<NT>(part, cur.hi[ks], wg_desc(tl.b_lo + koff));
-        }
-#pragma unroll
-        for (int ks = 0; ks < TC_KC / 2; ++ks)
-            wgmma_tf32_rs<NT>(part, cur.hi[ks], wg_desc(tl.b_hi + (uint32_t)ks * 32u));
-        wg_commit();
-        const int s1 = s + 1 == ring.depth ? 0 : s + 1;
-        const uint32_t phase1 = phase ^ (s1 == 0);
-        if constexpr (split_ahead) {
-            if (it + 1 < nkt) take(s1, phase1, nxt);
-        }
-        wg_wait<0>();
+    // after the wait that retired a stage's group: hand its sum to acc and its registers back to the compiler (the MMAs
+    // read f and wrote part until then: the fences keep the compiler from reusing or reading them before the wait)
+    auto retire = [&](int st, float (&part)[NT / 2], TcAFrag& f) {
         wg_fence_regs(part);
-        // the MMAs read cur's registers until the wait: keep the compiler from giving them to nxt or v before it
-        wg_fence_regs(cur.hi);
-        wg_fence_regs(cur.lo);
-        if (lane == 0) mbar_arrive(&ring.empty[s]);
+        wg_fence_regs(f.hi);
+        wg_fence_regs(f.lo);
+        if (lane == 0) mbar_arrive(&ring.empty[st]);
 #pragma unroll
         for (int j = 0; j < NT / 2; ++j) acc[j] += part[j];
-        if constexpr (split_ahead) cur = nxt;
-        s = s1;
-        phase = phase1;
+    };
+    int s = g % ring.depth;                     // stage of k-tile it
+    uint32_t phase = (g / ring.depth) & 1;      // parity of k-tile it's round
+    if constexpr (NT < 128) {
+        TcAFrag f[2];
+        float part[2][NT / 2];
+        int sp = s;                             // stage of k-tile it - 1
+        // k-tile it, B = it & 1: taken into f[B] and issued into part[B]; then k-tile it - 1, in flight in the other set,
+        // is retired.  The group of k-tile it is in flight at the end.
+        auto step = [&](auto B, bool first) {
+            constexpr int b = decltype(B)::value;
+            take(s, phase, f[b]);
+            tc_issue_stage<NT>(ring.tiles(base, s), f[b], part[b]);
+            if (!first) {
+                wg_wait<1>();
+                retire(sp, part[b ^ 1], f[b ^ 1]);
+            }
+            sp = s;
+            s = s + 1 == ring.depth ? 0 : s + 1;
+            phase ^= (s == 0);
+        };
+        // after the unit's last k-tile, in flight in set B
+        auto finish = [&](auto B) {
+            wg_wait<0>();
+            retire(sp, part[decltype(B)::value], f[decltype(B)::value]);
+        };
+        using Set0 = std::integral_constant<int, 0>;
+        using Set1 = std::integral_constant<int, 1>;
+        if (nkt > 0) {
+            step(Set0(), true);
+            for (int it = 1;; it += 2) {
+                if (it == nkt) { finish(Set0()); break; }
+                step(Set1(), false);
+                if (it + 1 == nkt) { finish(Set1()); break; }
+                step(Set0(), false);
+            }
+        }
+    } else {
+        constexpr bool ordered = !Feed::split_b;
+        TcAFrag f;
+        float part[NT / 2];
+        for (int it = 0; it < nkt; ++it) {
+            take(s, phase, f);
+            if constexpr (ordered) {
+                if (wg == 1) tc_token_wait<TC_BAR_WG0_ISSUED>();
+                else if (it > 0) tc_token_wait<TC_BAR_WG1_ISSUED>();
+            }
+            tc_issue_stage<NT>(ring.tiles(base, s), f, part);
+            if constexpr (ordered) {
+                if (wg == 0) tc_token_arrive<TC_BAR_WG0_ISSUED>();
+                else tc_token_arrive<TC_BAR_WG1_ISSUED>();
+            }
+            wg_wait<0>();
+            retire(s, part, f);
+            s = s + 1 == ring.depth ? 0 : s + 1;
+            phase ^= (s == 0);
+        }
+        if constexpr (ordered) {
+            if (wg == 0 && nkt > 0) tc_token_wait<TC_BAR_WG1_ISSUED>();
+        }
     }
 }
 
@@ -464,8 +544,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         // ===================== producers: thread == tile row =====================
         wg_regs_dec<TC_PRODUCER_REGS>();
         const int r = tid;
-        const int cpt = a.cpad >> 2;                 // chunks per tap
-        const int nchunks = a.ntaps * cpt;           // real chunks; the rest of Kp is zero padding
+        const int cpt = a.cpad >> 2;                 // chunks per tap; chunks of taps >= ntaps are Kp's zero padding
+        const int hwin = a.Hin * a.Win;              // channel-plane stride (a plane has < 2^31 pixels)
         if (r == 0) tma_prefetch_map(&a.wmap);
         int g = 0;                                   // k-tiles this CTA has gathered
         for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
@@ -498,48 +578,60 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 //      straight into the tile (tc_a_idx) with zeros where the im2col matrix has none.  The thread never
                 //      waits for its copies: its arrival on full[s] is made when they land, so up to `depth` stages of
                 //      loads are in flight.  The consumers read A with ld.shared, so no proxy fence is needed.
+                //      The producers issue one instruction stream per scheduler, and below N = 128 that stream is what
+                //      paces the stage ring, so each copy is one wide multiply-add from a base pointer and a
+                //      channel-plane step worked out once per tap.  A pixel without a value copies from its image's
+                //      base with step 0, and a channel past C_in from the last channel's address: every copy names a
+                //      valid address, and those copies read nothing (zero fill).
                 const int q0 = kt * TC_KC;
                 const int tap0 = q0 / cpt, c40 = q0 - tap0 * cpt;
+                // this thread's pixel under tap `tap` (Kp's zero padding past the last tap has none): the address of
+                // channel 4 c4 and the channel-plane step, 0 when there is no value
+                auto tap_src = [&](int tap, int c4, const float*& p, int& step) {
+                    const bool real = tap < a.ntaps;
+                    const int t = real ? tap : 0;
+                    const int iy = iy0 + a.off_y[t], ix = ix0 + a.off_x[t];
+                    const bool ok = mvalid && real && (unsigned)iy < (unsigned)a.Hin && (unsigned)ix < (unsigned)a.Win;
+                    p = xb + (ok ? c4 * 4 * hwin + iy * a.Win + ix : 0);
+                    step = ok ? hwin : 0;
+                };
                 if (c40 + TC_KC <= cpt) {
-                    // fast path (C_in % 32 == 0 layers): the whole stage reads one filter tap -> one bounds check,
-                    // one base pointer, 32 loads that differ only by the channel-plane stride
-                    bool ok = mvalid && tap0 < a.ntaps;
-                    int pix = 0;
-                    if (ok) {
-                        const int iy = iy0 + a.off_y[tap0], ix = ix0 + a.off_x[tap0];
-                        ok = (iy >= 0) && (iy < a.Hin) && (ix >= 0) && (ix < a.Win);
-                        pix = iy * a.Win + ix;
+                    // the whole stage reads one filter tap (C_in % 32 == 0 layers): one bounds check, one base
+                    // pointer, 32 copies one channel plane apart
+                    const float* p;
+                    int step;
+                    tap_src(tap0, c40, p, step);
+                    const int nv = a.Cin - c40 * 4;           // channels from the stage's first: >= 1
+                    if (nv >= TC_KC * 4) {
+#pragma unroll
+                        for (int k = 0; k < TC_KC * 4; ++k) cp_async_4(at + 4 * tc_a_idx(r, k), p + k * step, step != 0);
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < TC_KC * 4; ++k)
+                            cp_async_4(at + 4 * tc_a_idx(r, k), p + min(k, nv - 1) * step, step != 0 && k < nv);
                     }
-                    const float* p = ok ? xb + (long long)(c40 * 4) * HWin + pix : a.x;
-                    const int nv = ok ? (a.Cin - c40 * 4) : 0;
-#pragma unroll
-                    for (int c = 0; c < TC_KC; ++c)
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const bool v = c * 4 + j < nv;
-                            cp_async_4(at + 4 * tc_a_idx(r, 4 * c + j), v ? p + (c * 4 + j) * HWin : a.x, v);
-                        }
                 } else {
-                    int q = q0, tap = tap0, c4 = c40;
+                    // one tap per chunk of 4 channels; with C_in % 4 == 0 every chunk has its 4 channels
+                    auto chunks = [&](auto whole4) {
+                        int tap = tap0, c4 = c40;
 #pragma unroll
-                    for (int c = 0; c < TC_KC; ++c) {
-                        const float* p = a.x;
-                        int nv = 0;
-                        if (mvalid && q < nchunks) {
-                            const int iy = iy0 + a.off_y[tap], ix = ix0 + a.off_x[tap];
-                            if (iy >= 0 && iy < a.Hin && ix >= 0 && ix < a.Win) {
-                                p = xb + (long long)(c4 * 4) * HWin + (iy * a.Win + ix);
-                                nv = a.Cin - c4 * 4;
+                        for (int c = 0; c < TC_KC; ++c) {
+                            const float* p;
+                            int step;
+                            tap_src(tap, c4, p, step);
+                            const int nv = a.Cin - c4 * 4;    // >= 1: c4 < cpad / 4
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                if constexpr (decltype(whole4)::value)
+                                    cp_async_4(at + 4 * tc_a_idx(r, 4 * c + j), p + j * step, step != 0);
+                                else
+                                    cp_async_4(at + 4 * tc_a_idx(r, 4 * c + j), p + min(j, nv - 1) * step, step != 0 && j < nv);
                             }
+                            if (++c4 == cpt) { c4 = 0; ++tap; }
                         }
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const bool v = j < nv;
-                            cp_async_4(at + 4 * tc_a_idx(r, 4 * c + j), v ? p + j * HWin : a.x, v);
-                        }
-                        ++q;
-                        if (++c4 == cpt) { c4 = 0; ++tap; }
-                    }
+                    };
+                    if ((a.Cin & 3) == 0) chunks(std::true_type());
+                    else chunks(std::false_type());
                 }
                 cp_async_arrive(&ring.full[s]);
             }
