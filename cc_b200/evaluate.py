@@ -761,26 +761,38 @@ def flow_intrinsics(K, Hs, Ws, h=256, w=832, device=None):
     return torch.from_numpy(K).to(dev), torch.from_numpy(Kinv).to(dev)
 
 
-def _flow_frames(frames_u8, h, w):
+def _flow_frames(frames_u8, h, w, normalization='global'):
     """uint8 [B,F,Hs,Ws,3] -> F normalised fp32 [B,3,h,w] tensors, each frame stretched and resized as make3d_frames does
-    it (Scale hands imresize a float32 frame)."""
+    it (Scale hands imresize a float32 frame).  normalization 'global' is Normalize(.5, .5); 'local' is NormalizeLocally
+    over each sample's F frames (train.py builds its validation-flow transform with --data-normalization's normalize)."""
+    from .input_pipeline import NORMALIZATIONS, bytescale_frames, resize_frames, _prep
+    assert normalization in NORMALIZATIONS, normalization
     src = _on_library_device(frames_u8)
     assert src.dtype == torch.uint8 and src.dim() == 5 and src.size(4) == 3, (src.dtype, src.shape)
     B, F, Hs, Ws = (int(v) for v in src.shape[:4])
-    x = make3d_frames(src.reshape(B * F, Hs, Ws, 3), h, w).view(B, F, 3, h, w)
-    return [x[:, f].contiguous() for f in range(F)]
+    if normalization == 'global':
+        x = make3d_frames(src.reshape(B * F, Hs, Ws, 3), h, w).view(B, F, 3, h, w)
+        return [x[:, f].contiguous() for f in range(F)]
+    flat = src.reshape(B * F, Hs, Ws, 3)
+    if (Hs, Ws) != (h, w):
+        flat = resize_frames(bytescale_frames(flat), h, w)
+    par = torch.zeros(B, 4, device=src.device)                 # no flip, scale 1
+    par[:, 1:3] = 1.0
+    offs = torch.zeros(B, 2, dtype=torch.int32, device=src.device)
+    return _prep(flat.view(B, F, h, w, 3), par, offs, B, F, h, w, h, w, 'local')[0]
 
 
 @torch.no_grad()
 def flow_eval_batch(disp_net, pose_net, mask_net, flow_net, frames_u8, K, flow_gt, obj_map, THRESH=0.01, h=256, w=832,
-                    spatial_normalize=False, want_mask=False):
+                    spatial_normalize=False, want_mask=False, normalization='global'):
     """test_flow.py:112-140 for a batch of one frame size: frames_u8 uint8 [B,5,Hs,Ws,3] (target, then _08 _09 _11 _12),
     K the raw intrinsics [B,3,3] (or the (K, Kinv) pair flow_intrinsics returns), flow_gt [B,3,Hg,Wg], obj_map [B,Hg,Wg]
     (load_kitti_flow_samples' arrays; numpy arrays go to the library's device) -> flow_eval's fp32 [B,8] on the device
     (and the combined mask with want_mask).  The frames are stretched, resized and normalised as Scale does it, the four
     nets run at batch B (Back2Future on refs 1 and 2, another flow net on ref 2), flow_cam = pose2flow with pose[:, 2].
-    spatial_normalize: train.py's validate_flow_with_gt with --spatial-normalize.  No host synchronisation."""
-    x = _flow_frames(frames_u8, h, w)
+    spatial_normalize: train.py's validate_flow_with_gt with --spatial-normalize; normalization: its --data-normalization
+    ('global' or 'local', as _flow_frames takes it).  No host synchronisation."""
+    x = _flow_frames(frames_u8, h, w, normalization)
     Hs, Ws = int(frames_u8.shape[2]), int(frames_u8.shape[3])
     K, Kinv = K if isinstance(K, tuple) else flow_intrinsics(K, Hs, Ws, h, w, x[0].device)
     emask, flow_cam, flow_fwd = _flow_nets(disp_net, pose_net, mask_net, flow_net, x[0], x[1:], K, Kinv, spatial_normalize)

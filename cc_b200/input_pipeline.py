@@ -89,10 +89,19 @@ def rotate_affines(p, B, Hs, Ws):
     return np.array([pil_rotate_affine(ang[b], Ws, Hs) if rot[b] else IDENTITY_AFFINE for b in range(B)], np.float64)
 
 
+def to_device(a, device):
+    """A host array or tensor -> `device`.  To a GPU it goes through pinned memory, asynchronously: the host does not wait
+    for the device, and the caching host allocator keeps the pinned block until the copy has run."""
+    t = torch.as_tensor(a)
+    if torch.device(device).type == 'cuda' and not t.is_cuda:
+        t = t.pin_memory()
+    return t.to(device, non_blocking=True)
+
+
 def rotate_frames(src, affine):
     """src [B,F,H,W,3] uint8 on the device, affine [B,6] fp64 (host or device) -> rotated copy (ccb_rotate_frames_u8)."""
     B, F, H, W, _ = src.shape
-    aff = torch.as_tensor(affine, dtype=torch.float64).to(src.device, non_blocking=True).contiguous()
+    aff = to_device(torch.as_tensor(affine, dtype=torch.float64), src.device).contiguous()
     assert aff.shape == (B, 6)
     dst = torch.empty_like(src)
     _lib.call('ccb_rotate_frames_u8', src, aff, dst, B, F, H, W, src)
@@ -168,14 +177,15 @@ class DeviceAugment:
         if self.rotate:
             src = rotate_frames(src, rotate_affines(p, B, Hs, Ws))
         par = torch.from_numpy(np.stack([p['flip'], (p['scaled_w'] / Ws).astype(np.float32), (p['scaled_h'] / Hs).astype(np.float32),
-                                         np.zeros(B, np.float32)], 1).astype(np.float32)).to(self.device, non_blocking=True)
-        offs = torch.from_numpy(np.stack([p['offset_x'], p['offset_y']], 1).astype(np.int32)).to(self.device, non_blocking=True)
+                                         np.zeros(B, np.float32)], 1).astype(np.float32))
+        par = to_device(par, self.device)
+        offs = to_device(np.stack([p['offset_x'], p['offset_y']], 1).astype(np.int32), self.device)
         outs, self.stats = _prep(src, par, offs, B, F, Hs, Ws, H, W, self.normalization)
         K = augment_intrinsics(intrinsics.cpu().numpy() if torch.is_tensor(intrinsics) else intrinsics, p, Ws)
         Kinv = np.linalg.inv(K).astype(np.float32)                     # sequence_folders.py:61
         t = F // 2 if tgt_index is None else tgt_index                # sequence_folders.py:16-21: the target is the middle frame
         refs = [o for i, o in enumerate(outs) if i != t]
-        return outs[t], refs, torch.from_numpy(K).to(self.device), torch.from_numpy(Kinv).to(self.device)
+        return outs[t], refs, to_device(K, self.device), to_device(Kinv, self.device)
 
 
 def scale_intrinsics(K, Hs, Ws, h, w):

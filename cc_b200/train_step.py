@@ -223,7 +223,9 @@ class Trainer:
         self._captured = dict(lr=self.opt.lr, grad_scale=self.opt.grad_scale, fixed=self.fixed)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self.static_loss, _ = self.step(tgt, refs, K, Kinv)
+            self.static_loss, aux = self.step(tgt, refs, K, Kinv)
+        # the loss terms each replay writes (loss_2 stays the int 0 when w2 == 0), for the per-step loss log
+        self.static_terms = {k: v.detach() if torch.is_tensor(v) else v for k, v in aux.items() if k.startswith('loss_')}
         self._restore(snap)                                  # capture itself does not execute, but keep the contract explicit
         pyramid.clear()
         return self.graph
