@@ -316,6 +316,11 @@ def is_simulator():
     return _is_sim
 
 
+def device():
+    """The device the library's kernels run on: the CPU for the simulator build, else the current CUDA device."""
+    return torch.device('cpu') if is_simulator() else torch.device('cuda')
+
+
 def workspace(query, *args, like):
     """(scratch buffer, its size) for the entry point whose size query `query` is, called on `args`: fp32 for a
     `*_floats` query, uint8 for `*_bytes`, on `like`'s device; (None, 0) where nothing is needed.  A query's -1

@@ -34,6 +34,7 @@ import numpy as np
 import torch
 from .inverse_warp import pose2flow, pose_vec2mat
 from . import _lib, loss_functions as LF, models
+from .input_pipeline import device_tensor, flow_intrinsics, scale_frames
 
 
 def _to_net_input(img_hwc, device):
@@ -268,7 +269,7 @@ def kitti_flow_errors(gt_png, pred_png):
     """evaluate_flow.py compute_err (:44-53) of decoded KITTI flow images on the device (ccb_kitti_flow_errors): gt_png and
     pred_png uint16 [B,H,W,3] (or [H,W,3]; numpy arrays are copied to the current CUDA device) -> (errors fp64 [B,2] =
     aepe, Fl; counts int64 [B,2] = outliers, valid pixels), both on the device.  The script averages the per-image rows."""
-    dev = pred_png.device if torch.is_tensor(pred_png) else (torch.device('cpu') if _lib.is_simulator() else torch.device('cuda'))
+    dev = pred_png.device if torch.is_tensor(pred_png) else _lib.device()
     gt, pred = (torch.as_tensor(np.asarray(a) if not torch.is_tensor(a) else a).to(dev).contiguous() for a in (gt_png, pred_png))
     if gt.dim() == 3:
         gt, pred = gt[None], pred[None]
@@ -437,32 +438,16 @@ def load_make3d(img_file, depth_file, min_depth=1e-3, max_depth=70.0):
     return {'tgt': tgt, 'gt_depth': gt, 'mask': np.logical_and(gt > min_depth, gt < max_depth)}
 
 
-def _on_library_device(a):
-    """A tensor as it is; a numpy array copied to the library's device (the current CUDA device, or the CPU simulator)."""
-    if torch.is_tensor(a):
-        return a.contiguous()
-    dev = torch.device('cpu') if _lib.is_simulator() else torch.device('cuda')
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
 @torch.no_grad()
 def make3d_frames(crops_u8, h=256, w=256, resize=True):
     """The net input of test_make3d.py:98-106 for a batch: crops_u8 uint8 [B,Hs,Ws,3] (load_make3d's 'tgt'; numpy arrays
     go to the library's device) -> normalised fp32 [B,3,h,w] (or [B,3,Hs,Ws] without resizing).  Unless resize is False
-    or the crops already are h x w, each crop is contrast-stretched as scipy.misc.imresize stretches a float32 image
-    (input_pipeline.bytescale_frames) and resized as Pillow's BILINEAR (resize_frames); then (x/255 - 0.5)/0.5.
-    No host synchronisation."""
-    from .input_pipeline import bytescale_frames, resize_frames, _prep
-    src = _on_library_device(crops_u8)
-    assert src.dtype == torch.uint8 and src.dim() == 4 and src.size(3) == 3, (src.dtype, src.shape)
-    B, Hs, Ws = (int(v) for v in src.shape[:3])
-    if resize and (Hs, Ws) != (h, w):
-        src = resize_frames(bytescale_frames(src), h, w)
-    H, W = int(src.shape[1]), int(src.shape[2])
-    par = torch.zeros(B, 4, device=src.device)                 # no flip, scale 1 (filled on the device: capturable)
-    par[:, 1:3] = 1.0
-    offs = torch.zeros(B, 2, dtype=torch.int32, device=src.device)
-    return _prep(src, par, offs, B, 1, H, W, H, W, 'global')[0][0]
+    or the crops already are h x w, each crop is contrast-stretched and resized as scipy.misc.imresize does to a float32
+    image (input_pipeline.scale_frames); then (x/255 - 0.5)/0.5.  No host synchronisation."""
+    src = device_tensor(crops_u8)[:, None]
+    if not resize:
+        h, w = src.shape[2:4]
+    return scale_frames(src, h, w)[0][0]
 
 
 @torch.no_grad()
@@ -490,7 +475,7 @@ def make3d_eval_batch(disp_net, crops_u8, gt_depth, h=256, w=256, min_depth=1e-3
     No host synchronisation."""
     disp_net.eval()
     disp = disp_net(make3d_frames(crops_u8, h, w, resize))
-    gt = _on_library_device(gt_depth)
+    gt = device_tensor(gt_depth)
     H, W = int(gt.shape[1]), int(gt.shape[2])
     pred = spline_zoom(1 / disp[:, 0], H, W, min_depth, max_depth)
     return make3d_depth_errors(gt, pred, min_depth, max_depth)
@@ -604,7 +589,7 @@ def pose_errors(poses, gt=None, rotation_mode='euler'):
     final = torch.empty(S, L, 3, 4, device=poses.device, dtype=torch.float64)
     out = None
     if gt is not None:
-        gt = _on_library_device(gt).to(poses.device, torch.float64).contiguous()
+        gt = device_tensor(gt).to(poses.device, torch.float64).contiguous()
         assert gt.shape == (S, L, 3, 4), (gt.shape, poses.shape)
         out = torch.empty(S, 2, device=poses.device, dtype=torch.float64)
     rot = {'euler': _lib.ROT_EULER, 'quat': _lib.ROT_QUAT}[rotation_mode]
@@ -621,7 +606,7 @@ def pose_eval_batch(pose_net, frames_u8, snippets, gt_poses=None, rotation_mode=
     h x w); the snippets are gathered on the device (target = column L/2, refs = the others in order) and the pose net runs
     on all of them in one call.  No host synchronisation."""
     x = make3d_frames(frames_u8, h, w, resize)
-    idx = _on_library_device(snippets).to(x.device, torch.int64)
+    idx = device_tensor(snippets).to(x.device, torch.int64)
     L = int(idx.shape[1])
     mid = L // 2
     pose_net.eval()
@@ -750,53 +735,21 @@ def flow_eval(emask, flow_cam, flow_fwd, flow_gt, obj_map_gt, THRESH=0.01, epe_t
     return (out, mask) if want_mask else out
 
 
-def flow_intrinsics(K, Hs, Ws, h=256, w=832, device=None):
-    """ValidationFlow's intrinsics after Scale (custom_transforms.py:133-134) and their float32 inverse
-    (validation_flow.py:141), from the raw K [B,3,3] of load_kitti_flow_samples, on the host -> (K, Kinv) fp32 on
-    `device` (the library's device by default)."""
-    from .input_pipeline import scale_intrinsics
-    K = scale_intrinsics(K.cpu().numpy() if torch.is_tensor(K) else K, Hs, Ws, h, w)
-    Kinv = np.linalg.inv(K).astype(np.float32)
-    dev = device or (torch.device('cpu') if _lib.is_simulator() else torch.device('cuda'))
-    return torch.from_numpy(K).to(dev), torch.from_numpy(Kinv).to(dev)
-
-
-def _flow_frames(frames_u8, h, w, normalization='global'):
-    """uint8 [B,F,Hs,Ws,3] -> F normalised fp32 [B,3,h,w] tensors, each frame stretched and resized as make3d_frames does
-    it (Scale hands imresize a float32 frame).  normalization 'global' is Normalize(.5, .5); 'local' is NormalizeLocally
-    over each sample's F frames (train.py builds its validation-flow transform with --data-normalization's normalize)."""
-    from .input_pipeline import NORMALIZATIONS, bytescale_frames, resize_frames, _prep
-    assert normalization in NORMALIZATIONS, normalization
-    src = _on_library_device(frames_u8)
-    assert src.dtype == torch.uint8 and src.dim() == 5 and src.size(4) == 3, (src.dtype, src.shape)
-    B, F, Hs, Ws = (int(v) for v in src.shape[:4])
-    if normalization == 'global':
-        x = make3d_frames(src.reshape(B * F, Hs, Ws, 3), h, w).view(B, F, 3, h, w)
-        return [x[:, f].contiguous() for f in range(F)]
-    flat = src.reshape(B * F, Hs, Ws, 3)
-    if (Hs, Ws) != (h, w):
-        flat = resize_frames(bytescale_frames(flat), h, w)
-    par = torch.zeros(B, 4, device=src.device)                 # no flip, scale 1
-    par[:, 1:3] = 1.0
-    offs = torch.zeros(B, 2, dtype=torch.int32, device=src.device)
-    return _prep(flat.view(B, F, h, w, 3), par, offs, B, F, h, w, h, w, 'local')[0]
-
-
 @torch.no_grad()
 def flow_eval_batch(disp_net, pose_net, mask_net, flow_net, frames_u8, K, flow_gt, obj_map, THRESH=0.01, h=256, w=832,
                     spatial_normalize=False, want_mask=False, normalization='global'):
     """test_flow.py:112-140 for a batch of one frame size: frames_u8 uint8 [B,5,Hs,Ws,3] (target, then _08 _09 _11 _12),
-    K the raw intrinsics [B,3,3] (or the (K, Kinv) pair flow_intrinsics returns), flow_gt [B,3,Hg,Wg], obj_map [B,Hg,Wg]
-    (load_kitti_flow_samples' arrays; numpy arrays go to the library's device) -> flow_eval's fp32 [B,8] on the device
-    (and the combined mask with want_mask).  The frames are stretched, resized and normalised as Scale does it, the four
+    K the raw intrinsics [B,3,3] (or the (K, Kinv) pair flow_intrinsics returns), flow_gt [B,3,Hg,Wg],
+    obj_map [B,Hg,Wg] (load_kitti_flow_samples' arrays; numpy arrays go to the library's device) -> flow_eval's fp32 [B,8]
+    on the device (and the combined mask with want_mask).  The frames go through scale_frames (Scale), the four
     nets run at batch B (Back2Future on refs 1 and 2, another flow net on ref 2), flow_cam = pose2flow with pose[:, 2].
     spatial_normalize: train.py's validate_flow_with_gt with --spatial-normalize; normalization: its --data-normalization
-    ('global' or 'local', as _flow_frames takes it).  No host synchronisation."""
-    x = _flow_frames(frames_u8, h, w, normalization)
+    ('global' or 'local', as scale_frames takes it).  No host synchronisation."""
+    x, _ = scale_frames(frames_u8, h, w, normalization)
     Hs, Ws = int(frames_u8.shape[2]), int(frames_u8.shape[3])
     K, Kinv = K if isinstance(K, tuple) else flow_intrinsics(K, Hs, Ws, h, w, x[0].device)
     emask, flow_cam, flow_fwd = _flow_nets(disp_net, pose_net, mask_net, flow_net, x[0], x[1:], K, Kinv, spatial_normalize)
-    return flow_eval(emask, flow_cam, flow_fwd, _on_library_device(flow_gt), _on_library_device(obj_map), THRESH,
+    return flow_eval(emask, flow_cam, flow_fwd, device_tensor(flow_gt), device_tensor(obj_map), THRESH,
                      want_mask=want_mask)
 
 
@@ -805,10 +758,10 @@ def back2future_eval_batch(flow_net, frames_u8, flow_gt, obj_map, h=256, w=832):
     """test_back2future.py on KITTI-2015 for a batch of one frame size (frames, flow_gt and obj_map as flow_eval_batch takes
     them; the script's nlevels 5 and 6 give the same eval output from the same checkpoint) -> fp32 [B,4] on the device =
     compute_all_epes(gt, fwd, fwd, 1 - obj).  No host synchronisation."""
-    x = _flow_frames(frames_u8, h, w)
+    x, _ = scale_frames(frames_u8, h, w)
     flow_net.eval()
     flow_fwd = flow_net(x[0], x[2:4])[0]
-    return flow_eval(None, None, flow_fwd, _on_library_device(flow_gt), _on_library_device(obj_map))
+    return flow_eval(None, None, flow_fwd, device_tensor(flow_gt), device_tensor(obj_map))
 
 
 def load_flow_eval_nets(pretrained_disp, pretrained_pose, pretrained_mask, pretrained_flow, dispnet='DispResNet6',

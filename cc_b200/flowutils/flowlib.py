@@ -19,8 +19,7 @@ def flow_to_image(flow):
         return flow_colors(flow[None, None])[0]
     flow = np.asarray(flow)
     assert flow.ndim == 3 and flow.shape[0] == 2, flow.shape
-    dev = torch.device('cpu') if _lib.is_simulator() else torch.device('cuda')
-    levels = flow_colors(torch.from_numpy(np.ascontiguousarray(flow, np.float32))[None, None].to(dev))[0]
+    levels = flow_colors(torch.from_numpy(np.ascontiguousarray(flow, np.float32))[None, None].to(_lib.device()))[0]
     return levels.cpu().numpy() / 255.
 
 

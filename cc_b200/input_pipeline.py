@@ -19,12 +19,13 @@ The reference's other transforms run on the device as well, bit-exact with Pillo
   * NormalizeLocally (custom_transforms.py:33-44, --data-normalization local): normalization='local' writes v/255
     (ccb_prep_frames_unit) and normalises each sample by its own per-channel mean and unbiased std over all its frames
     (ccb_normalize_local);
-  * Scale(h, w) (custom_transforms.py:120-137, the validation-flow transform, train.py:189-190): DeviceScale resamples
-    the uint8 frames as Pillow's BILINEAR resize does (ccb_resize_u8, antialiased on a downscale), then normalises.
-The reference's loaders hand scipy.misc float32 copies of the uint8 frames (load_as_float), and scipy.misc byte-scales a
-float image to its own [min, max] before resampling; this pipeline takes the uint8 frames as they are, which is the
-same whenever a frame spans 0..255.  bytescale_frames restates that stretch where an evaluation needs it (Make3D,
-cc_b200.evaluate.make3d_frames)."""
+  * Scale(h, w) (custom_transforms.py:120-137, the validation-flow transform, train.py:189-190): scale_frames, behind
+    DeviceScale, the validations and every evaluation's net input, stretches each uint8 frame to its own [min, max]
+    (ccb_bytescale_u8), as scipy.misc.imresize does to the float32 copy the reference's loaders hand it (load_as_float),
+    resamples it as Pillow's BILINEAR resize does (ccb_resize_u8, antialiased on a downscale), then normalises.
+Documented deviation: scale_frames passes frames that already are h x w through as they are, as the reference's
+evaluation scripts do (test_make3d.py:101, test_pose.py:54); its Scale would imresize them too, which stretches a frame
+that does not span 0..255."""
 import math
 import random
 import numpy as np
@@ -96,6 +97,13 @@ def to_device(a, device):
     if torch.device(device).type == 'cuda' and not t.is_cuda:
         t = t.pin_memory()
     return t.to(device, non_blocking=True)
+
+
+def device_tensor(a):
+    """A tensor as it is (contiguous); a numpy array copied to the library's device (_lib.device())."""
+    if torch.is_tensor(a):
+        return a.contiguous()
+    return torch.from_numpy(np.ascontiguousarray(a)).to(_lib.device())
 
 
 def rotate_frames(src, affine):
@@ -196,12 +204,38 @@ def scale_intrinsics(K, Hs, Ws, h, w):
     return K
 
 
+def flow_intrinsics(K, Hs, Ws, h=256, w=832, device=None):
+    """ValidationFlow's intrinsics after Scale (scale_intrinsics) and their float32 inverse (validation_flow.py:137),
+    computed on the host from the raw K [B,3,3] -> (K, Kinv) fp32 on `device` (the library's device by default)."""
+    K = scale_intrinsics(K.cpu().numpy() if torch.is_tensor(K) else K, Hs, Ws, h, w)
+    Kinv = np.linalg.inv(K).astype(np.float32)
+    dev = device or _lib.device()
+    return torch.from_numpy(K).to(dev), torch.from_numpy(Kinv).to(dev)
+
+
+def scale_frames(frames_u8, h, w, normalization='global'):
+    """Compose([Scale(h, w), ArrayToTensor(), normalize]) on the frames: uint8 [B,F,Hs,Ws,3] (a numpy array goes to the
+    library's device) -> F tensors [B,3,h,w] and the 'local' statistics (None for 'global'), as _prep returns them.
+    Where (Hs, Ws) != (h, w) each frame is stretched (bytescale_frames) and resized (resize_frames) as imresize does to
+    a float32 frame; frames already h x w go through as they are.  The identity lookup parameters are filled on the
+    device, so the call makes no host synchronisation and can be captured in a CUDA graph."""
+    assert normalization in NORMALIZATIONS, normalization
+    src = device_tensor(frames_u8)
+    assert src.dtype == torch.uint8 and src.dim() == 5 and src.size(4) == 3, (src.dtype, src.shape)
+    B, F, Hs, Ws = (int(v) for v in src.shape[:4])
+    if (Hs, Ws) != (h, w):
+        src = resize_frames(bytescale_frames(src), h, w)
+    par = torch.zeros(B, 4, device=src.device)                 # no flip, scale 1
+    par[:, 1:3] = 1.0
+    offs = torch.zeros(B, 2, dtype=torch.int32, device=src.device)
+    return _prep(src, par, offs, B, F, h, w, h, w, normalization)
+
+
 class DeviceScale:
     """The validation-flow transform Compose([Scale(h, w), ArrayToTensor(), normalize]) (train.py:189-190):
-    frames_u8 [B,F,Hs,Ws,3] uint8 + intrinsics [B,3,3] -> (tgt, refs, K, Kinv) on `device`.  The frames are resampled as
-    Pillow's BILINEAR resize (antialiased when shrinking, as KITTI's ~375x1242 frames are to 256x832), then normalised
-    ('global' or 'local', as DeviceAugment).  K and K^-1 in float32 as custom_transforms.py:133-134 and
-    datasets/validation_flow.py:137 compute them.  The target is frame 0: validation_flow.py:130-133 orders the frames
+    frames_u8 [B,F,Hs,Ws,3] uint8 + intrinsics [B,3,3] -> (tgt, refs, K, Kinv) on `device`.  The frames go through
+    scale_frames ('global' or 'local', as DeviceAugment; the statistics of the last 'local' call are kept in
+    `self.stats`), K and K^-1 through flow_intrinsics.  The target is frame 0: validation_flow.py:130-133 orders the frames
     [tgt] + refs."""
 
     def __init__(self, device, h=256, w=832, normalization='global'):
@@ -209,14 +243,8 @@ class DeviceScale:
         self.device, self.h, self.w, self.normalization, self.stats = torch.device(device), h, w, normalization, None
 
     def __call__(self, frames_u8, intrinsics, tgt_index=0):
-        assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 5 and frames_u8.size(4) == 3
-        B, F, Hs, Ws, _ = frames_u8.shape
-        h, w = self.h, self.w
-        src = resize_frames(frames_u8.to(self.device, non_blocking=True).contiguous(), h, w)
-        par = torch.tensor([[0.0, 1.0, 1.0, 0.0]] * B, device=self.device)
-        offs = torch.zeros(B, 2, dtype=torch.int32, device=self.device)
-        outs, self.stats = _prep(src, par, offs, B, F, h, w, h, w, self.normalization)
-        K = scale_intrinsics(intrinsics.cpu().numpy() if torch.is_tensor(intrinsics) else intrinsics, Hs, Ws, h, w)
-        Kinv = np.linalg.inv(K).astype(np.float32)                     # validation_flow.py:137
+        Hs, Ws = frames_u8.shape[2:4]
+        outs, self.stats = scale_frames(frames_u8.to(self.device, non_blocking=True), self.h, self.w, self.normalization)
+        K, Kinv = flow_intrinsics(intrinsics, Hs, Ws, self.h, self.w, self.device)
         refs = [o for i, o in enumerate(outs) if i != tgt_index]
-        return outs[tgt_index], refs, torch.from_numpy(K).to(self.device), torch.from_numpy(Kinv).to(self.device)
+        return outs[tgt_index], refs, K, Kinv

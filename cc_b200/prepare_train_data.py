@@ -361,8 +361,8 @@ def main(argv=None, device=None):
     process is joined before it returns or raises."""
     args = parse_args(sys.argv[1:] if argv is None else argv)
     if device is None:
-        from .train import default_device
-        device = default_device()
+        from . import _lib
+        device = _lib.device()
     units, scenes_of = scene_sources(args)
     os.makedirs(args.dump_root, exist_ok=True)
     pool = multiprocessing.get_context('spawn').Pool(args.num_threads)

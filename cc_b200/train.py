@@ -29,7 +29,7 @@ import numpy as np
 import torch
 
 from . import _lib, pyramid, loss_functions as LF, evaluate as EV
-from .input_pipeline import DeviceAugment, draw_params, to_device
+from .input_pipeline import DeviceAugment, draw_params, scale_frames, to_device
 from .train_step import Trainer, HostFeeder, FLOWNETS
 
 SEQUENCE_LENGTH = 5
@@ -351,15 +351,15 @@ def run_epoch(trainer, loader, params, aug, log, print_freq=10, full_log=None, p
 # ---- validation ------------------------------------------------------------------------------------------------------
 @torch.no_grad()
 def validate_depth(disp_net, loader, device, normalization='global'):
-    """validate_depth_with_gt: the disp net in eval mode at batch B on the validation transform, 1 / disp, then
-    compute_errors(gt, depth.squeeze(1)); the six metrics summed on the device in batch order and divided by the count
-    (AverageMeter over 0-dim fp32 tensors) -> list of six 0-dim device tensors.  The net is left in eval mode."""
-    aug = DeviceAugment(device, flip=False, scale_crop=False, normalization=normalization)
+    """validate_depth_with_gt: the disp net in eval mode at batch B on the validation transform (ArrayToTensor and
+    normalize: scale_frames at the frames' own size), 1 / disp, then compute_errors(gt, depth.squeeze(1)); the six
+    metrics summed on the device in batch order and divided by the count (AverageMeter over 0-dim fp32 tensors) -> list
+    of six 0-dim device tensors.  The net is left in eval mode."""
     disp_net.eval()
     acc, count = torch.zeros(6, device=device), 0
     for frames, depth in loader:
-        B = frames.shape[0]
-        tgt, _, _, _ = aug(to_device(frames, device), np.tile(np.eye(3, dtype=np.float32), (B, 1, 1)))
+        H, W = frames.shape[2:4]
+        tgt = scale_frames(to_device(frames, device), H, W, normalization)[0][0]
         out = 1 / disp_net(tgt)
         acc += torch.stack(LF.compute_errors(to_device(depth, device), out.squeeze(1)))
         count += 1
@@ -490,14 +490,10 @@ def hyper_parameters(args):
                 beta1=args.momentum, beta2=args.beta, smoothness=args.smoothness_type)
 
 
-def default_device():
-    return torch.device('cpu') if _lib.is_simulator() else torch.device('cuda')
-
-
 def main(argv=None, device=None):
     """train.py main(): returns dict(save_path, train_losses, decisive_errors, trainer)."""
     args = parse_args(sys.argv[1:] if argv is None else argv)
-    dev = device or default_device()
+    dev = device or _lib.device()
     cuda = dev.type == 'cuda'
     save_path = os.path.join('checkpoints', args.name)
     print('=> will save everything to {}'.format(save_path))

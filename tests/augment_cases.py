@@ -1,6 +1,6 @@
 """Cases for the reference's remaining data transforms on the device (cc_b200.input_pipeline: RandomRotate, NormalizeLocally,
-Scale), against the fixture frozen from the reference (tests/golden/make_augment.py) and against the numpy restatements of
-Pillow (tests/augment_oracle.py).  Run by tests/test_augment.py on the CPU simulator and tests/test_gpu_augment.py on the
+Scale), against the fixture frozen from the reference (tests/golden/make_augment.py), against the numpy restatements of
+Pillow (tests/augment_oracle.py) and against oracle/make3d_eval.py's imresize.  Run by tests/test_augment.py on the CPU simulator and tests/test_gpu_augment.py on the
 H100.  The rotate and resize kernels are bit-exact with Pillow, so their bytes are compared with np.array_equal."""
 import random
 import numpy as np
@@ -126,8 +126,40 @@ def case_scale_transform_golden(device):
         assert np.array_equal(Kinv.cpu().numpy(), np.linalg.inv(g[name + '_K']))
 
 
+class _Net(torch.nn.Module):
+    """Stands in for one of flow_eval_batch's nets: records the inputs of each call and returns `out`."""
+
+    def __init__(self, out):
+        super().__init__()
+        self.out, self.calls = out, []
+
+    def forward(self, *args):
+        self.calls.append(args)
+        return self.out
+
+
+def case_scale_low_contrast(device, B=2, F=5, Hs=80, Ws=200, h=64, w=192, seed=9):
+    """(e) Scale on frames of 40..180, which imresize stretches to 0..255 before it resamples: DeviceScale's frames are
+    the frames flow_eval_batch hands its nets, bit for bit, and equal the oracle's imresize, normalised."""
+    from cc_b200 import evaluate as CE
+    from oracle import make3d_eval as OM
+    frames = np.random.RandomState(seed).randint(40, 181, size=(B, F, Hs, Ws, 3)).astype(np.uint8)
+    K = np.tile(np.array([[120.0, 0, 100.0], [0, 120.0, 40.0], [0, 0, 1]], np.float32), (B, 1, 1))
+    tgt, refs, _, _ = CI.DeviceScale(device, h, w)(torch.from_numpy(frames), K)
+    out = _stack(tgt, refs, 0)
+    pose = _Net(torch.zeros(B, F - 1, 6, device=device))
+    nets = [_Net(torch.ones(B, 1, h, w, device=device)), pose, _Net(torch.ones(B, F - 1, h, w, device=device)),
+            _Net(torch.zeros(B, 2, h, w, device=device))]
+    gt, obj = torch.ones(B, 3, Hs, Ws, device=device), torch.ones(B, Hs, Ws, device=device)
+    CE.flow_eval_batch(*nets, torch.from_numpy(frames).to(device), K, gt, obj, h=h, w=w)
+    fed = _stack(*pose.calls[0], 0)
+    assert np.array_equal(out, fed), 'DeviceScale against flow_eval_batch: max err %.3e' % np.abs(out - fed).max()
+    want = np.stack([np.concatenate([OM.net_input(frames[b, f], h, w) for f in range(F)]) for b in range(B)])
+    assert np.array_equal(out, want), 'DeviceScale against imresize: max err %.3e' % np.abs(out - want).max()
+
+
 AUGMENT_CASES = [case_rotate_kernel_fixture, case_resize_kernel_fixture, case_rotate_transform_golden, case_full_transform_golden,
-                 case_local_transform_golden, case_scale_transform_golden]
+                 case_local_transform_golden, case_scale_transform_golden, case_scale_low_contrast]
 
 
 # ---- full size, against the numpy restatements (no reference and no Pillow needed) -----------------------------------
@@ -183,7 +215,8 @@ def case_rotate_fullsize(device, B=4, F=5, H=256, W=832, seed=7):
 
 def case_scale_fullsize(device, F=5, Hs=375, Ws=1242, h=256, w=832, seed=8):
     """One KITTI-2015-sized sample (5 x 375x1242) to 256x832: resized bytes equal the oracle's, the normalised frames are
-    exactly (v/255 - .5)/.5 of them, and a repeat call gives the same bytes."""
+    exactly (v/255 - .5)/.5 of them, and a repeat call gives the same bytes.  Scaled to its own size, the sample goes
+    through unchanged: frames exactly (v/255 - .5)/.5 of the input, K as it was."""
     rs = np.random.RandomState(seed)
     frames = rs.randint(0, 256, size=(1, F, Hs, Ws, 3)).astype(np.uint8)
     src = torch.from_numpy(frames).to(device)
@@ -196,3 +229,7 @@ def case_scale_fullsize(device, F=5, Hs=375, Ws=1242, h=256, w=832, seed=8):
     out = _stack(tgt, refs, 0)
     assert np.array_equal(out, (_unit(want) - np.float32(0.5)) / np.float32(0.5))
     assert np.array_equal(Kd.cpu().numpy(), CI.scale_intrinsics(K, Hs, Ws, h, w))
+    tgt, refs, Kd, _ = CI.DeviceScale(device, Hs, Ws)(src, K)
+    out = _stack(tgt, refs, 0)
+    assert np.array_equal(out, (_unit(frames) - np.float32(0.5)) / np.float32(0.5)), 'equal size is not the identity'
+    assert np.array_equal(Kd.cpu().numpy(), K)

@@ -5,7 +5,7 @@ frames, nets and kernel chain inside a CUDA graph."""
 import numpy as np
 import pytest
 import torch
-from cc_b200 import evaluate as CE, models as CM, synth
+from cc_b200 import evaluate as CE, input_pipeline as CI, models as CM, synth
 from oracle import flow_eval as OF, make3d_eval as OM
 from tests import flow_eval_cases as FC
 from tests.util import assert_graph_replays, device_lib      # noqa: F401  (module fixture: the sm_90a library)
@@ -79,7 +79,7 @@ def test_back2future_eval_batch_against_oracle():
     gt, obj = _ground_truth(B, Hs, Ws, seed=13)
     net = _nets('Back2Future')[3]
     out = CE.back2future_eval_batch(net, frames, gt, obj, h, w).cpu().numpy()
-    x = CE._flow_frames(frames, h, w)
+    x, _ = CI.scale_frames(frames, h, w)
     fwd = net(x[0], x[2:4])[0].cpu()
     for k in range(B):
         want = OF.back2future_errors(fwd[k:k + 1], torch.from_numpy(gt[k:k + 1]), torch.from_numpy(obj[k:k + 1]))

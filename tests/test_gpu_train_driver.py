@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from cc_b200 import train as T, nn as cnn, evaluate as EV, loss_functions as LF
-from cc_b200.input_pipeline import DeviceAugment
+from cc_b200.input_pipeline import DeviceAugment, scale_frames
 from cc_b200.train_step import Trainer
 from oracle import metrics as OM
 from tests import train_cases as TC, flow_eval_cases as FC
@@ -265,8 +265,8 @@ def test_flow_validation(tmp_path):
     assert not torch.equal(avgs['global'], avgs['local'])
     # NormalizeLocally (custom_transforms.py:33-44) restated in fp64 on the globally normalised frames of one batch
     s = EV.load_kitti_flow_samples(fw, fw['groups'][next(iter(fw['groups']))][:2])
-    glob = EV._flow_frames(s['frames'], 256, 832, 'global')
-    loc = EV._flow_frames(s['frames'], 256, 832, 'local')
+    glob, _ = scale_frames(s['frames'], 256, 832, 'global')
+    loc, _ = scale_frames(s['frames'], 256, 832, 'local')
     v = torch.stack(glob, 1).double() * 0.5 + 0.5                      # [B,F,3,h,w] in [0, 1]
     flat = v.transpose(1, 2).reshape(v.shape[0], 3, -1)
     want = (v - flat.mean(2)[:, None, :, None, None]) / flat.std(2)[:, None, :, None, None]

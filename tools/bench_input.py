@@ -2,7 +2,8 @@
 """Developer micro-benchmark of the on-device input transforms (not bench.py): CUDA-event time per call after warm-up of
   * the train transform (cc_b200.input_pipeline.DeviceAugment: flip + scale-crop + normalise) at b4 x 5 frames x 256x832,
     rotation off / on (every sample rotated) x normalisation global / local;
-  * the validation Scale (DeviceScale) of one KITTI-2015-sized sample, 5 x 375x1242 -> 256x832.
+  * the validation Scale (DeviceScale: imresize's contrast stretch, Pillow's BILINEAR resize, normalise) of one
+    KITTI-2015-sized sample, 5 x 375x1242 -> 256x832.
 The uint8 frames are on the device before the timed window (the H2D copy is not timed).  Each row reports the
 algorithmic bytes (uint8 frames in + fp32 frames out) and that over the time, against the H100 SXM data sheet's
 3.35 TB/s, and the time the same batch takes on the host through Pillow (or, where Pillow is not installed, through the
@@ -20,6 +21,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from cc_b200 import input_pipeline as CI   # noqa: E402
+from oracle.make3d_eval import bytescale   # noqa: E402
 from tools.card import card                # noqa: E402
 
 PEAK_BW = 3.35e12      # H100 SXM HBM3, data sheet
@@ -125,8 +127,8 @@ def main():
                GBps=alg / (ms * 1e-3) / 1e9, share_of_3p35TBps=alg / (ms * 1e-3) / PEAK_BW)
     if args.host:
         def host_scale():
-            return [(torch.from_numpy(np.transpose(resize_fn(vframes[0, f], h, w), (2, 0, 1)).copy()).float() / 255 - 0.5) / 0.5
-                    for f in range(Fv)]
+            return [(torch.from_numpy(np.transpose(resize_fn(bytescale(vframes[0, f]), h, w), (2, 0, 1)).copy()).float() / 255
+                     - 0.5) / 0.5 for f in range(Fv)]
         row['host_ms'] = host_time(host_scale)
     res['rows']['valid_scale_global'] = row
     print(json.dumps(res, indent=1))
