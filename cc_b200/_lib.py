@@ -170,6 +170,9 @@ _SIGS = {
                               'int, int, float, float, float, float, float*, void*, long long, float*, ccb_stream_t'),
     'ccb_flow_color_workspace_bytes': ('long long', 'int, int, int, int'),
     'ccb_flow_color': (STATUS, 'const float*, int, int, int, int, void*, long long, unsigned char*, ccb_stream_t'),
+    'ccb_colorize_workspace_bytes': ('long long', 'int, int, int, int'),
+    'ccb_colorize': (STATUS, 'const float*, int, int, int, const unsigned char*, int, int, int, float, void*, long long, '
+                             'unsigned char*, ccb_stream_t'),
     'ccb_kitti_flow_errors_workspace_bytes': ('long long', 'int, int, int'),
     'ccb_kitti_flow_errors': (STATUS, 'const unsigned short*, const unsigned short*, int, int, int, void*, long long, '
                                       'double*, long long*, ccb_stream_t'),
@@ -191,6 +194,8 @@ _SIGS = {
                                 'int, int, ccb_stream_t'),
     'ccb_prep_frames_unit': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '
                                      'int, int, int, ccb_stream_t'),
+    'ccb_prep_frames_inference': (STATUS, 'const unsigned char*, float* const*, const float*, const int*, int, int, int, '
+                                          'int, int, int, ccb_stream_t'),
     'ccb_rotate_frames_u8': (STATUS, 'const unsigned char*, const double*, unsigned char*, int, int, int, int, '
                                      'ccb_stream_t'),
     'ccb_resize_u8_workspace_bytes': ('long long', 'int, int, int, int, int'),

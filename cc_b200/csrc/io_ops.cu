@@ -17,6 +17,7 @@
 //       pose evaluation of test_pose.py / test_sintel_pose.py: the snippet's pose algebra, ATE and RE, one thread per snippet
 //       KITTI-2015 flow evaluation of test_flow.py:112-140 / test_back2future.py: the combined mask and both
 //       compute_all_epes per sample, on the flow metrics' per-pixel body
+//       run_inference.py's images: utils.py tensor2array's colormaps through host-built uint8 tables
 //
 // All floating-point reductions are two-stage and deterministic (per-block partials in double, fixed-order finalize); the
 // segmentation counts are integer sums (atomics, the same in any order).
@@ -414,8 +415,10 @@ struct PrepArgs {
     int B, F, Hs, Ws, H, W;
 };
 
-// UNIT: ArrayToTensor alone (v / 255), for NormalizeLocally to follow; otherwise Normalize(.5, .5) as well.
-template <bool UNIT>
+// The value written: Normalize(.5, .5) after ArrayToTensor; ArrayToTensor alone (v / 255), for NormalizeLocally to follow;
+// or run_inference.py's (v / 255 - 0.5) / 0.2.  Each operation is one IEEE fp32 operation.
+enum PrepNorm { PREP_HALF, PREP_UNIT, PREP_FIFTH };
+template <int NORM>
 __global__ void __launch_bounds__(256) prep_frames_kernel(const PrepArgs a) {
     CCB_PDL_WAIT();
     const long long n = (long long)a.B * a.F * a.H * a.W;
@@ -441,7 +444,7 @@ __global__ void __launch_bounds__(256) prep_frames_kernel(const PrepArgs a) {
             const float v00 = (float)s[((long long)y0 * a.Ws + xa) * 3 + c], v01 = (float)s[((long long)y0 * a.Ws + xb) * 3 + c];
             const float v10 = (float)s[((long long)y1 * a.Ws + xa) * 3 + c], v11 = (float)s[((long long)y1 * a.Ws + xb) * 3 + c];
             const float v = (1.f - wy) * ((1.f - wx) * v00 + wx * v01) + wy * ((1.f - wx) * v10 + wx * v11);
-            d[(long long)c * a.H * a.W] = UNIT ? v / 255.f : (v / 255.f - 0.5f) / 0.5f;
+            d[(long long)c * a.H * a.W] = NORM == PREP_UNIT ? v / 255.f : (v / 255.f - 0.5f) / (NORM == PREP_HALF ? 0.5f : 0.2f);
         }
     }
 }
@@ -1010,6 +1013,64 @@ __global__ void __launch_bounds__(256) flow_color_kernel(const FlowColorArgs a) 
             const double level = floor(__dmul_rn(__dmul_rn(255.0, col), nan ? 0.0 : 1.0));
             o[c * n] = unknown ? (unsigned char)0 : (unsigned char)(int)level;
         }
+    }
+}
+
+// ================================================================================================
+// Colormaps of utils.py tensor2array (:36-53) as run_inference.py saves them, (255 * tensor2array(x, max_value,
+// colormap)).astype(uint8), through matplotlib's Colormap.__call__ on the float32 array:
+//   x = 1 / x first when inverted (depth from disparity); q = x / max, t = q * N, each rounded in fp32
+//   NaN -> black (the bad colour); t < 0 -> lut[0] (under); t >= N -> lut[N-1] (t == N, and over); else lut[trunc(t)]
+// The float tail, trunc(fp32(255 * fp32(lut64[i]))), is the host-built uint8 table lut [N,3].  max is the fixed value, or
+// each image's own maximum (tensor.max(): any NaN makes it NaN), taken as order-preserving keys with integer atomics.
+struct ColorizeArgs {
+    const float* maps;              // [B, H, W]
+    const unsigned char* lut;       // [N, 3]
+    unsigned long long* maxkey;     // [B]: ordered_key32 of the image's maximum, ~0 for NaN (per-image scale only)
+    unsigned char* out;             // [B, H, W, 3]
+    long long hw;
+    int N, invert;
+    float max_value;                // the fixed scale when maxkey is null
+};
+
+__device__ __forceinline__ float colorize_value(const ColorizeArgs& a, long long i) {
+    const float x = __ldg(a.maps + i);
+    return a.invert ? __fdiv_rn(1.f, x) : x;
+}
+
+__global__ void __launch_bounds__(256) colorize_max_kernel(const ColorizeArgs a) {
+    CCB_PDL_WAIT();
+    const long long base = (long long)blockIdx.y * a.hw;
+    unsigned long long m = 0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < a.hw; i += (long long)gridDim.x * 256) {
+        const float v = colorize_value(a, base + i);
+        const unsigned long long k = (v != v) ? ~0ull : (unsigned long long)ordered_key32(v);
+        m = (k > m) ? k : m;
+    }
+    warp_max_into(a.maxkey + blockIdx.y, m);
+}
+
+__global__ void __launch_bounds__(256) colorize_kernel(const ColorizeArgs a) {
+    CCB_PDL_WAIT();
+    const long long base = (long long)blockIdx.y * a.hw;
+    float mx = a.max_value;
+    if (a.maxkey) {
+        const unsigned long long k = a.maxkey[blockIdx.y];
+        mx = (k == ~0ull) ? __uint_as_float(0x7fc00000u) : ordered_value32((unsigned)k);
+    }
+    const float n = (float)a.N;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < a.hw; i += (long long)gridDim.x * 256) {
+        const float t = __fmul_rn(__fdiv_rn(colorize_value(a, base + i), mx), n);
+        unsigned char* o = a.out + (base + i) * 3;
+        if (t != t) {
+            o[0] = o[1] = o[2] = 0;
+            continue;
+        }
+        const int idx = (t < 0.f) ? 0 : (t >= n ? a.N - 1 : (int)t);
+        const unsigned char* c = a.lut + 3 * idx;
+        o[0] = __ldg(c);
+        o[1] = __ldg(c + 1);
+        o[2] = __ldg(c + 2);
     }
 }
 
@@ -1723,6 +1784,30 @@ extern "C" int ccb_flow_color(const float* flow, int B, int P, int H, int W, voi
     return check_launch("flow_color");
 }
 
+extern "C" long long ccb_colorize_workspace_bytes(int B, int H, int W, int per_image_max) {
+    if (B <= 0 || H <= 0 || W <= 0) return -1;
+    return per_image_max ? (long long)B * (long long)sizeof(unsigned long long) : 0;
+}
+
+extern "C" int ccb_colorize(const float* maps, int B, int H, int W, const unsigned char* lut, int N, int invert, int per_image_max,
+                            float max_value, void* work, long long work_bytes, unsigned char* out, ccb_stream_t stream) {
+    CCB_REQUIRE(maps && lut && out, CCB_ERR_ARG, "colorize: null pointer");
+    CCB_REQUIRE(B > 0 && H > 0 && W > 0, CCB_ERR_ARG, "colorize: bad sizes");
+    CCB_REQUIRE(N > 0 && N <= (1 << 24), CCB_ERR_ARG, "colorize: the table needs 1 .. 2^24 entries, got %d", N);
+    const long long need = ccb_colorize_workspace_bytes(B, H, W, per_image_max);
+    CCB_REQUIRE_WORK("colorize", "work", work, work_bytes, need);
+    ColorizeArgs a;
+    a.maps = maps; a.lut = lut; a.maxkey = need > 0 ? (unsigned long long*)work : nullptr; a.out = out;
+    a.hw = (long long)H * W; a.N = N; a.invert = invert != 0; a.max_value = max_value;
+    const dim3 grid(blocks_for(a.hw, 256, NUM_SMS * 4), B);
+    if (a.maxkey) {
+        cudaMemsetAsync(a.maxkey, 0, (size_t)need, (cudaStream_t)stream);
+        CCB_LAUNCH(colorize_max_kernel, grid, dim3(256), 0, stream, a);
+    }
+    CCB_LAUNCH(colorize_kernel, grid, dim3(256), 0, stream, a);
+    return check_launch("colorize");
+}
+
 extern "C" long long ccb_kitti_flow_errors_workspace_bytes(int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0) return -1;
     return (long long)B * blocks_for((long long)H * W, 2048, 128) * 3 * (long long)sizeof(double);
@@ -1868,7 +1953,7 @@ extern "C" int ccb_pose_errors(const float* poses, int S, int L, int rot_mode, c
     return check_launch("pose_errors");
 }
 
-template <bool UNIT>
+template <int NORM>
 static int prep_frames_launch(const char* what, const unsigned char* src_u8, float* const* dst, const float* params, const int* offs,
                               int B, int F, int Hs, int Ws, int H, int W, ccb_stream_t stream) {
     CCB_REQUIRE(src_u8 && dst && params && offs, CCB_ERR_ARG, "%s: null pointer", what);
@@ -1878,18 +1963,23 @@ static int prep_frames_launch(const char* what, const unsigned char* src_u8, flo
     a.src = src_u8; a.params = params; a.offs = offs; a.B = B; a.F = F; a.Hs = Hs; a.Ws = Ws; a.H = H; a.W = W;
     for (int f = 0; f < 8; ++f) a.dst[f] = (f < F) ? dst[f] : nullptr;
     for (int f = 0; f < F; ++f) CCB_REQUIRE(a.dst[f] != nullptr, CCB_ERR_ARG, "%s: dst[%d] is null", what, f);
-    CCB_LAUNCH(prep_frames_kernel<UNIT>, dim3(blocks_for((long long)B * F * H * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
+    CCB_LAUNCH(prep_frames_kernel<NORM>, dim3(blocks_for((long long)B * F * H * W, 256, NUM_SMS * 8)), dim3(256), 0, stream, a);
     return check_launch(what);
 }
 
 extern "C" int ccb_prep_frames(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B, int F,
                                int Hs, int Ws, int H, int W, ccb_stream_t stream) {
-    return prep_frames_launch<false>("prep_frames", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
+    return prep_frames_launch<PREP_HALF>("prep_frames", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
 }
 
 extern "C" int ccb_prep_frames_unit(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B,
                                     int F, int Hs, int Ws, int H, int W, ccb_stream_t stream) {
-    return prep_frames_launch<true>("prep_frames_unit", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
+    return prep_frames_launch<PREP_UNIT>("prep_frames_unit", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
+}
+
+extern "C" int ccb_prep_frames_inference(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B,
+                                         int F, int Hs, int Ws, int H, int W, ccb_stream_t stream) {
+    return prep_frames_launch<PREP_FIFTH>("prep_frames_inference", src_u8, dst, params, offs, B, F, Hs, Ws, H, W, stream);
 }
 
 extern "C" int ccb_rotate_frames_u8(const unsigned char* src, const double* affine, unsigned char* dst, int B, int F, int H, int W,

@@ -8,6 +8,9 @@
   flow_submission_sample  submit_flow.py:109-175                           KITTI-2015 test-set files of one sample
                         (flow_submission, flow_colors: the fused kernels; write_flow_submission: the script's files;
                         kitti_flow_errors: evaluate_flow.py compute_err :44-53 of decoded 16-bit PNGs)
+  colorize              utils.py tensor2array's 'bone' and 'rainbow' colormaps as run_inference.py saves them, in one
+                        call for a batch (colormap_table: matplotlib's lookup tables as uint8; cc_b200.run_inference
+                        runs the script)
   depth_eval_batch      test_disp.py:98-141 for a batch on the device, no host synchronisation
                         (velodyne_depth: generate_depth_map's ground truth; spline_zoom: scipy's zoom(order=3);
                         depth_errors: both scalings and compute_errors; depth_summary: the script's printed rows)
@@ -231,6 +234,72 @@ def flow_colors(flow):
     work, nbytes = _lib.workspace('ccb_flow_color_workspace_bytes', B, P, H, W, like=flow)
     out = torch.empty(B, 3, P * H, W, device=flow.device, dtype=torch.uint8)
     _lib.call('ccb_flow_color', flow, B, P, H, W, work, nbytes, out, flow)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# utils.py tensor2array's colormaps (run_inference.py): matplotlib's lookup tables built on the host, the lookup on the device
+
+# matplotlib's _bone_data (cm.get_cmap('bone', 10000)) and utils.py opencv_rainbow()'s stops (from_list(..., N=1000)):
+# per channel the (x, y0, y1) rows of LinearSegmentedColormap's segment data, and the table size
+_BONE = ([(0., 0., 0.), (0.746032, 0.652778, 0.652778), (1.0, 1.0, 1.0)],
+         [(0., 0., 0.), (0.365079, 0.319444, 0.319444), (0.746032, 0.777778, 0.777778), (1.0, 1.0, 1.0)],
+         [(0., 0., 0.), (0.365079, 0.444444, 0.444444), (1.0, 1.0, 1.0)])
+_RAINBOW_STOPS = ((0.000, (1.00, 0.00, 0.00)), (0.400, (1.00, 1.00, 0.00)), (0.600, (0.00, 1.00, 0.00)),
+                  (0.800, (0.00, 0.00, 1.00)), (1.000, (0.60, 0.00, 1.00)))
+COLORMAPS = {'bone': (_BONE, 10000),
+             'rainbow': (tuple([(x, c[k], c[k]) for x, c in _RAINBOW_STOPS] for k in range(3)), 1000)}
+
+
+def _segment_table(N, data):
+    """matplotlib's _create_lookup_table(N, data) with gamma 1: fp64 [N] in [0, 1]."""
+    a = np.array(data, np.float64)
+    x, y0, y1 = a[:, 0] * (N - 1), a[:, 1], a[:, 2]
+    xind = (N - 1) * np.linspace(0, 1, N)
+    ind = np.searchsorted(x, xind)[1:-1]
+    distance = (xind[1:-1] - x[ind - 1]) / (x[ind] - x[ind - 1])
+    lut = np.concatenate([[y1[0]], distance * (y0[ind] - y1[ind - 1]) + y1[ind - 1], [y0[-1]]])
+    return np.clip(lut, 0.0, 1.0)
+
+
+def colormap_table(name):
+    """The uint8 [N,3] table of COLORMAPS[name]: entry i is trunc(float32(255 * float32(lut[i]))), what
+    (255 * tensor2array(...)).astype(np.uint8) makes of colour i of matplotlib's fp64 table."""
+    data, N = COLORMAPS[name]
+    lut = np.stack([_segment_table(N, d) for d in data], 1).astype(np.float32)
+    return (np.float32(255) * lut).astype(np.uint8)
+
+
+_TABLES = {}
+
+
+def _device_table(name, device):
+    """colormap_table(name) on `device`, copied there once: later calls (and CUDA-graph captures) reuse it."""
+    key = (name, str(device))
+    if key not in _TABLES:
+        _TABLES[key] = torch.from_numpy(colormap_table(name)).to(device)
+    return _TABLES[key]
+
+
+@torch.no_grad()
+def colorize(maps, colormap, max_value=None, invert=False):
+    """(255 * tensor2array(x, max_value, colormap)).astype(np.uint8) of each map, HWC, on the device (ccb_colorize):
+    maps [B,H,W] (or [B,1,H,W]) -> uint8 [B,H,W,3].  invert takes 1/x first in fp32 (depth from disparity); max_value None
+    scales each image by its own maximum.  colormap is 'bone' or 'rainbow' (COLORMAPS).  No host synchronisation once
+    the colormap's table is on the device."""
+    if colormap not in COLORMAPS:
+        raise ValueError('colorize: colormap must be one of %s, got %r' % (sorted(COLORMAPS), colormap))
+    maps = _lib.f32(maps)
+    if maps.dim() == 4 and maps.size(1) == 1:
+        maps = maps[:, 0]
+    assert maps.dim() == 3, maps.shape
+    B, H, W = (int(v) for v in maps.shape)
+    lut = _device_table(colormap, maps.device)
+    per_image = max_value is None
+    work, nbytes = _lib.workspace('ccb_colorize_workspace_bytes', B, H, W, int(per_image), like=maps)
+    out = torch.empty(B, H, W, 3, device=maps.device, dtype=torch.uint8)
+    _lib.call('ccb_colorize', maps, B, H, W, lut, lut.shape[0], int(bool(invert)), int(per_image),
+              0.0 if per_image else float(max_value), work, nbytes, out, maps)
     return out
 
 

@@ -81,7 +81,9 @@ def augment_intrinsics(K, p, Ws):
     return K
 
 
-NORMALIZATIONS = ('global', 'local')
+# 'global' Normalize(.5, .5), 'local' NormalizeLocally (--data-normalization); 'inference' run_inference.py's (x/255 - .5)/.2
+NORMALIZATIONS = ('global', 'local', 'inference')
+_PREP_ENTRY = {'global': 'ccb_prep_frames', 'local': 'ccb_prep_frames_unit', 'inference': 'ccb_prep_frames_inference'}
 
 
 def rotate_affines(p, B, Hs, Ws):
@@ -151,10 +153,9 @@ def normalize_local(frames):
 
 def _prep(src, par, offs, B, F, Hs, Ws, H, W, normalization):
     """uint8 [B,F,Hs,Ws,3] on the device -> F tensors [B,3,H,W]: flip / scale-crop lookup, ArrayToTensor, then Normalize(.5,
-    .5) (global) or NormalizeLocally (local; returns its statistics, else None)."""
+    .5) (global), NormalizeLocally (local; returns its statistics, else None) or (x - .5)/.2 (inference)."""
     outs = [torch.empty(B, 3, H, W, device=src.device) for _ in range(F)]
-    fn = 'ccb_prep_frames' if normalization == 'global' else 'ccb_prep_frames_unit'
-    _lib.call(fn, src, outs, par, offs, B, F, Hs, Ws, H, W, src)
+    _lib.call(_PREP_ENTRY[normalization], src, outs, par, offs, B, F, Hs, Ws, H, W, src)
     return outs, (normalize_local(outs) if normalization == 'local' else None)
 
 
@@ -215,7 +216,7 @@ def flow_intrinsics(K, Hs, Ws, h=256, w=832, device=None):
 
 def scale_frames(frames_u8, h, w, normalization='global'):
     """Compose([Scale(h, w), ArrayToTensor(), normalize]) on the frames: uint8 [B,F,Hs,Ws,3] (a numpy array goes to the
-    library's device) -> F tensors [B,3,h,w] and the 'local' statistics (None for 'global'), as _prep returns them.
+    library's device) -> F tensors [B,3,h,w] and the 'local' statistics (None otherwise), as _prep returns them.
     Where (Hs, Ws) != (h, w) each frame is stretched (bytescale_frames) and resized (resize_frames) as imresize does to
     a float32 frame; frames already h x w go through as they are.  The identity lookup parameters are filled on the
     device, so the call makes no host synchronisation and can be captured in a CUDA graph."""

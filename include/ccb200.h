@@ -389,6 +389,14 @@ int ccb_flow_eval(const float* emask, const float* flow_cam, const float* flow_f
 long long ccb_flow_color_workspace_bytes(int B, int P, int H, int W);
 int ccb_flow_color(const float* flow, int B, int P, int H, int W, void* work, long long work_bytes, unsigned char* out,
                    ccb_stream_t stream);
+/* Colormaps of utils.py tensor2array as run_inference.py saves them, (255 * tensor2array(x, max, colormap)).astype(uint8),
+ * no host sync.  maps [B,H,W] fp32 (1/x first, in fp32, when invert != 0) -> out [B,H,W,3] uint8 through lut [N,3] uint8
+ * (device): t = (x / max) * N, each rounded in fp32; NaN is black, t < 0 takes lut[0], t >= N lut[N-1], else lut[trunc(t)].
+ * max is max_value, or each image's own maximum (any NaN makes it NaN, as torch.max) when per_image_max != 0; only then
+ * is a workspace needed. */
+long long ccb_colorize_workspace_bytes(int B, int H, int W, int per_image_max);
+int ccb_colorize(const float* maps, int B, int H, int W, const unsigned char* lut, int N, int invert, int per_image_max,
+                 float max_value, void* work, long long work_bytes, unsigned char* out, ccb_stream_t stream);
 /* KITTI flow scores of two 16-bit triplets each (evaluate_flow.py compute_err :44-53 on flow_read_png's decoding), no host
  * sync.  gt and pred [B,H,W,3] uint16 -> out [B,2] fp64 (aepe, Fl) and optionally counts [B,2] (outliers weighted by
  * valid_gt, sum of valid_gt).  fp64 block partials with a fixed-order finalize: the same bits on every run. */
@@ -460,6 +468,9 @@ int ccb_prep_frames(const unsigned char* src_u8, float* const* dst, const float*
 /* The same lookup writing v/255 only (ArrayToTensor without Normalize), for ccb_normalize_local to follow. */
 int ccb_prep_frames_unit(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B, int F,
                          int Hs, int Ws, int H, int W, ccb_stream_t stream);
+/* The same lookup writing run_inference.py's (v/255 - .5)/.2. */
+int ccb_prep_frames_inference(const unsigned char* src_u8, float* const* dst, const float* params, const int* offs, int B,
+                              int F, int Hs, int Ws, int H, int W, ccb_stream_t stream);
 /* RandomRotate (custom_transforms.py:75-85) = scipy.misc.imrotate = Pillow Image.rotate(angle, BILINEAR), bit-exact:
  * src, dst [B,F,H,W,3] uint8 (not in place); affine [B,6] fp64 maps an output pixel centre (x+.5, y+.5) to the input point
  * (a0 x + a1 y + a2, a3 x + a4 y + a5), as Pillow builds it (cc_b200.input_pipeline.pil_rotate_affine); the identity
