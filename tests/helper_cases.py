@@ -7,6 +7,7 @@ equivariance, (iii) the f1 <-> f2 symmetry, (iv) the zero-displacement channel, 
 import numpy as np
 import torch
 from tests.util import golden, T, assert_close
+from tests import layer_audit as LA
 from cc_b200 import synth, nn as cnn, loss_functions as CL, inverse_warp as CW
 from oracle import geometry as OG
 
@@ -135,6 +136,20 @@ def case_corr81_properties(device):
     d1, d2 = torch.autograd.grad((out * G).sum(), [f1r, f2r])
     lhs = float((out.detach() * G).sum())
     assert abs(float((f1 * d1).sum()) - lhs) <= 1e-4 * max(1.0, abs(lhs)) and abs(float((f2 * d2).sum()) - lhs) <= 1e-4 * max(1.0, abs(lhs))
+    # (vi) forward and both gradients held element by element to the layer audit's cost-volume bound, both tables: one
+    # channel; 6 and 13 channels, not a multiple of the kernel's channel group (the last chunk is ragged); h and w one
+    # past a multiple of the kernel's pixel tile
+    for (B_, C_, h_, w_) in ((1, 1, 17, 17), (2, 6, 17, 33), (1, 13, 33, 17)):
+        assert C_ == 1 or C_ % LA.CORR_CG
+        assert h_ % LA.CORR_CT == 1 and w_ % LA.CORR_CT == 1
+        a = torch.randn(B_, C_, h_, w_, generator=gen).to(device).requires_grad_(True)
+        b = torch.randn(B_, C_, h_, w_, generator=gen).to(device).requires_grad_(True)
+        G = torch.randn(B_, 81, h_, w_, generator=gen).to(device)
+        with LA.LayerAudit(report=False) as audit:
+            for rev in (False, True):
+                torch.autograd.grad((cnn.corr81(a, b, rev) * G).sum(), [a, b])
+        assert [(r['op'], r['phase']) for r in audit.rows] == [('corr81', 'fwd'), ('corr81', 'bwd')] * 2, audit.rows
+        assert {c for r in audit.rows for c in r['checks']} == {'out', 'd_f1', 'd_f2'}, audit.rows
 
 
 HELPER_CASES = [case_loss_helpers_golden, case_geometry_shims, case_corr81_properties]

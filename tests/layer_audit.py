@@ -578,6 +578,35 @@ def evaluate(op, checks, R=R):
     return res, max([v[0] for v in res.values()] or [0.0]), bad
 
 
+def assert_conv_within_bound(kind, x, w, stride, pad, bias=None, res=None, out_pad=0, act=None, slope=0.0, y=None, g=None,
+                             dx=None, dw=None, db=None, dres=None, what=''):
+    """One convolution (kind 'conv') or ConvTranspose2d (kind 'convT') call held element by element to the audit's
+    bound: the forward output y with its bias / residual / activation epilogue, and, given the upstream gradient g of y,
+    the gradients dx, dw, db (and dres) that were computed - the checks conv_fwd_checks / conv_bwd_checks (convT_*)
+    build, evaluated against R[kind] and REL_BAR.  act: an _lib.ACT_* code or its cc_b200.nn name (None, 'relu',
+    'leaky', 'sigmoid'); the backward differentiates it at y, so y is needed with an activation.  Unlike rel_err
+    against the largest |fp64| of the whole tensor, the bound scales with each element's own products: a k-stage that
+    lost its tf32 lo terms stands out at r = 20-230 where rel_err still reads 3e-5 to 1e-4 (tests/test_layer_audit.py).
+    Returns {check: worst r}."""
+    act = act if isinstance(act, int) else cnn.ACT[act]
+    checks = []
+    if kind == 'conv':
+        if y is not None:
+            checks += conv_fwd_checks(x, w, bias, res, stride, pad, act, slope, y)[0]
+        if g is not None:
+            checks += conv_bwd_checks(x, w, y, g, stride, pad, act, slope, dx=dx, dw=dw, db=db, dres=dres)[0]
+    else:
+        assert kind == 'convT' and res is None and dres is None, kind
+        if y is not None:
+            checks += convT_fwd_checks(x, w, bias, stride, pad, out_pad, act, slope, y)[0]
+        if g is not None:
+            checks += convT_bwd_checks(x, w, y, g, stride, pad, act, slope, dx=dx, dw=dw, db=db)[0]
+    assert checks, (kind, what, 'nothing to check')
+    out, _, bad = evaluate(kind, checks)
+    assert not bad, '%s %s over the bound (R = %.3g): %s' % (kind, what, R[kind], '; '.join(bad))
+    return {k: v[0] for k, v in out.items()}
+
+
 class LayerAudit:
     """with LayerAudit(nets={'disp': net, ...}) as audit: ... run forward / backward ...  (see the module docstring)"""
 

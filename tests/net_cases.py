@@ -3,10 +3,13 @@ GPU tests): product modules vs the golden fixtures frozen from the reference and
 import torch
 import torch.nn.functional as F
 from tests.util import golden, T, assert_close, key_with_stride, pick, conv_impl
+from tests import layer_audit as LA
 from cc_b200 import synth, nn as cnn, models as CM
 from oracle import nets as ON
 
 TOL = 1e-4
+# the fused epilogues every fprop of _conv_cross_check runs with a bias and a residual
+EPILOGUES = ('relu', 'sigmoid', 'leaky', None)
 
 
 def _wts(shape, seed, device):
@@ -14,7 +17,8 @@ def _wts(shape, seed, device):
 
 
 def case_conv_shapes(device, big=False):
-    """conv2d / conv_transpose2d forward + all gradients against torch on odd shapes."""
+    """conv2d / conv_transpose2d forward + all gradients against torch on odd shapes, and every result held element by
+    element to the layer audit's bound (layer_audit.assert_conv_within_bound)."""
     g = torch.Generator().manual_seed(0)
     cases = [  # B, Ci, H, W, Co, k, s, p, act, bias, res
         (2, 3, 13, 17, 8, 7, 2, 3, 'relu', True, False),
@@ -48,6 +52,8 @@ def case_conv_shapes(device, big=False):
         gb = torch.autograd.grad((z * wt).sum(), ins)
         for a_, b_, nm in zip(ga, gb, ('dx', 'dw', 'db/dres', 'dres')):
             assert_close(a_, b_, TOL, tag + ' ' + nm)
+        LA.assert_conv_within_bound('conv', x, w, s, p, bias=b, res=r, act=act, slope=0.2, y=y.detach(), g=wt, dx=ga[0], dw=ga[1],
+                                    db=ga[2] if bias else None, dres=ga[-1] if res else None, what=tag)
     tcases = [(2, 16, 5, 7, 8, 3, 2, 1, 1, 'relu'), (2, 24, 4, 6, 12, 4, 2, 1, 0, 'relu'), (1, 8, 3, 3, 5, 3, 1, 1, 0, None)]
     if big:
         tcases += [(4, 512, 2, 7, 512, 3, 2, 1, 1, 'relu'), (4, 96, 32, 104, 32, 4, 2, 1, 0, 'relu')]
@@ -65,11 +71,14 @@ def case_conv_shapes(device, big=False):
         gb = torch.autograd.grad((z * wt).sum(), [x, w, b])
         for a_, b_, nm in zip(ga, gb, ('dx', 'dw', 'db')):
             assert_close(a_, b_, TOL, tag + ' ' + nm)
+        LA.assert_conv_within_bound('convT', x, w, s, p, bias=b, out_pad=op, act=act, y=y.detach(), g=wt, dx=ga[0], dw=ga[1],
+                                    db=ga[2], what=tag)
 
 
 def case_conv_tc(device):
     """wgmma tensor-core path (IMPL_TC, 3xTF32) against torch fp64 on real layer shapes: fprop, dgrad (incl. strided parity
-    classes / ConvTranspose forward) and wgrad.  GPU only (the simulator has no tensor cores)."""
+    classes / ConvTranspose forward) and wgrad, each result also held element by element to the layer audit's bound
+    (layer_audit.assert_conv_within_bound).  GPU only (the simulator has no tensor cores)."""
     from cc_b200 import _lib
     g = torch.Generator().manual_seed(7)
     shapes = [(2, 32, 16, 24, 64, 3, 1, 1), (2, 17, 13, 20, 40, 3, 2, 1), (4, 128, 32, 104, 128, 3, 1, 1),
@@ -84,8 +93,9 @@ def case_conv_tc(device):
             xd, wd, bd = [t.detach().double().requires_grad_(True) for t in (x, w, b)]
             tag = f'tc {Ci}->{Co} k{k} s{s}'
             # fused epilogue (bias + LeakyReLU) in the forward ...
-            assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(F.conv2d(xd, wd, bd, s, p), 0.2), 1e-4,
-                         tag + ' fprop+leaky')
+            y = cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2)
+            assert_close(y, F.leaky_relu(F.conv2d(xd, wd, bd, s, p), 0.2), 1e-4, tag + ' fprop+leaky')
+            LA.assert_conv_within_bound('conv', x, w, s, p, bias=b, act='leaky', slope=0.2, y=y, what=tag + ' fprop+leaky')
             # ... gradients with a linear epilogue: a forward difference of 1e-6 flips LeakyReLU masks of
             # near-zero pre-activations, which changes dx by ~1e-2 for ANY two implementations
             zd = F.conv2d(xd, wd, bd, s, p)
@@ -97,6 +107,7 @@ def case_conv_tc(device):
             assert_close(gx, gd[0], 1e-4, tag + ' dgrad')
             assert_close(gw, gd[1], 1e-4, tag + ' wgrad')
             assert_close(gb, gd[2], 1e-4, tag + ' bias grad')
+            LA.assert_conv_within_bound('conv', x, w, s, p, bias=b, y=y.detach(), g=wt, dx=gx, dw=gw, db=gb, what=tag)
         # ConvTranspose2d forward == strided dgrad parity classes
         x = torch.randn(4, 96, 8, 28, generator=g).to(device).requires_grad_(True)      # small M per parity class: split-K
         b = torch.randn(32, generator=g).to(device)
@@ -111,14 +122,20 @@ def case_conv_tc(device):
             gb_ = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd])
             assert_close(ga[0], gb_[0], 1e-4, f'tc convT k{k} dx')
             assert_close(ga[1], gb_[1], 1e-4, f'tc convT k{k} dw')
+            LA.assert_conv_within_bound('convT', x, w, 2, 1, bias=b, out_pad=op, y=y.detach(), g=wt, dx=ga[0], dw=ga[1],
+                                        what=f'tc convT k{k} s2')
 
 
 def _conv_cross_check(device, shapes, seed, name):
     """Every shape through both convolution families - the wgmma tensor-core kernels (IMPL_TC, 3xTF32) and the CUDA-core
     FFMA kernels - each against torch fp64 and against each other: two independent implementations of the same
-    convolution, forward with a fused bias + LeakyReLU epilogue and with a linear one, data / weight / bias gradients."""
+    convolution, forward with a fused bias + LeakyReLU epilogue, with bias + residual under each activation of EPILOGUES
+    and with a linear one, data / weight / bias gradients.  Every result of both is also held element by element to the
+    layer audit's bound (layer_audit.assert_conv_within_bound).  Returns one row per shape and implementation: the
+    worst r of the forward outputs (y), the data (dx), weight (dw) and bias (db) gradients."""
     from cc_b200 import _lib
     g = torch.Generator().manual_seed(seed)
+    rows = []
     for (B, Ci, H, W, Co, k, s, p) in shapes:
         tag = f'{name} {Ci}->{Co} k{k} s{s} {H}x{W}'
         x = torch.randn(B, Ci, H, W, generator=g).to(device).requires_grad_(True)
@@ -127,18 +144,32 @@ def _conv_cross_check(device, shapes, seed, name):
         xd, wd, bd = [t.detach().double().requires_grad_(True) for t in (x, w, b)]
         zd = F.conv2d(xd, wd, bd, s, p)
         wt = _wts(zd.shape, 9, device)
+        res = _wts(zd.shape, 10, device)
         gd = torch.autograd.grad((zd * wt.double()).sum(), [xd, wd, bd])
         outs = {}
         for impl in (_lib.IMPL_TC, _lib.IMPL_FFMA):
+            worst = {}
+
+            def bound(what, **kw):
+                for c, r in LA.assert_conv_within_bound('conv', x, w, s, p, what=f'{tag} impl {impl} {what}', **kw).items():
+                    worst[c] = max(worst.get(c, 0.0), r)
             with conv_impl(impl):
-                assert_close(cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2), F.leaky_relu(zd, 0.2), 1e-4, f'{tag} impl {impl} fprop+leaky')
+                y = cnn.conv2d(x, w, b, None, s, p, 'leaky', 0.2)
+                assert_close(y, F.leaky_relu(zd, 0.2), 1e-4, f'{tag} impl {impl} fprop+leaky')
+                bound('fprop+leaky', bias=b, act='leaky', slope=0.2, y=y)
+                for act in EPILOGUES:
+                    y = cnn.conv2d(x, w, b, res, s, p, act, 0.2)
+                    bound(f'fprop+residual {act}', bias=b, res=res, act=act, slope=0.2, y=y)
                 y = cnn.conv2d(x, w, b, None, s, p, None, 0.2)
                 gx, gw, gb = torch.autograd.grad((y * wt).sum(), [x, w, b])
             outs[impl] = (y.detach(), gx, gw, gb)
             for got, ref, what in zip(outs[impl], (zd,) + tuple(gd), ('fprop', 'dgrad', 'wgrad', 'bias grad')):
                 assert_close(got, ref, 1e-4, f'{tag} impl {impl} {what}')
+            bound('fprop, dgrad, wgrad, bias grad', bias=b, y=y.detach(), g=wt, dx=gx, dw=gw, db=gb)
+            rows.append(dict(shape=[B, Ci, H, W, Co, k, s, p], impl=impl, r=worst))
         for a_, b_, what in zip(outs[_lib.IMPL_TC], outs[_lib.IMPL_FFMA], ('fprop', 'dgrad', 'wgrad', 'bias grad')):
             assert_close(a_, b_, 1e-4, f'{tag} tensor-core vs CUDA-core kernels {what}')
+    return rows
 
 
 def case_conv_tma_family(device):
@@ -406,6 +437,21 @@ def case_bn_upsample(device):
     assert_close(u, v, 1e-6, 'upsample2x')
     wt = _wts(u.shape, 4, device)
     assert_close(torch.autograd.grad((u * wt).sum(), [x2])[0], torch.autograd.grad((v * wt).sum(), [x2])[0], 1e-6, 'upsample2x bwd')
+    # every result held element by element to the layer audit's BatchNorm bound at the edges of the per-channel split:
+    # B * plane = BN_CHUNK (one full split), BN_CHUNK + 1 (a second split of one value) and two values per channel
+    # (torch refuses one in training mode)
+    for i, shape in enumerate([(2, 3, 64, 64), (1, 3, 3, 2731), (2, 3, 1, 1)]):
+        assert shape[0] * shape[2] * shape[3] == (LA.BN_CHUNK, LA.BN_CHUNK + 1, 2)[i], shape
+        xs = (torch.randn(shape, generator=g) * 2 + 5).to(device).requires_grad_(True)
+        bn3 = cnn.BatchNorm2d(3).to(device)
+        with torch.no_grad():
+            bn3.weight.copy_(torch.rand(3, generator=g) + 0.5); bn3.bias.copy_(torch.randn(3, generator=g))
+        with LA.LayerAudit(nets={'bn': bn3}, report=False) as audit:
+            y = bn3(xs)
+            torch.autograd.grad((y * _wts(y.shape, 11 + i, device)).sum(), [xs, bn3.weight, bn3.bias])
+        assert [(r['op'], r['phase']) for r in audit.rows] == [('bn', 'fwd'), ('bn', 'bwd')], audit.rows
+        assert set(audit.rows[0]['checks']) == {'mean', 'invstd', 'running_mean', 'running_var', 'y'}, audit.rows[0]
+        assert set(audit.rows[1]['checks']) == {'dx', 'dgamma', 'dbeta'}, audit.rows[1]
 
 
 def _load(mod, params, device):

@@ -253,10 +253,19 @@ def case_main(device, tmp, capsys, run):
     net = RI.load_disp_net(checkpoint(), 'DispNetS', device)
     prod = RI.infer(net, frames, *size, no_resize='--no-resize' in argv, output_disp='disp' in kinds,
                     output_depth='depth' in kinds)
+    # a --dataset-dir folder is listed in os.listdir order, which differs between file systems: the fixture holds the
+    # order of the machine that made it, so each image is matched by its output name - the last photo that writes it
+    source = {}
+    for i, f in enumerate(res['files']):
+        for kind, p in zip(('disp', 'depth'), RI.output_names(f, 'out')):
+            if kind in kinds:
+                source[os.path.basename(p)] = (i, kind)
+    assert sorted(source) == sorted(final), (sorted(source), sorted(final))
     differing = 0
     for n, k in final.items():
-        i, kind = k // len(kinds), kinds[k % len(kinds)]
-        disp = d['%s_disp_%d' % (run, i)][0, 0]
+        i, kind = source[n]
+        assert kind == kinds[k % len(kinds)], (n, kind)
+        disp = d['%s_disp_%d' % (run, k // len(kinds))][0, 0]
         want = np.ascontiguousarray(d['%s_saved_%d' % (run, k)].transpose(1, 2, 0))
         got = prod[i][kind].cpu().numpy()
         cm, mv, inv = ('bone', None, False) if kind == 'disp' else ('rainbow', 10, True)

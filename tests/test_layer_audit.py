@@ -1,9 +1,10 @@
 """The layer audit's checker (tests/layer_audit.py), without a GPU.
 
 fp32 torch ops stand in for the kernels: correct fp32 results must pass every bound, and each of six typical kernel
-bugs applied to an otherwise correct result must be flagged.  The wrappers must restore the autograd Functions on exit,
-also when the audit raises.  Then the audit runs on the CPU simulator build of the product kernels over the four
-networks, one forward and one backward each (DispResNet6 and PoseNetB6 at b2 64x128, MaskNet6 and Back2Future at
+bugs applied to an otherwise correct result must be flagged; so must three faults of the tensor-core convolutions'
+3xTF32 stage ring, emulated on the CPU, that rel_err's 1e-4 bar alone can miss.  The wrappers must restore the autograd
+Functions on exit, also when the audit raises.  Then the audit runs on the CPU simulator build of the product kernels
+over the four networks, one forward and one backward each (DispResNet6 and PoseNetB6 at b2 64x128, MaskNet6 and Back2Future at
 b1 64x64, FlowNetC6 at b1 64x128), which covers the CUDA-core convolutions and the BatchNorm, upsample, cost-volume and
 feature-warp kernels; and over the evaluation forwards in eval mode, which covers the eval-mode BatchNorm kernel.  Three
 mistakes in an eval-mode BatchNorm result (eps, the running mean, invstd) must each be flagged."""
@@ -45,6 +46,62 @@ def test_conv_forward_border_tap_dropped():
     z[1, 5, 0, 0] -= (x[1, :, 0, 0] * w[5, :, 1, 1]).sum()
     flagged, (r, rel, _) = _flagged('conv', LA.conv_fwd_checks(x, w, b, None, 1, 1, _lib.ACT_LEAKY, 0.2, F.leaky_relu(z, 0.2))[0], 'y')
     assert flagged and r > 1e3, r
+
+
+def _tf32(t):
+    """fp32 -> tf32, round to nearest with ties away from zero (cvt.rna.tf32.f32), by bit mask."""
+    return ((t.contiguous().view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+def _conv_3xtf32(x, w, stride, pad, fault=None):
+    """The wgmma convolution's arithmetic, emulated on the CPU: the im2col operand A [pixels, K] and the weights B [K, Co]
+    in the kernel's K order (tap-major, channels inner), split into tf32 hi and lo, k-stages of 32 whose
+    hi*hi + hi*lo + lo*hi products are summed in fp64, the result rounded to fp32.  fault: 'cross terms dropped' - the
+    last k-stage keeps hi*hi only; 'stale lo' - the last k-stage multiplies the previous stage's A lo; '2xTF32' - every
+    stage drops lo*hi.  The first two are what one ring-phase or buffer-parity slip does to a single stage."""
+    B, Ci, H, W = x.shape
+    Co, _, k, _ = w.shape
+    Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
+    a = F.unfold(x, k, padding=pad, stride=stride).view(B, Ci, k * k, Ho * Wo).permute(0, 3, 2, 1).reshape(B * Ho * Wo, -1)
+    b = w.permute(0, 2, 3, 1).reshape(Co, -1).t()
+    ah, bh = _tf32(a), _tf32(b)
+    al, bl = _tf32(a - ah), _tf32(b - bh)
+    ah, bh, al, bl = ah.double(), bh.double(), al.double(), bl.double()
+    K = a.shape[1]
+    acc = torch.zeros(a.shape[0], Co, dtype=torch.float64)
+    last = (K - 1) // 32 * 32
+    for k0 in range(0, K, 32):
+        sl = slice(k0, k0 + 32)
+        acc += ah[:, sl] @ bh[sl]
+        if fault == 'cross terms dropped' and k0 == last:
+            continue
+        alo = al[:, k0 - 32:k0 - 32 + (min(K, k0 + 32) - k0)] if fault == 'stale lo' and k0 == last else al[:, sl]
+        acc += ah[:, sl] @ bl[sl]
+        if fault != '2xTF32':
+            acc += alo @ bh[sl]
+    return acc.float().view(B, Ho * Wo, Co).permute(0, 2, 1).reshape(B, Co, Ho, Wo)
+
+
+@pytest.mark.parametrize('fault', ['cross terms dropped', 'stale lo', '2xTF32'])
+def test_conv_tf32_stage_fault_flagged(fault):
+    """Three plausible faults of the 3xTF32 stage ring, emulated on the CPU (no device kernel is touched) on shapes of
+    the ring tests' plan grid: the element-wise bound flags each on every shape (the correct emulation passes), while
+    rel_err's 1e-4 bar alone lets a one-stage fault through on at least one of them - why the convolution edge tests
+    hold every result to the bound."""
+    missed = []
+    for i, (B, Ci, H, W, Co, k, s, p) in enumerate([(2, 64, 16, 16, 64, 3, 1, 1), (2, 32, 8, 8, 20, 3, 1, 1),
+                                                     (1, 512, 8, 8, 64, 3, 1, 1)]):
+        g = _gen(30 + i)
+        x = torch.randn(B, Ci, H, W, generator=g)
+        w = torch.randn(Co, Ci, k, k, generator=g) / (Ci * k * k) ** 0.5
+        r_ok = _passes('conv', LA.conv_fwd_checks(x, w, None, None, s, p, _lib.ACT_NONE, 0.0, _conv_3xtf32(x, w, s, p))[0])
+        assert r_ok < 1, r_ok
+        flagged, (r, rel, _) = _flagged('conv', LA.conv_fwd_checks(x, w, None, None, s, p, _lib.ACT_NONE, 0.0,
+                                                                    _conv_3xtf32(x, w, s, p, fault))[0], 'y')
+        assert flagged and r > LA.R['conv'], (fault, (B, Ci, H, W, Co, k, s, p), r, rel)
+        if rel <= LA.REL_BAR:
+            missed.append(((B, Ci, H, W, Co, k, s, p), r, rel))
+    assert missed or fault == '2xTF32', (fault, 'rel_err alone catches it on every shape')
 
 
 def test_dgrad_parity_class_shifted():
