@@ -13,7 +13,9 @@
                         runs the script)
   depth_eval_batch      test_disp.py:98-141 for a batch on the device, no host synchronisation
                         (velodyne_depth: generate_depth_map's ground truth; spline_zoom: scipy's zoom(order=3);
-                        depth_errors: both scalings and compute_errors; depth_summary: the script's printed rows)
+                        depth_errors: both scalings and compute_errors; depth_summary: the script's printed rows;
+                        kitti_depth_framework / stillbox_depth_framework: the two test_frameworks' files and
+                        displacements; cc_b200.test_disp runs the script)
   make3d_eval_batch     test_make3d.py:97-148 for a batch on the device, no host synchronisation
                         (make3d_files / load_make3d: test_framework's files and samples; make3d_frames: imresize's contrast
                         stretch, Pillow's resize and the normalisation; make3d_depth_errors: the capped median scaling and
@@ -247,8 +249,13 @@ _BONE = ([(0., 0., 0.), (0.746032, 0.652778, 0.652778), (1.0, 1.0, 1.0)],
          [(0., 0., 0.), (0.365079, 0.444444, 0.444444), (1.0, 1.0, 1.0)])
 _RAINBOW_STOPS = ((0.000, (1.00, 0.00, 0.00)), (0.400, (1.00, 1.00, 0.00)), (0.600, (0.00, 1.00, 0.00)),
                   (0.800, (0.00, 0.00, 1.00)), (1.000, (0.60, 0.00, 1.00)))
+# matplotlib's _hot_data (cm.get_cmap('hot'), N = 256): test_disp.py's --output-dir images
+_HOT = ([(0., 0.0416, 0.0416), (0.365079, 1.0, 1.0), (1.0, 1.0, 1.0)],
+        [(0., 0., 0.), (0.365079, 0., 0.), (0.746032, 1.0, 1.0), (1.0, 1.0, 1.0)],
+        [(0., 0., 0.), (0.746032, 0., 0.), (1.0, 1.0, 1.0)])
 COLORMAPS = {'bone': (_BONE, 10000),
-             'rainbow': (tuple([(x, c[k], c[k]) for x, c in _RAINBOW_STOPS] for k in range(3)), 1000)}
+             'rainbow': (tuple([(x, c[k], c[k]) for x, c in _RAINBOW_STOPS] for k in range(3)), 1000),
+             'hot': (_HOT, 256)}
 
 
 def _segment_table(N, data):
@@ -285,7 +292,7 @@ def _device_table(name, device):
 def colorize(maps, colormap, max_value=None, invert=False):
     """(255 * tensor2array(x, max_value, colormap)).astype(np.uint8) of each map, HWC, on the device (ccb_colorize):
     maps [B,H,W] (or [B,1,H,W]) -> uint8 [B,H,W,3].  invert takes 1/x first in fp32 (depth from disparity); max_value None
-    scales each image by its own maximum.  colormap is 'bone' or 'rainbow' (COLORMAPS).  No host synchronisation once
+    scales each image by its own maximum.  colormap is a name of COLORMAPS.  No host synchronisation once
     the colormap's table is on the device."""
     if colormap not in COLORMAPS:
         raise ValueError('colorize: colormap must be one of %s, got %r' % (sorted(COLORMAPS), colormap))
@@ -450,11 +457,12 @@ def depth_errors(gt, pred, min_depth=1e-3, max_depth=80.0, crop='eigen', poses=N
 
 @torch.no_grad()
 def depth_eval_batch(disp_net, tgt, gt_depth, min_depth=1e-3, max_depth=80.0, crop='eigen', pose_net=None, refs=None,
-                     displacements=None, spatial_normalize=False):
+                     displacements=None, spatial_normalize=False, want_disp=False):
     """test_disp.py:100-141 for a batch: tgt [B,3,h,w] and refs (list of [B,3,h,w]) normalised device tensors (DeviceScale
     makes them from uint8 frames), gt_depth fp64 [B,H,W] (velodyne_depth), displacements [B,R] -> fp64 [B,2,7] on the
     device, row 0 scaled by the pose net's displacements (zeros without a pose net), row 1 by the median ratio.  The pose
-    net may return PoseExpNet's (mask, pose).  No host synchronisation."""
+    net may return PoseExpNet's (mask, pose).  want_disp also returns the disparity the errors come from, [B,1,h,w]
+    (after spatial_normalize).  No host synchronisation."""
     disp_net.eval()
     disp = disp_net(tgt)
     if spatial_normalize:
@@ -465,7 +473,8 @@ def depth_eval_batch(disp_net, tgt, gt_depth, min_depth=1e-3, max_depth=80.0, cr
     if pose_net is not None:
         pose_net.eval()
         poses = _pose(pose_net(tgt, refs))
-    return depth_errors(gt_depth, pred, min_depth, max_depth, crop, poses, displacements if poses is not None else None)
+    errors = depth_errors(gt_depth, pred, min_depth, max_depth, crop, poses, displacements if poses is not None else None)
+    return (errors, disp) if want_disp else errors
 
 
 def depth_summary(per_sample):
@@ -475,6 +484,96 @@ def depth_summary(per_sample):
     errors = np.zeros((2, 7, per_sample.shape[0]), np.float32)
     errors[:] = per_sample.transpose(1, 2, 0)
     return errors.mean(2)
+
+
+def _depth_shifts(seq_length, step=1):
+    """The reference frames' offsets of read_scene_data: -demi..-1, 1..demi (times step), demi = (seq_length - 1) // 2."""
+    demi = (seq_length - 1) // 2
+    return [step * i for i in list(range(-demi, 0)) + list(range(1, demi + 1))]
+
+
+def kitti_displacements(oxts_root, index, shifts, timestamps=None):
+    """kitti_eval's get_displacements: speed |oxts[8:11]| of frame `index` times |t_index - t_index+shift| per shift, the
+    times parsed as the reference parses them (strptime(ts[:-3]).timestamp(); only their differences are used, so the
+    time zone drops out).  timestamps: a dict that caches each drive's timestamps.txt across calls."""
+    import datetime
+    import os
+    cache = {} if timestamps is None else timestamps
+    if oxts_root not in cache:
+        with open(os.path.join(oxts_root, 'timestamps.txt')) as f:
+            cache[oxts_root] = [datetime.datetime.strptime(ts[:-3], '%Y-%m-%d %H:%M:%S.%f').timestamp()
+                                for ts in f.read().splitlines()]
+    t = cache[oxts_root]
+    speed = np.linalg.norm(np.genfromtxt(os.path.join(oxts_root, 'data', '{:010d}.txt'.format(index)))[8:11])
+    if not all(0 <= index + s < len(t) for s in shifts):
+        raise ValueError('%s: frames %s are outside the drive\'s %d timestamps' % (oxts_root, [index + s for s in shifts],
+                                                                                  len(t)))
+    return [speed * abs(t[index] - t[index + s]) for s in shifts]
+
+
+def kitti_depth_framework(root, test_files, seq_length=3, step=1):
+    """kitti_eval/depth_evaluation_utils.py test_framework_KITTI's read_scene_data -> one dict per test file that exists,
+    in list order: 'path' (root joined to the line), 'refs' (the frames at the shifts of _depth_shifts in the same folder,
+    always .png; a missing one is the target itself with shift 0, so its displacement is 0), 'velo' (the drive's
+    velodyne_points/data/<index>.bin), 'calib_dir' (root/<date>), 'cam' (the camera folder's last two digits) and
+    'displacements' (kitti_displacements).  Prints 'getting test metadata ... ' and '<path> missing' as the reference."""
+    import os
+    shifts = _depth_shifts(seq_length, step)
+    samples, timestamps = [], {}
+    print('getting test metadata ... ')
+    for sample in test_files:
+        tgt = os.path.join(root, sample)
+        parts = sample[:-4].split('/')
+        if len(parts) != 5:
+            raise ValueError('%s: a KITTI test file is <date>/<drive>/<camera>/data/<index>.<ext>' % sample)
+        date, scene, cam_id, _, index = parts
+        refs = [os.path.join(os.path.dirname(tgt), '{:010d}.png'.format(int(index) + s)) for s in shifts]
+        capped = list(shifts)
+        for i, r in enumerate(refs):
+            if not os.path.isfile(r):
+                refs[i], capped[i] = tgt, 0
+        if not os.path.isfile(tgt):
+            print('{} missing'.format(tgt))
+            continue
+        samples.append(dict(path=tgt, refs=refs, cam=int(cam_id[-2:]), calib_dir=os.path.join(root, date),
+                            velo=os.path.join(root, date, scene, 'velodyne_points', 'data', '{}.bin'.format(index[:10])),
+                            displacements=kitti_displacements(os.path.join(root, date, scene, 'oxts'), int(index), capped,
+                                                              timestamps)))
+    return samples
+
+
+def stillbox_depth_framework(root, test_files, seq_length=3, step=1):
+    """stillbox_eval/depth_evaluation_utils.py test_framework_stillbox's read_scene_data, as kitti_depth_framework: the
+    metadata.json of every directory under root; a line is <folder>/RGB_<scene>_<index>.<ext>; the reference indices are
+    clamped into the scene (at its edges a reference is the target itself, displacement 0); 'depth' is the scene's .npy of
+    the target and 'displacements' round(|speed|, 3) * time_step * |index - ref index|."""
+    import json
+    import os
+    meta = {}
+    for d in os.listdir(root):
+        if os.path.isdir(os.path.join(root, d)):
+            with open(os.path.join(root, d, 'metadata.json')) as f:
+                meta[d] = json.load(f)
+    shifts = _depth_shifts(seq_length, step)
+    samples = []
+    print('getting test metadata ... ')
+    for sample in test_files:
+        parts = sample.split('/')
+        names = parts[-1][:-4].split('_')
+        if len(parts) != 2 or len(names) != 3:
+            raise ValueError('%s: a Stillbox test file is <folder>/RGB_<scene>_<index>.<ext>' % sample)
+        folder, index = parts[0], int(names[2])
+        scene = meta[folder]['scenes'][int(names[1])]
+        tgt = os.path.join(root, sample)
+        if not os.path.isfile(tgt):
+            print('{} missing'.format(tgt))
+            continue
+        capped = [min(max(0, index + s), scene['length'] - 1) for s in shifts]
+        speed = np.around(np.linalg.norm(scene['speed']), decimals=3)
+        samples.append(dict(path=tgt, refs=[os.path.join(root, folder, '{}'.format(scene['imgs'][i])) for i in capped],
+                            depth=os.path.join(root, folder, '{}'.format(scene['depth'][index])),
+                            displacements=[speed * scene['time_step'] * abs(index - i) for i in capped]))
+    return samples
 
 
 # ------------------------------------------------------------------------------------------------

@@ -26,6 +26,7 @@ Documented deviations:
                 names it; the reference crashes on it, inside the net for RGBA.
   batching      the frames of one size run through the net together; the reference runs one image at a time."""
 import argparse
+import contextlib
 import fnmatch
 import multiprocessing
 import os
@@ -104,6 +105,39 @@ def encode(path, img):
     Image.fromarray(img).save(path)
 
 
+@contextlib.contextmanager
+def worker_pool(workers):
+    """`workers` spawned host processes for the block: closed when it ends, terminated when it raises, and joined before
+    the block is left either way."""
+    pool = multiprocessing.get_context('spawn').Pool(workers)
+    try:
+        yield pool
+        pool.close()
+    except BaseException:
+        pool.terminate()
+        raise
+    finally:
+        pool.join()
+
+
+def chunks_ahead(pool, fn, chunks):
+    """pool.map(fn, chunk) of each chunk in turn, the next chunk handed to the workers before this one is yielded: the
+    host work of chunk k + 1 overlaps the device work of chunk k."""
+    pending = pool.map_async(fn, chunks[0]) if chunks else None
+    for k in range(len(chunks)):
+        res = pending.get()
+        pending = pool.map_async(fn, chunks[k + 1]) if k + 1 < len(chunks) else None
+        yield res
+
+
+def host_arrays(tensors):
+    """Device tensors of any shapes -> numpy arrays of the same shapes, in one device-to-host copy."""
+    import torch
+    flat = torch.cat([t.reshape(-1) for t in tensors]).cpu().numpy()
+    ends = np.cumsum([t.numel() for t in tensors])
+    return [a.reshape(t.shape) for a, t in zip(np.split(flat, ends[:-1]), tensors)]
+
+
 # ---- device ------------------------------------------------------------------------------------------------------------
 def infer(disp_net, frames, img_height=128, img_width=416, no_resize=False, output_disp=True, output_depth=True):
     """run_inference.py:56-78 for a list of uint8 H x W x 3 frames (numpy or device tensors, any sizes) -> one dict per
@@ -147,7 +181,6 @@ def main(argv=None, device=None, workers=WORKERS):
     if not (args.output_disp or args.output_depth):
         print('You must at least output one value !')
         return None
-    import torch
     from . import _lib
     disp_net = load_disp_net(args.pretrained, args.dispnet, device or _lib.device())
     os.makedirs(args.output_dir, exist_ok=True)
@@ -161,22 +194,12 @@ def main(argv=None, device=None, workers=WORKERS):
         if args.output_depth:
             last[zname] = i
     chunks = [range(i, min(i + CHUNK, len(files))) for i in range(0, len(files), CHUNK)]
-    pool = multiprocessing.get_context('spawn').Pool(workers)
     written, writes = [], []
-    try:
-        load = lambda c: pool.map_async(decode, [files[i] for i in c])  # noqa: E731
-        pending = load(chunks[0]) if chunks else None
-        for k, c in enumerate(chunks):
-            frames = pending.get()
-            pending = load(chunks[k + 1]) if k + 1 < len(chunks) else None
+    with worker_pool(workers) as pool:
+        for c, frames in zip(chunks, chunks_ahead(pool, decode, [[files[i] for i in c] for c in chunks])):
             res = infer(disp_net, frames, args.img_height, args.img_width, args.no_resize, args.output_disp,
                         args.output_depth)
-            host = {}                             # each kind's images in one copy; with --no-resize their sizes differ
-            for kind in ('disp', 'depth'):
-                if kind in res[0]:
-                    flat = torch.cat([r[kind].reshape(-1) for r in res]).cpu().numpy()
-                    ends = np.cumsum([r[kind].numel() for r in res])
-                    host[kind] = [a.reshape(r[kind].shape) for a, r in zip(np.split(flat, ends[:-1]), res)]
+            host = {kind: host_arrays([r[kind] for r in res]) for kind in ('disp', 'depth') if kind in res[0]}
             jobs = []
             for j, i in enumerate(c):
                 for kind, name in zip(('disp', 'depth'), names[i]):
@@ -186,12 +209,6 @@ def main(argv=None, device=None, workers=WORKERS):
             writes.append(pool.starmap_async(encode, jobs))
         for wr in writes:
             wr.get()
-        pool.close()
-    except BaseException:
-        pool.terminate()
-        raise
-    finally:
-        pool.join()
     return dict(files=files, written=written)
 
 
